@@ -32,8 +32,15 @@
 //     warp moves the image into shared memory with two bulk copies when the previous pair's MMAs have retired.
 //
 // 12 warps (3 warpgroups):
-//   warp 0 producer (Xn ring) | warp 1 copier | warps 2-3 builders | warps 4-7 consumers, rows 0-63 of every tile |
-//   warps 8-11 consumers, rows 64-127
+//   warpgroup 0: warp 0 producer (Xn ring) | warp 1 copier | warps 2-3 builders      -> setmaxnreg 72 registers
+//   warpgroup 1: consumers, rows 0-63 of every tile | warpgroup 2: rows 64-127     -> setmaxnreg 208 registers
+//
+// Consumer schedule per tile: the L1 chain (one commit group per K chunk, the chunk before retired and its ring stages
+// released while the next one runs), then the two signs staggered by one phase so that each short L2 / L3 chain runs on
+// the tensor pipe under the other sign's tanh:
+//   epi1+ | L2+ . epi1- | L2- . epi2+ | L3+ . epi2- | L3- . epi3+ | epi3-      ("X . e": X in flight while e runs)
+// The waits inside the chains are warp-uniform (mbar_wait_warp): a divergent spin loop while wgmmas are in flight makes
+// ptxas serialize every wgmma of the kernel.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -48,6 +55,8 @@ constexpr int T2_STAGE = T2_MT * 128;          // 16 KB: 128 rows x 64 f16
 constexpr int T2_B1_CHUNK = T2_H * 128;        // 8 KB: 64 rows x 64 f16
 constexpr int T2_W3_BLOCK = T2_ACT_PAD * 128;  // 4 KB
 constexpr uint32_t T2_SPIN_LIMIT = 1u << 28;
+// registers per thread after the split: 128 x 72 + 256 x 208 = 62 464 <= 384 x 168 = 64 512 allocated at launch
+constexpr int T2_REGS_DATA = 72, T2_REGS_MATH = 208;
 
 // ---- raw PTX wrappers ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -72,6 +81,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         if (++spins > T2_SPIN_LIMIT) __trap();            // watchdog: trap instead of hanging the GPU
     }
 }
+// The same wait with the poll result agreed across the (converged) warp, so that the spin loop branches warp-uniformly.  The
+// consumer warpgroups wait with wgmmas in flight; a per-thread (divergent) spin loop there makes ptxas serialize every wgmma
+// of the kernel (warning C7520: each HGMMA then runs to completion before the next one is issued).
+__device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
+    uint32_t spins = 0;
+    while (!__all_sync(0xffffffffu, mbar_try(bar, parity))) {
+        if (++spins > T2_SPIN_LIMIT) __trap();            // watchdog: trap instead of hanging the GPU
+    }
+}
 __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
@@ -88,6 +106,9 @@ __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarr
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// per-thread register budget of the executing warpgroup (all four warps of the warpgroup must execute it)
+template <int N> __device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // keeps the compiler from moving accesses of an operand register across a wgmma / wait
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 __device__ __forceinline__ void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
@@ -290,168 +311,173 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
     }
     __syncthreads();
 
-    if (warp == T2_W_PROD) {
-        // ===================== producer: observation stages =====================
-        if (lane == 0) {
-            uint32_t stage = 0, phase = 0;
-            const int per_tile = NKC * NP;
-            for (int i = 0; i < my_pairs; ++i)
-                for (int m = 0; m < NMT; ++m)
-                    for (int s = 0; s < per_tile; ++s) {
-                        mbar_wait(&bars[B2_EMPTY + stage], phase ^ 1);
-                        mbar_expect_tx(&bars[B2_FULL + stage], T2_STAGE);
-                        bulk_g2s(smem + L.xst + stage * T2_STAGE, p.xnt + ((size_t)m * per_tile + s) * T2_STAGE, T2_STAGE,
-                                 &bars[B2_FULL + stage]);
-                        if (++stage == NST) { stage = 0; phase ^= 1; }
-                    }
-        }
-    } else if (warp == T2_W_COPY) {
-        // ===================== copier: eps1 by TMA from the shadows (or from the image), W2/W3/bias from the image =====================
-        const T2Image I = t2_image<SPLIT>(NKC, !p.use_tma);
-        const uint8_t* my_images = p.images + (size_t)blockIdx.x * 2 * I.total;
-        const uint32_t w_bytes = 2u * NP * (T2_B1_CHUNK + T2_W3_BLOCK);
-        for (int i = 0; i < my_pairs; ++i) {
-            const uint32_t b = i & 1, u = i >> 1;
-            const uint8_t* img = my_images + (size_t)b * I.total;
-            const int pair = blockIdx.x + i * gridDim.x;
-            const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, p.err);
-            mbar_wait(&bars[B2_IMG_READY + b], u & 1);                             // builders have finished image i
-            if (i > 0) mbar_wait(&bars[B2_EPS_FREE], (i - 1) & 1);                 // previous pair's last L1 has retired
+    if (warp < T2_CONS_WARP0) {
+        // warpgroup 0 (producer, copier, builders) only moves data: its registers go to the two consumer warpgroups
+        reg_dealloc<T2_REGS_DATA>();
+        if (warp == T2_W_PROD) {
+            // ===================== producer: observation stages =====================
             if (lane == 0) {
-                mbar_expect_tx(&bars[B2_EPS_TX], (uint32_t)(NP * NKC * T2_B1_CHUNK));
-                if (p.use_tma) {
-                    const long long at = slice + p.w1;
-                    const int unit0 = (int)(((long long)(at & 7) * (long long)p.shadow_stride + (at - (at & 7))) >> 3);
-#pragma unroll
-                    for (int pc = 0; pc < NP; ++pc)
-                        for (int kc = 0; kc < NKC; ++kc)
-                            tma_load_3d(smem + L.b1 + (size_t)(kc * NP + pc) * T2_B1_CHUNK, pc ? &maps.lo : &maps.hi, 0, unit0 + 8 * kc, 0,
-                                        &bars[B2_EPS_TX]);
-                } else {
-                    for (int c = 0; c < NP * NKC; ++c)
-                        bulk_g2s(smem + L.b1 + (size_t)c * T2_B1_CHUNK, img + I.b1 + (size_t)c * T2_B1_CHUNK, T2_B1_CHUNK, &bars[B2_EPS_TX]);
-                }
-            }
-            mbar_wait(&bars[B2_EPS_TX], i & 1);
-            if (p.use_tma) {
-                // the unit holding column `obs` received the first elements of the next row: it carries the bias element
-                // eps_b1[n] (the observation tile has a constant 1 there) and zeros (obs % 8 == 0 on this path)
-                const int kcb = p.obs >> 6, ub = (p.obs & 63) >> 3;
-#pragma unroll
-                for (int rr = 0; rr < 2; ++rr) {
-                    const int n = 2 * lane + rr;
-                    const float eb = ldg_stream(p.table + slice + p.b1 + n);
-                    __half hi, lo;
-                    split_h1(eb, hi, lo);
-                    const uint32_t off = (uint32_t)(kcb * NP) * T2_B1_CHUNK + n * 128 + ((ub ^ (n & 7)) << 4);      // [kc][piece] blocks
-                    *(uint4*)(smem + L.b1 + off) = make_uint4((uint32_t)__half_as_ushort(hi), 0, 0, 0);
-                    if (SPLIT) *(uint4*)(smem + L.b1 + T2_B1_CHUNK + off) = make_uint4((uint32_t)__half_as_ushort(lo), 0, 0, 0);
-                }
-                fence_async_smem();
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bars[B2_EPS_READY]);
-            if (i > 0) mbar_wait(&bars[B2_W_FREE], (i - 1) & 1);                   // previous pair's last L3 has retired
-            if (lane == 0) {
-                mbar_expect_tx(&bars[B2_W_READY], w_bytes + 1024);
-                bulk_g2s(smem + L.w2, img + I.w2, w_bytes, &bars[B2_W_READY]);     // W2 [sign][piece], W3 [sign][piece]: contiguous in both
-                bulk_g2s((uint8_t*)bias_all + (i & 1) * 1024, img + I.bias, 1024, &bars[B2_W_READY]);
-            }
-            mbar_wait(&bars[B2_W_READY], i & 1);                                   // landed: the image slot may be rewritten
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bars[B2_IMG_FREE + b]);
-        }
-    } else if (warp < T2_CONS_WARP0) {
-        // ===================== builder warps: W2+-, W3+-, biases (and eps1 without the shadows) one pair ahead =====================
-        const int btid = tid - T2_BLD_WARP0 * 32;
-        constexpr int BT = T2_BLD_WARPS * 32;
-        const T2Image I = t2_image<SPLIT>(NKC, !p.use_tma);
-        uint8_t* my_images = p.images + (size_t)blockIdx.x * 2 * I.total;
-        const float sg = p.sigma;
-        for (int j = 0; j < my_pairs; ++j) {
-            const int pair = blockIdx.x + j * gridDim.x;
-            mbar_wait(&bars[B2_IMG_FREE + (j & 1)], (((uint32_t)j >> 1) & 1) ^ 1);
-            const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, nullptr);
-            const float* __restrict__ eps = p.table + slice;
-            uint8_t* img = my_images + (size_t)(j & 1) * I.total;
-            // W2+- / W3+-: element pairs (n, k), (n, k+1); theta +- sigma*eps with the reference's two roundings
-            const int n2 = T2_H * T2_H / 2, n3 = T2_ACT_PAD * T2_H / 2;
-            for (int e2 = btid; e2 < n2 + n3; e2 += BT) {
-                const bool l3 = e2 >= n2;
-                const int k2 = 2 * (l3 ? e2 - n2 : e2);
-                const int n = k2 >> 6, kk = k2 & 63;
-                const int off = (l3 ? p.w3 : p.w2) + k2;
-                const bool live = !l3 || n < p.act;
-                float wp0 = 0.f, wp1 = 0.f, wn0 = 0.f, wn1 = 0.f;
-                if (live) {
-                    const float d0 = __fmul_rn(sg, ldg_stream(eps + off)), d1 = __fmul_rn(sg, ldg_stream(eps + off + 1));
-                    const float t0 = __ldg(p.theta + off), t1 = __ldg(p.theta + off + 1);
-                    wp0 = __fadd_rn(t0, d0); wp1 = __fadd_rn(t1, d1); wn0 = __fadd_rn(t0, -d0); wn1 = __fadd_rn(t1, -d1);
-                }
-                const uint32_t blk = l3 ? T2_W3_BLOCK : T2_B1_CHUNK;
-                uint8_t* base = img + (l3 ? I.w3 : I.w2) + sw128_off(n, kk);
-                if (SPLIT) {
-                    __half h0, l0, h1, l1;
-                    split_h1(wp0, h0, l0); split_h1(wp1, h1, l1);
-                    *(uint32_t*)(base + 0 * blk) = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-                    *(uint32_t*)(base + 1 * blk) = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-                    split_h1(wn0, h0, l0); split_h1(wn1, h1, l1);
-                    *(uint32_t*)(base + 2 * blk) = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-                    *(uint32_t*)(base + 3 * blk) = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-                } else {
-                    *(uint32_t*)(base + 0 * blk) = pack_h2(wp0, wp1);
-                    *(uint32_t*)(base + 1 * blk) = pack_h2(wn0, wn1);
-                }
-            }
-            {
-                float* bias = (float*)(img + I.bias);
-                for (int e = btid; e < T2_H + T2_ACT_PAD; e += BT) {
-                    if (e < T2_H) {
-                        const float d = __fmul_rn(sg, ldg_stream(eps + p.b2 + e)), t = __ldg(p.theta + p.b2 + e);
-                        bias[e] = __fadd_rn(t, d); bias[T2_H + e] = __fadd_rn(t, -d);
-                    } else {
-                        const int j2 = e - T2_H;
-                        float vp = 0.f, vn = 0.f;
-                        if (j2 < p.act) {
-                            const float d = __fmul_rn(sg, ldg_stream(eps + p.b3 + j2)), t = __ldg(p.theta + p.b3 + j2);
-                            vp = __fadd_rn(t, d); vn = __fadd_rn(t, -d);
+                uint32_t stage = 0, phase = 0;
+                const int per_tile = NKC * NP;
+                for (int i = 0; i < my_pairs; ++i)
+                    for (int m = 0; m < NMT; ++m)
+                        for (int s = 0; s < per_tile; ++s) {
+                            mbar_wait(&bars[B2_EMPTY + stage], phase ^ 1);
+                            mbar_expect_tx(&bars[B2_FULL + stage], T2_STAGE);
+                            bulk_g2s(smem + L.xst + stage * T2_STAGE, p.xnt + ((size_t)m * per_tile + s) * T2_STAGE, T2_STAGE,
+                                     &bars[B2_FULL + stage]);
+                            if (++stage == NST) { stage = 0; phase ^= 1; }
                         }
-                        bias[2 * T2_H + j2] = vp; bias[2 * T2_H + T2_ACT_PAD + j2] = vn;
+            }
+        } else if (warp == T2_W_COPY) {
+            // ===================== copier: eps1 by TMA from the shadows (or from the image), W2/W3/bias from the image =====================
+            const T2Image I = t2_image<SPLIT>(NKC, !p.use_tma);
+            const uint8_t* my_images = p.images + (size_t)blockIdx.x * 2 * I.total;
+            const uint32_t w_bytes = 2u * NP * (T2_B1_CHUNK + T2_W3_BLOCK);
+            for (int i = 0; i < my_pairs; ++i) {
+                const uint32_t b = i & 1, u = i >> 1;
+                const uint8_t* img = my_images + (size_t)b * I.total;
+                const int pair = blockIdx.x + i * gridDim.x;
+                const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, p.err);
+                mbar_wait(&bars[B2_IMG_READY + b], u & 1);                             // builders have finished image i
+                if (i > 0) mbar_wait(&bars[B2_EPS_FREE], (i - 1) & 1);                 // previous pair's last L1 has retired
+                if (lane == 0) {
+                    mbar_expect_tx(&bars[B2_EPS_TX], (uint32_t)(NP * NKC * T2_B1_CHUNK));
+                    if (p.use_tma) {
+                        const long long at = slice + p.w1;
+                        const int unit0 = (int)(((long long)(at & 7) * (long long)p.shadow_stride + (at - (at & 7))) >> 3);
+#pragma unroll
+                        for (int pc = 0; pc < NP; ++pc)
+                            for (int kc = 0; kc < NKC; ++kc)
+                                tma_load_3d(smem + L.b1 + (size_t)(kc * NP + pc) * T2_B1_CHUNK, pc ? &maps.lo : &maps.hi, 0, unit0 + 8 * kc, 0,
+                                            &bars[B2_EPS_TX]);
+                    } else {
+                        for (int c = 0; c < NP * NKC; ++c)
+                            bulk_g2s(smem + L.b1 + (size_t)c * T2_B1_CHUNK, img + I.b1 + (size_t)c * T2_B1_CHUNK, T2_B1_CHUNK, &bars[B2_EPS_TX]);
                     }
                 }
+                mbar_wait(&bars[B2_EPS_TX], i & 1);
+                if (p.use_tma) {
+                    // the unit holding column `obs` received the first elements of the next row: it carries the bias element
+                    // eps_b1[n] (the observation tile has a constant 1 there) and zeros (obs % 8 == 0 on this path)
+                    const int kcb = p.obs >> 6, ub = (p.obs & 63) >> 3;
+#pragma unroll
+                    for (int rr = 0; rr < 2; ++rr) {
+                        const int n = 2 * lane + rr;
+                        const float eb = ldg_stream(p.table + slice + p.b1 + n);
+                        __half hi, lo;
+                        split_h1(eb, hi, lo);
+                        const uint32_t off = (uint32_t)(kcb * NP) * T2_B1_CHUNK + n * 128 + ((ub ^ (n & 7)) << 4);      // [kc][piece] blocks
+                        *(uint4*)(smem + L.b1 + off) = make_uint4((uint32_t)__half_as_ushort(hi), 0, 0, 0);
+                        if (SPLIT) *(uint4*)(smem + L.b1 + T2_B1_CHUNK + off) = make_uint4((uint32_t)__half_as_ushort(lo), 0, 0, 0);
+                    }
+                    fence_async_smem();
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars[B2_EPS_READY]);
+                if (i > 0) mbar_wait(&bars[B2_W_FREE], (i - 1) & 1);                   // previous pair's last L3 has retired
+                if (lane == 0) {
+                    mbar_expect_tx(&bars[B2_W_READY], w_bytes + 1024);
+                    bulk_g2s(smem + L.w2, img + I.w2, w_bytes, &bars[B2_W_READY]);     // W2 [sign][piece], W3 [sign][piece]: contiguous in both
+                    bulk_g2s((uint8_t*)bias_all + (i & 1) * 1024, img + I.bias, 1024, &bars[B2_W_READY]);
+                }
+                mbar_wait(&bars[B2_W_READY], i & 1);                                   // landed: the image slot may be rewritten
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars[B2_IMG_FREE + b]);
             }
-            if (!p.use_tma) {
-                // eps1 (unscaled) converted from the float32 slice: rows of 64, K padded to nkc*64, column `obs` = eps_b1
-                const int Kp = NKC * T2_KC;
-                for (int e2 = btid; e2 < T2_H * Kp / 2; e2 += BT) {
-                    const int n = (2 * e2) / Kp, k = (2 * e2) - n * Kp;
-                    float x0 = 0.f, x1 = 0.f;
-                    if (k < p.obs) x0 = ldg_stream(eps + p.w1 + (size_t)n * p.obs + k); else if (k == p.obs) x0 = ldg_stream(eps + p.b1 + n);
-                    if (k + 1 < p.obs) x1 = ldg_stream(eps + p.w1 + (size_t)n * p.obs + k + 1); else if (k + 1 == p.obs) x1 = ldg_stream(eps + p.b1 + n);
-                    uint8_t* dst = img + I.b1 + (size_t)((k >> 6) * NP) * T2_B1_CHUNK + sw128_off(n, k & 63);     // [kc][piece] blocks
+        } else {
+            // ===================== builder warps: W2+-, W3+-, biases (and eps1 without the shadows) one pair ahead =====================
+            const int btid = tid - T2_BLD_WARP0 * 32;
+            constexpr int BT = T2_BLD_WARPS * 32;
+            const T2Image I = t2_image<SPLIT>(NKC, !p.use_tma);
+            uint8_t* my_images = p.images + (size_t)blockIdx.x * 2 * I.total;
+            const float sg = p.sigma;
+            for (int j = 0; j < my_pairs; ++j) {
+                const int pair = blockIdx.x + j * gridDim.x;
+                mbar_wait(&bars[B2_IMG_FREE + (j & 1)], (((uint32_t)j >> 1) & 1) ^ 1);
+                const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, nullptr);
+                const float* __restrict__ eps = p.table + slice;
+                uint8_t* img = my_images + (size_t)(j & 1) * I.total;
+                // W2+- / W3+-: element pairs (n, k), (n, k+1); theta +- sigma*eps with the reference's two roundings
+                const int n2 = T2_H * T2_H / 2, n3 = T2_ACT_PAD * T2_H / 2;
+                for (int e2 = btid; e2 < n2 + n3; e2 += BT) {
+                    const bool l3 = e2 >= n2;
+                    const int k2 = 2 * (l3 ? e2 - n2 : e2);
+                    const int n = k2 >> 6, kk = k2 & 63;
+                    const int off = (l3 ? p.w3 : p.w2) + k2;
+                    const bool live = !l3 || n < p.act;
+                    float wp0 = 0.f, wp1 = 0.f, wn0 = 0.f, wn1 = 0.f;
+                    if (live) {
+                        const float d0 = __fmul_rn(sg, ldg_stream(eps + off)), d1 = __fmul_rn(sg, ldg_stream(eps + off + 1));
+                        const float t0 = __ldg(p.theta + off), t1 = __ldg(p.theta + off + 1);
+                        wp0 = __fadd_rn(t0, d0); wp1 = __fadd_rn(t1, d1); wn0 = __fadd_rn(t0, -d0); wn1 = __fadd_rn(t1, -d1);
+                    }
+                    const uint32_t blk = l3 ? T2_W3_BLOCK : T2_B1_CHUNK;
+                    uint8_t* base = img + (l3 ? I.w3 : I.w2) + sw128_off(n, kk);
                     if (SPLIT) {
                         __half h0, l0, h1, l1;
-                        split_h1(x0, h0, l0); split_h1(x1, h1, l1);
-                        *(uint32_t*)dst = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-                        *(uint32_t*)(dst + T2_B1_CHUNK) = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+                        split_h1(wp0, h0, l0); split_h1(wp1, h1, l1);
+                        *(uint32_t*)(base + 0 * blk) = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
+                        *(uint32_t*)(base + 1 * blk) = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+                        split_h1(wn0, h0, l0); split_h1(wn1, h1, l1);
+                        *(uint32_t*)(base + 2 * blk) = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
+                        *(uint32_t*)(base + 3 * blk) = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
                     } else {
-                        *(uint32_t*)dst = pack_h2(x0, x1);
+                        *(uint32_t*)(base + 0 * blk) = pack_h2(wp0, wp1);
+                        *(uint32_t*)(base + 1 * blk) = pack_h2(wn0, wn1);
                     }
                 }
+                {
+                    float* bias = (float*)(img + I.bias);
+                    for (int e = btid; e < T2_H + T2_ACT_PAD; e += BT) {
+                        if (e < T2_H) {
+                            const float d = __fmul_rn(sg, ldg_stream(eps + p.b2 + e)), t = __ldg(p.theta + p.b2 + e);
+                            bias[e] = __fadd_rn(t, d); bias[T2_H + e] = __fadd_rn(t, -d);
+                        } else {
+                            const int j2 = e - T2_H;
+                            float vp = 0.f, vn = 0.f;
+                            if (j2 < p.act) {
+                                const float d = __fmul_rn(sg, ldg_stream(eps + p.b3 + j2)), t = __ldg(p.theta + p.b3 + j2);
+                                vp = __fadd_rn(t, d); vn = __fadd_rn(t, -d);
+                            }
+                            bias[2 * T2_H + j2] = vp; bias[2 * T2_H + T2_ACT_PAD + j2] = vn;
+                        }
+                    }
+                }
+                if (!p.use_tma) {
+                    // eps1 (unscaled) converted from the float32 slice: rows of 64, K padded to nkc*64, column `obs` = eps_b1
+                    const int Kp = NKC * T2_KC;
+                    for (int e2 = btid; e2 < T2_H * Kp / 2; e2 += BT) {
+                        const int n = (2 * e2) / Kp, k = (2 * e2) - n * Kp;
+                        float x0 = 0.f, x1 = 0.f;
+                        if (k < p.obs) x0 = ldg_stream(eps + p.w1 + (size_t)n * p.obs + k); else if (k == p.obs) x0 = ldg_stream(eps + p.b1 + n);
+                        if (k + 1 < p.obs) x1 = ldg_stream(eps + p.w1 + (size_t)n * p.obs + k + 1); else if (k + 1 == p.obs) x1 = ldg_stream(eps + p.b1 + n);
+                        uint8_t* dst = img + I.b1 + (size_t)((k >> 6) * NP) * T2_B1_CHUNK + sw128_off(n, k & 63);     // [kc][piece] blocks
+                        if (SPLIT) {
+                            __half h0, l0, h1, l1;
+                            split_h1(x0, h0, l0); split_h1(x1, h1, l1);
+                            *(uint32_t*)dst = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
+                            *(uint32_t*)(dst + T2_B1_CHUNK) = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
+                        } else {
+                            *(uint32_t*)dst = pack_h2(x0, x1);
+                        }
+                    }
+                }
+                __threadfence();                                             // image visible device-wide (L2)
+                asm volatile("fence.proxy.async;" ::: "memory");             // ... and to the async proxy that will copy it
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars[B2_IMG_READY + (j & 1)]);
+                if (j + 1 < my_pairs) {                                      // L2 prefetch of the next pair's operands
+                    const long long nidx = es_checked_slice(p.idx[blockIdx.x + (j + 1) * gridDim.x], p.P, p.table_len, nullptr);
+                    const char* nxt = (const char*)(p.table + nidx);
+                    const int lines = (p.b3 + p.act) * 4 / 128 + 2;
+                    const int skip = p.use_tma ? p.b1 * 4 / 128 : 0;         // with the shadows eps1 comes by TMA
+                    for (int l = skip + btid; l < lines; l += BT) prefetch_l2(nxt + (size_t)l * 128);
+                }
             }
-            __threadfence();                                             // image visible device-wide (L2)
-            asm volatile("fence.proxy.async;" ::: "memory");             // ... and to the async proxy that will copy it
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&bars[B2_IMG_READY + (j & 1)]);
-            if (j + 1 < my_pairs) {                                      // L2 prefetch of the next pair's operands
-                const long long nidx = es_checked_slice(p.idx[blockIdx.x + (j + 1) * gridDim.x], p.P, p.table_len, nullptr);
-                const char* nxt = (const char*)(p.table + nidx);
-                const int lines = (p.b3 + p.act) * 4 / 128 + 2;
-                const int skip = p.use_tma ? p.b1 * 4 / 128 : 0;         // with the shadows eps1 comes by TMA
-                for (int l = skip + btid; l < lines; l += BT) prefetch_l2(nxt + (size_t)l * 128);
-            }
-        }
+    }
     } else {
+        reg_alloc<T2_REGS_MATH>();
         // ===================== consumer warpgroups: MMAs and epilogues of 64 rows of every tile =====================
         const int cw = warp - T2_CONS_WARP0;                  // 0..7
         const int half = cw >> 2;                             // rows 64*half .. 64*half + 63 of the tile
@@ -471,7 +497,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
             const float* bias = bias_all + (i & 1) * 256;
             double fit_p = 0.0, fit_n = 0.0;
             float pp0 = 0.f, pp1 = 0.f, pp2 = 0.f, pn0 = 0.f, pn1 = 0.f, pn2 = 0.f;     // position sums of this thread's rows
-            mbar_wait(&bars[B2_EPS_READY], i & 1);
+            mbar_wait_warp(&bars[B2_EPS_READY], i & 1);
             for (int m = 0; m < NMT; ++m) {
                 // ---- L1: V = Xn . eps1^T (SPLIT: x_hi.eps_hi + x_hi.eps_lo + x_lo.eps_hi), chunk by chunk through the ring ----
                 float v[32];
@@ -480,8 +506,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 uint32_t prev = 0;
                 for (int kc = 0; kc < NKC; ++kc) {
                     const uint32_t st = stage;
-                    mbar_wait(&bars[B2_FULL + st], phase);
-                    if (SPLIT) mbar_wait(&bars[B2_FULL + st + 1], phase);
+                    mbar_wait_warp(&bars[B2_FULL + st], phase);
+                    if (SPLIT) mbar_wait_warp(&bars[B2_FULL + st + 1], phase);
                     const uint64_t ah = a_desc0 + st * STAGE_D, al = ah + STAGE_D;
                     const uint64_t bh = b1_desc0 + (uint64_t)kc * NP * B1_D, bl = bh + B1_D;
 #pragma unroll
@@ -508,28 +534,24 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     if (SPLIT) mbar_arrive(&bars[B2_EMPTY + prev + 1]);
                     if (m == NMT - 1) mbar_arrive(&bars[B2_EPS_FREE]);            // the pair's last L1 has retired
                 }
-                if (m == 0) mbar_wait(&bars[B2_W_READY], i & 1);                  // W2, W3 and the biases of the pair in place?
+                if (m == 0) mbar_wait_warp(&bars[B2_W_READY], i & 1);                  // W2, W3 and the biases of the pair in place?
 
                 const int ta = m * T2_MT + r0, tb = ta + 8;                        // time steps of this thread's two rows
                 const float* __restrict__ urow = p.ubase + (size_t)ta * T2_H + 2 * q;
-#pragma unroll 1
-                for (int sgn = 0; sgn < 2; ++sgn) {
-                    const float s = sgn ? -sg : sg;
-                    // ---- epi1: h1 = tanh(U +- sigma V) ----
-                    uint32_t hh[16], hl[16];
-                    {
-                        float z[32];
+                // ---- epi1: h1 = tanh(U +- sigma V) ----
+                auto epi1 = [&](float s, uint32_t (&hh)[16], uint32_t (&hl)[16]) {
+                    float z[32];
 #pragma unroll
-                        for (int c = 0; c < 8; ++c) {
-                            const float2 u0 = __ldg(reinterpret_cast<const float2*>(urow + 8 * c));
-                            const float2 u1 = __ldg(reinterpret_cast<const float2*>(urow + 8 * T2_H + 8 * c));
-                            z[4 * c + 0] = __fmaf_rn(v[4 * c + 0], s, u0.x); z[4 * c + 1] = __fmaf_rn(v[4 * c + 1], s, u0.y);
-                            z[4 * c + 2] = __fmaf_rn(v[4 * c + 2], s, u1.x); z[4 * c + 3] = __fmaf_rn(v[4 * c + 3], s, u1.y);
-                        }
-                        act_pack<SPLIT>(z, hh, hl);
+                    for (int c = 0; c < 8; ++c) {
+                        const float2 u0 = __ldg(reinterpret_cast<const float2*>(urow + 8 * c));
+                        const float2 u1 = __ldg(reinterpret_cast<const float2*>(urow + 8 * T2_H + 8 * c));
+                        z[4 * c + 0] = __fmaf_rn(v[4 * c + 0], s, u0.x); z[4 * c + 1] = __fmaf_rn(v[4 * c + 1], s, u0.y);
+                        z[4 * c + 2] = __fmaf_rn(v[4 * c + 2], s, u1.x); z[4 * c + 3] = __fmaf_rn(v[4 * c + 3], s, u1.y);
                     }
-                    // ---- L2: D2 = h1 . W2^T (SPLIT: h_hi.w_hi + h_hi.w_lo + h_lo.w_hi) ----
-                    float d2[32];
+                    act_pack<SPLIT>(z, hh, hl);
+                };
+                // ---- L2: D2 = h1 . W2^T (SPLIT: h_hi.w_hi + h_hi.w_lo + h_lo.w_hi), one commit group ----
+                auto mma2 = [&](int sgn, const uint32_t (&hh)[16], const uint32_t (&hl)[16], float (&d2)[32]) {
                     const uint64_t w2h = w2d + (uint64_t)(sgn * NP) * B1_D, w2l = w2h + B1_D;
                     reg_fence(d2);
                     wg_fence();
@@ -544,21 +566,20 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                         }
                     }
                     wg_commit();
-                    wg_wait<0>();
-                    reg_fence(d2); reg_fence(hh); reg_fence(hl);
-                    // ---- epi2: h2 = tanh(D2 + b2) ----
-                    {
-                        const float* b2 = bias + sgn * T2_H + 2 * q;
+                };
+                // ---- epi2: h2 = tanh(D2 + b2) ----
+                auto epi2 = [&](int sgn, float (&d2)[32], uint32_t (&hh)[16], uint32_t (&hl)[16]) {
+                    const float* b2 = bias + sgn * T2_H + 2 * q;
 #pragma unroll
-                        for (int c = 0; c < 8; ++c) {
-                            const float2 bb = *reinterpret_cast<const float2*>(b2 + 8 * c);
-                            d2[4 * c + 0] = __fadd_rn(d2[4 * c + 0], bb.x); d2[4 * c + 1] = __fadd_rn(d2[4 * c + 1], bb.y);
-                            d2[4 * c + 2] = __fadd_rn(d2[4 * c + 2], bb.x); d2[4 * c + 3] = __fadd_rn(d2[4 * c + 3], bb.y);
-                        }
-                        act_pack<SPLIT>(d2, hh, hl);
+                    for (int c = 0; c < 8; ++c) {
+                        const float2 bb = *reinterpret_cast<const float2*>(b2 + 8 * c);
+                        d2[4 * c + 0] = __fadd_rn(d2[4 * c + 0], bb.x); d2[4 * c + 1] = __fadd_rn(d2[4 * c + 1], bb.y);
+                        d2[4 * c + 2] = __fadd_rn(d2[4 * c + 2], bb.x); d2[4 * c + 3] = __fadd_rn(d2[4 * c + 3], bb.y);
                     }
-                    // ---- L3: D3 = h2 . W3^T (N = 32) ----
-                    float d3[16];
+                    act_pack<SPLIT>(d2, hh, hl);
+                };
+                // ---- L3: D3 = h2 . W3^T (N = 32), one commit group ----
+                auto mma3 = [&](int sgn, const uint32_t (&hh)[16], const uint32_t (&hl)[16], float (&d3)[16]) {
                     const uint64_t w3h = w3d + (uint64_t)(sgn * NP) * W3_D, w3l = w3h + W3_D;
                     reg_fence(d3);
                     wg_fence();
@@ -573,10 +594,9 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                         }
                     }
                     wg_commit();
-                    wg_wait<0>();
-                    reg_fence(d3); reg_fence(hh); reg_fence(hl);
-                    if (sgn == 1 && m == NMT - 1 && lane == 0) mbar_arrive(&bars[B2_W_FREE]);   // the pair's last L3 has retired
-                    // ---- epi3: a = tanh(D3 + b3) [+ action noise]; r_t = <a_t, c_t>; positions ----
+                };
+                // ---- epi3: a = tanh(D3 + b3) [+ action noise]; r_t = <a_t, c_t>; positions ----
+                auto epi3 = [&](int sgn, const float (&d3)[16]) {
                     const float* b3 = bias + 2 * T2_H + sgn * T2_ACT_PAD;
                     float ra = 0.f, rb = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f;
 #pragma unroll
@@ -602,7 +622,32 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     const double r2 = (q == 0) ? (double)ra + (double)rb : 0.0;   // rows beyond T contribute 0
                     if (sgn) { fit_n += r2; pn0 += q0; pn1 += q1; pn2 += q2; }
                     else     { fit_p += r2; pp0 += q0; pp1 += q1; pp2 += q2; }
-                }
+                };
+                // The + sign runs one phase ahead of the - sign, so every L2 / L3 chain is in flight on the tensor pipe while the
+                // tanh of the other sign runs: L2+ under epi1-, L2- under epi2+, L3+ under epi2-, L3- under epi3+.  Each wait
+                // leaves the most recent group in flight; the reg_fences after it keep the retired chain's A fragments alive
+                // until then, and its accumulators from being read before.
+                uint32_t hp[16], lp[16], hn[16], ln[16];
+                float d2p[32], d2n[32], d3p[16], d3n[16];
+                epi1(sg, hp, lp);
+                mma2(0, hp, lp, d2p);
+                epi1(-sg, hn, ln);
+                mma2(1, hn, ln, d2n);
+                wg_wait<1>();
+                reg_fence(d2p); reg_fence(hp); if (SPLIT) reg_fence(lp);
+                epi2(0, d2p, hp, lp);
+                mma3(0, hp, lp, d3p);
+                wg_wait<1>();
+                reg_fence(d2n); reg_fence(hn); if (SPLIT) reg_fence(ln);
+                epi2(1, d2n, hn, ln);
+                mma3(1, hn, ln, d3n);
+                wg_wait<1>();
+                reg_fence(d3p); reg_fence(hp); if (SPLIT) reg_fence(lp);
+                epi3(0, d3p);
+                wg_wait<0>();
+                reg_fence(d3n); reg_fence(hn); if (SPLIT) reg_fence(ln);
+                if (m == NMT - 1 && lane == 0) mbar_arrive(&bars[B2_W_FREE]);   // the pair's last L3 has retired
+                epi3(1, d3n);
             }
             // ---- this warp's sums of the pair -> shared memory; the last of the 8 warps adds them in warp order and writes the
             //      pair's results (no global scratch, no device-wide fence: a CTA-scope release/acquire on a shared counter) ----
