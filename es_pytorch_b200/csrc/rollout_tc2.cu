@@ -22,7 +22,9 @@
 //
 // Operand staging:
 //   * Xn: pre-tiled once per generation into the exact shared-memory image of every (tile, K chunk[, piece]) stage
-//     (rollout_tc2_prep_kernel) -> one 16 KB cp.async.bulk per stage into a ring;
+//     (rollout_tc2_prep_kernel).  The ring holds 8 KB slots, one warpgroup's 64 rows of a stage each (one cp.async.bulk per
+//     slot), filled as one FIFO in the order (pair, tile, warpgroup, K chunk, piece); each slot is released by the 4 warps of
+//     the warpgroup that reads it.  SPLIT: 8 slots = 4 K chunks of lookahead, otherwise 16 slots = 16 chunks;
 //   * eps1 (82 % of a perturbation): the library keeps float16 shadows of the table (hi, and lo for SPLIT) in 8 copies shifted
 //     by 0..7 elements; in copy idx % 8 every row of eps1 is 16-byte aligned, and ONE 3-D TMA tensor copy per K chunk
 //     (dims {64 elements, origin in 16-byte units, 64 rows of stride obs*2 bytes}: overlapping strides, 128-byte swizzle)
@@ -30,15 +32,21 @@
 //     (Shapes without 16-byte aligned rows, or no memory for the shadows: builder warps convert the float32 slice.)
 //   * theta2/3 +- sigma*eps2/3 and the biases: builder warps compute them one pair ahead into an L2-resident image, a copier
 //     warp moves the image into shared memory with two bulk copies when the previous pair's MMAs have retired.
+//   * with the shadows, the copier also prefetches the next pair's eps1 into L2 (TMA prefetch, same maps and coordinates)
+//     one pair ahead, so the eps1 copy at the pair boundary reads L2 and not HBM.
 //
 // 12 warps (3 warpgroups):
 //   warpgroup 0: warp 0 producer (Xn ring) | warp 1 copier | warps 2-3 builders      -> setmaxnreg 72 registers
 //   warpgroup 1: consumers, rows 0-63 of every tile | warpgroup 2: rows 64-127     -> setmaxnreg 208 registers
 //
-// Consumer schedule per tile: the L1 chain (one commit group per K chunk, the chunk before retired and its ring stages
+// Consumer schedule per tile: the L1 chain (one commit group per K chunk, the chunk before retired and its ring slots
 // released while the next one runs), then the two signs staggered by one phase so that each short L2 / L3 chain runs on
 // the tensor pipe under the other sign's tanh:
 //   epi1+ | L2+ . epi1- | L2- . epi2+ | L3+ . epi2- | L3- . epi3+ | epi3-      ("X . e": X in flight while e runs)
+// The FIFO order of the ring staggers the two warpgroups by one L1 chain: warpgroup 1's chain of tile m is fed after
+// warpgroup 0's, so it runs while warpgroup 0 is in its epilogues, and warpgroup 0's chain of tile m + 1 runs under warpgroup
+// 1's epilogues.  No other synchronisation orders the warpgroups (an explicit turn token on top of the FIFO order measured no
+// faster at float32-equivalent precision and slower with single float16 products).
 // The waits inside the chains are warp-uniform (mbar_wait_warp): a divergent spin loop while wgmmas are in flight makes
 // ptxas serialize every wgmma of the kernel.
 #include <cuda.h>
@@ -51,7 +59,9 @@ namespace {
 constexpr int T2_THREADS = 384;
 constexpr int T2_W_PROD = 0, T2_W_COPY = 1, T2_BLD_WARP0 = 2, T2_BLD_WARPS = 2, T2_CONS_WARP0 = 4, T2_CONS_WARPS = 8;
 constexpr int T2_H = 64, T2_MT = 128, T2_KC = 64, T2_ACT_PAD = 32;
-constexpr int T2_STAGE = T2_MT * 128;          // 16 KB: 128 rows x 64 f16
+constexpr int T2_STAGE = T2_MT * 128;          // 16 KB: 128 rows x 64 f16 (one tile's K chunk piece in the xnt image)
+constexpr int T2_SLOT = T2_STAGE / 2;          // 8 KB: the 64 rows of one consumer warpgroup (one observation ring slot)
+constexpr int T2_WG_WARPS = T2_CONS_WARPS / 2; // warps per consumer warpgroup
 constexpr int T2_B1_CHUNK = T2_H * 128;        // 8 KB: 64 rows x 64 f16
 constexpr int T2_W3_BLOCK = T2_ACT_PAD * 128;  // 4 KB
 constexpr uint32_t T2_SPIN_LIMIT = 1u << 28;
@@ -98,6 +108,14 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 __device__ __forceinline__ void tma_load_3d(void* dst_smem, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(dst_smem)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// the same box fetched into L2 only
+__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* map, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// first 16-byte unit of a slice's eps1 in the shifted shadow copy where its rows are 16-byte aligned
+__device__ __forceinline__ int t2_shadow_unit(long long at, size_t shadow_stride) {
+    return (int)(((long long)(at & 7) * (long long)shadow_stride + (at - (at & 7))) >> 3);
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
@@ -235,7 +253,7 @@ struct T2Params {
 
 template <bool SPLIT> struct T2Cfg {
     static constexpr int NP = SPLIT ? 2 : 1;              // pieces per operand
-    static constexpr int NST = SPLIT ? 4 : 8;             // observation stages in the ring
+    static constexpr int NSLOT = SPLIT ? 8 : 16;          // 8 KB slots in the observation ring (a power of 2)
 };
 
 struct T2Smem { uint32_t b1, xst, w2, w3, bias, red, bars, total; };
@@ -244,7 +262,7 @@ template <bool SPLIT> __host__ __device__ inline T2Smem t2_layout(int nkc) {
     T2Smem L;
     uint32_t o = 0;
     L.b1 = o;   o += (uint32_t)C::NP * nkc * T2_B1_CHUNK;         // [kc][piece][64 rows x 128 B]
-    L.xst = o;  o += (uint32_t)C::NST * T2_STAGE;
+    L.xst = o;  o += (uint32_t)C::NSLOT * T2_SLOT;
     L.w2 = o;   o += 2u * C::NP * T2_B1_CHUNK;                    // [sign][piece][64 rows x 128 B]
     L.w3 = o;   o += 2u * C::NP * T2_W3_BLOCK;                    // [sign][piece][32 rows x 128 B]
     L.bias = o; o += 2 * 1024;                                    // double-buffered by pair parity
@@ -267,8 +285,9 @@ template <bool SPLIT> __host__ __device__ inline T2Image t2_image(int nkc, int w
     return I;
 }
 
-enum { B2_FULL = 0, B2_EMPTY = 8, B2_EPS_TX = 16, B2_EPS_READY, B2_EPS_FREE, B2_W_READY, B2_W_FREE, B2_IMG_READY,
+enum { B2_FULL = 0, B2_EMPTY = 16, B2_EPS_TX = 32, B2_EPS_READY, B2_EPS_FREE, B2_W_READY, B2_W_FREE, B2_IMG_READY,
        B2_IMG_FREE = B2_IMG_READY + 2, B2_COUNT = B2_IMG_FREE + 2 };
+static_assert(T2Cfg<true>::NSLOT <= B2_EMPTY && T2Cfg<false>::NSLOT <= B2_EMPTY, "barrier enum too small for the ring");
 static_assert(B2_COUNT * 8 + 16 <= 1024, "barrier block too small");
 
 // tanh of an accumulator fragment (+ bias / + U +- sigma V) packed into the A fragments of the next layer: the m64nN
@@ -288,7 +307,7 @@ template <bool SPLIT, bool NOISE>
 __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid_constant__ T2Params p,
                                                                      const __grid_constant__ T2Maps maps) {
     using C = T2Cfg<SPLIT>;
-    constexpr int NP = C::NP, NST = C::NST;
+    constexpr int NP = C::NP, NSLOT = C::NSLOT;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     const T2Smem L = t2_layout<SPLIT>(p.nkc);
@@ -303,7 +322,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
     if (tid == 0) {
         ((unsigned*)(smem + L.red + 2 * T2_CONS_WARPS * 64))[0] = 0;
         ((unsigned*)(smem + L.red + 2 * T2_CONS_WARPS * 64))[1] = 0;
-        for (int s = 0; s < NST; ++s) { mbar_init(&bars[B2_FULL + s], 1); mbar_init(&bars[B2_EMPTY + s], T2_CONS_WARPS); }
+        for (int s = 0; s < NSLOT; ++s) { mbar_init(&bars[B2_FULL + s], 1); mbar_init(&bars[B2_EMPTY + s], T2_WG_WARPS); }
         mbar_init(&bars[B2_EPS_TX], 1); mbar_init(&bars[B2_EPS_READY], 1); mbar_init(&bars[B2_EPS_FREE], T2_CONS_WARPS);
         mbar_init(&bars[B2_W_READY], 1); mbar_init(&bars[B2_W_FREE], T2_CONS_WARPS);
         for (int b = 0; b < 2; ++b) { mbar_init(&bars[B2_IMG_READY + b], T2_BLD_WARPS); mbar_init(&bars[B2_IMG_FREE + b], 1); }
@@ -315,19 +334,23 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
         // warpgroup 0 (producer, copier, builders) only moves data: its registers go to the two consumer warpgroups
         reg_dealloc<T2_REGS_DATA>();
         if (warp == T2_W_PROD) {
-            // ===================== producer: observation stages =====================
+            // ===================== producer: observation ring =====================
+            // One FIFO of 8 KB slots in the order (pair, tile, warpgroup half, K chunk, piece): a slot is one warpgroup's 64
+            // rows of a 16 KB stage image, so warpgroup 1's chain of a tile is fed after warpgroup 0's, and warpgroup 0's chain
+            // of the next tile after that.
             if (lane == 0) {
-                uint32_t stage = 0, phase = 0;
+                uint32_t slot = 0, phase = 0;
                 const int per_tile = NKC * NP;
                 for (int i = 0; i < my_pairs; ++i)
                     for (int m = 0; m < NMT; ++m)
-                        for (int s = 0; s < per_tile; ++s) {
-                            mbar_wait(&bars[B2_EMPTY + stage], phase ^ 1);
-                            mbar_expect_tx(&bars[B2_FULL + stage], T2_STAGE);
-                            bulk_g2s(smem + L.xst + stage * T2_STAGE, p.xnt + ((size_t)m * per_tile + s) * T2_STAGE, T2_STAGE,
-                                     &bars[B2_FULL + stage]);
-                            if (++stage == NST) { stage = 0; phase ^= 1; }
-                        }
+                        for (int h = 0; h < 2; ++h)
+                            for (int s = 0; s < per_tile; ++s) {
+                                mbar_wait(&bars[B2_EMPTY + slot], phase ^ 1);
+                                mbar_expect_tx(&bars[B2_FULL + slot], T2_SLOT);
+                                bulk_g2s(smem + L.xst + slot * T2_SLOT, p.xnt + ((size_t)m * per_tile + s) * T2_STAGE + h * T2_SLOT,
+                                         T2_SLOT, &bars[B2_FULL + slot]);
+                                if (++slot == NSLOT) { slot = 0; phase ^= 1; }
+                            }
             }
         } else if (warp == T2_W_COPY) {
             // ===================== copier: eps1 by TMA from the shadows (or from the image), W2/W3/bias from the image =====================
@@ -344,8 +367,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 if (lane == 0) {
                     mbar_expect_tx(&bars[B2_EPS_TX], (uint32_t)(NP * NKC * T2_B1_CHUNK));
                     if (p.use_tma) {
-                        const long long at = slice + p.w1;
-                        const int unit0 = (int)(((long long)(at & 7) * (long long)p.shadow_stride + (at - (at & 7))) >> 3);
+                        const int unit0 = t2_shadow_unit(slice + p.w1, p.shadow_stride);
 #pragma unroll
                         for (int pc = 0; pc < NP; ++pc)
                             for (int kc = 0; kc < NKC; ++kc)
@@ -375,6 +397,14 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&bars[B2_EPS_READY]);
+                if (p.use_tma && lane == 0 && i + 1 < my_pairs) {
+                    // the next pair's eps1 rows into L2 now, so that its TMA at the pair boundary does not wait on HBM
+                    const long long nslice = es_checked_slice(p.idx[pair + gridDim.x], p.P, p.table_len, nullptr);
+                    const int nunit0 = t2_shadow_unit(nslice + p.w1, p.shadow_stride);
+#pragma unroll
+                    for (int pc = 0; pc < NP; ++pc)
+                        for (int kc = 0; kc < NKC; ++kc) tma_prefetch_3d(pc ? &maps.lo : &maps.hi, 0, nunit0 + 8 * kc, 0);
+                }
                 if (i > 0) mbar_wait(&bars[B2_W_FREE], (i - 1) & 1);                   // previous pair's last L3 has retired
                 if (lane == 0) {
                     mbar_expect_tx(&bars[B2_W_READY], w_bytes + 1024);
@@ -485,13 +515,15 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
         const int r0 = half * 64 + (cw & 3) * 16 + (lane >> 2);   // this thread's rows: r0 and r0 + 8
         const float sg = p.sigma;
         const bool want_pos = p.behv_pos != nullptr;
-        const uint64_t a_desc0 = wg_desc_sw128(smem_u32(smem + L.xst + half * (T2_STAGE / 2)));
+        const uint64_t a_desc0 = wg_desc_sw128(smem_u32(smem + L.xst));
         const uint64_t b1_desc0 = wg_desc_sw128(smem_u32(smem + L.b1));
         const uint64_t w2d = wg_desc_sw128(smem_u32(smem + L.w2)), w3d = wg_desc_sw128(smem_u32(smem + L.w3));
-        constexpr uint64_t STAGE_D = T2_STAGE >> 4, B1_D = T2_B1_CHUNK >> 4, W3_D = T2_W3_BLOCK >> 4;
+        constexpr uint64_t SLOT_D = T2_SLOT >> 4, B1_D = T2_B1_CHUNK >> 4, W3_D = T2_W3_BLOCK >> 4;
         double* red = (double*)(smem + L.red);                // [pair parity][8 warps][8]: per-pair sums of every consumer warp
         unsigned* red_cnt = (unsigned*)(smem + L.red + 2 * T2_CONS_WARPS * 64);
-        uint32_t stage = 0, phase = 0;
+        // The ring holds the chains of both warpgroups in turn: warpgroup 0's slots of tile m, then warpgroup 1's, then
+        // warpgroup 0's of tile m + 1, ...  `fifo` is the ring position of this warpgroup's next slot.
+        uint32_t fifo = (uint32_t)(half * NKC * NP);
         for (int i = 0; i < my_pairs; ++i) {
             const int pair = blockIdx.x + i * gridDim.x;
             const float* bias = bias_all + (i & 1) * 256;
@@ -505,10 +537,10 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 wg_fence();
                 uint32_t prev = 0;
                 for (int kc = 0; kc < NKC; ++kc) {
-                    const uint32_t st = stage;
+                    const uint32_t st = fifo & (NSLOT - 1), phase = (fifo / NSLOT) & 1;
                     mbar_wait_warp(&bars[B2_FULL + st], phase);
                     if (SPLIT) mbar_wait_warp(&bars[B2_FULL + st + 1], phase);
-                    const uint64_t ah = a_desc0 + st * STAGE_D, al = ah + STAGE_D;
+                    const uint64_t ah = a_desc0 + st * SLOT_D, al = ah + SLOT_D;
                     const uint64_t bh = b1_desc0 + (uint64_t)kc * NP * B1_D, bl = bh + B1_D;
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
@@ -519,14 +551,14 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                         }
                     }
                     wg_commit();
-                    if (kc > 0) {                                  // chunk kc - 1 has retired: its stages go back to the producer
+                    if (kc > 0) {                                  // chunk kc - 1 has retired: its slots go back to the producer
                         wg_wait<1>();
                         if (lane == 0) { mbar_arrive(&bars[B2_EMPTY + prev]); if (SPLIT) mbar_arrive(&bars[B2_EMPTY + prev + 1]); }
                     }
                     prev = st;
-                    stage += NP;
-                    if (stage == NST) { stage = 0; phase ^= 1; }
+                    fifo += NP;
                 }
+                fifo += (uint32_t)(NKC * NP);                      // the other warpgroup's chain of this tile
                 wg_wait<0>();
                 reg_fence(v);
                 if (lane == 0) {
