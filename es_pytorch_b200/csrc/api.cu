@@ -207,33 +207,34 @@ int es_obstat_accumulate_coins(es_ctx* ctx, double* sum, double* sumsq, double* 
                                            n_coins, chance, (cudaStream_t)stream);
 }
 
+// the checks the open- and closed-loop rollouts share; `ptrs`: the entry point's own pointers are set
+static int es_rollout_check(const char* fn, bool ptrs, const EsRollout& r) {
+    ES_REQUIRE(ptrs && r.table && r.idx && r.theta && r.layer_sizes && r.rew_vec && r.fit_pos && r.fit_neg, "%s: NULL pointer", fn);
+    ES_REQUIRE(r.n_layers >= 1 && r.n_layers <= ES_MAX_LAYERS, "%s: n_layers must be in [1,%d]", fn, ES_MAX_LAYERS);
+    ES_REQUIRE(r.n_pairs >= 0 && r.T >= 1 && r.fit_stride >= 1, "%s: bad sizes", fn);
+    ES_REQUIRE((r.behv_pos == nullptr) == (r.behv_neg == nullptr), "%s: behv_pos/behv_neg must both be set or NULL", fn);
+    int64_t count = 0;
+    for (int l = 0; l < r.n_layers; ++l) {
+        ES_REQUIRE(r.layer_sizes[l] > 0 && r.layer_sizes[l + 1] > 0, "%s: layer size <= 0", fn);
+        count += (int64_t)r.layer_sizes[l] * r.layer_sizes[l + 1] + r.layer_sizes[l + 1];
+    }
+    ES_REQUIRE(count == r.P, "%s: layer sizes give %lld params, P=%d", fn, (long long)count, r.P);
+    ES_REQUIRE(r.table_len > r.P, "%s: table smaller than the network", fn);
+    return ES_OK;
+}
+
 int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
                               const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
                               const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
                               float* behv_pos, float* behv_neg, const float* act_noise, int mode, void* stream) {
     ES_ENTER(ctx);
-    ES_REQUIRE(table && idx && theta && layer_sizes && obsn && rew_vec && fit_pos && fit_neg,
-               "es_rollout_openloop: NULL pointer");
-    ES_REQUIRE(n_layers >= 1 && n_layers <= ES_MAX_LAYERS, "es_rollout_openloop: n_layers must be in [1,%d]",
-               ES_MAX_LAYERS);
-    ES_REQUIRE(n_pairs >= 0 && T >= 1 && fit_stride >= 1, "es_rollout_openloop: bad sizes");
-    ES_REQUIRE((behv_pos == nullptr) == (behv_neg == nullptr), "es_rollout_openloop: behv_pos/behv_neg must both be set or NULL");
-    int64_t count = 0;
-    for (int l = 0; l < n_layers; ++l) {
-        ES_REQUIRE(layer_sizes[l] > 0 && layer_sizes[l + 1] > 0, "es_rollout_openloop: layer size <= 0");
-        count += (int64_t)layer_sizes[l] * layer_sizes[l + 1] + layer_sizes[l + 1];
-    }
-    ES_REQUIRE(count == P, "es_rollout_openloop: layer sizes give %lld params, P=%d", (long long)count, P);
-    ES_REQUIRE(table_len > P, "es_rollout_openloop: table smaller than the network");
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev};
+    const int rc = es_rollout_check("es_rollout_openloop", obsn != nullptr, r);
+    if (rc) return rc;
     if (n_pairs == 0) return ES_OK;
-    if (mode == ES_ROLLOUT_F32)
-        return es_impl_rollout_f32(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn,
-                                   rew_vec, T, pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg,
-                                   act_noise, (cudaStream_t)stream);
-    if (mode == ES_ROLLOUT_TC || mode == ES_ROLLOUT_TC3)
-        return es_impl_rollout_tc2(ctx, mode == ES_ROLLOUT_TC3, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers,
-                                   obsn, rew_vec, T, pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg,
-                                   act_noise, (cudaStream_t)stream);
+    if (mode == ES_ROLLOUT_F32) return es_impl_rollout_f32(ctx, r, (cudaStream_t)stream);
+    if (mode == ES_ROLLOUT_TC || mode == ES_ROLLOUT_TC3) return es_impl_rollout_tc2(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
     es_set_error("es_rollout_openloop: unknown mode %d", mode);
     return ES_ERR_INVALID;
 }
@@ -253,28 +254,20 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
                           double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
                           double* ob_count, void* stream) {
     ES_ENTER(ctx);
-    ES_REQUIRE(table && idx && theta && layer_sizes && ob_mean && ob_std && obs0 && env_a && env_b && rew_vec && fit_pos && fit_neg,
-               "es_rollout_closedloop: NULL pointer");
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev};
+    const int rc = es_rollout_check("es_rollout_closedloop", ob_mean && ob_std && obs0 && env_a && env_b, r);
+    if (rc) return rc;
     if (n_layers != 3) {
         es_set_error("es_rollout_closedloop: two hidden layers (n_layers == 3) supported, got %d", n_layers);
         return ES_ERR_UNSUPPORTED;
     }
-    ES_REQUIRE(n_pairs >= 0 && T >= 1 && fit_stride >= 1 && band >= 1, "es_rollout_closedloop: bad sizes");
-    ES_REQUIRE((behv_pos == nullptr) == (behv_neg == nullptr), "es_rollout_closedloop: behv_pos/behv_neg must both be set or NULL");
+    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop: band must be in [1, obs_dim]");
     ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
                "es_rollout_closedloop: ob_sum/ob_sumsq/ob_count must all be set or NULL");
-    int64_t count = 0;
-    for (int l = 0; l < n_layers; ++l) {
-        ES_REQUIRE(layer_sizes[l] > 0 && layer_sizes[l + 1] > 0, "es_rollout_closedloop: layer size <= 0");
-        count += (int64_t)layer_sizes[l] * layer_sizes[l + 1] + layer_sizes[l + 1];
-    }
-    ES_REQUIRE(count == P, "es_rollout_closedloop: layer sizes give %lld params, P=%d", (long long)count, P);
-    ES_REQUIRE(table_len > P, "es_rollout_closedloop: table smaller than the network");
-    ES_REQUIRE(band <= layer_sizes[0], "es_rollout_closedloop: band wider than the observation");
     if (n_pairs == 0) return ES_OK;
-    return es_impl_rollout_closed(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, ob_mean, ob_std, ob_clip, obs0,
-                                  env_a, band, env_b, rew_vec, T, pos_scale, coin_words, save_obs_chance, fit_pos, fit_neg, fit_stride,
-                                  behv_pos, behv_neg, ob_sum, ob_sumsq, ob_count, (cudaStream_t)stream);
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
 }
 
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,

@@ -72,6 +72,54 @@ int es_ctx_counters(es_ctx* ctx, size_t n, unsigned** out);
 
 static inline int es_div_up(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// flat offsets of the parameters of an obs-h1-h2-act MLP in state-dict order (src/core/policy.py:33-35):
+// W1 [h1][obs], b1, W2 [h2][h1], b2, W3 [act][h2], b3
+struct EsMlpOffsets { int w1, b1, w2, b2, w3, b3; };
+__host__ __device__ inline EsMlpOffsets es_mlp_offsets(int obs, int h1, int h2, int act) {
+    EsMlpOffsets o;
+    o.w1 = 0; o.b1 = h1 * obs; o.w2 = o.b1 + h1; o.b2 = o.w2 + h2 * h1; o.w3 = o.b2 + h2; o.b3 = o.w3 + act * h2;
+    return o;
+}
+
+// one rollout call of the antithetic pairs idx[0 .. n_pairs), validated by api.cu
+struct EsRollout {
+    const float* table;
+    int64_t table_len;
+    const int64_t* idx;
+    int n_pairs;
+    const float* theta;
+    int P;
+    float sigma;
+    const int* layer_sizes;     // [n_layers + 1]
+    int n_layers;
+    const float* obsn;          // open loop: normalised observations [T][obs]
+    const float* rew_vec;       // [T][act]
+    int T;
+    float pos_scale;
+    double* fit_pos;
+    double* fit_neg;
+    int fit_stride;
+    float* behv_pos;            // [n_pairs][3] or NULL
+    float* behv_neg;
+    const float* act_noise;     // open loop: scaled action noise [n_pairs][2][T][act] (mt_gauss.cu) or NULL
+    int* err;                   // the ctx's error word (es_checked_slice)
+};
+// the closed-loop env, the observation normalisation and the ObStat increments of es_rollout_closedloop
+struct EsClosedEnv {
+    const double* ob_mean;
+    const double* ob_std;
+    double ob_clip;
+    const float* obs0;
+    const float* env_a;         // [band][obs]
+    int band;
+    const float* env_b;         // [act][obs]
+    const uint32_t* coins;      // [n_pairs][4] save_obs coin words or NULL
+    double save_obs_chance;
+    double* ob_sum;             // [obs], or NULL with ob_sumsq and ob_count
+    double* ob_sumsq;
+    double* ob_count;           // [2]
+};
+
 // ---- entry points implemented one per .cu file (called from api.cu) -------------------------
 int es_impl_draw_indices(es_ctx*, uint32_t*, int32_t*, int, int, uint64_t, int, int64_t*, uint32_t*, cudaStream_t);
 int es_impl_mt_skip(es_ctx*, uint32_t*, int32_t*, int, int, cudaStream_t);
@@ -84,18 +132,14 @@ int es_impl_obstat_accumulate_coins(es_ctx*, double*, double*, double*, const fl
                                     const uint32_t*, int, double, cudaStream_t);
 int es_impl_draw_noisy(es_ctx*, uint32_t*, int32_t*, int32_t*, double*, int, int, uint64_t, int, int, double, int64_t*, uint32_t*,
                        float*, cudaStream_t);
-// (the trailing const float* of the rollouts: scaled action noise [n_pairs][2][T][act], or NULL)
-int es_impl_rollout_f32(es_ctx*, const float*, int64_t, const int64_t*, int, const float*, int, float, const int*, int,
-                        const float*, const float*, int, float, double*, double*, int, float*, float*, const float*, cudaStream_t);
-int es_impl_rollout_f32x(es_ctx*, const float*, int64_t, const int64_t*, int, const float*, int, float, const int*, int,
-                         const float*, const float*, int, float, double*, double*, int, float*, float*, const float*, cudaStream_t);
-int es_impl_rollout_tc2(es_ctx*, int split, const float*, int64_t, const int64_t*, int, const float*, int, float, const int*,
-                        int, const float*, const float*, int, float, double*, double*, int, float*, float*, const float*,
-                        cudaStream_t);
+int es_impl_rollout_f32(es_ctx*, const EsRollout&, cudaStream_t);
+int es_impl_rollout_f32x(es_ctx*, const EsRollout&, cudaStream_t);
+int es_impl_rollout_tc2(es_ctx*, const EsRollout&, int split, cudaStream_t);
 void es_tc2_free_shadows(es_ctx* ctx);
-int es_impl_rollout_closed(es_ctx*, const float*, int64_t, const int64_t*, int, const float*, int, float, const int*, const double*,
-                           const double*, double, const float*, const float*, int, const float*, const float*, int, float,
-                           const uint32_t*, double, double*, double*, int, float*, float*, double*, double*, double*, cudaStream_t);
+int es_impl_rollout_closed(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
+// U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
+int es_launch_ubase(es_ctx*, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
+                    float* ubase, cudaStream_t);
 int es_impl_novelty(es_ctx*, const float*, int, const double*, int, int, double*, int, cudaStream_t);
 int es_impl_rank_transform(es_ctx*, const double*, const double*, int, int, int, double, double, int, int, int,
                            const int64_t*, float*, double*, int32_t*, double*, int32_t*, int64_t*, cudaStream_t);
@@ -118,14 +162,48 @@ __device__ __forceinline__ long long es_checked_slice(long long i, int P, long l
     }
     return i;
 }
-__device__ __forceinline__ float es_warp_sum(float v) {
+// Policy.pheno (src/core/policy.py:61-64): `params = self.flat_params + self.std * noise` for noise and -noise, the product
+// and the sum rounded separately
+__device__ __forceinline__ void es_pheno_pm(float sigma, float e, float t, float& w_plus, float& w_minus) {
+    const float d = __fmul_rn(sigma, e);
+    w_plus = __fadd_rn(t, d);
+    w_minus = __fadd_rn(t, -d);
+}
+template <typename T> __device__ __forceinline__ T es_warp_sum(T v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
-__device__ __forceinline__ int es_warp_sum_i(int v) {
+// the warp-wide sums of v[0..7] in 9 shuffles (transposing butterfly): lane L returns the sum over the lanes of v[L / 4]
+__device__ __forceinline__ float es_warp_sum8(const float (&v)[8], int lane) {
+    const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4;
+    float a[4], b[2], c;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    for (int i = 0; i < 4; ++i) a[i] = (h16 ? v[i + 4] : v[i]) + __shfl_xor_sync(0xffffffffu, h16 ? v[i] : v[i + 4], 16);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) b[i] = (h8 ? a[i + 2] : a[i]) + __shfl_xor_sync(0xffffffffu, h8 ? a[i] : a[i + 2], 8);
+    c = (h4 ? b[1] : b[0]) + __shfl_xor_sync(0xffffffffu, h4 ? b[0] : b[1], 4);
+    c += __shfl_xor_sync(0xffffffffu, c, 2);
+    c += __shfl_xor_sync(0xffffffffu, c, 1);
+    return c;
+}
+// a float32 pair held in one 64-bit register (element 0 in the low half), updated by two independent, identically rounded
+// FMAs (sm_90 has no packed f32x2 FMA)
+typedef unsigned long long es_f32x2;
+__device__ __forceinline__ es_f32x2 es_pack2(float lo, float hi) {
+    es_f32x2 v;
+    asm("mov.b64 %0, {%1, %2};" : "=l"(v) : "f"(lo), "f"(hi));
     return v;
+}
+__device__ __forceinline__ void es_unpack2(es_f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
+__device__ __forceinline__ es_f32x2 es_fma2(es_f32x2 a, es_f32x2 b, es_f32x2 c) {
+    float a0, a1, b0, b1, c0, c1;
+    es_unpack2(a, a0, a1); es_unpack2(b, b0, b1); es_unpack2(c, c0, c1);
+    return es_pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+__device__ __forceinline__ float es_hsum2(es_f32x2 v) {
+    float a, b;
+    es_unpack2(v, a, b);
+    return a + b;
 }
 #endif

@@ -13,10 +13,10 @@ __global__ void perturb_kernel(const float* __restrict__ theta, const float* __r
     float* op = out_pos + (size_t)k * P;
     float* on = out_neg ? out_neg + (size_t)k * P : nullptr;
     for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < P; p += gridDim.x * blockDim.x) {
-        const float d = __fmul_rn(sigma, __ldg(eps + p));   // std * noise
-        const float t = theta[p];
-        op[p] = __fadd_rn(t, d);                            // flat_params + (std*noise)
-        if (on) on[p] = __fadd_rn(t, -d);                   // flat_params + std*(-noise)
+        float wp, wm;
+        es_pheno_pm(sigma, __ldg(eps + p), theta[p], wp, wm);
+        op[p] = wp;
+        if (on) on[p] = wm;
     }
 }
 
@@ -121,7 +121,7 @@ __global__ void coin_count_kernel(const uint32_t* __restrict__ coins, int n_coin
         const double u = ((double)(w.x >> 5) * 67108864.0 + (double)(w.y >> 6)) / 9007199254740992.0;   // legacy random_sample
         c += (u < chance) ? 1 : 0;
     }
-    c = es_warp_sum_i(c);
+    c = es_warp_sum(c);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);
 }
 

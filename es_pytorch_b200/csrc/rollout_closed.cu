@@ -86,40 +86,14 @@ __device__ __forceinline__ float cl_tanh(float x) {
     const float e = __expf(2.f * x);
     return 1.f - __fdividef(2.f, 1.f + e);
 }
-// float32 pairs: (+, -) of a weight times (x+, x-) of an input, held in one 64-bit register and updated by two independent,
-// identically rounded FMAs (sm_90 has no packed f32x2 FMA)
-typedef unsigned long long cl_u64;
-__device__ __forceinline__ cl_u64 cl_pk(float lo, float hi) {
-    cl_u64 v;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(v) : "f"(lo), "f"(hi));
-    return v;
-}
-__device__ __forceinline__ void cl_unpk(cl_u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ cl_u64 cl_fma2(cl_u64 a, cl_u64 b, cl_u64 c) {
-    float a0, a1, b0, b1, c0, c1;
-    cl_unpk(a, a0, a1); cl_unpk(b, b0, b1); cl_unpk(c, c0, c1);
-    return cl_pk(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-// Transposing butterfly: the warp-wide sums of v[0..7] in 9 shuffles; lane 4 q (and its three neighbours) returns the sum of v[q]
-__device__ __forceinline__ float cl_warp_sum8(const float (&v)[8], int lane) {
-    const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4;
-    float a[4], b[2], c;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) a[i] = (h16 ? v[i + 4] : v[i]) + __shfl_xor_sync(0xffffffffu, h16 ? v[i] : v[i + 4], 16);
-#pragma unroll
-    for (int i = 0; i < 2; ++i) b[i] = (h8 ? a[i + 2] : a[i]) + __shfl_xor_sync(0xffffffffu, h8 ? a[i] : a[i + 2], 8);
-    c = (h4 ? b[1] : b[0]) + __shfl_xor_sync(0xffffffffu, h4 ? b[0] : b[1], 4);
-    c += __shfl_xor_sync(0xffffffffu, c, 2);
-    c += __shfl_xor_sync(0xffffffffu, c, 1);
-    return c;
-}
+// the float32 pairs (es_f32x2) of this kernel hold (+, -) of a weight times (x+, x-) of an input
 // the four rows of a warp: z[r] (+, -) -> tanh(z + bias) of row 4 w + r, written by the lane that ends up with that sum
-__device__ __forceinline__ void cl_finish_rows(const cl_u64 (&z)[4], int warp, int lane, int rows, const float* __restrict__ bias_p,
+__device__ __forceinline__ void cl_finish_rows(const es_f32x2 (&z)[4], int warp, int lane, int rows, const float* __restrict__ bias_p,
                                                const float* __restrict__ bias_m, float* __restrict__ out2) {
     float v[8];
 #pragma unroll
-    for (int r = 0; r < 4; ++r) cl_unpk(z[r], v[2 * r], v[2 * r + 1]);
-    const float c = cl_warp_sum8(v, lane);
+    for (int r = 0; r < 4; ++r) es_unpack2(z[r], v[2 * r], v[2 * r + 1]);
+    const float c = es_warp_sum8(v, lane);
     if ((lane & 3) == 0) {
         const int q = lane >> 2, o = 4 * warp + (q >> 1), sg = q & 1;
         out2[2 * o + sg] = (o < rows) ? cl_tanh(c + (sg ? bias_m : bias_p)[o]) : 0.f;
@@ -134,8 +108,8 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
     double* __restrict__ nrstd = nmean + p.obs;
     double* __restrict__ rfit = reinterpret_cast<double*>(cl_smem + L.racc);        // [2]
     float* __restrict__ rpos = cl_smem + L.racc + 4;                                  // [2][3]
-    cl_u64* __restrict__ W2 = reinterpret_cast<cl_u64*>(cl_smem + L.w2);
-    cl_u64* __restrict__ W3 = reinterpret_cast<cl_u64*>(cl_smem + L.w3);
+    es_f32x2* __restrict__ W2 = reinterpret_cast<es_f32x2*>(cl_smem + L.w2);
+    es_f32x2* __restrict__ W3 = reinterpret_cast<es_f32x2*>(cl_smem + L.w3);
     float* __restrict__ bias = cl_smem + L.bias;
     float* __restrict__ envA = cl_smem + L.env_a;
     float* __restrict__ envB = cl_smem + L.env_b;
@@ -150,8 +124,7 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int obs = p.obs, h1 = p.h1, h2 = p.h2, act = p.act, T = p.T, band = p.band, half = p.band >> 1;
     const int act_pad = L.act_pad, o2s = L.o2_stride;
-    // flat parameter layout (state-dict order, src/core/policy.py:33-35): W1 [h1][obs], b1, W2 [h2][h1], b2, W3 [act][h2], b3
-    const int off_b1 = h1 * obs, off_w2 = off_b1 + h1, off_b2 = off_w2 + h2 * h1, off_w3 = off_b2 + h2, off_b3 = off_w3 + act * h2;
+    const EsMlpOffsets off = es_mlp_offsets(obs, h1, h2, act);
     const bool l3_warp = 4 * warp < act;                        // warps that hold rows of layer 3
     const bool rew_warp = warp == CL_WARPS - 1;
 
@@ -175,12 +148,13 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
         const float* __restrict__ eps = p.table + base;
         const float* __restrict__ th = p.theta;
         const float sg = p.sigma;
-        // theta +- sigma * eps: the product and the sum are rounded separately (numpy: flat + std * noise)
-        auto wpm = [&](int at) {
-            const float t = th[at], se = __fmul_rn(sg, eps[at]);
-            return cl_pk(__fadd_rn(t, se), __fsub_rn(t, se));
+        auto wpm = [&](int at) {                                   // (theta + sigma eps, theta - sigma eps)
+            const float t = th[at];
+            float wp, wm;
+            es_pheno_pm(sg, eps[at], t, wp, wm);
+            return es_pack2(wp, wm);
         };
-        cl_u64 w1[4][JL];                                          // (w+, w-) of rows 4 warp + r, elements 32 j + lane
+        es_f32x2 w1[4][JL];                                        // (w+, w-) of rows 4 warp + r, elements 32 j + lane
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
 #pragma unroll
@@ -194,17 +168,17 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
 #pragma unroll
             for (int j = 0; j < CL_J23; ++j) {
                 const int o = 4 * warp + r, k = 32 * j + lane;
-                W2[(o * CL_J23 + j) * 32 + lane] = (o < h2 && k < h1) ? wpm(off_w2 + o * h1 + k) : 0ull;
-                W3[(o * CL_J23 + j) * 32 + lane] = (o < act && k < h2) ? wpm(off_w3 + o * h2 + k) : 0ull;
+                W2[(o * CL_J23 + j) * 32 + lane] = (o < h2 && k < h1) ? wpm(off.w2 + o * h1 + k) : 0ull;
+                W3[(o * CL_J23 + j) * 32 + lane] = (o < act && k < h2) ? wpm(off.w3 + o * h2 + k) : 0ull;
             }
         }
         if (tid < CL_H) {
             float a, b;
-            cl_unpk(tid < h1 ? wpm(off_b1 + tid) : 0ull, a, b);
+            es_unpack2(tid < h1 ? wpm(off.b1 + tid) : 0ull, a, b);
             bias[tid] = a; bias[CL_H + tid] = b;
-            cl_unpk(tid < h2 ? wpm(off_b2 + tid) : 0ull, a, b);
+            es_unpack2(tid < h2 ? wpm(off.b2 + tid) : 0ull, a, b);
             bias[2 * CL_H + tid] = a; bias[3 * CL_H + tid] = b;
-            cl_unpk(tid < act ? wpm(off_b3 + tid) : 0ull, a, b);
+            es_unpack2(tid < act ? wpm(off.b3 + tid) : 0ull, a, b);
             bias[4 * CL_H + tid] = a; bias[5 * CL_H + tid] = b;
         }
         for (int i = tid; i < obs; i += CL_THREADS) {
@@ -236,41 +210,41 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
             }
             // ---- layer 1: 4 rows x JL elements per lane, weights in registers, every input read once per warp ----
             {
-                cl_u64 z[4] = {0ull, 0ull, 0ull, 0ull};
-                const cl_u64* __restrict__ xv = reinterpret_cast<const cl_u64*>(x2) + lane;
+                es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
+                const es_f32x2* __restrict__ xv = reinterpret_cast<const es_f32x2*>(x2) + lane;
 #pragma unroll
                 for (int j = 0; j < JL; ++j) {
-                    const cl_u64 x = xv[32 * j];
+                    const es_f32x2 x = xv[32 * j];
 #pragma unroll
-                    for (int r = 0; r < 4; ++r) z[r] = cl_fma2(w1[r][j], x, z[r]);
+                    for (int r = 0; r < 4; ++r) z[r] = es_fma2(w1[r][j], x, z[r]);
                 }
                 cl_finish_rows(z, warp, lane, h1, bias, bias + CL_H, reinterpret_cast<float*>(h1v));
             }
             __syncthreads();
             // ---- layer 2 ----
             {
-                cl_u64 z[4] = {0ull, 0ull, 0ull, 0ull};
-                const cl_u64* __restrict__ hv = reinterpret_cast<const cl_u64*>(h1v) + lane;
-                const cl_u64* __restrict__ wr = W2 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
+                es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
+                const es_f32x2* __restrict__ hv = reinterpret_cast<const es_f32x2*>(h1v) + lane;
+                const es_f32x2* __restrict__ wr = W2 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
 #pragma unroll
                 for (int j = 0; j < CL_J23; ++j) {
-                    const cl_u64 x = hv[32 * j];
+                    const es_f32x2 x = hv[32 * j];
 #pragma unroll
-                    for (int r = 0; r < 4; ++r) z[r] = cl_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
+                    for (int r = 0; r < 4; ++r) z[r] = es_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
                 }
                 cl_finish_rows(z, warp, lane, h2, bias + 2 * CL_H, bias + 3 * CL_H, reinterpret_cast<float*>(h2v));
             }
             __syncthreads();
             // ---- layer 3 (only the warps that hold its rows) ----
             if (l3_warp) {
-                cl_u64 z[4] = {0ull, 0ull, 0ull, 0ull};
-                const cl_u64* __restrict__ hv = reinterpret_cast<const cl_u64*>(h2v) + lane;
-                const cl_u64* __restrict__ wr = W3 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
+                es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
+                const es_f32x2* __restrict__ hv = reinterpret_cast<const es_f32x2*>(h2v) + lane;
+                const es_f32x2* __restrict__ wr = W3 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
 #pragma unroll
                 for (int j = 0; j < CL_J23; ++j) {
-                    const cl_u64 x = hv[32 * j];
+                    const es_f32x2 x = hv[32 * j];
 #pragma unroll
-                    for (int r = 0; r < 4; ++r) z[r] = cl_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
+                    for (int r = 0; r < 4; ++r) z[r] = es_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
                 }
                 cl_finish_rows(z, warp, lane, act, bias + 4 * CL_H, bias + 5 * CL_H, reinterpret_cast<float*>(a2));
             }
@@ -371,21 +345,17 @@ int cl_launch(es_ctx* ctx, const ClParams& p, cudaStream_t stream) {
 
 }  // namespace
 
-int es_impl_rollout_closed(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
-                           int n_params, float sigma, const int* dims, const double* ob_mean, const double* ob_std, double ob_clip,
-                           const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec, int T,
-                           float pos_scale, const uint32_t* coins, double chance, double* fit_pos, double* fit_neg, int fit_stride,
-                           float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count,
-                           cudaStream_t stream) {
+int es_impl_rollout_closed(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {
+    const int* dims = r.layer_sizes;
     ClParams p;
-    p.table = table; p.table_len = table_len; p.idx = idx; p.n_pairs = n_pairs; p.theta = theta; p.sigma = sigma;
-    p.obs = dims[0]; p.h1 = dims[1]; p.h2 = dims[2]; p.act = dims[3]; p.T = T; p.n_params = n_params;
-    p.ob_mean = ob_mean; p.ob_std = ob_std; p.ob_clip = ob_clip;
-    p.obs0 = obs0; p.env_a = env_a; p.env_b = env_b; p.band = band; p.crew = rew_vec; p.pos_scale = pos_scale;
-    p.coins = coins; p.chance = chance;
-    p.fit_pos = fit_pos; p.fit_neg = fit_neg; p.fit_stride = fit_stride; p.behv_pos = behv_pos; p.behv_neg = behv_neg;
-    p.ob_sum = ob_sum; p.ob_sumsq = ob_sumsq; p.ob_count = ob_count;
-    p.err = ctx->err_dev;
+    p.table = r.table; p.table_len = r.table_len; p.idx = r.idx; p.n_pairs = r.n_pairs; p.theta = r.theta; p.sigma = r.sigma;
+    p.obs = dims[0]; p.h1 = dims[1]; p.h2 = dims[2]; p.act = dims[3]; p.T = r.T; p.n_params = r.P;
+    p.ob_mean = env.ob_mean; p.ob_std = env.ob_std; p.ob_clip = env.ob_clip;
+    p.obs0 = env.obs0; p.env_a = env.env_a; p.env_b = env.env_b; p.band = env.band; p.crew = r.rew_vec; p.pos_scale = r.pos_scale;
+    p.coins = env.coins; p.chance = env.save_obs_chance;
+    p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.fit_stride = r.fit_stride; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
+    p.ob_sum = env.ob_sum; p.ob_sumsq = env.ob_sumsq; p.ob_count = env.ob_count;
+    p.err = r.err;
     if (p.h1 > CL_H || p.h2 > CL_H || p.act > CL_A || p.obs > 384 || p.band > CL_HALO || p.obs < p.band || (p.band & 1)) {
         es_set_error("es_rollout_closedloop: supports even band <= obs <= 384, hidden <= %d, act <= %d, band <= %d (got %d-%d-%d-%d, band %d)",
                      CL_H, CL_A, CL_HALO, p.obs, p.h1, p.h2, p.act, p.band);

@@ -80,13 +80,14 @@ __device__ __forceinline__ void rf_stage_weights(float* __restrict__ W, const fl
         const int in = d.in[l], cnt = d.in[l] * d.out[l];
         for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
             const int n = i / in, k = i - n * in;
-            const float dlt = __fmul_rn(sigma, __ldg(eps + d.w_off[l] + i));     // std * noise
-            const float t = __ldg(theta + d.w_off[l] + i);
-            W[d.sw_off[l] + n * d.pitch[l] + k] = __fadd_rn(t, neg ? -dlt : dlt);
+            float wp, wm;
+            es_pheno_pm(sigma, __ldg(eps + d.w_off[l] + i), __ldg(theta + d.w_off[l] + i), wp, wm);
+            W[d.sw_off[l] + n * d.pitch[l] + k] = neg ? wm : wp;
         }
         for (int i = threadIdx.x; i < d.out[l]; i += blockDim.x) {
-            const float dlt = __fmul_rn(sigma, __ldg(eps + d.b_off[l] + i));
-            W[d.sb_off[l] + i] = __fadd_rn(__ldg(theta + d.b_off[l] + i), neg ? -dlt : dlt);
+            float wp, wm;
+            es_pheno_pm(sigma, __ldg(eps + d.b_off[l] + i), __ldg(theta + d.b_off[l] + i), wp, wm);
+            W[d.sb_off[l] + i] = neg ? wm : wp;
         }
     }
 }
@@ -226,28 +227,25 @@ rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ 
 
 static int rf_round4(int x) { return (x + 3) & ~3; }
 
-int es_impl_rollout_f32(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
-                        const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
-                        const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
-                        float* behv_pos, float* behv_neg, const float* act_noise, cudaStream_t stream) {
+int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     // obs-64-64-act networks with enough pairs to fill the GPU: the packed-FMA kernel of rollout_f32x.cu (one CTA per pair);
     // fewer pairs than half the SMs (single evaluations, es.step's noiseless evaluation) stay here, where the episode's time
     // tiles are split over the idle SMs.  ES_F32_GENERAL=1 forces this kernel (tests compare the two).
-    if (2 * n_pairs >= ctx->sm_count && !getenv("ES_F32_GENERAL")) {
-        const int rc = es_impl_rollout_f32x(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec,
-                                            T, pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, stream);
+    if (2 * r.n_pairs >= ctx->sm_count && !getenv("ES_F32_GENERAL")) {
+        const int rc = es_impl_rollout_f32x(ctx, r, stream);
         if (rc != ES_ERR_UNSUPPORTED) return rc;
     }
+    const int n_pairs = r.n_pairs, T = r.T, n_layers = r.n_layers;
     RfDesc d;
     memset(&d, 0, sizeof(d));
     d.n_layers = n_layers;
-    d.P = P;
-    d.table_len = table_len;
-    d.err = ctx->err_dev;
+    d.P = r.P;
+    d.table_len = r.table_len;
+    d.err = r.err;
     int off = 0, soff = 0, xmax = 0;
     for (int l = 0; l < n_layers; ++l) {
-        d.in[l] = layer_sizes[l];
-        d.out[l] = layer_sizes[l + 1];
+        d.in[l] = r.layer_sizes[l];
+        d.out[l] = r.layer_sizes[l + 1];
         d.in4[l] = rf_round4(d.in[l]);
         d.pitch[l] = ((d.in4[l] >> 2) & 1) ? d.in4[l] : d.in4[l] + 4;   // (pitch/4) odd -> conflict-free float4 rows
         d.w_off[l] = off; off += d.in[l] * d.out[l];
@@ -303,21 +301,23 @@ int es_impl_rollout_f32(es_ctx* ctx, const float* table, int64_t table_len, cons
                 if (rc) return rc;
             }
         }
-        double* fp = fit_pos + (size_t)p0 * fit_stride;
-        double* fn = fit_neg + (size_t)p0 * fit_stride;
-        float* bp = behv_pos ? behv_pos + (size_t)p0 * 3 : nullptr;
-        float* bn = behv_neg ? behv_neg + (size_t)p0 * 3 : nullptr;
-        const float* an = act_noise ? act_noise + (size_t)p0 * 2 * T * layer_sizes[n_layers] : nullptr;
+        double* fp = r.fit_pos + (size_t)p0 * r.fit_stride;
+        double* fn = r.fit_neg + (size_t)p0 * r.fit_stride;
+        float* bp = r.behv_pos ? r.behv_pos + (size_t)p0 * 3 : nullptr;
+        float* bn = r.behv_neg ? r.behv_neg + (size_t)p0 * 3 : nullptr;
+        const float* an = r.act_noise ? r.act_noise + (size_t)p0 * 2 * T * r.layer_sizes[n_layers] : nullptr;
         if (gw) {
-            rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(table, idx + p0, theta, sigma, d, wglobal);
+            rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, d, wglobal);
             ES_LAUNCHED(ctx);
             ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)act_smem));
             rollout_f32_kernel<true><<<dim3(2 * np, n_splits), RF_THREADS, act_smem, stream>>>(
-                table, idx + p0, theta, sigma, d, obsn, rew_vec, T, pos_scale, fp, fn, fit_stride, bp, bn, part, tickets, wglobal, an);
+                r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
+                wglobal, an);
         } else {
             ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));
             rollout_f32_kernel<false><<<dim3(2 * np, n_splits), RF_THREADS, smem_w, stream>>>(
-                table, idx + p0, theta, sigma, d, obsn, rew_vec, T, pos_scale, fp, fn, fit_stride, bp, bn, part, tickets, nullptr, an);
+                r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
+                nullptr, an);
         }
         ES_LAUNCHED(ctx);
     }

@@ -47,12 +47,11 @@
 // warpgroup 0's, so it runs while warpgroup 0 is in its epilogues, and warpgroup 0's chain of tile m + 1 runs under warpgroup
 // 1's epilogues.  No other synchronisation orders the warpgroups (an explicit turn token on top of the FIFO order measured no
 // faster at float32-equivalent precision and slower with single float16 products).
-// The waits inside the chains are warp-uniform (mbar_wait_warp): a divergent spin loop while wgmmas are in flight makes
-// ptxas serialize every wgmma of the kernel.
-#include <cuda.h>
+// The waits inside the chains are warp-uniform (mbar_wait_warp, pipeline.cuh).
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include "common.cuh"
+#include "pipeline.cuh"
 
 namespace {
 
@@ -64,61 +63,13 @@ constexpr int T2_SLOT = T2_STAGE / 2;          // 8 KB: the 64 rows of one consu
 constexpr int T2_WG_WARPS = T2_CONS_WARPS / 2; // warps per consumer warpgroup
 constexpr int T2_B1_CHUNK = T2_H * 128;        // 8 KB: 64 rows x 64 f16
 constexpr int T2_W3_BLOCK = T2_ACT_PAD * 128;  // 4 KB
-constexpr uint32_t T2_SPIN_LIMIT = 1u << 28;
 // registers per thread after the split: 128 x 72 + 256 x 208 = 62 464 <= 384 x 168 = 64 512 allocated at launch
 constexpr int T2_REGS_DATA = 72, T2_REGS_MATH = 208;
 
-// ---- raw PTX wrappers ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t spins = 0;
-    while (!mbar_try(bar, parity)) {
-        if (++spins > T2_SPIN_LIMIT) __trap();            // watchdog: trap instead of hanging the GPU
-    }
-}
-// The same wait with the poll result agreed across the (converged) warp, so that the spin loop branches warp-uniformly.  The
-// consumer warpgroups wait with wgmmas in flight; a per-thread (divergent) spin loop there makes ptxas serialize every wgmma
-// of the kernel (warning C7520: each HGMMA then runs to completion before the next one is issued).
-__device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity) {
-    uint32_t spins = 0;
-    while (!__all_sync(0xffffffffu, mbar_try(bar, parity))) {
-        if (++spins > T2_SPIN_LIMIT) __trap();            // watchdog: trap instead of hanging the GPU
-    }
-}
-__device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// 3-D TMA tensor copy (tile mode): coordinates {element, origin unit, row}
-__device__ __forceinline__ void tma_load_3d(void* dst_smem, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-                 ::"r"(smem_u32(dst_smem)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-// the same box fetched into L2 only
-__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* map, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(map), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
 // first 16-byte unit of a slice's eps1 in the shifted shadow copy where its rows are 16-byte aligned
 __device__ __forceinline__ int t2_shadow_unit(long long at, size_t shadow_stride) {
     return (int)(((long long)(at & 7) * (long long)shadow_stride + (at - (at & 7))) >> 3);
 }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 // ---- wgmma (warpgroup-wide, asynchronous; D in registers) -----------------------------------------------------------
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -210,11 +161,6 @@ __device__ __forceinline__ float ldg_stream(const float* p) {
     return v;
 }
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // K-major, 128-byte-swizzled operand tile: rows of 128 B, 8-row atoms of 1024 B (SBO); sm_90 wgmma descriptor
 __device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t saddr) {
@@ -245,7 +191,7 @@ struct T2Params {
     int use_tma;                  // eps1 by TMA from the shadows; 0: the builders convert the float32 slice
     int n_pairs, obs, act, T, nkc, n_mtiles, fit_stride;
     float sigma, pos_scale;
-    int w1, b1, w2, b2, w3, b3;   // flat parameter offsets
+    EsMlpOffsets off;
     long long table_len;
     int P;
     int* err;
@@ -367,7 +313,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 if (lane == 0) {
                     mbar_expect_tx(&bars[B2_EPS_TX], (uint32_t)(NP * NKC * T2_B1_CHUNK));
                     if (p.use_tma) {
-                        const int unit0 = t2_shadow_unit(slice + p.w1, p.shadow_stride);
+                        const int unit0 = t2_shadow_unit(slice + p.off.w1, p.shadow_stride);
 #pragma unroll
                         for (int pc = 0; pc < NP; ++pc)
                             for (int kc = 0; kc < NKC; ++kc)
@@ -386,7 +332,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
 #pragma unroll
                     for (int rr = 0; rr < 2; ++rr) {
                         const int n = 2 * lane + rr;
-                        const float eb = ldg_stream(p.table + slice + p.b1 + n);
+                        const float eb = ldg_stream(p.table + slice + p.off.b1 + n);
                         __half hi, lo;
                         split_h1(eb, hi, lo);
                         const uint32_t off = (uint32_t)(kcb * NP) * T2_B1_CHUNK + n * 128 + ((ub ^ (n & 7)) << 4);      // [kc][piece] blocks
@@ -400,7 +346,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 if (p.use_tma && lane == 0 && i + 1 < my_pairs) {
                     // the next pair's eps1 rows into L2 now, so that its TMA at the pair boundary does not wait on HBM
                     const long long nslice = es_checked_slice(p.idx[pair + gridDim.x], p.P, p.table_len, nullptr);
-                    const int nunit0 = t2_shadow_unit(nslice + p.w1, p.shadow_stride);
+                    const int nunit0 = t2_shadow_unit(nslice + p.off.w1, p.shadow_stride);
 #pragma unroll
                     for (int pc = 0; pc < NP; ++pc)
                         for (int kc = 0; kc < NKC; ++kc) tma_prefetch_3d(pc ? &maps.lo : &maps.hi, 0, nunit0 + 8 * kc, 0);
@@ -428,19 +374,18 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, nullptr);
                 const float* __restrict__ eps = p.table + slice;
                 uint8_t* img = my_images + (size_t)(j & 1) * I.total;
-                // W2+- / W3+-: element pairs (n, k), (n, k+1); theta +- sigma*eps with the reference's two roundings
+                // W2+- / W3+-: element pairs (n, k), (n, k+1)
                 const int n2 = T2_H * T2_H / 2, n3 = T2_ACT_PAD * T2_H / 2;
                 for (int e2 = btid; e2 < n2 + n3; e2 += BT) {
                     const bool l3 = e2 >= n2;
                     const int k2 = 2 * (l3 ? e2 - n2 : e2);
                     const int n = k2 >> 6, kk = k2 & 63;
-                    const int off = (l3 ? p.w3 : p.w2) + k2;
+                    const int at = (l3 ? p.off.w3 : p.off.w2) + k2;
                     const bool live = !l3 || n < p.act;
                     float wp0 = 0.f, wp1 = 0.f, wn0 = 0.f, wn1 = 0.f;
                     if (live) {
-                        const float d0 = __fmul_rn(sg, ldg_stream(eps + off)), d1 = __fmul_rn(sg, ldg_stream(eps + off + 1));
-                        const float t0 = __ldg(p.theta + off), t1 = __ldg(p.theta + off + 1);
-                        wp0 = __fadd_rn(t0, d0); wp1 = __fadd_rn(t1, d1); wn0 = __fadd_rn(t0, -d0); wn1 = __fadd_rn(t1, -d1);
+                        es_pheno_pm(sg, ldg_stream(eps + at), __ldg(p.theta + at), wp0, wn0);
+                        es_pheno_pm(sg, ldg_stream(eps + at + 1), __ldg(p.theta + at + 1), wp1, wn1);
                     }
                     const uint32_t blk = l3 ? T2_W3_BLOCK : T2_B1_CHUNK;
                     uint8_t* base = img + (l3 ? I.w3 : I.w2) + sw128_off(n, kk);
@@ -461,15 +406,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     float* bias = (float*)(img + I.bias);
                     for (int e = btid; e < T2_H + T2_ACT_PAD; e += BT) {
                         if (e < T2_H) {
-                            const float d = __fmul_rn(sg, ldg_stream(eps + p.b2 + e)), t = __ldg(p.theta + p.b2 + e);
-                            bias[e] = __fadd_rn(t, d); bias[T2_H + e] = __fadd_rn(t, -d);
+                            es_pheno_pm(sg, ldg_stream(eps + p.off.b2 + e), __ldg(p.theta + p.off.b2 + e), bias[e], bias[T2_H + e]);
                         } else {
                             const int j2 = e - T2_H;
                             float vp = 0.f, vn = 0.f;
-                            if (j2 < p.act) {
-                                const float d = __fmul_rn(sg, ldg_stream(eps + p.b3 + j2)), t = __ldg(p.theta + p.b3 + j2);
-                                vp = __fadd_rn(t, d); vn = __fadd_rn(t, -d);
-                            }
+                            if (j2 < p.act) es_pheno_pm(sg, ldg_stream(eps + p.off.b3 + j2), __ldg(p.theta + p.off.b3 + j2), vp, vn);
                             bias[2 * T2_H + j2] = vp; bias[2 * T2_H + T2_ACT_PAD + j2] = vn;
                         }
                     }
@@ -480,8 +421,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     for (int e2 = btid; e2 < T2_H * Kp / 2; e2 += BT) {
                         const int n = (2 * e2) / Kp, k = (2 * e2) - n * Kp;
                         float x0 = 0.f, x1 = 0.f;
-                        if (k < p.obs) x0 = ldg_stream(eps + p.w1 + (size_t)n * p.obs + k); else if (k == p.obs) x0 = ldg_stream(eps + p.b1 + n);
-                        if (k + 1 < p.obs) x1 = ldg_stream(eps + p.w1 + (size_t)n * p.obs + k + 1); else if (k + 1 == p.obs) x1 = ldg_stream(eps + p.b1 + n);
+                        if (k < p.obs) x0 = ldg_stream(eps + p.off.w1 + (size_t)n * p.obs + k); else if (k == p.obs) x0 = ldg_stream(eps + p.off.b1 + n);
+                        if (k + 1 < p.obs) x1 = ldg_stream(eps + p.off.w1 + (size_t)n * p.obs + k + 1); else if (k + 1 == p.obs) x1 = ldg_stream(eps + p.off.b1 + n);
                         uint8_t* dst = img + I.b1 + (size_t)((k >> 6) * NP) * T2_B1_CHUNK + sw128_off(n, k & 63);     // [kc][piece] blocks
                         if (SPLIT) {
                             __half h0, l0, h1, l1;
@@ -500,8 +441,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 if (j + 1 < my_pairs) {                                      // L2 prefetch of the next pair's operands
                     const long long nidx = es_checked_slice(p.idx[blockIdx.x + (j + 1) * gridDim.x], p.P, p.table_len, nullptr);
                     const char* nxt = (const char*)(p.table + nidx);
-                    const int lines = (p.b3 + p.act) * 4 / 128 + 2;
-                    const int skip = p.use_tma ? p.b1 * 4 / 128 : 0;         // with the shadows eps1 comes by TMA
+                    const int lines = (p.off.b3 + p.act) * 4 / 128 + 2;
+                    const int skip = p.use_tma ? p.off.b1 * 4 / 128 : 0;         // with the shadows eps1 comes by TMA
                     for (int l = skip + btid; l < lines; l += BT) prefetch_l2(nxt + (size_t)l * 128);
                 }
             }
@@ -684,8 +625,9 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
             // ---- this warp's sums of the pair -> shared memory; the last of the 8 warps adds them in warp order and writes the
             //      pair's results (no global scratch, no device-wide fence: a CTA-scope release/acquire on a shared counter) ----
             double* mine = red + ((size_t)(i & 1) * T2_CONS_WARPS + cw) * 8;
-            const double fitp = warp_sum_d(fit_p), fitn = warp_sum_d(fit_n);
-            const double ps[6] = {warp_sum_d(pp0), warp_sum_d(pp1), warp_sum_d(pp2), warp_sum_d(pn0), warp_sum_d(pn1), warp_sum_d(pn2)};
+            const double fitp = es_warp_sum(fit_p), fitn = es_warp_sum(fit_n);
+            const double ps[6] = {es_warp_sum<double>(pp0), es_warp_sum<double>(pp1), es_warp_sum<double>(pp2),
+                                  es_warp_sum<double>(pn0), es_warp_sum<double>(pn1), es_warp_sum<double>(pn2)};
             if (lane == 0) {
                 mine[0] = fitp; mine[1] = fitn;
 #pragma unroll
@@ -738,11 +680,13 @@ __global__ void rollout_tc2_prep_kernel(const float* __restrict__ obsn, int T, i
     }
 }
 
-// U[t][n] = b1[n] + sum_k Xn[t][k] * theta1[n][k], accumulated in float64 (k ascending) and rounded once to float32.
-// Output: row-major [n_mtiles * 128][64] (0 beyond T).
+// U[t][n] = b1[n] + sum_k Xn[t][k] * theta1[n][k], the unperturbed part of layer 1 that the pair kernels (this file and
+// rollout_f32x.cu) share between the two signs of a pair: accumulated in float64 (k ascending) and rounded once to float32, so
+// that splitting z1+- = U +- sigma V adds no rounding of its own to the theta term.  Output: row-major [n_tiles * 128][64]
+// (0 beyond T).
 constexpr int T2_UB_ROWS = 8, T2_UB_KT = 64, T2_UB_RPT = T2_UB_ROWS / 4;
-__global__ void __launch_bounds__(256) rollout_tc2_ubase_kernel(const float* __restrict__ obsn, const float* __restrict__ theta,
-                                                                 int w1, int b1, int T, int obs, float* __restrict__ ubase) {
+__global__ void __launch_bounds__(256) rollout_ubase_kernel(const float* __restrict__ obsn, const float* __restrict__ theta,
+                                                             int w1, int b1, int T, int obs, float* __restrict__ ubase) {
     __shared__ float s_w[T2_UB_KT][T2_H + 1];
     __shared__ float s_x[T2_UB_ROWS][T2_UB_KT];
     const int n = threadIdx.x & 63, rg = threadIdx.x >> 6;
@@ -815,8 +759,7 @@ int t2_encode_map(CUtensorMap* map, void* base, size_t stride, int obs) {
 }
 
 template <bool SPLIT>
-int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, const float* theta, int T, int n_pairs,
-              cudaStream_t stream) {
+int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, cudaStream_t stream) {
     const T2Smem L = t2_layout<SPLIT>(p.nkc);
     const size_t smem = (size_t)L.total + 1024;       // + alignment slack
     if (smem > 227 * 1024) {
@@ -826,7 +769,7 @@ int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, c
     constexpr int NP = SPLIT ? 2 : 1;
     const size_t xnt_bytes = (size_t)p.n_mtiles * p.nkc * NP * T2_STAGE;
     const size_t ub_bytes = (size_t)p.n_mtiles * T2_MT * T2_H * sizeof(float);
-    const int grid = n_pairs < ctx->sm_count ? n_pairs : ctx->sm_count;
+    const int grid = p.n_pairs < ctx->sm_count ? p.n_pairs : ctx->sm_count;
     const size_t img_bytes = (((size_t)grid * 2 * t2_image<SPLIT>(p.nkc, !p.use_tma).total) + 255) & ~(size_t)255;
     void* scratch = nullptr;
     int rc = es_ctx_scratch(ctx, xnt_bytes + ub_bytes + img_bytes, &scratch);
@@ -840,10 +783,10 @@ int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, c
         const size_t total = (size_t)p.n_mtiles * p.nkc * T2_MT * T2_KC;
         int blocks = es_div_up((int64_t)total, 256);
         if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
-        rollout_tc2_prep_kernel<SPLIT><<<blocks, 256, 0, stream>>>(obsn, T, p.obs, p.nkc, p.n_mtiles, xnt);
+        rollout_tc2_prep_kernel<SPLIT><<<blocks, 256, 0, stream>>>(obsn, p.T, p.obs, p.nkc, p.n_mtiles, xnt);
         ES_LAUNCHED(ctx);
-        rollout_tc2_ubase_kernel<<<p.n_mtiles * T2_MT / T2_UB_ROWS, 256, 0, stream>>>(obsn, theta, p.w1, p.b1, T, p.obs, ubase);
-        ES_LAUNCHED(ctx);
+        rc = es_launch_ubase(ctx, obsn, p.theta, p.off, p.T, p.obs, p.n_mtiles, ubase, stream);
+        if (rc) return rc;
     }
     if (p.act_noise) {
         ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc2_kernel<SPLIT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -858,6 +801,13 @@ int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, c
 
 }  // namespace
 
+int es_launch_ubase(es_ctx* ctx, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
+                    float* ubase, cudaStream_t stream) {
+    rollout_ubase_kernel<<<n_tiles * T2_MT / T2_UB_ROWS, 256, 0, stream>>>(obsn, theta, off.w1, off.b1, T, obs, ubase);
+    ES_LAUNCHED(ctx);
+    return ES_OK;
+}
+
 void es_tc2_free_shadows(es_ctx* ctx) {
     if (ctx->sh16_hi) cudaFree(ctx->sh16_hi);
     if (ctx->sh16_lo) cudaFree(ctx->sh16_lo);
@@ -867,26 +817,23 @@ void es_tc2_free_shadows(es_ctx* ctx) {
     ctx->sh16_src = nullptr;
 }
 
-int es_impl_rollout_tc2(es_ctx* ctx, int split, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
-                        const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
-                        const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
-                        float* behv_pos, float* behv_neg, const float* act_noise, cudaStream_t stream) {
-    if (n_layers != 3 || layer_sizes[1] != T2_H || layer_sizes[2] != T2_H || layer_sizes[3] > T2_ACT_PAD || layer_sizes[0] > 1023) {
+int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t stream) {
+    const int* ls = r.layer_sizes;
+    if (r.n_layers != 3 || ls[1] != T2_H || ls[2] != T2_H || ls[3] > T2_ACT_PAD || ls[0] > 1023) {
         es_set_error("es_rollout_openloop(TC): the tensor-core path covers obs(<=1023)-64-64-act(<=32) tanh MLPs; "
                      "use ES_ROLLOUT_F32 for other shapes");
         return ES_ERR_UNSUPPORTED;
     }
     T2Params p;
     memset(&p, 0, sizeof(p));
-    p.table = table; p.idx = idx; p.theta = theta; p.act_noise = act_noise; p.rew_vec = rew_vec;
-    p.fit_pos = fit_pos; p.fit_neg = fit_neg; p.behv_pos = behv_pos; p.behv_neg = behv_neg;
-    p.n_pairs = n_pairs; p.obs = layer_sizes[0]; p.act = layer_sizes[3]; p.T = T; p.fit_stride = fit_stride;
-    p.sigma = sigma; p.pos_scale = pos_scale;
+    p.table = r.table; p.idx = r.idx; p.theta = r.theta; p.act_noise = r.act_noise; p.rew_vec = r.rew_vec;
+    p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
+    p.n_pairs = r.n_pairs; p.obs = ls[0]; p.act = ls[3]; p.T = r.T; p.fit_stride = r.fit_stride;
+    p.sigma = r.sigma; p.pos_scale = r.pos_scale;
     p.nkc = es_div_up(p.obs + 1, T2_KC);                 // + the constant-1 column that carries the L1 bias
-    p.n_mtiles = es_div_up(T, T2_MT);
-    p.w1 = 0; p.b1 = p.obs * T2_H; p.w2 = p.b1 + T2_H; p.b2 = p.w2 + T2_H * T2_H; p.w3 = p.b2 + T2_H;
-    p.b3 = p.w3 + T2_H * p.act;
-    p.table_len = table_len; p.P = P; p.err = ctx->err_dev;
+    p.n_mtiles = es_div_up(r.T, T2_MT);
+    p.off = es_mlp_offsets(p.obs, T2_H, T2_H, p.act);
+    p.table_len = r.table_len; p.P = r.P; p.err = r.err;
 
     // float16 shadows of the table (hi always, lo when a split rollout asks for it): 8 shifted copies each, built once per
     // (table pointer, length) and addressed through two TMA tensor maps.  Needs 16-byte aligned rows in every slice (obs % 8
@@ -894,15 +841,15 @@ int es_impl_rollout_tc2(es_ctx* ctx, int split, const float* table, int64_t tabl
     T2Maps maps;
     memset(&maps, 0, sizeof(maps));
     p.use_tma = 0;
-    if (p.obs % 8 == 0 && !getenv("ES_TC_NO_SHADOW") && !ctx->sh16_failed) {
-        const size_t stride = ((size_t)table_len + 64 * (size_t)p.obs + 79) & ~(size_t)7;       // room for the last slice's rows
-        const bool fresh = ctx->sh16_src != table || ctx->sh16_len != table_len || ctx->sh16_stride != stride || ctx->sh16_obs != p.obs;
+    if (p.obs % 8 == 0 && !ctx->sh16_failed) {
+        const size_t stride = ((size_t)r.table_len + 64 * (size_t)p.obs + 79) & ~(size_t)7;       // room for the last slice's rows
+        const bool fresh = ctx->sh16_src != r.table || ctx->sh16_len != r.table_len || ctx->sh16_stride != stride || ctx->sh16_obs != p.obs;
         if (fresh) es_tc2_free_shadows(ctx);
         bool ok = true;
         if (!ctx->sh16_hi) {
             ok = cudaMalloc(&ctx->sh16_hi, 8 * stride * sizeof(__half)) == cudaSuccess;
             if (ok) {
-                rollout_tc2_shadow_kernel<<<dim3(ctx->sm_count * 8, 8), 256, 0, stream>>>(table, table_len, stride, (__half*)ctx->sh16_hi, nullptr);
+                rollout_tc2_shadow_kernel<<<dim3(ctx->sm_count * 8, 8), 256, 0, stream>>>(r.table, r.table_len, stride, (__half*)ctx->sh16_hi, nullptr);
                 ES_LAUNCHED(ctx);
             }
         }
@@ -910,7 +857,7 @@ int es_impl_rollout_tc2(es_ctx* ctx, int split, const float* table, int64_t tabl
             ok = cudaMalloc(&ctx->sh16_lo, 8 * stride * sizeof(__half)) == cudaSuccess;
             if (ok) {
                 // (recomputes hi: simpler than a second kernel, runs once per table)
-                rollout_tc2_shadow_kernel<<<dim3(ctx->sm_count * 8, 8), 256, 0, stream>>>(table, table_len, stride, (__half*)ctx->sh16_hi,
+                rollout_tc2_shadow_kernel<<<dim3(ctx->sm_count * 8, 8), 256, 0, stream>>>(r.table, r.table_len, stride, (__half*)ctx->sh16_hi,
                                                                                         (__half*)ctx->sh16_lo);
                 ES_LAUNCHED(ctx);
             }
@@ -930,12 +877,11 @@ int es_impl_rollout_tc2(es_ctx* ctx, int split, const float* table, int64_t tabl
             es_tc2_free_shadows(ctx);
             ctx->sh16_failed = 1;
         } else {
-            ctx->sh16_src = table; ctx->sh16_len = table_len; ctx->sh16_stride = stride; ctx->sh16_obs = p.obs;
+            ctx->sh16_src = r.table; ctx->sh16_len = r.table_len; ctx->sh16_stride = stride; ctx->sh16_obs = p.obs;
             maps = *(T2Maps*)ctx->sh16_maps;
             p.use_tma = 1;
             p.shadow_stride = stride;
         }
     }
-    return split ? t2_launch<true>(ctx, p, maps, obsn, theta, T, n_pairs, stream)
-                 : t2_launch<false>(ctx, p, maps, obsn, theta, T, n_pairs, stream);
+    return split ? t2_launch<true>(ctx, p, maps, r.obsn, stream) : t2_launch<false>(ctx, p, maps, r.obsn, stream);
 }
