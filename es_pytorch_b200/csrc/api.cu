@@ -137,18 +137,25 @@ int es_sm_count(const es_ctx* ctx) { return ctx ? ctx->sm_count : -1; }
     ES_CHECK_CUDA(cudaSetDevice((ctx)->device));                             \
     do { int _a = es_async_error((ctx), __func__); if (_a) return _a; } while (0)
 
+// the randint bound of es_draw_indices and es_draw_noisy: NoiseTable.sample_idx raises ValueError when upper_bound <= 0
+// (noisetable.py:39), and ranges >= 2^32 take numpy's 64-bit draw path
+static int es_randint_check(const char* fn, uint64_t upper_bound) {
+    ES_REQUIRE(upper_bound >= 1, "%s: upper_bound must be >= 1 (network too large for noise table)", fn);
+    if (upper_bound - 1 >= 0xFFFFFFFFull) {
+        es_set_error("%s: ranges >= 2^32 use numpy's 64-bit draw path, not implemented", fn);
+        return ES_ERR_UNSUPPORTED;
+    }
+    return ES_OK;
+}
+
 int es_draw_indices(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int n_streams, int n_per_stream,
                     uint64_t upper_bound, int extra_words, int64_t* idx_out, uint32_t* extra_out, void* stream) {
     ES_ENTER(ctx);
     ES_REQUIRE(mt_key && mt_pos && idx_out, "es_draw_indices: NULL pointer");
     ES_REQUIRE(n_streams >= 0 && n_per_stream >= 0, "es_draw_indices: negative count");
     ES_REQUIRE(extra_words >= 0 && extra_words <= 7, "es_draw_indices: extra_words must be in [0,7]");
-    // NoiseTable.sample_idx raises ValueError when upper_bound <= 0 (noisetable.py:39)
-    ES_REQUIRE(upper_bound >= 1, "es_draw_indices: upper_bound must be >= 1 (network too large for noise table)");
-    if (upper_bound - 1 >= 0xFFFFFFFFull) {
-        es_set_error("es_draw_indices: ranges >= 2^32 use numpy's 64-bit draw path, not implemented");
-        return ES_ERR_UNSUPPORTED;
-    }
+    const int rc = es_randint_check("es_draw_indices", upper_bound);
+    if (rc) return rc;
     if (n_streams == 0 || n_per_stream == 0) return ES_OK;
     return es_impl_draw_indices(ctx, mt_key, mt_pos, n_streams, n_per_stream, upper_bound, extra_words, idx_out,
                                 extra_out, (cudaStream_t)stream);
@@ -278,12 +285,8 @@ int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_g
     ES_REQUIRE(n_streams >= 0 && n_per_stream >= 0 && normals_per_eval >= 0, "es_draw_noisy: negative count");
     ES_REQUIRE(coins_per_eval >= 0 && coins_per_eval <= 8, "es_draw_noisy: coins_per_eval must be in [0,8]");
     ES_REQUIRE(coins_per_eval == 0 || coin_out, "es_draw_noisy: coin_out is NULL");
-    // NoiseTable.sample_idx raises ValueError when upper_bound <= 0 (noisetable.py:39)
-    ES_REQUIRE(upper_bound >= 1, "es_draw_noisy: upper_bound must be >= 1 (network too large for noise table)");
-    if (upper_bound - 1 >= 0xFFFFFFFFull) {
-        es_set_error("es_draw_noisy: ranges >= 2^32 use numpy's 64-bit draw path, not implemented");
-        return ES_ERR_UNSUPPORTED;
-    }
+    const int rc = es_randint_check("es_draw_noisy", upper_bound);
+    if (rc) return rc;
     if (n_streams == 0 || n_per_stream == 0) return ES_OK;
     return es_impl_draw_noisy(ctx, mt_key, mt_pos, has_gauss, gauss, n_streams, n_per_stream, upper_bound, coins_per_eval,
                               normals_per_eval, scale, idx_out, coin_out, noise_out, (cudaStream_t)stream);

@@ -3,6 +3,7 @@
 // All float32 arithmetic mirrors the reference one IEEE operation at a time
 // (__fmul_rn / __fadd_rn / ... so ptxas cannot contract a*b+c into an FMA).
 #include "common.cuh"
+#include "mt19937.cuh"
 
 // ---- a3: theta +- sigma*eps  (src/core/policy.py:61-64) ----------------------------------------
 __global__ void perturb_kernel(const float* __restrict__ theta, const float* __restrict__ table,
@@ -118,8 +119,7 @@ __global__ void coin_count_kernel(const uint32_t* __restrict__ coins, int n_coin
     int c = 0;
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n_coins; e += gridDim.x * blockDim.x) {
         const uint2 w = *reinterpret_cast<const uint2*>(coins + 2 * (size_t)e);
-        const double u = ((double)(w.x >> 5) * 67108864.0 + (double)(w.y >> 6)) / 9007199254740992.0;   // legacy random_sample
-        c += (u < chance) ? 1 : 0;
+        c += (mt19937_random_sample(w.x, w.y) < chance) ? 1 : 0;
     }
     c = es_warp_sum(c);
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);

@@ -14,23 +14,9 @@
 // registers), a shuffle scan composes them inside each warp and the warp totals are chained through shared memory, and
 // each thread then replays its chunk from its true entry state and writes indices/extras at its true output offset.
 #include "common.cuh"
+#include "mt19937.cuh"
 
-constexpr int MT_N = 624, MT_M = 397;
 constexpr int MT_MAXS = 8;  // machine states: 0 = seeking an index, j>0 = j extra words still to consume
-
-__device__ __forceinline__ uint32_t mt_twist(uint32_t u, uint32_t v) {
-    const uint32_t y = (u & 0x80000000u) | (v & 0x7FFFFFFFu);
-    return (y >> 1) ^ ((y & 1u) ? 0x9908B0DFu : 0u);
-}
-
-__device__ __forceinline__ uint32_t mt_temper(uint32_t y) {
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9D2C5680u;
-    y ^= (y << 15) & 0xEFC60000u;
-    y ^= y >> 18;
-    return y;
-}
-
 constexpr int MT_THREADS = 128, MT_WARPS = MT_THREADS / 32;
 
 // transition function of a run of words: entry state s -> (exit state, indices emitted), packed in registers:
@@ -81,24 +67,24 @@ __device__ __forceinline__ MtFn mtfn_shfl_up(const MtFn& f, int d) {
 // next 624-word block of the MT19937 state, by all MT_THREADS threads of the CTA (three dependency-free phases):
 // new[i] = x[i+397] ^ twist(old[i], old[i+1]); x is old for i < 227, new after
 __device__ __forceinline__ void mt_regenerate(uint32_t* mt, int tid) {
-    constexpr int D = MT_N - MT_M;                                   // 227
+    constexpr int D = MT_DW;
     uint32_t y[(D + MT_THREADS - 1) / MT_THREADS];
     // phase A: i in [0,227)
-    for (int c = 0, i = tid; i < D; i += MT_THREADS, ++c) y[c] = mt[i + MT_M] ^ mt_twist(mt[i], mt[i + 1]);
+    for (int c = 0, i = tid; i < D; i += MT_THREADS, ++c) y[c] = mt[i + MT_MW] ^ mt19937_twist(mt[i], mt[i + 1]);
     __syncthreads();
     for (int c = 0, i = tid; i < D; i += MT_THREADS, ++c) mt[i] = y[c];
     __syncthreads();
     // phase B: i in [227,454) uses new[i-227], old[i], old[i+1]
-    for (int c = 0, i = D + tid; i < 2 * D; i += MT_THREADS, ++c) y[c] = mt[i - D] ^ mt_twist(mt[i], mt[i + 1]);
+    for (int c = 0, i = D + tid; i < 2 * D; i += MT_THREADS, ++c) y[c] = mt[i - D] ^ mt19937_twist(mt[i], mt[i + 1]);
     __syncthreads();
     for (int c = 0, i = D + tid; i < 2 * D; i += MT_THREADS, ++c) mt[i] = y[c];
     __syncthreads();
     // phase C: i in [454,623) uses new[i-227] (phase B), old[i], old[i+1]
-    for (int c = 0, i = 2 * D + tid; i < MT_N - 1; i += MT_THREADS, ++c) y[c] = mt[i - D] ^ mt_twist(mt[i], mt[i + 1]);
+    for (int c = 0, i = 2 * D + tid; i < MT_NW - 1; i += MT_THREADS, ++c) y[c] = mt[i - D] ^ mt19937_twist(mt[i], mt[i + 1]);
     __syncthreads();
-    for (int c = 0, i = 2 * D + tid; i < MT_N - 1; i += MT_THREADS, ++c) mt[i] = y[c];
+    for (int c = 0, i = 2 * D + tid; i < MT_NW - 1; i += MT_THREADS, ++c) mt[i] = y[c];
     __syncthreads();
-    if (tid == 0) mt[MT_N - 1] = mt[MT_M - 1] ^ mt_twist(mt[MT_N - 1], mt[0]);
+    if (tid == 0) mt[MT_NW - 1] = mt[MT_MW - 1] ^ mt19937_twist(mt[MT_NW - 1], mt[0]);
     __syncthreads();
 }
 
@@ -107,23 +93,23 @@ __device__ __forceinline__ void mt_regenerate(uint32_t* mt, int tid) {
 // fit_fn, which draws its save_obs coin first, simple_example.py:38 / obj.py:54).
 __global__ void __launch_bounds__(MT_THREADS) mt_skip_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos,
                                                              int n_words) {
-    __shared__ uint32_t mt[MT_N];
+    __shared__ uint32_t mt[MT_NW];
     const int tid = threadIdx.x;
-    uint32_t* key = mt_key + (size_t)blockIdx.x * MT_N;
+    uint32_t* key = mt_key + (size_t)blockIdx.x * MT_NW;
     int pos = mt_pos[blockIdx.x];
-    if (pos + n_words <= MT_N) {                       // common case: no regeneration, the key is untouched
+    if (pos + n_words <= MT_NW) {                       // common case: no regeneration, the key is untouched
         if (tid == 0) mt_pos[blockIdx.x] = pos + n_words;
         return;
     }
-    for (int i = tid; i < MT_N; i += MT_THREADS) mt[i] = key[i];
+    for (int i = tid; i < MT_NW; i += MT_THREADS) mt[i] = key[i];
     __syncthreads();
     int left = n_words;
     while (left > 0) {
-        if (pos >= MT_N) { mt_regenerate(mt, tid); pos = 0; }
-        const int take = min(left, MT_N - pos);
+        if (pos >= MT_NW) { mt_regenerate(mt, tid); pos = 0; }
+        const int take = min(left, MT_NW - pos);
         pos += take; left -= take;
     }
-    for (int i = tid; i < MT_N; i += MT_THREADS) key[i] = mt[i];
+    for (int i = tid; i < MT_NW; i += MT_THREADS) key[i] = mt[i];
     if (tid == 0) mt_pos[blockIdx.x] = pos;
 }
 
@@ -132,38 +118,38 @@ template <int ST>
 __global__ void __launch_bounds__(MT_THREADS)
 mt_draw_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int n_per_stream, uint32_t rng,
                uint32_t mask, int extra, int64_t* __restrict__ idx_out, uint32_t* __restrict__ extra_out) {
-    __shared__ uint32_t mt[MT_N];
-    __shared__ uint32_t tw[MT_N];
+    __shared__ uint32_t mt[MT_NW];
+    __shared__ uint32_t tw[MT_NW];
     __shared__ MtFn s_warp[MT_WARPS];          // inclusive function of each warp, then of everything before it
     __shared__ MtFn s_block;
     __shared__ int s_stop[MT_WARPS];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int stream_id = blockIdx.x;
-    uint32_t* key = mt_key + (size_t)stream_id * MT_N;
+    uint32_t* key = mt_key + (size_t)stream_id * MT_NW;
     int64_t* out = idx_out + (size_t)stream_id * n_per_stream;
     uint32_t* xout = extra_out ? extra_out + (size_t)stream_id * n_per_stream * extra : nullptr;
     const int S = ST > 0 ? ST : extra + 1;
 
-    for (int i = tid; i < MT_N; i += MT_THREADS) mt[i] = key[i];
+    for (int i = tid; i < MT_NW; i += MT_THREADS) mt[i] = key[i];
     int pos = mt_pos[stream_id];
     __syncthreads();
 
     int produced = 0;  // indices emitted so far
     int state = 0;     // machine state at `pos`
     while (produced < n_per_stream || state > 0) {
-        if (pos >= MT_N) {
+        if (pos >= MT_NW) {
             mt_regenerate(mt, tid);
             pos = 0;
         }
         // temper the available words
-        for (int i = pos + tid; i < MT_N; i += MT_THREADS) tw[i] = mt_temper(mt[i]);
+        for (int i = pos + tid; i < MT_NW; i += MT_THREADS) tw[i] = mt19937_temper(mt[i]);
         __syncthreads();
 
-        const int avail = MT_N - pos;
+        const int avail = MT_NW - pos;
         const int C = (avail + MT_THREADS - 1) / MT_THREADS;  // words per thread (<= 5)
         const int b = pos + tid * C;
-        const int e = min(MT_N, b + C);
+        const int e = min(MT_NW, b + C);
         const int len = max(0, e - b);
 
         // accept bits of this thread's chunk, in a register: bit i <=> word b+i passes the masked rejection test
@@ -224,7 +210,7 @@ mt_draw_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int 
         const int blk_state = (int)mtfn_st(blk, state);
         const int blk_count = (int)mtfn_cn(blk, state);
         // (4) replay with the mask; stop where the machine is seeking and everything requested is out
-        int stop = MT_N;  // first unconsumed position if the stream ends inside this thread's chunk
+        int stop = MT_NW;  // first unconsumed position if the stream ends inside this thread's chunk
         {
             int cur = 0;
             // leading extra words of the previous thread's last draw
@@ -247,7 +233,7 @@ mt_draw_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int 
             }
         }
         // a thread whose chunk starts after the end also reports its start
-        if (b < e && stop == MT_N && st == 0 && base >= n_per_stream) stop = e;
+        if (b < e && stop == MT_NW && st == 0 && base >= n_per_stream) stop = e;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) stop = min(stop, __shfl_xor_sync(0xffffffffu, stop, o));
         if (lane == 0) s_stop[warp] = stop;
@@ -256,33 +242,32 @@ mt_draw_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int 
 #pragma unroll
         for (int w = 1; w < MT_WARPS; ++w) stop = min(stop, s_stop[w]);
 
-        if (produced + blk_count >= n_per_stream && stop < MT_N) {
+        if (produced + blk_count >= n_per_stream && stop < MT_NW) {
             // the stream finished inside this block at `stop` (state 0 there)
             pos = stop;
             produced = n_per_stream;
             state = 0;
         } else if (produced + blk_count >= n_per_stream && blk_state == 0) {
-            pos = MT_N;  // finished exactly at the block end
+            pos = MT_NW;  // finished exactly at the block end
             produced = n_per_stream;
             state = 0;
         } else {
-            pos = MT_N;
+            pos = MT_NW;
             produced += blk_count;
             state = blk_state;
         }
         __syncthreads();
     }
 
-    for (int i = tid; i < MT_N; i += MT_THREADS) key[i] = mt[i];
+    for (int i = tid; i < MT_NW; i += MT_THREADS) key[i] = mt[i];
     if (tid == 0) mt_pos[stream_id] = pos;
 }
 
 int es_impl_draw_indices(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int n_streams, int n_per_stream,
                          uint64_t upper_bound, int extra_words, int64_t* idx_out, uint32_t* extra_out,
                          cudaStream_t stream) {
-    const uint32_t rng = (uint32_t)(upper_bound - 1);
-    uint32_t mask = rng;
-    mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
+    const Mt19937Bound bd = mt19937_randint_bound(upper_bound);
+    const uint32_t rng = bd.rng, mask = bd.mask;
     if (rng == 0) {
         // numpy returns `low` without consuming any random word when the range is empty
         ES_CHECK_CUDA(cudaMemsetAsync(idx_out, 0, sizeof(int64_t) * (size_t)n_streams * n_per_stream, stream));

@@ -16,7 +16,7 @@
 //
 // One CTA per stream.  The state lives in a ring of MG_RING 624-word blocks in shared memory (raw words for the recurrence and
 // for the state handed back, tempered words for the attempt windows), regenerated ahead of the cursor by the whole CTA with two
-// barriers per block (see `ensure`).  What the time goes to, measured with cycle counters (MG_PROFILE) and ncu on the way from
+// barriers per block (see `ensure`).  What the time goes to, measured with cycle counters and ncu on the way from
 // 109 ms to 72 ms per K = 10 000, T*act = 17 000 generation with 8 streams: the regeneration (69 blocks per rollout) is the
 // limiter and it is instruction-issue bound (issue slots 61 %): the textbook three dependent 227-word phases cost ~1 100 cycles
 // per block with 4 or 10 warps; ONE pass that recomputes up to three twists per word is as slow (~100 instructions per word);
@@ -40,26 +40,19 @@
 
 namespace {
 
-constexpr int MG_N = 624, MG_M = 397, MG_D = MG_N - MG_M;      // 227
 constexpr int MG_THREADS = 736, MG_WARPS = MG_THREADS / 32;    // 23 warps: see the word <-> thread map of the regeneration
 static_assert(MG_WARPS <= 32, "one shuffle scan over the warp totals");
 constexpr int MG_RING = 20;                                    // blocks in the ring (raw + tempered + one block of twists: 102 KB of shared memory)
-constexpr int MG_RW = MG_RING * MG_N, MG_RQ = MG_RW / 4;       // ring words; the tempered ring is stored as 4 quarter rings (see mg_tw_slot)
+constexpr int MG_RW = MG_RING * MT_NW, MG_RQ = MG_RW / 4;      // ring words; the tempered ring is stored as 4 quarter rings (see mg_tw_slot)
 static_assert(MG_RW % 4 == 0, "quarter rings");
 constexpr int MG_APT = 2;                                      // attempts per thread and step (consecutive attempts)
 constexpr int MG_WIN = 4 * MG_APT * MG_THREADS;                // words tested per step (5888 = 9.4 blocks)
-static_assert((MG_RING - 2) * MG_N >= MG_WIN + MG_N, "the ring holds the cursor's block and a whole window ahead of it");
+static_assert((MG_RING - 2) * MT_NW >= MG_WIN + MT_NW, "the ring holds the cursor's block and a whole window ahead of it");
 
-__device__ __forceinline__ uint32_t mg_twist(uint32_t u, uint32_t v) { return mt19937_twist(u, v); }
-__device__ __forceinline__ uint32_t mg_temper(uint32_t y) { return mt19937_temper(y); }
 // Where ring word k (0 <= k < MG_RW) of the TEMPERED stream lives: word k sits in quarter ring k % 4 at k / 4, so that the four
 // words of consecutive attempts (k = s + 4a + q) are consecutive in shared memory for a fixed q: the attempt windows read
 // without bank conflicts (stride-4 or stride-8 word reads were 4- / 8-way conflicts and half of a window step's time)
 __device__ __forceinline__ int mg_tw_slot(int k) { return (k & 3) * MG_RQ + (k >> 2); }
-// legacy_double: (a >> 5, b >> 6) -> [0, 1) with 53 bits
-__device__ __forceinline__ double mg_double(uint32_t a, uint32_t b) {
-    return __dmul_rn(__dadd_rn(__dmul_rn((double)(a >> 5), 67108864.0), (double)(b >> 6)), 1.0 / 9007199254740992.0);
-}
 struct MgShared {
     int wtot[2][MG_WARPS];
     int end;
@@ -69,6 +62,23 @@ struct MgShared {
 // two, so the cache state only depends on the parity of N and of e (c0 = the stream's incoming has_gauss)
 __device__ __forceinline__ int mg_cached(int c0, int N, int e) { return (N & 1) ? (c0 ^ (e & 1)) : c0; }
 
+// What the finishing kernels write once per evaluation e of a stream (ce = mg_cached(c0, N, e); g0, cache: the stream's
+// incoming and outgoing cached gaussian; out: the evaluation's N values)
+__device__ __forceinline__ void mg_cache_edges(int e, int n_eval, int c0, int ce, int N, double scale, const double* __restrict__ g0,
+                                               float* __restrict__ out, double* __restrict__ cache) {
+    if (e == 0 && ce && N > 0) out[0] = (float)__dmul_rn(*g0, scale);              // the stream's incoming cached gaussian
+    if (e == n_eval - 1 && !mg_cached(c0, N, n_eval)) *cache = 0.0;                // nothing cached afterwards
+    if (N == 0 && e == 0 && c0) *cache = *g0;                                      // no draws at all: the cache is untouched
+}
+// the pair g of an accepted attempt: values p and p + 1 of the evaluation; a value N is the cache
+__device__ __forceinline__ void mg_store_pair(double2 g, int p, int N, bool last_eval, double scale, float* __restrict__ out,
+                                              double* __restrict__ cache) {
+    out[p] = (float)__dmul_rn(g.x, scale);
+    if (p + 1 < N) out[p + 1] = (float)__dmul_rn(g.y, scale);
+    else if (!last_eval) out[N] = (float)__dmul_rn(g.y, scale);        // = value 0 of the stream's next evaluation
+    else *cache = g.y;                                                 // the cache the stream hands back
+}
+
 __global__ void __launch_bounds__(MG_THREADS, 1)
 mt_gauss_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int32_t* __restrict__ has_gauss_io,
                 const double* __restrict__ gauss_io, int n_pairs, uint32_t rng, uint32_t mask, int coins, int N,
@@ -76,15 +86,15 @@ mt_gauss_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int
                 int32_t* __restrict__ c0_out, double* __restrict__ gauss0_out) {
     extern __shared__ uint32_t mg_smem[];
     uint32_t* s_raw = mg_smem;                                 // [MG_RING][624] raw state words (the recurrence, the state handed back)
-    uint32_t* s_tw = mg_smem + MG_RING * MG_N;                 // [MG_RING][624] tempered words (what the consumers read)
-    uint32_t* s_T = mg_smem + 2 * MG_RING * MG_N;              // [624] twists of the block being regenerated
+    uint32_t* s_tw = mg_smem + MG_RING * MT_NW;                // [MG_RING][624] tempered words (what the consumers read)
+    uint32_t* s_T = mg_smem + 2 * MG_RING * MT_NW;             // [624] twists of the block being regenerated
     __shared__ MgShared sh;
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int sid = blockIdx.x;
-    for (int i = tid; i < MG_N; i += MG_THREADS) {
-        const uint32_t y = mt_key[(size_t)sid * MG_N + i];
-        s_raw[i] = y; s_tw[mg_tw_slot(i)] = mg_temper(y);
+    for (int i = tid; i < MT_NW; i += MG_THREADS) {
+        const uint32_t y = mt_key[(size_t)sid * MT_NW + i];
+        s_raw[i] = y; s_tw[mg_tw_slot(i)] = mt19937_temper(y);
     }
     const long long cur0 = mt_pos[sid];
     const int c0 = has_gauss_io[sid] ? 1 : 0;
@@ -93,55 +103,32 @@ mt_gauss_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int
 
     // the cursor as (block, offset in the block, offset in the ring): 32-bit bookkeeping, no 64-bit divisions per step
     int gen_b = 0;                                             // newest generated block (block 0 = the incoming state)
-#ifdef MG_PROFILE
-    long long pr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    const long long t_start = clock64();
-#endif
-    int cblk = (int)(cur0 / MG_N), coff = (int)(cur0 % MG_N), cring = (int)(cur0 % (MG_RING * MG_N));
+    int cblk = (int)(cur0 / MT_NW), coff = (int)(cur0 % MT_NW), cring = (int)(cur0 % (MG_RING * MT_NW));
     auto advance = [&](int n) {
         coff += n;
-        while (coff >= MG_N) { coff -= MG_N; ++cblk; }
+        while (coff >= MT_NW) { coff -= MT_NW; ++cblk; }
         cring += n;
-        if (cring >= MG_RING * MG_N) cring -= MG_RING * MG_N;
+        if (cring >= MG_RING * MT_NW) cring -= MG_RING * MT_NW;
     };
-    // Next block of the recurrence into ring slot (b + 1) % MG_RING by the whole CTA.  The recurrence
-    // N[i] = N[i-227] ^ tw(O[i], O[i+1]) is XOR-linear in its first term, so with the 623 twists T[k] = tw(O[k], O[k+1]) of the
-    // OLD block (one per thread, exchanged through shared memory) every new word is a few XORs of old words and twists -- two
-    // barriers per block instead of the three dependent 227-word phases of the textbook form:
-    //   i <  227:  N[i] = O[i+397] ^ T[i]
-    //   i <  454:  N[i] = O[i+170] ^ T[i-227] ^ T[i]
-    //   i <  623:  N[i] = O[i-57]  ^ T[i-454] ^ T[i-227] ^ T[i]
-    //   N[623] = N[396] ^ tw(O[623], N[0])
-    // (recomputing the twists instead of sharing them -- one barrier, ~100 instructions per word -- measured slower.)
-    // word of this thread in the regeneration: every warp stays inside one of the three ranges and all three ranges run the SAME
-    // code (an unused twist index points at s_T[623], which holds 0); the odd word out (N[623], the longest expression) has a
-    // warp of its own: threads 0-226 | 256-482 | 512-680 | 704.  Everything that does not depend on the block is computed once.
-    const int my_i = (tid < 256) ? (tid < MG_D ? tid : -1) : (tid < 512) ? (tid - 256 < MG_D ? tid - 256 + MG_D : -1)
-                   : (tid < 704) ? (tid - 512 < MG_N - 1 - 2 * MG_D ? tid - 512 + 2 * MG_D : -1) : (tid == 704 ? MG_N - 1 : -1);
-    const bool plain = my_i >= 0 && my_i < MG_N - 1;
-    const int r_o = !plain ? 0 : (my_i < MG_D ? my_i + MG_M : my_i < 2 * MG_D ? my_i + MG_M - MG_D : my_i + MG_M - 2 * MG_D);
-    const int r_a = plain ? my_i : MG_N - 1;
-    const int r_b = (plain && my_i >= MG_D) ? my_i - MG_D : MG_N - 1;
-    const int r_c = (plain && my_i >= 2 * MG_D) ? my_i - 2 * MG_D : MG_N - 1;
-    const int r_tw = my_i >= 0 ? (my_i & 3) * MG_RQ + (my_i >> 2) : 0;       // mg_tw_slot(nslot * 624 + i) = r_tw + nslot * 156
-    if (tid == 0) s_T[MG_N - 1] = 0;
+    // Next block of the recurrence into ring slot (b + 1) % MG_RING by the whole CTA, with two barriers per block instead of the
+    // three dependent 227-word phases of the textbook form: the twists of the old block are shared through s_T and every thread
+    // forms one new word (Mt19937Regen).  (Recomputing the twists instead of sharing them -- one barrier, ~100 instructions per
+    // word -- measured slower.)  Everything that does not depend on the block is computed once.
+    Mt19937Regen rg;
+    rg.init(tid);
+    const int r_tw = rg.my_i >= 0 ? (rg.my_i & 3) * MG_RQ + (rg.my_i >> 2) : 0;   // mg_tw_slot(nslot * 624 + i) = r_tw + nslot * 156
+    if (tid == 0) s_T[MT_NW - 1] = 0;
     auto ensure = [&](int n) {                                 // the next n words are in the ring (n uniform over the CTA)
-        const int blocks = cblk + (coff + n + MG_N - 1) / MG_N;               // blocks [0, blocks) are needed
+        const int blocks = cblk + (coff + n + MT_NW - 1) / MT_NW;              // blocks [0, blocks) are needed
         while (gen_b + 1 < blocks) {
-            const uint32_t* __restrict__ O = s_raw + (gen_b % MG_RING) * MG_N;
+            const uint32_t* __restrict__ O = s_raw + (gen_b % MG_RING) * MT_NW;
             const int nslot = (gen_b + 1) % MG_RING;
-            uint32_t* __restrict__ dst = s_raw + nslot * MG_N;
-            if (tid < MG_N - 1) s_T[tid] = mg_twist(O[tid], O[tid + 1]);
+            uint32_t* __restrict__ dst = s_raw + nslot * MT_NW;
+            if (tid < MT_NW - 1) s_T[tid] = mt19937_twist(O[tid], O[tid + 1]);
             __syncthreads();
-            if (plain) {
-                const uint32_t y = O[r_o] ^ s_T[r_a] ^ s_T[r_b] ^ s_T[r_c];
-                dst[my_i] = y; s_tw[r_tw + nslot * (MG_N / 4)] = mg_temper(y);
-            } else if (my_i == MG_N - 1) {
-                const uint32_t n0 = O[MG_M] ^ s_T[0];
-                const uint32_t n396 = O[396 + MG_M - MG_D] ^ s_T[396 - MG_D] ^ s_T[396];
-                const uint32_t y = n396 ^ mg_twist(O[MG_N - 1], n0);
-                dst[my_i] = y; s_tw[r_tw + nslot * (MG_N / 4)] = mg_temper(y);
-            }
+            auto put = [&](uint32_t y) { dst[rg.my_i] = y; s_tw[r_tw + nslot * (MT_NW / 4)] = mt19937_temper(y); };
+            if (rg.plain) put(rg.word(O, s_T));
+            else if (rg.my_i == MT_NW - 1) put(mt19937_last_word(O, s_T));
             __syncthreads();
             ++gen_b;
         }
@@ -180,9 +167,7 @@ mt_gauss_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int
             while (need > 0) {
                 // only as many words as the remaining attempts can use at the usual acceptance rate are regenerated up front
                 ensure(MG_WIN);
-                // this thread's MG_APT consecutive attempts (4 words each).  x = 2 u - 1 with u = (a >> 5, b >> 6) / 2^53: the
-                // 53-bit integer converts exactly, and one fused multiply-add rounds the exact value of 2 u - 1 once -- the
-                // reference's (2.0 * u) - 1.0 rounds the same exact value once (2 u is exact)
+                // this thread's MG_APT consecutive attempts (4 words each)
                 uint32_t wd[MG_APT][4];
                 bool acc[MG_APT];
                 unsigned bal[MG_APT];
@@ -196,13 +181,7 @@ mt_gauss_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int
                         if (k4 >= MG_RQ) k4 -= MG_RQ;
                         wd[j][q] = s_tw[((ph + q) & 3) * MG_RQ + k4];
                     }
-                    // u = (a >> 5, b >> 6) as a 53-bit integer, exactly, in float64; x = 2 u / 2^53 - 1: one fused multiply-add rounds
-                    // the exact value once, like the reference's (2.0 * u) - 1.0 (2 u is exact)
-                    const double v1 = fma((double)(wd[j][0] >> 5), 67108864.0, (double)(wd[j][1] >> 6));
-                    const double v2 = fma((double)(wd[j][2] >> 5), 67108864.0, (double)(wd[j][3] >> 6));
-                    const double x1 = fma(v1, 1.0 / 4503599627370496.0, -1.0), x2 = fma(v2, 1.0 / 4503599627370496.0, -1.0);
-                    const double r2 = __dadd_rn(__dmul_rn(x1, x1), __dmul_rn(x2, x2));
-                    acc[j] = r2 < 1.0 && r2 != 0.0;
+                    acc[j] = mt19937_polar_accept(wd[j][0], wd[j][1], wd[j][2], wd[j][3]);
                     bal[j] = __ballot_sync(0xffffffffu, acc[j]);
                 }
                 const unsigned buf = step & 1;
@@ -242,26 +221,19 @@ mt_gauss_kernel(uint32_t* __restrict__ mt_key, int32_t* __restrict__ mt_pos, int
             }
         }
     }
-#ifdef MG_PROFILE
-    if (sid == 0 && (tid == 0 || tid == 300 || tid == 623))
-        printf("tid %d: %lld blocks: twist %lld, bar1 %lld, xor+temper %lld, bar2 %lld cycles per block; total kernel %lld cycles, %u steps\n", tid, pr[4],
-               pr[0] / max(pr[4], 1LL), pr[1] / max(pr[4], 1LL), pr[2] / max(pr[4], 1LL), pr[3] / max(pr[4], 1LL), clock64() - t_start, step);
-#endif
     // ---- hand the state back: the block the cursor is in (position 624 = block exhausted), and its position ----
     const bool at_end = coff == 0 && (cblk > 0);
     const int b_last = at_end ? cblk - 1 : cblk;
     ensure(0);                                                 // (block b_last is in the ring: the cursor has been there)
-    const uint32_t* last = s_raw + (b_last % MG_RING) * MG_N;
-    for (int i = tid; i < MG_N; i += MG_THREADS) mt_key[(size_t)sid * MG_N + i] = last[i];
+    const uint32_t* last = s_raw + (b_last % MG_RING) * MT_NW;
+    for (int i = tid; i < MT_NW; i += MG_THREADS) mt_key[(size_t)sid * MT_NW + i] = last[i];
     if (tid == 0) {
-        mt_pos[sid] = at_end ? MG_N : coff;
+        mt_pos[sid] = at_end ? MT_NW : coff;
         has_gauss_io[sid] = mg_cached(c0, N, 2 * n_pairs);     // (the cached VALUE is written by the finishing kernel)
     }
 }
 
-// The recorded attempts -> gaussians, on the whole GPU: attempt r of evaluation e gives values c_e + 2r (f*x2) and c_e + 2r + 1
-// (f*x1) of the evaluation's N; a value N (the second of the last attempt) is the cache: the first value of the stream's next
-// evaluation, or the cached gaussian the stream hands back.
+// The recorded attempts -> gaussians, on the whole GPU: attempt r of evaluation e gives values c_e + 2r and c_e + 2r + 1.
 __global__ void __launch_bounds__(256)
 mt_gauss_finish_kernel(const uint4* __restrict__ acc4, int a_max, const int32_t* __restrict__ c0_in, const double* __restrict__ gauss0,
                        int n_streams, int n_pairs, int N, double scale, float* __restrict__ noise_out, double* __restrict__ gauss_io) {
@@ -275,23 +247,10 @@ mt_gauss_finish_kernel(const uint4* __restrict__ acc4, int a_max, const int32_t*
         const int ce = mg_cached(c0, N, e);
         const int need = (N - ce + 1) >> 1;
         float* out = noise_out + (size_t)ge * N;
-        if (r == 0) {
-            if (e == 0 && ce && N > 0) out[0] = (float)__dmul_rn(gauss0[sid], scale);     // the stream's incoming cached gaussian
-            if (e == 2 * n_pairs - 1 && !mg_cached(c0, N, 2 * n_pairs)) gauss_io[sid] = 0.0;   // nothing cached afterwards
-            if (N == 0 && e == 0 && c0) gauss_io[sid] = gauss0[sid];                       // no draws at all: the cache is untouched
-        }
+        if (r == 0) mg_cache_edges(e, 2 * n_pairs, c0, ce, N, scale, gauss0 + sid, out, gauss_io + sid);
         if (r >= need) continue;
         const uint4 w = acc4[i];
-        const double x1 = __dadd_rn(__dmul_rn(2.0, mg_double(w.x, w.y)), -1.0);
-        const double x2 = __dadd_rn(__dmul_rn(2.0, mg_double(w.z, w.w)), -1.0);
-        const double r2 = __dadd_rn(__dmul_rn(x1, x1), __dmul_rn(x2, x2));
-        const double f = sqrt(__ddiv_rn(__dmul_rn(-2.0, log(r2)), r2));
-        const int p = ce + 2 * r;
-        out[p] = (float)__dmul_rn(__dmul_rn(f, x2), scale);
-        const double g2 = __dmul_rn(f, x1);
-        if (p + 1 < N) out[p + 1] = (float)__dmul_rn(g2, scale);
-        else if (e + 1 < 2 * n_pairs) out[N] = (float)__dmul_rn(g2, scale);              // = value 0 of the stream's next evaluation
-        else gauss_io[sid] = g2;                                                          // the cache the stream hands back
+        mg_store_pair(mt19937_polar_pair(w.x, w.y, w.z, w.w), ce + 2 * r, N, e == 2 * n_pairs - 1, scale, out, gauss_io + sid);
     }
 }
 
@@ -356,20 +315,6 @@ __global__ void __launch_bounds__(640) mj_lists_kernel() {
 // the two block / twist buffers so that every shared-memory address is a per-thread register plus an immediate (the first
 // version recomputed them and issued ~110 instructions per warp and block; the kernel is issue-bound).
 constexpr int MF_WARPS = 21, MF_THREADS = 32 * MF_WARPS;
-struct MjTaps { int o, a, b, c; };
-__device__ __forceinline__ MjTaps mj_taps(int i) {            // N[i] = O[o] ^ T[a] ^ T[b] ^ T[c], 0 <= i <= 622
-    MjTaps m;
-    m.o = i < MT_DW ? i + MT_MW : (i < 2 * MT_DW ? i + MT_MW - MT_DW : i + MT_MW - 2 * MT_DW);
-    m.a = i;
-    m.b = i >= MT_DW ? i - MT_DW : MT_NW - 1;
-    m.c = i >= 2 * MT_DW ? i - 2 * MT_DW : MT_NW - 1;
-    return m;
-}
-__device__ __forceinline__ uint32_t mj_last_word(const uint32_t* __restrict__ O, const uint32_t* __restrict__ T) {     // N[623]
-    const uint32_t n0 = O[MT_MW] ^ T[0];
-    const uint32_t n396 = O[396 + MT_MW - MT_DW] ^ T[396 - MT_DW] ^ T[396];
-    return n396 ^ mt19937_twist(O[MT_NW - 1], n0);
-}
 
 // segments in the order the CTAs should start: most jumps first, so that the long CTAs do not end up in the last wave
 __device__ __forceinline__ int mj_jumps(unsigned block) {       // non-zero hexadecimal digits = jumps to reach the block
@@ -403,7 +348,7 @@ mt_fill_kernel(const uint32_t* __restrict__ mt_key, int n_streams, int n_seg, in
     const bool owner = (lane < 31 && iw < MT_NW - 1) || last;
     const bool tail_warp = warp == MF_WARPS - 1;
     const int i = iw < MT_NW - 1 ? iw : MT_NW - 2;             // (clamped: whole warps take part in the shuffle)
-    const MjTaps tp = mj_taps(i);
+    const Mt19937Taps tp = mt19937_taps(i);
     uint32_t* __restrict__ out = words + (size_t)sid * stride_words;
     for (int j = tid; j < MT_NW; j += MF_THREADS) {
         const uint32_t y = mt_key[(size_t)sid * MT_NW + j];
@@ -419,7 +364,7 @@ mt_fill_kernel(const uint32_t* __restrict__ mt_key, int n_streams, int n_seg, in
         constexpr bool OUT = decltype(out_tag)::value;
         uint32_t n = O[tp.o] ^ T[tp.a] ^ T[tp.b] ^ T[tp.c];
         if (tail_warp) {
-            if (last) n = mj_last_word(O, T);
+            if (last) n = mt19937_last_word(O, T);
         }
         const uint32_t nx = __shfl_down_sync(0xffffffffu, n, 1);
         const uint32_t tw = mt19937_twist(n, nx);
@@ -496,18 +441,7 @@ mt_fill_kernel(const uint32_t* __restrict__ mt_key, int n_streams, int n_seg, in
     if (b < Lb) regen(Yes(), X0, T0, X1, T1, opw);
 }
 
-// ---- the accept bit of every possible attempt, in parallel: one CTA per (stream, chunk of 4096 words), thread q looks at the
-//      four attempts that start at words 4 q .. 4 q + 3 of the chunk (one per phase) ----
-__device__ __forceinline__ bool mj_accept(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3) {
-    // x = 2 u - 1 with u = (a >> 5, b >> 6) / 2^53: the 53-bit integer is exact in float64 and one fused multiply-add rounds
-    // the exact value of 2 u - 1 once, like the reference's (2.0 * u) - 1.0 (2 u is exact); r2 with two roundings as in C
-    const double v1 = fma((double)(w0 >> 5), 67108864.0, (double)(w1 >> 6));
-    const double v2 = fma((double)(w2 >> 5), 67108864.0, (double)(w3 >> 6));
-    const double x1 = fma(v1, 1.0 / 4503599627370496.0, -1.0), x2 = fma(v2, 1.0 / 4503599627370496.0, -1.0);
-    const double r2 = __dadd_rn(__dmul_rn(x1, x1), __dmul_rn(x2, x2));
-    return r2 < 1.0 && r2 != 0.0;
-}
-
+// ---- the accept bit of every possible attempt, in parallel ----
 // One WARP per chunk (4096 words = 1024 attempts of each phase): 32 steps of 128 words; lane l holds words 4 l .. 4 l + 3 of a step
 // (one 16-byte load), takes the next three from lane l + 1 (lane 31: from the next step's first load, which is already in
 // flight), and tests the four attempts that start at its words; lane s keeps the ballots of step s, so the 32 mask words of a
@@ -531,10 +465,10 @@ mt_flags_kernel(const uint32_t* __restrict__ words, size_t stride_words, int n_c
         b.z = __shfl_down_sync(0xffffffffu, cur.z, 1);
         const uint32_t n0 = __shfl_sync(0xffffffffu, nxt1.x, 0), n1 = __shfl_sync(0xffffffffu, nxt1.y, 0), n2 = __shfl_sync(0xffffffffu, nxt1.z, 0);
         if (lane == 31) { b.x = n0; b.y = n1; b.z = n2; }
-        const unsigned b0 = __ballot_sync(0xffffffffu, mj_accept(cur.x, cur.y, cur.z, cur.w));
-        const unsigned b1 = __ballot_sync(0xffffffffu, mj_accept(cur.y, cur.z, cur.w, b.x));
-        const unsigned b2 = __ballot_sync(0xffffffffu, mj_accept(cur.z, cur.w, b.x, b.y));
-        const unsigned b3 = __ballot_sync(0xffffffffu, mj_accept(cur.w, b.x, b.y, b.z));
+        const unsigned b0 = __ballot_sync(0xffffffffu, mt19937_polar_accept(cur.x, cur.y, cur.z, cur.w));
+        const unsigned b1 = __ballot_sync(0xffffffffu, mt19937_polar_accept(cur.y, cur.z, cur.w, b.x));
+        const unsigned b2 = __ballot_sync(0xffffffffu, mt19937_polar_accept(cur.z, cur.w, b.x, b.y));
+        const unsigned b3 = __ballot_sync(0xffffffffu, mt19937_polar_accept(cur.w, b.x, b.y, b.z));
         if (lane == s) { keep[0] = b0; keep[1] = b1; keep[2] = b2; keep[3] = b3; }
         cur = nxt1; nxt1 = nxt2; nxt2 = nxt3; nxt3 = far;
     }
@@ -719,17 +653,13 @@ mt_emit_kernel(const uint32_t* __restrict__ words, size_t stride_words, const ui
     const int c0 = c0_in[sid], ce = mg_cached(c0, N, e);
     const int need = (N - ce + 1) >> 1;
     float* out = noise_out + (size_t)ge * N;
-    if (tid == 0) {
-        if (e == 0 && ce && N > 0) out[0] = (float)__dmul_rn(gauss0[sid], scale);          // the stream's incoming cached gaussian
-        if (e == 2 * n_pairs - 1 && !mg_cached(c0, N, 2 * n_pairs)) gauss_io[sid] = 0.0;    // nothing cached afterwards
-        if (N == 0 && e == 0 && c0) gauss_io[sid] = gauss0[sid];
-    }
+    if (tid == 0) mg_cache_edges(e, 2 * n_pairs, c0, ce, N, scale, gauss0 + sid, out, gauss_io + sid);
     const uint32_t* __restrict__ gw = words + (size_t)sid * stride_words + reg_start[ge];
     int found = 0;
     for (unsigned it = 0; found < need; ++it) {
         const uint32_t* __restrict__ wp = gw + (size_t)4 * (it * 1024u + tid);
         const uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3);
-        const bool acc = mj_accept(w0, w1, w2, w3);
+        const bool acc = mt19937_polar_accept(w0, w1, w2, w3);
         const unsigned bal = __ballot_sync(0xffffffffu, acc);
         if (lane == 0) s_wt[it & 1][warp] = __popc(bal);
         __syncthreads();
@@ -741,21 +671,145 @@ mt_emit_kernel(const uint32_t* __restrict__ words, size_t stride_words, const ui
         }
         const int total = __shfl_sync(0xffffffffu, scan, 31);
         const int rank = found + (warp ? __shfl_sync(0xffffffffu, scan, warp - 1) : 0) + __popc(bal & ((1u << lane) - 1u));
-        if (acc && rank < need) {
-            const double v1 = fma((double)(w0 >> 5), 67108864.0, (double)(w1 >> 6));
-            const double v2 = fma((double)(w2 >> 5), 67108864.0, (double)(w3 >> 6));
-            const double x1 = fma(v1, 1.0 / 4503599627370496.0, -1.0), x2 = fma(v2, 1.0 / 4503599627370496.0, -1.0);
-            const double r2 = __dadd_rn(__dmul_rn(x1, x1), __dmul_rn(x2, x2));
-            const double f = sqrt(__ddiv_rn(__dmul_rn(-2.0, log(r2)), r2));
-            const int p = ce + 2 * rank;
-            out[p] = (float)__dmul_rn(__dmul_rn(f, x2), scale);
-            const double g2 = __dmul_rn(f, x1);
-            if (p + 1 < N) out[p + 1] = (float)__dmul_rn(g2, scale);
-            else if (e + 1 < 2 * n_pairs) out[N] = (float)__dmul_rn(g2, scale);            // = value 0 of the stream's next evaluation
-            else gauss_io[sid] = g2;                                                        // the cache the stream hands back
-        }
+        if (acc && rank < need)
+            mg_store_pair(mt19937_polar_pair(w0, w1, w2, w3), ce + 2 * rank, N, e == 2 * n_pairs - 1, scale, out, gauss_io + sid);
         found += total;
     }
+}
+
+// ---- how one es_draw_noisy call runs: the sequential kernel, or the jump-ahead path and the sizes of its buffers ----
+struct MgPlan {
+    bool jump;
+    int lb_log2;                  // segments of 2^lb_log2 blocks, n_seg per stream
+    long long n_seg, n_chunks;    // n_chunks chunks of MJ_CW words per stream
+    size_t gen_words, stride_words;
+};
+
+// How many words can a stream consume?  Per rollout ceil(N / 2) accepted attempts at acceptance pi / 4 (a negative binomial
+// count), 4 words each; per pair one index draw (~1.08 words with rejections, bounded generously) and the coins.  The
+// jump-ahead pass generates the mean + 12 sigma of the total (+ slack); the walk flags an overflow.
+int mg_plan(const es_ctx* ctx, int n_streams, int n_pairs, int coins, int N, MgPlan& pl) {
+    const double p_acc = 0.78539816339744830962, n_acc = (N + 1) / 2;
+    const double att_mean = n_acc / p_acc, att_sd = sqrt(n_acc * (1.0 - p_acc)) / p_acc;
+    const double evals = 2.0 * n_pairs;
+    const double words_max = 624.0 + n_pairs * (8.0 + 4.0 * coins) + 4.0 * (evals * att_mean + 12.0 * sqrt(evals) * att_sd + 64.0) +
+                             2.0 * MG_WIN + 16.0 * MT_NW;
+    const long long blocks_needed = (long long)(words_max / MT_NW) + 1;
+    // jump-ahead when a stream is long enough to be worth splitting (ES_MT_JUMP=0 / 1 overrides; ES_MT_JUMP_LB: log2 of the
+    // segment length in blocks, for tests)
+    const char* ej = getenv("ES_MT_JUMP");
+    const bool forced = ej && atoi(ej) != 0;
+    pl = MgPlan{};
+    if (!(ej ? forced : blocks_needed >= 2048)) return ES_OK;
+    int lb = 3;
+    const char* el = getenv("ES_MT_JUMP_LB");
+    if (el) lb = atoi(el);
+    else
+        while (lb < MJ_BITS_RANGE - 1 && (long long)n_streams * ((blocks_needed + (1LL << lb) - 1) >> lb) > 4LL * ctx->sm_count) ++lb;
+    if (lb < 0) lb = 0;
+    if (lb > MJ_BITS_RANGE - 1) lb = MJ_BITS_RANGE - 1;
+    const long long n_seg = (blocks_needed + (1LL << lb) - 1) >> lb;
+    if (((n_seg << lb) >> MJ_BITS_RANGE) != 0 || (double)(n_seg << lb) * MT_NW > 4.0e9 || n_seg > 65535) {
+        // the block index of a segment start must fit the available jumps (2^20 blocks = 654 M words per stream) and a
+        // 32-bit word index: longer streams take the sequential kernel unless the jump-ahead path was asked for explicitly
+        if (!forced) return ES_OK;
+        es_set_error("es_draw_noisy: %lld blocks per stream exceed the jump-ahead range (2^%d blocks)", n_seg << lb, MJ_BITS_RANGE);
+        return ES_ERR_UNSUPPORTED;
+    }
+    pl.jump = true;
+    pl.lb_log2 = lb;
+    pl.n_seg = n_seg;
+    // (whole chunks of MJ_CW words, + one chunk of padding: the flags kernel reads 4 words past every attempt start)
+    pl.gen_words = (size_t)(1 + (n_seg << lb)) * MT_NW;
+    pl.n_chunks = (long long)((pl.gen_words + MJ_CW - 1) / MJ_CW);
+    pl.stride_words = (size_t)(pl.n_chunks + 1) * MJ_CW;
+    return ES_OK;
+}
+
+struct MgDraw {                   // the arguments of one es_draw_noisy call
+    uint32_t* mt_key; int32_t* mt_pos; int32_t* has_gauss; double* gauss;
+    int n_streams, n_pairs;
+    uint32_t rng, mask;
+    int coins, N;
+    double scale;
+    int64_t* idx_out; uint32_t* extra_out; float* noise_out;
+};
+
+size_t mg_pad(size_t b) { return (b + 255) & ~(size_t)255; }
+
+int mg_launch_jump(es_ctx* ctx, const MgDraw& d, const MgPlan& pl, cudaStream_t stream) {
+    // scratch: the streams' words | accept masks [stream][phase][chunk][32] | chunk counts -> prefixes [stream][phase][chunk]
+    //          | first word of every rollout [stream][2 n] | incoming cache per stream
+    const size_t n_eval = (size_t)d.n_streams * 2 * d.n_pairs;
+    const size_t words_bytes = mg_pad((size_t)d.n_streams * pl.stride_words * sizeof(uint32_t));
+    const size_t mask_bytes = mg_pad((size_t)d.n_streams * 4 * pl.n_chunks * 32 * sizeof(uint32_t));
+    const size_t cnt_bytes = mg_pad((size_t)d.n_streams * 4 * pl.n_chunks * sizeof(uint32_t));
+    const size_t reg_bytes = mg_pad(n_eval * sizeof(uint32_t));
+    const size_t c0_bytes = mg_pad((size_t)d.n_streams * sizeof(int32_t)), g0_bytes = mg_pad((size_t)d.n_streams * sizeof(double));
+    const size_t ord_bytes = mg_pad((size_t)pl.n_seg * sizeof(uint16_t));
+    void* scratch = nullptr;
+    int rc = es_ctx_scratch(ctx, words_bytes + mask_bytes + cnt_bytes + reg_bytes + c0_bytes + g0_bytes + ord_bytes, &scratch);
+    if (rc) return rc;
+    char* at = (char*)scratch;
+    uint32_t* words = (uint32_t*)at; at += words_bytes;
+    uint32_t* masks = (uint32_t*)at; at += mask_bytes;
+    uint32_t* counts = (uint32_t*)at; at += cnt_bytes;
+    uint32_t* reg_start = (uint32_t*)at; at += reg_bytes;
+    int32_t* c0 = (int32_t*)at; at += c0_bytes;
+    double* gauss0 = (double*)at; at += g0_bytes;
+    uint16_t* order = (uint16_t*)at;
+    if (!ctx->mj_lists_ready) {
+        mj_lists_kernel<<<MJ_NPOLY, 640, 0, stream>>>();
+        ES_LAUNCHED(ctx);
+        ctx->mj_lists_ready = 1;
+    }
+    mj_order_kernel<<<1, 1024, 0, stream>>>((int)pl.n_seg, pl.lb_log2, order);
+    ES_LAUNCHED(ctx);
+    const size_t smem = (size_t)(MJ_WIN_BLOCKS + 6) * MT_NW * sizeof(uint32_t);
+    ES_CHECK_CUDA(cudaFuncSetAttribute(mt_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    mt_fill_kernel<<<(unsigned)(d.n_streams * pl.n_seg), MF_THREADS, smem, stream>>>(d.mt_key, d.n_streams, (int)pl.n_seg, pl.lb_log2,
+                                                                                   order, words, pl.stride_words);
+    ES_LAUNCHED(ctx);
+    mt_flags_kernel<<<dim3((unsigned)((pl.n_chunks + MFL_WARPS - 1) / MFL_WARPS), (unsigned)d.n_streams), 32 * MFL_WARPS, 0, stream>>>(
+        words, pl.stride_words, (int)pl.n_chunks, masks, counts);
+    ES_LAUNCHED(ctx);
+    mt_scan_kernel<<<d.n_streams * 4, 1024, 0, stream>>>(counts, (int)pl.n_chunks);
+    ES_LAUNCHED(ctx);
+    mt_walk_kernel<<<d.n_streams, 32, 0, stream>>>(d.mt_key, d.mt_pos, d.has_gauss, d.gauss, d.n_pairs, d.rng, d.mask, d.coins, d.N,
+                                                   d.idx_out, d.extra_out, reg_start, c0, gauss0, words, pl.stride_words,
+                                                   (int)pl.n_chunks, masks, counts, (uint32_t)(pl.gen_words - 8), ctx->err_dev);
+    ES_LAUNCHED(ctx);
+    mt_emit_kernel<<<(unsigned)n_eval, 1024, 0, stream>>>(words, pl.stride_words, reg_start, c0, gauss0, d.n_pairs, d.N, d.scale,
+                                                          d.noise_out, d.gauss);
+    ES_LAUNCHED(ctx);
+    return ES_OK;
+}
+
+int mg_launch_sequential(es_ctx* ctx, const MgDraw& d, cudaStream_t stream) {
+    // scratch: the accepted attempts' words [stream][evaluation][a_max] (16 bytes per two gaussians), the incoming cache per
+    // stream
+    const size_t n_eval = (size_t)d.n_streams * 2 * d.n_pairs;
+    const int a_max = (d.N + 1) / 2 > 0 ? (d.N + 1) / 2 : 1;
+    const size_t acc_bytes = mg_pad(n_eval * a_max * sizeof(uint4));
+    const size_t c0_bytes = mg_pad((size_t)d.n_streams * sizeof(int32_t)), g0_bytes = mg_pad((size_t)d.n_streams * sizeof(double));
+    void* scratch = nullptr;
+    int rc = es_ctx_scratch(ctx, acc_bytes + c0_bytes + g0_bytes, &scratch);
+    if (rc) return rc;
+    uint4* acc4 = (uint4*)scratch;
+    int32_t* c0 = (int32_t*)((char*)scratch + acc_bytes);
+    double* gauss0 = (double*)((char*)scratch + acc_bytes + c0_bytes);
+    const size_t smem = (size_t)(2 * MG_RING + 1) * MT_NW * sizeof(uint32_t);
+    ES_CHECK_CUDA(cudaFuncSetAttribute(mt_gauss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    mt_gauss_kernel<<<d.n_streams, MG_THREADS, smem, stream>>>(d.mt_key, d.mt_pos, d.has_gauss, d.gauss, d.n_pairs, d.rng, d.mask,
+                                                               d.coins, d.N, d.idx_out, d.extra_out, acc4, a_max, c0, gauss0);
+    ES_LAUNCHED(ctx);
+    const long long total = (long long)n_eval * a_max;
+    int blocks = es_div_up(total, 256);
+    if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
+    mt_gauss_finish_kernel<<<blocks, 256, 0, stream>>>(acc4, a_max, c0, gauss0, d.n_streams, d.n_pairs, d.N, d.scale, d.noise_out,
+                                                       d.gauss);
+    ES_LAUNCHED(ctx);
+    return ES_OK;
 }
 
 }  // namespace
@@ -763,120 +817,15 @@ mt_emit_kernel(const uint32_t* __restrict__ words, size_t stride_words, const ui
 int es_impl_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,
                        int n_per_stream, uint64_t upper_bound, int coins, int normals_per_eval, double scale, int64_t* idx_out,
                        uint32_t* extra_out, float* noise_out, cudaStream_t stream) {
-    const uint32_t rng = (uint32_t)(upper_bound - 1);
-    uint32_t mask = rng;
-    mask |= mask >> 1; mask |= mask >> 2; mask |= mask >> 4; mask |= mask >> 8; mask |= mask >> 16;
-    if (rng == 0) {
+    const Mt19937Bound bd = mt19937_randint_bound(upper_bound);
+    if (bd.rng == 0) {
         es_set_error("es_draw_noisy: upper_bound == 1 is not supported");
         return ES_ERR_UNSUPPORTED;
     }
-    const int N = normals_per_eval;
-    // ---- how many words can a stream consume?  Per rollout ceil(N / 2) accepted attempts at acceptance pi / 4 (a negative
-    //      binomial count), 4 words each; per pair one index draw (~1.08 words with rejections, bounded generously) and the
-    //      coins.  The jump-ahead pass generates the mean + 12 sigma of the total (+ slack); the walk flags an overflow. ----
-    const double p_acc = 0.78539816339744830962, n_acc = (N + 1) / 2;
-    const double att_mean = n_acc / p_acc, att_sd = sqrt(n_acc * (1.0 - p_acc)) / p_acc;
-    const double evals = 2.0 * n_per_stream;
-    const double words_max = 624.0 + n_per_stream * (8.0 + 4.0 * coins) + 4.0 * (evals * att_mean + 12.0 * sqrt(evals) * att_sd + 64.0) +
-                             2.0 * MG_WIN + 16.0 * MT_NW;
-    const long long blocks_needed = (long long)(words_max / MT_NW) + 1;
-    // jump-ahead when a stream is long enough to be worth splitting (ES_MT_JUMP=0 / 1 overrides; ES_MT_JUMP_LB: log2 of the
-    // segment length in blocks, for tests)
-    const char* ej = getenv("ES_MT_JUMP");
-    bool jump = ej ? atoi(ej) != 0 : blocks_needed >= 2048;
-    int lb_log2 = 3;
-    if (jump) {
-        const char* el = getenv("ES_MT_JUMP_LB");
-        if (el) lb_log2 = atoi(el);
-        else
-            while (lb_log2 < MJ_BITS_RANGE - 1 && (long long)n_streams * ((blocks_needed + (1LL << lb_log2) - 1) >> lb_log2) > 4LL * ctx->sm_count) ++lb_log2;
-        if (lb_log2 < 0) lb_log2 = 0;
-        if (lb_log2 > MJ_BITS_RANGE - 1) lb_log2 = MJ_BITS_RANGE - 1;
-    }
-    long long n_seg = jump ? (blocks_needed + (1LL << lb_log2) - 1) >> lb_log2 : 0;
-    if (jump && (((n_seg << lb_log2) >> MJ_BITS_RANGE) != 0 || (double)(n_seg << lb_log2) * MT_NW > 4.0e9 || n_seg > 65535)) {
-        // the block index of a segment start must fit the available jumps (2^20 blocks = 654 M words per stream) and a
-        // 32-bit word index: longer streams take the sequential kernel unless the jump-ahead path was asked for explicitly
-        if (ej && atoi(ej) != 0) {
-            es_set_error("es_draw_noisy: %lld blocks per stream exceed the jump-ahead range (2^%d blocks)", n_seg << lb_log2, MJ_BITS_RANGE);
-            return ES_ERR_UNSUPPORTED;
-        }
-        jump = false;
-        n_seg = 0;
-    }
-    // (whole chunks of MJ_CW words, + one chunk of padding: the flags kernel reads 4 words past every attempt start)
-    const size_t gen_words = jump ? (size_t)(1 + (n_seg << lb_log2)) * MT_NW : 0;
-    const long long n_chunks = jump ? (long long)((gen_words + MJ_CW - 1) / MJ_CW) : 0;
-    const size_t stride_words = jump ? (size_t)(n_chunks + 1) * MJ_CW : 0;
-    const int a_max = (N + 1) / 2 > 0 ? (N + 1) / 2 : 1;
-    const size_t n_eval = (size_t)n_streams * 2 * n_per_stream;
-    auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    const size_t c0_bytes = pad((size_t)n_streams * sizeof(int32_t)), g0_bytes = pad((size_t)n_streams * sizeof(double));
-    if (jump) {
-        // scratch: the streams' words | accept masks [stream][phase][chunk][32] | chunk counts -> prefixes [stream][phase][chunk]
-        //          | first word of every rollout [stream][2 n] | incoming cache per stream
-        const size_t words_bytes = pad((size_t)n_streams * stride_words * sizeof(uint32_t));
-        const size_t mask_bytes = pad((size_t)n_streams * 4 * n_chunks * 32 * sizeof(uint32_t));
-        const size_t cnt_bytes = pad((size_t)n_streams * 4 * n_chunks * sizeof(uint32_t));
-        const size_t reg_bytes = pad(n_eval * sizeof(uint32_t));
-        const size_t ord_bytes = pad((size_t)n_seg * sizeof(uint16_t));
-        void* scratch = nullptr;
-        int rc = es_ctx_scratch(ctx, words_bytes + mask_bytes + cnt_bytes + reg_bytes + c0_bytes + g0_bytes + ord_bytes, &scratch);
-        if (rc) return rc;
-        char* at = (char*)scratch;
-        uint32_t* words = (uint32_t*)at; at += words_bytes;
-        uint32_t* masks = (uint32_t*)at; at += mask_bytes;
-        uint32_t* counts = (uint32_t*)at; at += cnt_bytes;
-        uint32_t* reg_start = (uint32_t*)at; at += reg_bytes;
-        int32_t* c0 = (int32_t*)at; at += c0_bytes;
-        double* gauss0 = (double*)at; at += g0_bytes;
-        uint16_t* order = (uint16_t*)at;
-        if (!ctx->mj_lists_ready) {
-            mj_lists_kernel<<<MJ_NPOLY, 640, 0, stream>>>();
-            ES_LAUNCHED(ctx);
-            ctx->mj_lists_ready = 1;
-        }
-        mj_order_kernel<<<1, 1024, 0, stream>>>((int)n_seg, lb_log2, order);
-        ES_LAUNCHED(ctx);
-        const size_t smem = (size_t)(MJ_WIN_BLOCKS + 6) * MT_NW * sizeof(uint32_t);
-        ES_CHECK_CUDA(cudaFuncSetAttribute(mt_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mt_fill_kernel<<<(unsigned)(n_streams * n_seg), MF_THREADS, smem, stream>>>(mt_key, n_streams, (int)n_seg, lb_log2, order, words,
-                                                                                    stride_words);
-        ES_LAUNCHED(ctx);
-        mt_flags_kernel<<<dim3((unsigned)((n_chunks + MFL_WARPS - 1) / MFL_WARPS), (unsigned)n_streams), 32 * MFL_WARPS, 0, stream>>>(
-            words, stride_words, (int)n_chunks, masks, counts);
-        ES_LAUNCHED(ctx);
-        mt_scan_kernel<<<n_streams * 4, 1024, 0, stream>>>(counts, (int)n_chunks);
-        ES_LAUNCHED(ctx);
-        mt_walk_kernel<<<n_streams, 32, 0, stream>>>(mt_key, mt_pos, has_gauss, gauss, n_per_stream, rng, mask, coins, N, idx_out, extra_out,
-                                                     reg_start, c0, gauss0, words, stride_words, (int)n_chunks, masks, counts,
-                                                     (uint32_t)(gen_words - 8), ctx->err_dev);
-        ES_LAUNCHED(ctx);
-        mt_emit_kernel<<<(unsigned)n_eval, 1024, 0, stream>>>(words, stride_words, reg_start, c0, gauss0, n_per_stream, N, scale,
-                                                              noise_out, gauss);
-        ES_LAUNCHED(ctx);
-        return ES_OK;
-    }
-    // sequential kernel.  scratch: the accepted attempts' words [stream][evaluation][a_max] (16 bytes per two gaussians), the
-    // incoming cache per stream
-    const size_t acc_bytes = pad(n_eval * a_max * sizeof(uint4));
-    void* scratch = nullptr;
-    int rc = es_ctx_scratch(ctx, acc_bytes + c0_bytes + g0_bytes, &scratch);
+    MgPlan pl;
+    const int rc = mg_plan(ctx, n_streams, n_per_stream, coins, normals_per_eval, pl);
     if (rc) return rc;
-    uint4* acc4 = (uint4*)scratch;
-    int32_t* c0 = (int32_t*)((char*)scratch + acc_bytes);
-    double* gauss0 = (double*)((char*)scratch + acc_bytes + c0_bytes);
-    {
-        const size_t smem = (size_t)(2 * MG_RING + 1) * MG_N * sizeof(uint32_t);
-        ES_CHECK_CUDA(cudaFuncSetAttribute(mt_gauss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mt_gauss_kernel<<<n_streams, MG_THREADS, smem, stream>>>(mt_key, mt_pos, has_gauss, gauss, n_per_stream, rng, mask, coins, N,
-                                                                 idx_out, extra_out, acc4, a_max, c0, gauss0);
-        ES_LAUNCHED(ctx);
-    }
-    const long long total = (long long)n_eval * a_max;
-    int blocks = es_div_up(total, 256);
-    if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
-    mt_gauss_finish_kernel<<<blocks, 256, 0, stream>>>(acc4, a_max, c0, gauss0, n_streams, n_per_stream, N, scale, noise_out, gauss);
-    ES_LAUNCHED(ctx);
-    return ES_OK;
+    const MgDraw d = {mt_key, mt_pos, has_gauss, gauss, n_streams, n_per_stream, bd.rng, bd.mask, coins, normals_per_eval, scale,
+                      idx_out, extra_out, noise_out};
+    return pl.jump ? mg_launch_jump(ctx, d, pl, stream) : mg_launch_sequential(ctx, d, stream);
 }

@@ -22,6 +22,7 @@
 // Four barriers per step.
 #include <math.h>
 #include "common.cuh"
+#include "mt19937.cuh"
 
 namespace {
 
@@ -190,12 +191,12 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
         }
         if (tid < 2) rfit[tid] = 0.0;
         if (tid < 6) rpos[tid] = 0.f;
-        // the save_obs coins of the pair's two evaluations (legacy random_sample: (a >> 5, b >> 6) / 2^53 < chance)
+        // the save_obs coins of the pair's two evaluations (legacy random_sample < chance)
         bool save_p = false, save_m = false;
         if (p.coins) {
             const uint32_t* c = p.coins + (size_t)pair * 4;
-            save_p = ((double)(c[0] >> 5) * 67108864.0 + (double)(c[1] >> 6)) / 9007199254740992.0 < p.chance;
-            save_m = ((double)(c[2] >> 5) * 67108864.0 + (double)(c[3] >> 6)) / 9007199254740992.0 < p.chance;
+            save_p = mt19937_random_sample(c[0], c[1]) < p.chance;
+            save_m = mt19937_random_sample(c[2], c[3]) < p.chance;
         }
         const bool keep_stat = p.ob_sum && (save_p || save_m);
         __syncthreads();
