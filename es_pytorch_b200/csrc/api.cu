@@ -230,13 +230,16 @@ static int es_rollout_check(const char* fn, bool ptrs, const EsRollout& r) {
     return ES_OK;
 }
 
-int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
-                              const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
-                              const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
-                              float* behv_pos, float* behv_neg, const float* act_noise, int mode, void* stream) {
+int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                 const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
+                                 const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
+                                 float* behv_pos, float* behv_neg, const float* act_noise, int n_episodes, int mode, void* stream) {
     ES_ENTER(ctx);
+    ES_REQUIRE(n_episodes >= 1, "es_rollout_openloop: n_episodes must be >= 1, got %d", n_episodes);
+    // without action noise the episodes are identical and their mean is exactly the one episode (E copies of a float32 value
+    // sum exactly in float64, and (E r) / E == r)
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev};
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
     const int rc = es_rollout_check("es_rollout_openloop", obsn != nullptr, r);
     if (rc) return rc;
     if (n_pairs == 0) return ES_OK;
@@ -244,6 +247,14 @@ int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len
     if (mode == ES_ROLLOUT_TC || mode == ES_ROLLOUT_TC3) return es_impl_rollout_tc2(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
     es_set_error("es_rollout_openloop: unknown mode %d", mode);
     return ES_ERR_INVALID;
+}
+
+int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                              const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
+                              const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
+                              float* behv_pos, float* behv_neg, const float* act_noise, int mode, void* stream) {
+    return es_rollout_openloop_episodes(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T,
+                                        pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, 1, mode, stream);
 }
 
 int es_rollout_openloop(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
@@ -262,7 +273,7 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
                           double* ob_count, void* stream) {
     ES_ENTER(ctx);
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev};
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1};
     const int rc = es_rollout_check("es_rollout_closedloop", ob_mean && ob_std && obs0 && env_a && env_b, r);
     if (rc) return rc;
     if (n_layers != 3) {

@@ -101,8 +101,9 @@ struct EsRollout {
     int fit_stride;
     float* behv_pos;            // [n_pairs][3] or NULL
     float* behv_neg;
-    const float* act_noise;     // open loop: scaled action noise [n_pairs][2][T][act] (mt_gauss.cu) or NULL
+    const float* act_noise;     // open loop: scaled action noise [n_pairs][2][n_episodes][T][act] (mt_gauss.cu) or NULL
     int* err;                   // the ctx's error word (es_checked_slice)
+    int n_episodes;             // episodes per evaluation, averaged per step (>= 1; 1 when act_noise is NULL)
 };
 // the closed-loop env, the observation normalisation and the ObStat increments of es_rollout_closedloop
 struct EsClosedEnv {

@@ -111,12 +111,12 @@ rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ 
                    const float* __restrict__ rew_vec, int T, float pos_scale, double* __restrict__ fit_pos,
                    double* __restrict__ fit_neg, int fit_stride, float* __restrict__ behv_pos,
                    float* __restrict__ behv_neg, double* __restrict__ part, unsigned* __restrict__ tickets,
-                   const float* __restrict__ wglobal, const float* __restrict__ act_noise) {
+                   const float* __restrict__ wglobal, const float* __restrict__ act_noise, int n_eps) {
     extern __shared__ __align__(16) float smem[];
     float* Wsm = GW ? const_cast<float*>(wglobal) + (size_t)blockIdx.x * d.w_floats : smem;    // [w_floats]
     float* Xa = GW ? smem : smem + d.w_floats;          // [RF_TM][xpitch]
     float* Xb = Xa + RF_TM * d.xpitch;                  // [RF_TM][xpitch]
-    float* s_rew = Xb + RF_TM * d.xpitch;               // [RF_TM]
+    double* s_rew = (double*)(Xb + RF_TM * d.xpitch);   // [RF_TM]
     __shared__ double s_fit;
     __shared__ float s_pos[3];
 
@@ -162,31 +162,37 @@ rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ 
             __syncthreads();
             float* tmp = xin; xin = xout; xout = tmp;
         }
-        // xin now holds the actions [RF_TM][act_dim]
-        if (act_noise) {
-            // a += rs.randn(act) * ac_std (src/nn/nn.py:47-48): the scaled gaussians of this evaluation, drawn in stream order
-            // by mt_gauss.cu; reward and position see the noisy action (the env receives it, gym_runner.py:53)
-            const float* __restrict__ nz = act_noise + ((size_t)blockIdx.x * T + t0) * act_dim;
-            for (int i = threadIdx.x; i < rows * act_dim; i += RF_THREADS) {
-                const int r = i / act_dim, j = i - r * act_dim;
-                xin[r * d.xpitch + j] = __fadd_rn(xin[r * d.xpitch + j], __ldg(nz + i));
-            }
-            __syncthreads();
-        }
+        // xin now holds the actions [RF_TM][act_dim].  Per step and episode e < n_eps: a += rs.randn(act) * ac_std
+        // (src/nn/nn.py:47-48, the scaled gaussians of episode e drawn in stream order by mt_gauss.cu; the env receives the noisy
+        // action, gym_runner.py:53), r_e = <a, c_t> in float32; the step's reward is (r_0 + .. + r_{n_eps-1}) / n_eps in float64,
+        // episodes in order (obj.py:54-63).  The last episode's noisy action stays in xin for the position integrator.
         if (threadIdx.x < rows) {
             const int r = threadIdx.x;
-            const float* a = xin + r * d.xpitch;
+            float* a = xin + r * d.xpitch;
             const float* c = rew_vec + (size_t)(t0 + r) * act_dim;
-            float acc = 0.f;
-            for (int j = 0; j < act_dim; ++j) acc = __fadd_rn(acc, __fmul_rn(a[j], __ldg(c + j)));
-            s_rew[r] = acc;
+            double s = 0.0;
+            for (int e = 0; e < n_eps; ++e) {
+                const float* __restrict__ nz = act_noise ? act_noise + (((size_t)blockIdx.x * n_eps + e) * T + t0 + r) * act_dim : nullptr;
+                const bool last = e == n_eps - 1;
+                float acc = 0.f;
+                for (int j = 0; j < act_dim; ++j) {
+                    float v = a[j];
+                    if (nz) {
+                        v = __fadd_rn(v, __ldg(nz + j));
+                        if (last) a[j] = v;
+                    }
+                    acc = __fadd_rn(acc, __fmul_rn(v, __ldg(c + j)));
+                }
+                s += (double)acc;
+            }
+            s_rew[r] = s / n_eps;
         }
         __syncthreads();
         if (threadIdx.x == 0) {
             double f = s_fit;
             float p0 = s_pos[0], p1 = s_pos[1], p2 = s_pos[2];
             for (int r = 0; r < rows; ++r) {
-                f += (double)s_rew[r];
+                f += s_rew[r];
                 const float* a = xin + r * d.xpitch;
                 p0 = __fadd_rn(p0, __fmul_rn(pos_scale, a[0 % act_dim]));
                 p1 = __fadd_rn(p1, __fmul_rn(pos_scale, a[1 % act_dim]));
@@ -257,7 +263,7 @@ int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     for (int l = 0; l < n_layers; ++l) { d.sb_off[l] = soff; soff += rf_round4(d.out[l]); }
     d.w_floats = rf_round4(soff);
     d.xpitch = xmax;
-    const size_t act_smem = (2 * (size_t)RF_TM * d.xpitch + RF_TM) * sizeof(float);
+    const size_t act_smem = 2 * (size_t)RF_TM * d.xpitch * sizeof(float) + RF_TM * sizeof(double);
     const size_t smem_w = (size_t)d.w_floats * sizeof(float) + act_smem;
     const bool gw = smem_w > 227 * 1024;              // weights do not fit beside the activation tiles: global scratch
     if (act_smem > 227 * 1024) {
@@ -305,19 +311,20 @@ int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
         double* fn = r.fit_neg + (size_t)p0 * r.fit_stride;
         float* bp = r.behv_pos ? r.behv_pos + (size_t)p0 * 3 : nullptr;
         float* bn = r.behv_neg ? r.behv_neg + (size_t)p0 * 3 : nullptr;
-        const float* an = r.act_noise ? r.act_noise + (size_t)p0 * 2 * T * r.layer_sizes[n_layers] : nullptr;
+        const int n_eps = r.act_noise ? r.n_episodes : 1;
+        const float* an = r.act_noise ? r.act_noise + (size_t)p0 * 2 * n_eps * T * r.layer_sizes[n_layers] : nullptr;
         if (gw) {
             rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, d, wglobal);
             ES_LAUNCHED(ctx);
             ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)act_smem));
             rollout_f32_kernel<true><<<dim3(2 * np, n_splits), RF_THREADS, act_smem, stream>>>(
                 r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
-                wglobal, an);
+                wglobal, an, n_eps);
         } else {
             ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));
             rollout_f32_kernel<false><<<dim3(2 * np, n_splits), RF_THREADS, smem_w, stream>>>(
                 r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
-                nullptr, an);
+                nullptr, an, n_eps);
         }
         ES_LAUNCHED(ctx);
     }

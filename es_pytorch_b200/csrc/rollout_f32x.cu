@@ -46,7 +46,7 @@ struct FxParams {
     const float* xst;        // [n_tiles][nkc][FX_MT][FX_XP] stage images of the normalised observations
     const float* ubase;      // [n_tiles * FX_MT][FX_H] row-major (es_launch_ubase)
     const float* rew;        // [T][act]
-    const float* act_noise;  // [n_pairs][2][T][act] scaled action noise (mt_gauss.cu) or NULL
+    const float* act_noise;  // [n_pairs][2][n_eps][T][act] scaled action noise (mt_gauss.cu) or NULL
     double* fit_pos;
     double* fit_neg;
     float* behv_pos;
@@ -57,6 +57,7 @@ struct FxParams {
     long long table_len;
     int P;
     int* err;
+    int n_eps;               // episodes per evaluation (1 without action noise)
 };
 
 struct FxSmem { uint32_t e1, xs, h, w2, w3, bias, posb, red, bars, total; int e1p, act4; };
@@ -107,6 +108,9 @@ __device__ __forceinline__ void fx_tile_mma(const ulonglong2* __restrict__ A, in
     }
 }
 
+// NOISE: the action-noise variant (noise loads and the episode loop in the layer-3 epilogue), a separate instantiation so that
+// the noise-free kernel keeps its own register allocation
+template <bool NOISE>
 __global__ void __launch_bounds__(FX_THREADS, 1) rollout_f32x_kernel(const __grid_constant__ FxParams p) {
     extern __shared__ __align__(128) uint8_t fx_smem[];
     const FxSmem L = fx_layout(p.obs, p.act);
@@ -284,22 +288,51 @@ __global__ void __launch_bounds__(FX_THREADS, 1) rollout_f32x_kernel(const __gri
                     const bool unit = lane < p.act;
                     const float b3 = bias[sgn * (FX_H + 32) + FX_H + n3];
                     const int tb = m * FX_MT + r0;                                     // time step of row 0 of this warp
-                    const float* __restrict__ nz = p.act_noise ? p.act_noise + (((size_t)pair * 2 + sgn) * p.T + tb) * p.act + lane : nullptr;
-                    float v[8];
+                    if (!NOISE) {          // (the parent kernel's epilogue, kept as it was: the same code for the same SASS)
+                        const float* __restrict__ nz = p.act_noise ? p.act_noise + (((size_t)pair * 2 + sgn) * p.T + tb) * p.act + lane : nullptr;
+                        float v[8];
 #pragma unroll
-                    for (int a = 0; a < 8; ++a) {
-                        float av = tanhf(es_hsum2(acc3[a]) + b3);
-                        const bool live = unit && tb + a < p.T;
-                        if (nz && live) av = __fadd_rn(av, __ldg(nz + a * p.act));     // a += randn * ac_std (nn.py:47-48)
-                        v[a] = live ? av * __ldg(p.rew + (size_t)(tb + a) * p.act + lane) : 0.f;
-                        if (want_pos) {
+                        for (int a = 0; a < 8; ++a) {
+                            float av = tanhf(es_hsum2(acc3[a]) + b3);
+                            const bool live = unit && tb + a < p.T;
+                            if (nz && live) av = __fadd_rn(av, __ldg(nz + a * p.act));     // a += randn * ac_std (nn.py:47-48)
+                            v[a] = live ? av * __ldg(p.rew + (size_t)(tb + a) * p.act + lane) : 0.f;
+                            if (want_pos) {
 #pragma unroll
-                            for (int jj = 0; jj < 3; ++jj)
-                                if (lane == jj % p.act) posb[(r0 + a) * 4 + jj] = av;   // action component jj % act
+                                for (int jj = 0; jj < 3; ++jj)
+                                    if (lane == jj % p.act) posb[(r0 + a) * 4 + jj] = av;   // action component jj % act
+                            }
                         }
+                        const float r = es_warp_sum8(v, lane);             // lanes 4 q .. 4 q + 3: the reward of row q
+                        if ((lane & 3) == 0) { if (sgn) fs1 += (double)r; else fs0 += (double)r; }
+                    } else {
+                        const float* __restrict__ nz = p.act_noise + (((size_t)pair * 2 + sgn) * p.n_eps * p.T + tb) * p.act + lane;
+                        float act[8];
+#pragma unroll
+                        for (int a = 0; a < 8; ++a) act[a] = tanhf(es_hsum2(acc3[a]) + b3);
+                        // episode e sees a + its own noise (a += randn * ac_std, nn.py:47-48); the row's float32 rewards are
+                        // summed over the episodes in float64, in order, and divided by n_eps (obj.py:54-63); the positions
+                        // follow the last episode
+                        double re = 0.0;
+#pragma unroll 1
+                        for (int e = 0; e < p.n_eps; ++e) {
+                            float v[8];
+#pragma unroll
+                            for (int a = 0; a < 8; ++a) {
+                                float av = act[a];
+                                const bool live = unit && tb + a < p.T;
+                                if (live) av = __fadd_rn(av, __ldg(nz + (size_t)e * p.T * p.act + a * p.act));
+                                v[a] = live ? av * __ldg(p.rew + (size_t)(tb + a) * p.act + lane) : 0.f;
+                                if (want_pos && e == p.n_eps - 1) {
+#pragma unroll
+                                    for (int jj = 0; jj < 3; ++jj)
+                                        if (lane == jj % p.act) posb[(r0 + a) * 4 + jj] = av;   // action component jj % act
+                                }
+                            }
+                            re += (double)es_warp_sum8(v, lane);           // lanes 4 q .. 4 q + 3: the reward of row q
+                        }
+                        if ((lane & 3) == 0) { const double r = re / p.n_eps; if (sgn) fs1 += r; else fs0 += r; }
                     }
-                    const float r = es_warp_sum8(v, lane);             // lanes 4 q .. 4 q + 3: the reward of row q
-                    if ((lane & 3) == 0) { if (sgn) fs1 += (double)r; else fs0 += (double)r; }
                 }
                 __syncthreads();                                 // H is free again; the position columns are visible
                 if (want_pos && tid < 3) {
@@ -360,6 +393,7 @@ int es_impl_rollout_f32x(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     p.sigma = r.sigma; p.pos_scale = r.pos_scale;
     p.off = es_mlp_offsets(p.obs, FX_H, FX_H, p.act);
     p.table_len = r.table_len; p.P = r.P; p.err = r.err;
+    p.n_eps = r.act_noise ? r.n_episodes : 1;
 
     const size_t xst_bytes = (size_t)p.n_tiles * p.nkc * FX_STAGE_FLOATS * sizeof(float);
     const size_t ub_bytes = (size_t)p.n_tiles * FX_MT * FX_H * sizeof(float);
@@ -379,8 +413,13 @@ int es_impl_rollout_f32x(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
         if (rc) return rc;
     }
     const int grid = r.n_pairs < ctx->sm_count ? r.n_pairs : ctx->sm_count;
-    ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32x_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-    rollout_f32x_kernel<<<grid, FX_THREADS, L.total, stream>>>(p);
+    if (p.act_noise) {
+        ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32x_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
+        rollout_f32x_kernel<true><<<grid, FX_THREADS, L.total, stream>>>(p);
+    } else {
+        ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32x_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
+        rollout_f32x_kernel<false><<<grid, FX_THREADS, L.total, stream>>>(p);
+    }
     ES_LAUNCHED(ctx);
     return ES_OK;
 }

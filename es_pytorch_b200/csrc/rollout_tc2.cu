@@ -181,7 +181,7 @@ struct T2Params {
     const uint8_t* xnt;           // [n_mtiles][nkc][pieces][16 KB stage image]
     const float* ubase;           // [n_mtiles * 128][64] row-major
     const float* rew_vec;         // [T][act]
-    const float* act_noise;       // [n_pairs][2][T][act] scaled action noise (mt_gauss.cu) or NULL
+    const float* act_noise;       // [n_pairs][2][n_eps][T][act] scaled action noise (mt_gauss.cu) or NULL
     uint8_t* images;              // [gridDim.x][2][image bytes]
     double* fit_pos;
     double* fit_neg;
@@ -195,6 +195,7 @@ struct T2Params {
     long long table_len;
     int P;
     int* err;
+    int n_eps;                    // episodes per evaluation (NOISE instantiations; 1 otherwise)
 };
 
 template <bool SPLIT> struct T2Cfg {
@@ -247,8 +248,8 @@ template <bool SPLIT> __device__ __forceinline__ void act_pack(const float (&z)[
     }
 }
 
-// NOISE: the action-noise variant (loads of the noise array in the layer-3 epilogue); a separate instantiation so that the
-// registers it needs do not cost the noise-free kernel anything
+// NOISE: the action-noise variant (loads of the noise array and the episode loop in the layer-3 epilogue); a separate
+// instantiation so that the registers it needs do not cost the noise-free kernel anything
 template <bool SPLIT, bool NOISE>
 __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid_constant__ T2Params p,
                                                                      const __grid_constant__ T2Maps maps) {
@@ -569,9 +570,15 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     wg_commit();
                 };
                 // ---- epi3: a = tanh(D3 + b3) [+ action noise]; r_t = <a_t, c_t>; positions ----
-                auto epi3 = [&](int sgn, const float (&d3)[16]) {
+                // With action noise, episode ep of n_eps sees a + its own noise; the two rows' float32 rewards are summed over
+                // the episodes in float64, in order, and divided by n_eps (obj.py:54-63); the positions are the last episode's.
+                // The first episode is straight-line code as in the single-episode kernel; the others loop and recompute the
+                // tanh (keeping the 16 actions live across the loop would cost registers).  (epi3_episode serves the NOISE
+                // instantiations only.)
+                auto epi3_episode = [&](int sgn, const float (&d3)[16], const float* __restrict__ nz, float& ra, float& rb,
+                                        float& q0, float& q1, float& q2) {
                     const float* b3 = bias + 2 * T2_H + sgn * T2_ACT_PAD;
-                    float ra = 0.f, rb = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f;
+                    ra = 0.f; rb = 0.f; q0 = 0.f; q1 = 0.f; q2 = 0.f;
 #pragma unroll
                     for (int c = 0; c < 4; ++c) {
 #pragma unroll
@@ -581,8 +588,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                             const float z = __fadd_rn(d3[4 * c + e], b3[col]);
                             float a = SPLIT ? tanh_acc(z) : tanh_fast(z);
                             if (col < p.act && t < p.T) {
-                                if (NOISE && p.act_noise)       // a += rs.randn(act) * ac_std (src/nn/nn.py:47-48), drawn by mt_gauss.cu
-                                    a += __ldg(p.act_noise + (((size_t)pair * 2 + sgn) * p.T + t) * p.act + col);
+                                if (NOISE && nz)                // a += rs.randn(act) * ac_std (src/nn/nn.py:47-48), drawn by mt_gauss.cu
+                                    a += __ldg(nz + (size_t)t * p.act + col);
                                 const float r = a * __ldg(p.rew_vec + (size_t)t * p.act + col);
                                 if (e & 2) rb += r; else ra += r;
                                 // position integrator: action components 0, 1, 2
@@ -592,7 +599,47 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     }
                     ra += __shfl_xor_sync(0xffffffffu, ra, 1); ra += __shfl_xor_sync(0xffffffffu, ra, 2);
                     rb += __shfl_xor_sync(0xffffffffu, rb, 1); rb += __shfl_xor_sync(0xffffffffu, rb, 2);
-                    const double r2 = (q == 0) ? (double)ra + (double)rb : 0.0;   // rows beyond T contribute 0
+                };
+                auto epi3 = [&](int sgn, const float (&d3)[16]) {
+                    if (!NOISE) {          // the noise-free kernels keep the single-episode epilogue as it was (same SASS)
+                        const float* b3 = bias + 2 * T2_H + sgn * T2_ACT_PAD;
+                        float ra = 0.f, rb = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f;
+#pragma unroll
+                        for (int c = 0; c < 4; ++c) {
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                const int col = 8 * c + 2 * q + (e & 1);
+                                const int t = (e & 2) ? tb : ta;
+                                const float z = __fadd_rn(d3[4 * c + e], b3[col]);
+                                const float a = SPLIT ? tanh_acc(z) : tanh_fast(z);
+                                if (col < p.act && t < p.T) {
+                                    const float r = a * __ldg(p.rew_vec + (size_t)t * p.act + col);
+                                    if (e & 2) rb += r; else ra += r;
+                                    q0 += (col == 0) ? a : 0.f; q1 += (col == 1) ? a : 0.f; q2 += (col == 2) ? a : 0.f;
+                                }
+                            }
+                        }
+                        ra += __shfl_xor_sync(0xffffffffu, ra, 1); ra += __shfl_xor_sync(0xffffffffu, ra, 2);
+                        rb += __shfl_xor_sync(0xffffffffu, rb, 1); rb += __shfl_xor_sync(0xffffffffu, rb, 2);
+                        const double r2 = (q == 0) ? (double)ra + (double)rb : 0.0;   // rows beyond T contribute 0
+                        if (sgn) { fit_n += r2; pn0 += q0; pn1 += q1; pn2 += q2; }
+                        else     { fit_p += r2; pp0 += q0; pp1 += q1; pp2 += q2; }
+                        return;
+                    }
+                    const int n_ep = p.n_eps;
+                    const float* __restrict__ nz = p.act_noise ? p.act_noise + ((size_t)pair * 2 + sgn) * n_ep * p.T * p.act : nullptr;
+                    float ra, rb, q0, q1, q2;
+                    epi3_episode(sgn, d3, nz, ra, rb, q0, q1, q2);
+                    double r2 = (q == 0) ? (double)ra + (double)rb : 0.0;   // rows beyond T contribute 0
+                    if (n_ep > 1) {
+                        double sa = (double)ra, sb = (double)rb;
+#pragma unroll 1
+                        for (int ep = 1; ep < n_ep; ++ep) {
+                            epi3_episode(sgn, d3, nz + (size_t)ep * p.T * p.act, ra, rb, q0, q1, q2);
+                            sa += (double)ra; sb += (double)rb;
+                        }
+                        if (q == 0) r2 = sa / n_ep + sb / n_ep;
+                    }
                     if (sgn) { fit_n += r2; pn0 += q0; pn1 += q1; pn2 += q2; }
                     else     { fit_p += r2; pp0 += q0; pp1 += q1; pp2 += q2; }
                 };
@@ -834,6 +881,7 @@ int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t
     p.n_mtiles = es_div_up(r.T, T2_MT);
     p.off = es_mlp_offsets(p.obs, T2_H, T2_H, p.act);
     p.table_len = r.table_len; p.P = r.P; p.err = r.err;
+    p.n_eps = r.act_noise ? r.n_episodes : 1;
 
     // float16 shadows of the table (hi always, lo when a split rollout asks for it): 8 shifted copies each, built once per
     // (table pointer, length) and addressed through two TMA tensor maps.  Needs 16-byte aligned rows in every slice (obs % 8

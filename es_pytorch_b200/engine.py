@@ -247,8 +247,11 @@ class Engine:
     # ------------------------------------------------------------------ a3+a4+a5
     def rollout(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], obsn, rew_vec, pos_scale: float,
                 fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None, behv_neg=None, mode: int = ES_ROLLOUT_F32,
-                act_noise=None):
-        """``act_noise``: float32 [n_pairs, 2, T, act] scaled action noise (``draw_noisy``), added to every action."""
+                act_noise=None, episodes: int = 1):
+        """``act_noise``: float32 [n_pairs, 2, episodes, T, act] scaled action noise (``draw_noisy``), added to every action.
+        ``episodes`` > 1 (obj.py:54-63's eps_per_policy): every evaluation is the per-step mean of that many episodes, each
+        with its own noise rows; behaviour is the last episode's.  Without ``act_noise`` the episodes are identical and the
+        result is the single episode's."""
         d = self.device
         _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
         _req(obsn, torch.float32, 'obsn', d); _req(rew_vec, torch.float32, 'rew_vec', d)
@@ -260,9 +263,12 @@ class Engine:
         if behv_pos is not None:
             _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
             assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
+        episodes = int(episodes)
+        if episodes < 1:
+            raise ValueError(f'episodes must be >= 1, got {episodes}')
         if act_noise is not None:
             _req(act_noise, torch.float32, 'act_noise', d)
-            assert act_noise.numel() == n * 2 * T * layer_sizes[-1]
+            assert act_noise.numel() == n * 2 * episodes * T * layer_sizes[-1]
         ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
         if mode in (ES_ROLLOUT_TC, ES_ROLLOUT_TC3):
             # the library keeps a bf16 shadow of the table keyed by (pointer, length); a different tensor object (the
@@ -271,11 +277,11 @@ class Engine:
             if ref is None or ref() is not table or ver != table._version:
                 check(self.lib.es_noise_table_changed(self._ctx), 'es_noise_table_changed')
                 self._tc_table = (weakref.ref(table), table._version)
-        check(self.lib.es_rollout_openloop_noisy(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta),
-                                                 theta.numel(), float(sigma), ls, len(layer_sizes) - 1, _ptr(obsn),
-                                                 _ptr(rew_vec), T, float(pos_scale), _ptr(fit_pos), _ptr(fit_neg),
-                                                 int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(act_noise), int(mode),
-                                                 self.stream), 'es_rollout_openloop')
+        check(self.lib.es_rollout_openloop_episodes(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta),
+                                                    theta.numel(), float(sigma), ls, len(layer_sizes) - 1, _ptr(obsn),
+                                                    _ptr(rew_vec), T, float(pos_scale), _ptr(fit_pos), _ptr(fit_neg),
+                                                    int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(act_noise),
+                                                    episodes, int(mode), self.stream), 'es_rollout_openloop')
 
     def rollout_closed(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
                        obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,

@@ -71,7 +71,7 @@ class DeviceGeneration:
                  optim: Optimizer, ob_clip: float = 5.0, pos_scale: float = 0.05, coins_per_eval: int = 0,
                  save_obs_chance: float = 0.0, archive: Optional[torch.Tensor] = None, nov_k: int = 10,
                  moo_w: float = 1.0, rollout_mode: int = ES_ROLLOUT_F32, comm: Optional[dist.Comm] = None,
-                 engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None):
+                 engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1):
         self.eng = engine or get_engine()
         # closed-loop variant of the synthetic env (gym.synthetic_env.ClosedLoopEnv): (obs_0 [obs], A^T [band, obs], B^T [act, obs]);
         # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop
@@ -97,6 +97,11 @@ class DeviceGeneration:
         # FeedForward._action_std (nn.py:47-48): != 0 -> every step adds rs.randn(act) * ac_std, drawn from the rank streams
         self.ac_std = float(ac_std or 0.0)
         self.act_noise = None
+        # episodes per evaluation (obj.py:54-63, eps_per_policy): with action noise every evaluation draws episodes x T x act
+        # gaussians after its coin and its fitness is the per-step mean over the episodes; without noise the episodes are
+        # identical and the result is the single episode's
+        self.episodes = int(episodes)
+        assert self.episodes >= 1
         assert self.coins_per_eval in (0, 1), 'fit_fns draw at most one save_obs coin per evaluation'
 
         # per-rank MT19937 streams, resident on the device between generations
@@ -188,10 +193,12 @@ class DeviceGeneration:
         self.version += 1
         with self._timed('draw_indices'):
             if self.ac_std != 0.0:
-                # indices, coins and the action noise of every rollout, in the reference's stream order (mt_gauss.cu)
-                nrm = self.T * self.act_dim
+                # indices, coins and the action noise of every rollout, in the reference's stream order (mt_gauss.cu); the
+                # episodes of one evaluation are back to back in the stream
+                nrm = self.episodes * self.T * self.act_dim
                 if self.act_noise is None or self.act_noise.shape != (self.k_local, 2, nrm):
-                    self.act_noise = e.empty((self.k_local, 2, nrm), torch.float32)
+                    self.act_noise = None
+                    self.act_noise = self._alloc_act_noise(nrm)
                 e.draw_noisy(self.mt_key, self.mt_pos, self.mt_has, self.mt_gauss, n_per_stream, self.table.numel() - self.P,
                              self.coins_per_eval, nrm, self.ac_std, self.idx, self.extras, self.act_noise)
             else:
@@ -237,7 +244,8 @@ class DeviceGeneration:
             e.rollout(self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.obsn, self.rew_vec,
                       self.pos_scale, fp, fn, self.n_obj, None if self.behv is None else self.behv[0],
                       None if self.behv is None else self.behv[1], self.rollout_mode,
-                      act_noise=self.act_noise if self.ac_std != 0.0 else None)
+                      act_noise=self.act_noise if self.ac_std != 0.0 else None,
+                      episodes=self.episodes if self.ac_std != 0.0 else 1)
         if self.n_obj == 2:
             # second objective column = novelty of the final (x, y) (training_result.py:95-97)
             e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
@@ -252,6 +260,19 @@ class DeviceGeneration:
             s, q = self._colsum
             e.obstat_accumulate_coins(self.gen_sum, self.gen_sumsq, self.gen_count, s, q, self.T,
                                       self.extras.view(-1, 2), self.save_obs_chance)
+
+    def _alloc_act_noise(self, nrm: int) -> torch.Tensor:
+        """The [k_local, 2, episodes * T * act] float32 buffer of the generation's action noise."""
+        if nrm > 2 ** 31 - 1:
+            raise ValueError(f'{self.episodes} episodes x {self.T} steps x {self.act_dim} actions = {nrm} gaussians per evaluation: '
+                             f'more than the 2^31 - 1 the draw kernel indexes')
+        nbytes = self.k_local * 2 * nrm * 4
+        try:
+            return self.eng.empty((self.k_local, 2, nrm), torch.float32)
+        except torch.cuda.OutOfMemoryError as exc:
+            raise MemoryError(f'the action-noise buffer of {self.k_local} pairs x 2 x {self.episodes} episodes x {self.T} steps x '
+                              f'{self.act_dim} actions needs {nbytes / 2 ** 30:.2f} GiB of device memory, which could not be '
+                              f'allocated: use fewer pairs per process or fewer episodes') from exc
 
     def update(self, fpos: torch.Tensor, fneg: torch.Tensor, all_weights: bool = False):
         """Ranker.rank + es.approx_grad on the device (rankers.py:46-50, es.py:98-101).  ``all_weights``: finalise the weights

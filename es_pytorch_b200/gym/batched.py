@@ -5,8 +5,14 @@ The reference's ``fit_fn`` is an opaque per-policy python callback (src/core/es.
 which forces one rollout per call.  A ``BatchedRollout`` is still callable like that (it is
 what ``es.step`` uses for the noiseless evaluation, es.py:48) but it also *describes* the
 evaluation -- env, episode length, how many ``rs.random()`` coins the script's fit_fn draws
-per evaluation, which TrainingResult adaptor it builds -- so the generation can run on the
-device with the same RNG consumption and the same results layout.
+per evaluation, how many episodes it averages, which TrainingResult adaptor it builds -- so
+the generation can run on the device with the same RNG consumption and the same results layout.
+
+``episodes`` is obj.py's ``eps_per_policy`` (obj.py:54-63): the fit_fn draws its coin, runs
+``max(1, episodes)`` episodes and returns the per-step mean of their rewards (float64, episodes
+in order), with the last episode's behaviour.  With action noise every episode draws its own
+T x act gaussians from the stream; without it the episodes are identical and the mean is
+exactly the single episode (E copies of a float32 sum exactly in float64, and (E r) / E == r).
 """
 from __future__ import annotations
 
@@ -25,7 +31,7 @@ class BatchedRollout:
     def __init__(self, env, max_steps: int, coins_per_eval: int = 1, save_obs_chance: float = 0.0,
                  archive: Optional[np.ndarray] = None, nov_k: int = 10,
                  rank_streams: Optional[Sequence[np.random.RandomState]] = None,
-                 rollout_mode: int = _lib.ES_ROLLOUT_F32):
+                 rollout_mode: int = _lib.ES_ROLLOUT_F32, episodes: int = 1):
         if not (getattr(env, 'is_synthetic_openloop', False) or getattr(env, 'is_synthetic_closedloop', False)):
             raise TypeError('BatchedRollout needs a synthetic env (es_pytorch_b200.gym.synthetic_env: open- or closed-loop)')
         self.env = env
@@ -36,6 +42,13 @@ class BatchedRollout:
         self.nov_k = int(nov_k)
         self.rank_streams = list(rank_streams) if rank_streams is not None else None
         self.rollout_mode = rollout_mode
+        if isinstance(episodes, bool) or not isinstance(episodes, (int, np.integer)):
+            raise TypeError(f'episodes must be an integer, got {episodes!r}')
+        if episodes < 0:
+            raise ValueError(f'episodes must be >= 0 (0 means 1, as max(1, eps_per_policy) in obj.py), got {episodes}')
+        self.episodes = max(1, int(episodes))
+        if self.episodes > 1 and self.archive is not None:
+            raise ValueError('episodes > 1 with a novelty archive: no reference script averages episodes for novelty search')
         self._gen = None            # cached DeviceGeneration (see core.es)
         self._streams_in_use = None  # the RandomState streams of the last batched evaluation (set by core.es)
         self.stream_env_from_host = False   # True: re-upload the env's obs/reward streams every generation
@@ -72,8 +85,27 @@ class BatchedRollout:
             from .gym_runner import _device_episode_closed
             total, pos, _ = _device_episode_closed(model, self.env, self.max_steps)
             return self.result_from_device(total, pos)
-        rews, behv, obs, steps = run_model(model, self.env, self.max_steps, noise_rs)
+        episodes = self.episodes if (noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0) else 1
+        if episodes > 1:
+            rews, behv, steps = self._run_episodes(model, noise_rs, episodes)
+        else:
+            rews, behv, obs, steps = run_model(model, self.env, self.max_steps, noise_rs)
         no_obs = np.array([np.zeros(self.env.observation_space.shape)])
         if self.archive is None:
             return RewardResult(rews, behv, no_obs, steps)
         return NSRResult(rews, behv[-3:], no_obs, steps, self.archive, self.nov_k)
+
+    def _run_episodes(self, model, rs, episodes: int):
+        """obj.py:57-60 with action noise: ``episodes`` runs of run_model drawing from ``rs``, rewards summed per step in
+        float64 in episode order and divided by the count.  A tanh MLP on the open-loop env runs all episodes as one launch
+        (one forward, the episodes' noise rows back to back) and reports the total of the per-step means."""
+        from .gym_runner import _device_episode
+        if getattr(self.env, 'is_synthetic_openloop', False) and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp():
+            total, pos, T = _device_episode(model, self.env, self.max_steps, rs, episodes)
+            return [total], [float(pos[0]), float(pos[1]), float(pos[2])] * int(self.max_steps), T - 1
+        rews = np.zeros(self.max_steps)
+        for _ in range(episodes):
+            rew, behv, _, steps = run_model(model, self.env, self.max_steps, rs)
+            rews[:len(rew)] += np.array(rew)
+        rews /= episodes
+        return rews.tolist(), behv, steps

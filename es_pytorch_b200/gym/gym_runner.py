@@ -35,7 +35,9 @@ def hbaselines_pos(env):
     return tuple(env.wrapped_env.get_body_com('torso')[:3])
 
 
-def _device_episode(model, env, max_steps: int, rs=None):
+def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
+    """One evaluation as one launch.  ``episodes`` > 1 with action noise: the per-step mean over that many episodes
+    (obj.py:54-63), their noise drawn back to back from ``rs``; returns the last episode's final position."""
     from ..engine import get_engine
     from ..core.policy import Policy
     eng = get_engine()
@@ -55,12 +57,14 @@ def _device_episode(model, env, max_steps: int, rs=None):
     ac_std = float(getattr(model, '_action_std', 0) or 0)
     if rs is not None and ac_std != 0:
         # nn.py:47-48: T calls of rs.randn(act) * ac_std; one call of rs.randn(T * act) consumes the stream identically
-        # (legacy gaussians are produced one by one, cached second value included).  [pair 0][+ | -][T][act]: both
+        # (legacy gaussians are produced one by one, cached second value included).  [pair 0][+ | -][episodes][T][act]: both
         # evaluations of the sigma = 0 "pair" see the same noise, only the first is used.
-        nz = (rs.randn(T * sizes[-1]) * ac_std).astype(np.float32)
+        nz = (rs.randn(episodes * T * sizes[-1]) * ac_std).astype(np.float32)
         noise = eng.to_device(np.stack([nz, nz]).reshape(1, 2, -1))
+    else:
+        episodes = 1
     eng.rollout(table, idx, theta, 0.0, sizes, obsn, rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1,
-                behv[0:1].view(-1), behv[1:2].view(-1), act_noise=noise)
+                behv[0:1].view(-1), behv[1:2].view(-1), act_noise=noise, episodes=episodes)
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 

@@ -120,6 +120,21 @@ int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len
                               double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
                               const float* act_noise, int mode, void* stream);
 
+/* The same with E = n_episodes episodes per evaluation, the reference's eps_per_policy (obj.py:54-63 runs run_model E times
+ * and averages the reward lists).  act_noise dev float [n_pairs][2 (+,-)][E][T][act_dim]: episode e of an evaluation adds
+ * its own noise row to the same forward pass (the open-loop observations do not depend on the actions).  Per step t the
+ * float32 rewards r_{e,t} are summed over the episodes in float64 in episode order and divided by E (float64); fitness is
+ * the float64 sum of these means in step order.  behv_pos/behv_neg hold the LAST episode's final position.  The array is
+ * what es_draw_noisy wrote with normals_per_eval = E * T * act_dim (the E episodes back to back in the stream).
+ * act_noise == NULL: the episodes are identical and their mean is exactly the single episode (E copies of a float32 value
+ * sum exactly in float64 for E < 2^29, and (E r) / E == r), so any n_episodes >= 1 gives es_rollout_openloop's result.
+ * n_episodes == 1 is es_rollout_openloop_noisy, bit for bit, in every mode.                                          */
+int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                 const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                 const float* obsn, const float* rew_vec, int T, float pos_scale,
+                                 double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                                 const float* act_noise, int n_episodes, int mode, void* stream);
+
 /* ---- a3 + a4 + a5 on the CLOSED-LOOP synthetic env (SURVEY.md section 8d's optional variant; never part of the headline) --
  * obs_{t+1} = tanh(A obs_t + B a_t): the observation depends on the policy's own actions, so the episode runs step by step
  * with one pair's perturbed weights resident on chip (rollout_closed.cu).  Replaces the same reference loop as
@@ -150,7 +165,11 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
  * coin words, final key / position / has_gauss bit-exact; the cached gaussian to <= 1 ulp of float64, log() being CUDA's).
  *   has_gauss dev int32 [n_streams], gauss dev double [n_streams]   in/out  (RandomState.get_state()[3], [4])
  *   coin_out  dev uint32 [n_streams*n_per_stream][4*coins_per_eval]  (+ coins then - coins) or NULL when coins_per_eval == 0
- *   noise_out dev float [n_streams*n_per_stream][2][normals_per_eval] = float32(gaussian * scale), scale = ac_std          */
+ *   noise_out dev float [n_streams*n_per_stream][2][normals_per_eval] = float32(gaussian * scale), scale = ac_std
+ * E episodes per evaluation (es_rollout_openloop_episodes): normals_per_eval = E * T * act_dim.  Long streams are drawn by
+ * MT19937 jump-ahead over the whole GPU; a stream needing more than 2^20 blocks (~654 M words) falls back to the sequential
+ * kernel (correct, slower); its scratch (16 bytes per two gaussians) or the jump-ahead word buffer failing to allocate
+ * returns ES_ERR_NOMEM with the size in es_last_error().                                                              */
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,
                   int n_per_stream, uint64_t upper_bound, int coins_per_eval, int normals_per_eval, double scale,
                   int64_t* idx_out, uint32_t* coin_out, float* noise_out, void* stream);
