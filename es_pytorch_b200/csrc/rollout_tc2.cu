@@ -864,11 +864,24 @@ void es_tc2_free_shadows(es_ctx* ctx) {
     ctx->sh16_src = nullptr;
 }
 
+// the largest obs_dim whose layout fits in shared memory: 511 (TC, 8 K chunks) / 383 (TC3, 6 K chunks)
+template <bool SPLIT> static int t2_max_obs() {
+    int nkc = 1;
+    while ((size_t)t2_layout<SPLIT>(nkc + 1).total + 1024 <= 227 * 1024) ++nkc;
+    return nkc * T2_KC - 1;                              // nkc = ceil((obs + 1) / 64)
+}
+
 int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t stream) {
     const int* ls = r.layer_sizes;
-    if (r.n_layers != 3 || ls[1] != T2_H || ls[2] != T2_H || ls[3] > T2_ACT_PAD || ls[0] > 1023) {
-        es_set_error("es_rollout_openloop(TC): the tensor-core path covers obs(<=1023)-64-64-act(<=32) tanh MLPs; "
-                     "use ES_ROLLOUT_F32 for other shapes");
+    const int max_obs = split ? t2_max_obs<true>() : t2_max_obs<false>();
+    if (r.n_layers != 3 || ls[1] != T2_H || ls[2] != T2_H || ls[3] > T2_ACT_PAD) {
+        es_set_error("es_rollout_openloop(TC%s): the tensor-core path covers obs(<=%d)-64-64-act(<=32) tanh MLPs; "
+                     "use ES_ROLLOUT_F32 for other shapes", split ? "3" : "", max_obs);
+        return ES_ERR_UNSUPPORTED;
+    }
+    if (ls[0] > max_obs) {                               // refused before any float16 shadow of the table is built
+        es_set_error("es_rollout_openloop(TC%s): obs_dim %d needs more than 227 KB of shared memory (this mode covers "
+                     "obs_dim <= %d)", split ? "3" : "", ls[0], max_obs);
         return ES_ERR_UNSUPPORTED;
     }
     T2Params p;

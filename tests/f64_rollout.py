@@ -1,0 +1,88 @@
+"""Float64 reference of the open-loop rollout: what every device rollout mode approximates.
+
+TEST INFRASTRUCTURE ONLY.  It takes the float32 data the kernels get and evaluates them in float64 without intermediate
+rounding, so a kernel can be judged on its own rather than against another float32 implementation:
+
+* the weights are ``theta +- f64(sigma) * eps`` exactly (``sigma`` is passed to the kernels as a float32), any number of
+  layers, state-dict flat layout (``weight[out, in]`` row-major, then ``bias[out]``, layer after layer);
+* every layer is ``tanh(x W^T + b)`` over the whole episode as one float64 matrix product;
+* episode ``e`` acts ``a_t + nz_e,t`` (``act_noise`` [n_pairs, 2, E, T, act], the scaled float32 gaussians) and earns
+  ``<a, c_t>``; the step's reward is the mean over the episodes and the fitness is its sum over t;
+* the reward mass ``sum_t mean_e sum_j |a_tj c_tj|`` is the scale of the fitness error of any implementation whose actions
+  carry a relative error: a float32 dot product is within ``act * 2^-24`` of it per step and an action error ``d`` moves it
+  by at most ``d`` times it.  It bounds ``sum_t |r_t|`` from above and equals it unless the products of one step cancel
+  (a single step can earn ~0 from large products);
+* the behaviour is the last episode's ``pos_scale * sum_t a_t[i % act]`` for i = 0, 1, 2.
+
+The observations ``obsn`` are taken as given: normalisation happens before the rollout and has its own bit-exact tests.
+"""
+from __future__ import annotations
+
+from typing import Optional, Sequence
+
+import numpy as np
+
+
+def layer_slices(layer_sizes: Sequence[int]):
+    """[(w_off, b_off, n_in, n_out)] of every layer in the flat parameter vector."""
+    out, off = [], 0
+    for fi, fo in zip(layer_sizes[:-1], layer_sizes[1:]):
+        out.append((off, off + fi * fo, fi, fo))
+        off += fi * fo + fo
+    return out
+
+
+def n_params(layer_sizes: Sequence[int]) -> int:
+    return sum(fi * fo + fo for fi, fo in zip(layer_sizes[:-1], layer_sizes[1:]))
+
+
+def perturbed(table: np.ndarray, i: int, theta: np.ndarray, sigma: float, sign: float) -> np.ndarray:
+    """theta + sign * f64(f32(sigma)) * table[i : i + P], exact in float64."""
+    P = len(theta)
+    s = float(np.float32(sigma))
+    return theta.astype(np.float64) + sign * s * table[int(i):int(i) + P].astype(np.float64)
+
+
+def episode(w: np.ndarray, layer_sizes: Sequence[int], obsn: np.ndarray, rew_vec: np.ndarray, pos_scale: float,
+            noise: Optional[np.ndarray] = None):
+    """One evaluation of the flat float64 weights ``w``.  ``noise``: [E, T, act] or None (one noiseless episode).
+    Returns (per-step reward [T] (mean over the episodes), its mass sum_j |a_tj c_tj| [T] (mean over the episodes),
+    behaviour [3], position magnitude [3]), all float64.  The
+    magnitude is sum_t |partial sum_t| + sum_t |term_t| of each position component: a float32 sum of those terms in step
+    order is within 2^-24 times it of the exact sum (to first order), which is what the position checks build on."""
+    a = obsn.astype(np.float64)
+    for wo, bo, fi, fo in layer_slices(layer_sizes):
+        a = np.tanh(a @ w[wo:wo + fi * fo].reshape(fo, fi).T + w[bo:bo + fo])
+    c = rew_vec.astype(np.float64)
+    act = a.shape[1]
+    if noise is None:
+        noise = np.zeros((1,) + a.shape, dtype=np.float32)
+    rew, rabs = np.zeros(a.shape[0]), np.zeros(a.shape[0])
+    for nz in noise:
+        an = a + nz.astype(np.float64)
+        rew += (an * c).sum(axis=1)
+        rabs += np.abs(an * c).sum(axis=1)
+    rew /= len(noise)
+    rabs /= len(noise)
+    terms = float(pos_scale) * an[:, [j % act for j in range(3)]]
+    behv = terms.sum(axis=0)
+    mag = np.abs(np.cumsum(terms, axis=0)).sum(axis=0) + np.abs(terms).sum(axis=0)
+    return rew, rabs, behv, mag
+
+
+def rollout_f64(table, idx, theta, sigma, layer_sizes, obsn, rew_vec, pos_scale, act_noise=None, episodes: int = 1,
+                pairs: Optional[Sequence[int]] = None):
+    """The truth of ``Engine.rollout`` for the pairs ``pairs`` (default: all).  Returns float64 arrays
+    (fitness [2, n], behaviour [2, n, 3], reward mass [2, n], position magnitude [2, n, 3]) with row 0 the +eps
+    and row 1 the -eps evaluation."""
+    idx = np.asarray(idx)
+    pairs = range(len(idx)) if pairs is None else pairs
+    T, act = rew_vec.shape
+    fit, mass = np.zeros((2, len(pairs))), np.zeros((2, len(pairs)))
+    behv, mag = np.zeros((2, len(pairs), 3)), np.zeros((2, len(pairs), 3))
+    for n, k in enumerate(pairs):
+        for s, sign in enumerate((1.0, -1.0)):
+            nz = None if act_noise is None else np.asarray(act_noise[k, s]).reshape(episodes, T, act)
+            r, ra, b, m = episode(perturbed(table, idx[k], theta, sigma, sign), layer_sizes, obsn, rew_vec, pos_scale, nz)
+            fit[s, n], behv[s, n], mass[s, n], mag[s, n] = r.sum(), b, ra.sum(), m
+    return fit, behv, mass, mag
