@@ -117,6 +117,9 @@ static int es_async_error(es_ctx* ctx, const char* where) {
             es_set_error("%s: es_draw_noisy consumed more MT19937 words than its jump-ahead pass had generated (a > 12 sigma "
                          "event of the polar method's acceptance count, or a bug): the draws of that call are invalid; set "
                          "ES_MT_JUMP=0 to use the sequential kernel", where);
+        else if (code == ES_ASYNC_RANDN_OVERFLOW)
+            es_set_error("%s: es_randn needed more MT19937 words than its windows had generated (a > 12 sigma event of the "
+                         "polar method's acceptance count, or a bug): the values of that call are invalid", where);
         else
             es_set_error("%s: a previous kernel reported error %d", where, code);
         return ES_ERR_INVALID;
@@ -301,6 +304,22 @@ int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_g
     if (n_streams == 0 || n_per_stream == 0) return ES_OK;
     return es_impl_draw_noisy(ctx, mt_key, mt_pos, has_gauss, gauss, n_streams, n_per_stream, upper_bound, coins_per_eval,
                               normals_per_eval, scale, idx_out, coin_out, noise_out, (cudaStream_t)stream);
+}
+
+int es_randn(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int64_t n, float* out,
+             void* stream) {
+    ES_ENTER(ctx);
+    ES_REQUIRE(n >= 0, "es_randn: negative count");
+    ES_REQUIRE(mt_key && mt_pos && has_gauss && gauss && (out || n == 0), "es_randn: NULL pointer");
+    if (n == 0) return ES_OK;
+    return es_impl_randn(ctx, mt_key, mt_pos, has_gauss, gauss, n, out, (cudaStream_t)stream);
+}
+
+int es_randn_plan(es_ctx* ctx, int64_t n, size_t* scratch_bytes, int* n_windows) {
+    ES_REQUIRE(ctx && scratch_bytes && n_windows, "es_randn_plan: NULL pointer");
+    ES_REQUIRE(n >= 0, "es_randn_plan: negative count");
+    if (n == 0) { *scratch_bytes = 0; *n_windows = 0; return ES_OK; }
+    return es_impl_randn_plan(ctx, n, scratch_bytes, n_windows);
 }
 
 int es_novelty(es_ctx* ctx, const float* behv, int n, const double* archive, int A, int k, double* out, int out_stride,

@@ -39,6 +39,7 @@ struct es_ctx {
 
 #define ES_ASYNC_BAD_INDEX 1
 #define ES_ASYNC_RNG_OVERFLOW 2      // es_draw_noisy (jump-ahead path): the stream consumed more words than were generated ahead
+#define ES_ASYNC_RANDN_OVERFLOW 3    // es_randn: the n values needed more words than its windows generated
 
 void es_set_error(const char* fmt, ...);
 
@@ -133,6 +134,8 @@ int es_impl_obstat_accumulate_coins(es_ctx*, double*, double*, double*, const fl
                                     const uint32_t*, int, double, cudaStream_t);
 int es_impl_draw_noisy(es_ctx*, uint32_t*, int32_t*, int32_t*, double*, int, int, uint64_t, int, int, double, int64_t*, uint32_t*,
                        float*, cudaStream_t);
+int es_impl_randn(es_ctx*, uint32_t*, int32_t*, int32_t*, double*, int64_t, float*, cudaStream_t);
+int es_impl_randn_plan(const es_ctx*, int64_t, size_t*, int*);
 int es_impl_rollout_f32(es_ctx*, const EsRollout&, cudaStream_t);
 int es_impl_rollout_f32x(es_ctx*, const EsRollout&, cudaStream_t);
 int es_impl_rollout_tc2(es_ctx*, const EsRollout&, int split, cudaStream_t);

@@ -35,6 +35,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <type_traits>
+#include <vector>
 #include "common.cuh"
 #include "mt19937.cuh"
 
@@ -685,6 +686,19 @@ struct MgPlan {
     size_t gen_words, stride_words;
 };
 
+// log2 of the jump-ahead segment length in blocks: the shortest segments that leave at most ~4 segments per SM over all
+// streams (ES_MT_JUMP_LB overrides it, for tests)
+int mj_segment_lb(long long n_streams, long long blocks, int sm_count) {
+    int lb = 3;
+    const char* el = getenv("ES_MT_JUMP_LB");
+    if (el) lb = atoi(el);
+    else
+        while (lb < MJ_BITS_RANGE - 1 && n_streams * ((blocks + (1LL << lb) - 1) >> lb) > 4LL * sm_count) ++lb;
+    if (lb < 0) lb = 0;
+    if (lb > MJ_BITS_RANGE - 1) lb = MJ_BITS_RANGE - 1;
+    return lb;
+}
+
 // How many words can a stream consume?  Per rollout ceil(N / 2) accepted attempts at acceptance pi / 4 (a negative binomial
 // count), 4 words each; per pair one index draw (~1.08 words with rejections, bounded generously) and the coins.  The
 // jump-ahead pass generates the mean + 12 sigma of the total (+ slack); the walk flags an overflow.
@@ -701,13 +715,7 @@ int mg_plan(const es_ctx* ctx, int n_streams, int n_pairs, int coins, int N, MgP
     const bool forced = ej && atoi(ej) != 0;
     pl = MgPlan{};
     if (!(ej ? forced : blocks_needed >= 2048)) return ES_OK;
-    int lb = 3;
-    const char* el = getenv("ES_MT_JUMP_LB");
-    if (el) lb = atoi(el);
-    else
-        while (lb < MJ_BITS_RANGE - 1 && (long long)n_streams * ((blocks_needed + (1LL << lb) - 1) >> lb) > 4LL * ctx->sm_count) ++lb;
-    if (lb < 0) lb = 0;
-    if (lb > MJ_BITS_RANGE - 1) lb = MJ_BITS_RANGE - 1;
+    const int lb = mj_segment_lb(n_streams, blocks_needed, ctx->sm_count);
     const long long n_seg = (blocks_needed + (1LL << lb) - 1) >> lb;
     if (((n_seg << lb) >> MJ_BITS_RANGE) != 0 || (double)(n_seg << lb) * MT_NW > 4.0e9 || n_seg > 65535) {
         // the block index of a segment start must fit the available jumps (2^20 blocks = 654 M words per stream) and a
@@ -737,6 +745,24 @@ struct MgDraw {                   // the arguments of one es_draw_noisy call
 
 size_t mg_pad(size_t b) { return (b + 255) & ~(size_t)255; }
 
+// the tempered words of blocks 0 .. n_seg << lb_log2 of every stream, from the streams' keys (block 0), into words
+int mj_launch_fill(es_ctx* ctx, const uint32_t* mt_key, int n_streams, int n_seg, int lb_log2, uint16_t* order, uint32_t* words,
+                   size_t stride_words, cudaStream_t stream) {
+    if (!ctx->mj_lists_ready) {
+        mj_lists_kernel<<<MJ_NPOLY, 640, 0, stream>>>();
+        ES_LAUNCHED(ctx);
+        ctx->mj_lists_ready = 1;
+    }
+    mj_order_kernel<<<1, 1024, 0, stream>>>(n_seg, lb_log2, order);
+    ES_LAUNCHED(ctx);
+    const size_t smem = (size_t)(MJ_WIN_BLOCKS + 6) * MT_NW * sizeof(uint32_t);
+    ES_CHECK_CUDA(cudaFuncSetAttribute(mt_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    mt_fill_kernel<<<(unsigned)(n_streams * n_seg), MF_THREADS, smem, stream>>>(mt_key, n_streams, n_seg, lb_log2, order, words,
+                                                                               stride_words);
+    ES_LAUNCHED(ctx);
+    return ES_OK;
+}
+
 int mg_launch_jump(es_ctx* ctx, const MgDraw& d, const MgPlan& pl, cudaStream_t stream) {
     // scratch: the streams' words | accept masks [stream][phase][chunk][32] | chunk counts -> prefixes [stream][phase][chunk]
     //          | first word of every rollout [stream][2 n] | incoming cache per stream
@@ -758,18 +784,8 @@ int mg_launch_jump(es_ctx* ctx, const MgDraw& d, const MgPlan& pl, cudaStream_t 
     int32_t* c0 = (int32_t*)at; at += c0_bytes;
     double* gauss0 = (double*)at; at += g0_bytes;
     uint16_t* order = (uint16_t*)at;
-    if (!ctx->mj_lists_ready) {
-        mj_lists_kernel<<<MJ_NPOLY, 640, 0, stream>>>();
-        ES_LAUNCHED(ctx);
-        ctx->mj_lists_ready = 1;
-    }
-    mj_order_kernel<<<1, 1024, 0, stream>>>((int)pl.n_seg, pl.lb_log2, order);
-    ES_LAUNCHED(ctx);
-    const size_t smem = (size_t)(MJ_WIN_BLOCKS + 6) * MT_NW * sizeof(uint32_t);
-    ES_CHECK_CUDA(cudaFuncSetAttribute(mt_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    mt_fill_kernel<<<(unsigned)(d.n_streams * pl.n_seg), MF_THREADS, smem, stream>>>(d.mt_key, d.n_streams, (int)pl.n_seg, pl.lb_log2,
-                                                                                   order, words, pl.stride_words);
-    ES_LAUNCHED(ctx);
+    rc = mj_launch_fill(ctx, d.mt_key, d.n_streams, (int)pl.n_seg, pl.lb_log2, order, words, pl.stride_words, stream);
+    if (rc) return rc;
     mt_flags_kernel<<<dim3((unsigned)((pl.n_chunks + MFL_WARPS - 1) / MFL_WARPS), (unsigned)d.n_streams), 32 * MFL_WARPS, 0, stream>>>(
         words, pl.stride_words, (int)pl.n_chunks, masks, counts);
     ES_LAUNCHED(ctx);
@@ -812,7 +828,244 @@ int mg_launch_sequential(es_ctx* ctx, const MgDraw& d, cudaStream_t stream) {
     return ES_OK;
 }
 
+// =====================================================================================================================
+// es_randn: n gaussians in a row from ONE stream, rs.randn(n) -- numpy's noise table.  Every attempt of the call starts at
+// word p0 + 4 a (p0: the incoming position), so all attempts share the phase ph = p0 & 3 and nothing has to be walked:
+// attempt a's values are c0 + 2 r and c0 + 2 r + 1, r = the number of accepted attempts before it (c0: the incoming cache
+// bit).  The stream is processed in windows of at most MR_WINDOW_BLOCKS blocks so that the scratch stays bounded; a window
+// is the jump-ahead path's fill (block 0 = the window's base state) + the accept masks and chunk prefixes of mt_flags_kernel
+// / mt_scan_kernel.  Window w + 1 starts from window w's last block (untempered from its words): the two windows overlap by
+// that block, so an attempt that starts in window w's own L blocks but ends in the next block is whole in window w, and no
+// window jumps further than its own length.  In its local numbering a window of L blocks owns the attempts a of phase ph
+// with a_lo <= a < 156 L (a_lo = p0 >> 2 in window 0, else 0): the next window's first attempt is its attempt 0.
+// =====================================================================================================================
+constexpr long long MR_WINDOW_BLOCKS = 3LL << 15;               // 98 304 blocks = 61 M words = 245 MB of words per window
+constexpr int MR_EMIT_WARPS = 8;
+
+struct MrState {                  // what the windows hand on to each other (device scratch)
+    long long base;               // rank among the call's accepted attempts of the window's attempt a = base + cum(a)
+    long long next;               // the next window's base
+    double g0;                    // the incoming cached gaussian
+    int c0, ph, a_lo;             // the incoming cache bit, the attempts' phase, the window's first attempt
+};
+
+// accepted attempts of phase ph before attempt a of the window (one warp; mph / cph: the phase's masks and chunk prefixes)
+__device__ __forceinline__ uint32_t mr_cum(const uint32_t* __restrict__ mph, const uint32_t* __restrict__ cph, uint32_t a, int lane) {
+    const uint32_t c = a >> 10, r = a & 1023u;
+    const uint32_t m = mph[(size_t)c * 32 + lane];
+    const int below = __reduce_add_sync(0xffffffffu, lane < (int)(r >> 5) ? __popc(m)
+                                                     : (lane == (int)(r >> 5) ? __popc(m & ((1u << (r & 31)) - 1u)) : 0));
+    return cph[c] + (uint32_t)below;
+}
+
+// One warp per window, after the prefixes: the window's rank offsets, the next window's base state; in window 0 the incoming
+// cache; in the window that holds the attempt giving value n - 1, the outgoing state (found with the prefix tables as
+// mt_walk_kernel does).
+__global__ void __launch_bounds__(32)
+mr_window_kernel(int w, int last, int64_t L, const uint32_t* __restrict__ words, int n_chunks, const uint32_t* __restrict__ masks,
+                 const uint32_t* __restrict__ cumul, uint32_t* __restrict__ key_next, uint32_t* __restrict__ mt_key,
+                 int32_t* __restrict__ mt_pos, int32_t* __restrict__ has_gauss, double* __restrict__ gauss, int64_t n,
+                 float* __restrict__ out, MrState* __restrict__ st, int* __restrict__ err) {
+    const int lane = threadIdx.x;
+    const unsigned FULL = 0xffffffffu;
+    int c0, ph, a_lo;
+    long long base_in = 0;
+    if (w == 0) {                                              // the incoming state, read before anything below writes it
+        const int p0 = mt_pos[0];
+        c0 = has_gauss[0] ? 1 : 0;
+        const double g0 = gauss[0];
+        ph = p0 & 3;
+        a_lo = p0 >> 2;
+        __syncwarp();
+        if (lane == 0) {
+            st->c0 = c0; st->g0 = g0; st->ph = ph;
+            if (c0) out[0] = (float)g0;                         // the cached gaussian is value 0 (the host ensures n >= 1)
+        }
+    } else {
+        c0 = st->c0; ph = st->ph; a_lo = 0;
+        base_in = st->next;
+    }
+    const long long A = (n - c0 + 1) >> 1;                     // accepted attempts the call needs
+    const uint32_t* __restrict__ mph = masks + (size_t)ph * n_chunks * 32;
+    const uint32_t* __restrict__ cph = cumul + (size_t)ph * n_chunks;
+    const uint32_t a_hi = (uint32_t)(L * (MT_NW / 4));
+    const long long base = w == 0 ? -(long long)mr_cum(mph, cph, (uint32_t)a_lo, lane) : base_in;
+    const long long next = base + mr_cum(mph, cph, a_hi, lane);
+    if (lane == 0) { st->base = base; st->next = next; st->a_lo = a_lo; }
+    if (!last)
+        for (int i = lane; i < MT_NW; i += 32) key_next[i] = mt19937_untemper(words[(size_t)L * MT_NW + i]);
+    if (A == 0) {                                              // n == 1 served by the cache: nothing cached afterwards
+        if (w == 0 && lane == 0) { has_gauss[0] = 0; gauss[0] = 0.0; }
+        return;
+    }
+    if (last && next < A) {                                    // (the host plans the mean + 12 sigma of the words needed)
+        if (lane == 0 && err) *(volatile int*)err = ES_ASYNC_RANDN_OVERFLOW;
+        return;
+    }
+    if (!(base <= A - 1 && A - 1 < next)) return;
+    // the (k + 1)-th accepted attempt of the window gives value n - 1: its chunk is the last one whose prefix is <= k
+    const uint32_t k = (uint32_t)(A - 1 - base);
+    uint32_t lo = 0, hi = (uint32_t)n_chunks - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (cph[mid] <= k) lo = mid; else hi = mid - 1u;
+    }
+    const uint32_t want = k - cph[lo] + 1u;                    // 1-based among the chunk's accepted attempts
+    const uint32_t m1 = mph[(size_t)lo * 32 + lane];
+    int inc = __popc(m1);
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int up = __shfl_up_sync(FULL, inc, d);
+        if (lane >= d) inc += up;
+    }
+    const int Lw = __ffs((int)__ballot_sync(FULL, (uint32_t)inc >= want)) - 1;
+    const uint32_t mL = __shfl_sync(FULL, m1, Lw);
+    const int kth = (int)want - (__shfl_sync(FULL, inc, Lw) - __popc(mL));
+    const int bit = __ffs((int)__ballot_sync(FULL, ((mL >> lane) & 1u) && __popc(mL & ((1u << lane) - 1u)) == kth - 1)) - 1;
+    const uint32_t a1 = (lo << 10) + 32u * (uint32_t)Lw + (uint32_t)bit;
+    // the stream after that attempt: the raw words behind the tempered words of the cursor's block, and the position
+    const uint32_t end = 4u * a1 + (uint32_t)ph + 4u;
+    const uint32_t blk = end / MT_NW, off = end % MT_NW;
+    const bool at_end = off == 0 && blk > 0;
+    const uint32_t b_last = at_end ? blk - 1 : blk;
+    for (int i = lane; i < MT_NW; i += 32) mt_key[i] = mt19937_untemper(words[(size_t)b_last * MT_NW + i]);
+    if (lane == 0) {
+        const int cached = (int)(c0 + 2 * A - n);              // the last attempt's second value is value n: the cache
+        mt_pos[0] = at_end ? MT_NW : (int32_t)off;
+        has_gauss[0] = cached;
+        if (!cached) gauss[0] = 0.0;                           // (otherwise mr_emit_kernel writes it)
+    }
+}
+
+// The gaussians of one window, one warp per chunk of 1 024 attempts: lane l takes attempt 32 j + l in step j, its rank is the
+// chunk's prefix + the accepted attempts of the chunk's mask words before j + those of lower lanes in word j.
+__global__ void __launch_bounds__(32 * MR_EMIT_WARPS)
+mr_emit_kernel(const uint32_t* __restrict__ words, int64_t L, int n_chunks, const uint32_t* __restrict__ masks,
+               const uint32_t* __restrict__ cumul, const MrState* __restrict__ st, int64_t n, float* __restrict__ out,
+               double* __restrict__ gauss) {
+    const int lane = threadIdx.x & 31;
+    const int c = blockIdx.x * MR_EMIT_WARPS + (threadIdx.x >> 5);
+    if (c >= n_chunks) return;
+    const int c0 = st->c0, ph = st->ph;
+    const uint32_t a_lo = (uint32_t)st->a_lo, a_hi = (uint32_t)(L * (MT_NW / 4));
+    const long long A = (n - c0 + 1) >> 1;
+    const long long r0 = st->base + cumul[(size_t)ph * n_chunks + c];
+    if (r0 >= A) return;                                       // the call's values end before this chunk
+    const uint32_t m = masks[((size_t)ph * n_chunks + c) * 32 + lane];
+    int inc = __popc(m);
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int up = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc += up;
+    }
+    const int excl = inc - __popc(m);
+    const uint32_t below = (1u << lane) - 1u;
+    const uint32_t* __restrict__ wc = words + (size_t)c * MJ_CW + ph + 4 * lane;
+    for (int j = 0; j < 32; ++j) {
+        const uint32_t mj = __shfl_sync(0xffffffffu, m, j);
+        const long long r = r0 + __shfl_sync(0xffffffffu, excl, j) + __popc(mj & below);
+        const uint32_t a = ((uint32_t)c << 10) + 32u * (uint32_t)j + (uint32_t)lane;
+        if (!((mj >> lane) & 1u) || a < a_lo || a >= a_hi || r < 0 || r >= A) continue;
+        const uint32_t* __restrict__ wp = wc + 128 * j;
+        const double2 g = mt19937_polar_pair(__ldg(wp), __ldg(wp + 1), __ldg(wp + 2), __ldg(wp + 3));
+        const long long v = c0 + 2 * r;
+        out[v] = (float)g.x;
+        if (v + 1 < n) out[v + 1] = (float)g.y;
+        else *gauss = g.y;                                     // value n: the cache the stream hands back
+    }
+}
+
+// The windows of one es_randn call: each covers L = n_seg << lb blocks of its own; together they cover the mean + 12 sigma of
+// the words n values can take (~2.55 words per value), so the last window's prefix shows whether the draw was complete.
+struct MrWindow { int n_seg, lb; long long L, n_chunks; };
+struct MrPlan {
+    std::vector<MrWindow> win;
+    // scratch: the window's words (+ a chunk of padding: mt_flags_kernel reads past every attempt start) | accept masks
+    //          [phase][chunk][32] | chunk counts -> prefixes [phase][chunk] | the next window's key | segment order | MrState
+    size_t words_bytes, mask_bytes, cnt_bytes, key_bytes, ord_bytes, bytes;
+};
+
+std::vector<MrWindow> mr_windows(const es_ctx* ctx, int64_t n) {
+    const double p_acc = 0.78539816339744830962, n_acc = (double)((n + 1) / 2);
+    const double words_max = 2.0 * MT_NW + 4.0 * (n_acc / p_acc + 12.0 * sqrt(n_acc * (1.0 - p_acc)) / p_acc + 64.0);
+    long long left = (long long)(words_max / MT_NW) + 1;
+    long long per = MR_WINDOW_BLOCKS;
+    const char* ew = getenv("ES_RANDN_WINDOW_BLOCKS");          // (tests: many small windows)
+    if (ew) per = atoll(ew);
+    if (per < 1) per = 1;
+    if (per > (1LL << (MJ_BITS_RANGE - 1))) per = 1LL << (MJ_BITS_RANGE - 1);
+    std::vector<MrWindow> win;
+    while (left > 0) {
+        const long long want = left < per ? left : per;
+        int lb = mj_segment_lb(1, want, ctx->sm_count);
+        while (((want + (1LL << lb) - 1) >> lb) > 65535) ++lb;                 // (mj_order_kernel: 16-bit segment numbers)
+        MrWindow wd;
+        wd.lb = lb;
+        wd.n_seg = (int)((want + (1LL << lb) - 1) >> lb);
+        wd.L = (long long)wd.n_seg << lb;
+        wd.n_chunks = ((1 + wd.L) * MT_NW + MJ_CW - 1) / MJ_CW;
+        win.push_back(wd);
+        left -= wd.L;
+    }
+    return win;
+}
+
+MrPlan mr_plan(const es_ctx* ctx, int64_t n) {
+    MrPlan pl;
+    pl.win = mr_windows(ctx, n);
+    long long nc = 0, ns = 0;
+    for (const MrWindow& w : pl.win) { nc = w.n_chunks > nc ? w.n_chunks : nc; ns = w.n_seg > ns ? w.n_seg : ns; }
+    pl.words_bytes = mg_pad((size_t)(nc + 1) * MJ_CW * sizeof(uint32_t));
+    pl.mask_bytes = mg_pad((size_t)4 * nc * 32 * sizeof(uint32_t));
+    pl.cnt_bytes = mg_pad((size_t)4 * nc * sizeof(uint32_t));
+    pl.key_bytes = mg_pad(MT_NW * sizeof(uint32_t));
+    pl.ord_bytes = mg_pad((size_t)ns * sizeof(uint16_t));
+    pl.bytes = pl.words_bytes + pl.mask_bytes + pl.cnt_bytes + pl.key_bytes + pl.ord_bytes + mg_pad(sizeof(MrState));
+    return pl;
+}
+
 }  // namespace
+
+int es_impl_randn_plan(const es_ctx* ctx, int64_t n, size_t* scratch_bytes, int* n_windows) {
+    const MrPlan pl = mr_plan(ctx, n);
+    *scratch_bytes = pl.bytes;
+    *n_windows = (int)pl.win.size();
+    return ES_OK;
+}
+
+int es_impl_randn(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int64_t n, float* out,
+                  cudaStream_t stream) {
+    const MrPlan pl = mr_plan(ctx, n);
+    const std::vector<MrWindow>& win = pl.win;
+    void* scratch = nullptr;
+    int rc = es_ctx_scratch(ctx, pl.bytes, &scratch);
+    if (rc) return rc;
+    char* at = (char*)scratch;
+    uint32_t* words = (uint32_t*)at; at += pl.words_bytes;
+    uint32_t* masks = (uint32_t*)at; at += pl.mask_bytes;
+    uint32_t* counts = (uint32_t*)at; at += pl.cnt_bytes;
+    uint32_t* key_next = (uint32_t*)at; at += pl.key_bytes;
+    uint16_t* order = (uint16_t*)at; at += pl.ord_bytes;
+    MrState* st = (MrState*)at;
+    for (size_t w = 0; w < win.size(); ++w) {
+        const MrWindow& wd = win[w];
+        const int n_chunks = (int)wd.n_chunks;
+        rc = mj_launch_fill(ctx, w == 0 ? mt_key : key_next, 1, wd.n_seg, wd.lb, order, words, (size_t)(n_chunks + 1) * MJ_CW, stream);
+        if (rc) return rc;
+        mt_flags_kernel<<<dim3((unsigned)((n_chunks + MFL_WARPS - 1) / MFL_WARPS), 1), 32 * MFL_WARPS, 0, stream>>>(
+            words, (size_t)(n_chunks + 1) * MJ_CW, n_chunks, masks, counts);
+        ES_LAUNCHED(ctx);
+        mt_scan_kernel<<<4, 1024, 0, stream>>>(counts, n_chunks);                 // (the phase is only known on the device)
+        ES_LAUNCHED(ctx);
+        mr_window_kernel<<<1, 32, 0, stream>>>((int)w, w + 1 == win.size(), wd.L, words, n_chunks, masks, counts, key_next, mt_key,
+                                               mt_pos, has_gauss, gauss, n, out, st, ctx->err_dev);
+        ES_LAUNCHED(ctx);
+        mr_emit_kernel<<<(unsigned)((n_chunks + MR_EMIT_WARPS - 1) / MR_EMIT_WARPS), 32 * MR_EMIT_WARPS, 0, stream>>>(
+            words, wd.L, n_chunks, masks, counts, st, n, out, gauss);
+        ES_LAUNCHED(ctx);
+    }
+    return ES_OK;
+}
 
 int es_impl_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,
                        int n_per_stream, uint64_t upper_bound, int coins, int normals_per_eval, double scale, int64_t* idx_out,

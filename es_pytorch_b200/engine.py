@@ -192,6 +192,31 @@ class Engine:
                                      _ptr(coin_out), _ptr(noise_out), self.stream), 'es_draw_noisy')
         return idx_out, coin_out, noise_out
 
+    def randn(self, mt_key, mt_pos, has_gauss, gauss, n: int, out=None):
+        """``rs.randn(n).astype(np.float32)`` of ONE stream (es_randn): mt_key int32 [624] (or [1, 624]), mt_pos /
+        has_gauss int32 [1], gauss float64 [1] -- ``RandomState.get_state()[1:5]`` --, updated in place to the state numpy
+        leaves behind.  Returns float32 [n] (``out`` when given)."""
+        d = self.device
+        n = int(n)
+        if n < 0:
+            raise ValueError(f'n must be >= 0, got {n}')
+        _req(mt_key, torch.int32, 'mt_key', d); _req(mt_pos, torch.int32, 'mt_pos', d)
+        _req(has_gauss, torch.int32, 'has_gauss', d); _req(gauss, torch.float64, 'gauss', d)
+        assert mt_key.numel() == ES_MT_N and mt_pos.numel() == 1 and has_gauss.numel() == 1 and gauss.numel() == 1
+        if out is None:
+            out = self.empty((n,), torch.float32)
+        _req(out, torch.float32, 'out', d)
+        assert out.numel() == n
+        check(self.lib.es_randn(self._ctx, _ptr(mt_key), _ptr(mt_pos), _ptr(has_gauss), _ptr(gauss), n, _ptr(out), self.stream),
+              'es_randn')
+        return out
+
+    def randn_plan(self, n: int):
+        """(scratch bytes, windows) of ``randn(..., n)``."""
+        nbytes, windows = C.c_size_t(), C.c_int()
+        check(self.lib.es_randn_plan(self._ctx, int(n), C.byref(nbytes), C.byref(windows)), 'es_randn_plan')
+        return int(nbytes.value), int(windows.value)
+
     # ------------------------------------------------------------------ a3
     def perturb(self, theta, table, idx, sigma: float, want_neg: bool = True):
         d = self.device

@@ -17,6 +17,7 @@
 #ifndef ES_B200_H
 #define ES_B200_H
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -173,6 +174,19 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,
                   int n_per_stream, uint64_t upper_bound, int coins_per_eval, int normals_per_eval, double scale,
                   int64_t* idx_out, uint32_t* coin_out, float* noise_out, void* stream);
+
+/* ---- the noise table: rs.randn(n) of ONE stream -------------------------------------------------------------------
+ * out[i] = (float)g_i, the n values numpy's legacy RandomState.randn(n).astype(np.float32) returns from the stream state
+ * (mt_key [624] raw words, mt_pos, has_gauss, gauss: RandomState.get_state()[1..4], device memory), which is updated in place
+ * to what numpy leaves behind.  Any incoming state is accepted: a position anywhere in the block, a cached gaussian (it is
+ * out[0]).  Key, position and has_gauss are bit-exact; a value (and the outgoing cached gaussian) can differ from numpy's in
+ * its last float64 bit (CUDA's log vs glibc's), which moves the float32 value by one ulp when the float64 value lies next to
+ * a float32 rounding midpoint.  The stream is drawn by MT19937 jump-ahead over the whole GPU in windows of at most 98 304
+ * blocks (245 MB of words): the scratch does not grow with n.  n == 0 changes nothing (out may then be NULL).           */
+int es_randn(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int64_t n, float* out,
+             void* stream);
+/* what es_randn(n) allocates: its scratch in bytes (the ctx's scratch grows to it + 25 %, never shrinks) and its windows */
+int es_randn_plan(es_ctx* ctx, int64_t n, size_t* scratch_bytes, int* n_windows);
 
 /* The tensor-core rollouts keep float16 shadows of the noise table (8 shifted copies of f16(table), 2 bytes x 8 x table_len
  * of HBM; ES_ROLLOUT_TC3 a second set for the low-order parts), built on first use and keyed by the table's device pointer,
