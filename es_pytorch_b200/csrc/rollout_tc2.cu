@@ -34,6 +34,11 @@
 //     warp moves the image into shared memory with two bulk copies when the previous pair's MMAs have retired.
 //   * with the shadows, the copier also prefetches the next pair's eps1 into L2 (TMA prefetch, same maps and coordinates)
 //     one pair ahead, so the eps1 copy at the pair boundary reads L2 and not HBM.
+//   * U and the reward weights c (the same for every pair): each consumer thread loads its 32 values of U for a tile into
+//     registers before the tile's L1 chain, which hides the load, and its 16 values of c once per tile; both signs use the
+//     registers.  Loaded once per sign inside the epilogues, their latency sat between the wgmma chains (pointing them at
+//     rows already in L1 recovered only a small part of what this saves).  The NOISE instantiations still load c element by
+//     element in the epilogue: holding it in registers there spills at 208.
 //
 // 12 warps (3 warpgroups):
 //   warpgroup 0: warp 0 producer (Xn ring) | warp 1 copier | warps 2-3 builders      -> setmaxnreg 72 registers
@@ -473,6 +478,18 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
             float pp0 = 0.f, pp1 = 0.f, pp2 = 0.f, pn0 = 0.f, pn1 = 0.f, pn2 = 0.f;     // position sums of this thread's rows
             mbar_wait_warp(&bars[B2_EPS_READY], i & 1);
             for (int m = 0; m < NMT; ++m) {
+                const int ta = m * T2_MT + r0, tb = ta + 8;                        // time steps of this thread's two rows
+                // U of this thread's two rows, loaded once for both signs (issued before the L1 chain, which hides the latency)
+                float u[32];
+                {
+                    const float* __restrict__ urow = p.ubase + (size_t)ta * T2_H + 2 * q;
+#pragma unroll
+                    for (int c = 0; c < 8; ++c) {
+                        const float2 u0 = __ldg(reinterpret_cast<const float2*>(urow + 8 * c));
+                        const float2 u1 = __ldg(reinterpret_cast<const float2*>(urow + 8 * T2_H + 8 * c));
+                        u[4 * c + 0] = u0.x; u[4 * c + 1] = u0.y; u[4 * c + 2] = u1.x; u[4 * c + 3] = u1.y;
+                    }
+                }
                 // ---- L1: V = Xn . eps1^T (SPLIT: x_hi.eps_hi + x_hi.eps_lo + x_lo.eps_hi), chunk by chunk through the ring ----
                 float v[32];
                 reg_fence(v);
@@ -510,18 +527,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 }
                 if (m == 0) mbar_wait_warp(&bars[B2_W_READY], i & 1);                  // W2, W3 and the biases of the pair in place?
 
-                const int ta = m * T2_MT + r0, tb = ta + 8;                        // time steps of this thread's two rows
-                const float* __restrict__ urow = p.ubase + (size_t)ta * T2_H + 2 * q;
                 // ---- epi1: h1 = tanh(U +- sigma V) ----
                 auto epi1 = [&](float s, uint32_t (&hh)[16], uint32_t (&hl)[16]) {
                     float z[32];
 #pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const float2 u0 = __ldg(reinterpret_cast<const float2*>(urow + 8 * c));
-                        const float2 u1 = __ldg(reinterpret_cast<const float2*>(urow + 8 * T2_H + 8 * c));
-                        z[4 * c + 0] = __fmaf_rn(v[4 * c + 0], s, u0.x); z[4 * c + 1] = __fmaf_rn(v[4 * c + 1], s, u0.y);
-                        z[4 * c + 2] = __fmaf_rn(v[4 * c + 2], s, u1.x); z[4 * c + 3] = __fmaf_rn(v[4 * c + 3], s, u1.y);
-                    }
+                    for (int k = 0; k < 32; ++k) z[k] = __fmaf_rn(v[k], s, u[k]);
                     act_pack<SPLIT>(z, hh, hl);
                 };
                 // ---- L2: D2 = h1 . W2^T (SPLIT: h_hi.w_hi + h_hi.w_lo + h_lo.w_hi), one commit group ----
@@ -575,6 +585,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 // The first episode is straight-line code as in the single-episode kernel; the others loop and recompute the
                 // tanh (keeping the 16 actions live across the loop would cost registers).  (epi3_episode serves the NOISE
                 // instantiations only.)
+                float rw[16];                                                      // c_t of this thread's D3 elements (!NOISE)
                 auto epi3_episode = [&](int sgn, const float (&d3)[16], const float* __restrict__ nz, float& ra, float& rb,
                                         float& q0, float& q1, float& q2) {
                     const float* b3 = bias + 2 * T2_H + sgn * T2_ACT_PAD;
@@ -601,7 +612,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     rb += __shfl_xor_sync(0xffffffffu, rb, 1); rb += __shfl_xor_sync(0xffffffffu, rb, 2);
                 };
                 auto epi3 = [&](int sgn, const float (&d3)[16]) {
-                    if (!NOISE) {          // the noise-free kernels keep the single-episode epilogue as it was (same SASS)
+                    if (!NOISE) {          // the noise-free kernels: one episode, c from registers
                         const float* b3 = bias + 2 * T2_H + sgn * T2_ACT_PAD;
                         float ra = 0.f, rb = 0.f, q0 = 0.f, q1 = 0.f, q2 = 0.f;
 #pragma unroll
@@ -613,7 +624,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                                 const float z = __fadd_rn(d3[4 * c + e], b3[col]);
                                 const float a = SPLIT ? tanh_acc(z) : tanh_fast(z);
                                 if (col < p.act && t < p.T) {
-                                    const float r = a * __ldg(p.rew_vec + (size_t)t * p.act + col);
+                                    const float r = a * rw[4 * c + e];
                                     if (e & 2) rb += r; else ra += r;
                                     q0 += (col == 0) ? a : 0.f; q1 += (col == 1) ? a : 0.f; q2 += (col == 2) ? a : 0.f;
                                 }
@@ -661,6 +672,18 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 reg_fence(d2n); reg_fence(hn); if (SPLIT) reg_fence(ln);
                 epi2(1, d2n, hn, ln);
                 mma3(1, hn, ln, d3n);
+                // c_t of this thread's 16 elements of D3, loaded once for both signs (NOISE: element by element in epi3_episode)
+                if (!NOISE) {
+#pragma unroll
+                    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            const int col = 8 * c + 2 * q + (e & 1);
+                            const int t = (e & 2) ? tb : ta;
+                            rw[4 * c + e] = (col < p.act && t < p.T) ? __ldg(p.rew_vec + (size_t)t * p.act + col) : 0.f;
+                        }
+                    }
+                }
                 wg_wait<1>();
                 reg_fence(d3p); reg_fence(hp); if (SPLIT) reg_fence(lp);
                 epi3(0, d3p);
