@@ -247,7 +247,11 @@ int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_
     if (rc) return rc;
     if (n_pairs == 0) return ES_OK;
     if (mode == ES_ROLLOUT_F32) return es_impl_rollout_f32(ctx, r, (cudaStream_t)stream);
-    if (mode == ES_ROLLOUT_TC || mode == ES_ROLLOUT_TC3) return es_impl_rollout_tc2(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
+    if (mode == ES_ROLLOUT_TC || mode == ES_ROLLOUT_TC3) {
+        // the shipped configs' wide policies (rollout_tcw.cu); obs-64-64-act and everything else: rollout_tc2.cu
+        if (es_tcw_covers(r)) return es_impl_rollout_tcw(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
+        return es_impl_rollout_tc2(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
+    }
     es_set_error("es_rollout_openloop: unknown mode %d", mode);
     return ES_ERR_INVALID;
 }

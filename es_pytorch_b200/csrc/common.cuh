@@ -140,6 +140,9 @@ int es_impl_rollout_f32(es_ctx*, const EsRollout&, cudaStream_t);
 int es_impl_rollout_f32x(es_ctx*, const EsRollout&, cudaStream_t);
 int es_impl_rollout_tc2(es_ctx*, const EsRollout&, int split, cudaStream_t);
 void es_tc2_free_shadows(es_ctx* ctx);
+// tanh MLPs with 2 to 4 hidden layers of widths in {64, 128, 192, 256}, obs <= 256, act <= 32, other than obs-64-64-act
+bool es_tcw_covers(const EsRollout&);
+int es_impl_rollout_tcw(es_ctx*, const EsRollout&, int split, cudaStream_t);
 int es_impl_rollout_closed(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
 int es_launch_ubase(es_ctx*, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,

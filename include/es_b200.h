@@ -101,7 +101,11 @@ int es_normalise_obs(es_ctx* ctx, const float* obs, const double* mean, const do
  *                          population spread of the float32 result, see DESIGN.md)
  *         ES_ROLLOUT_TC3 = wgmma tensor-core path at float32-equivalent accuracy: every operand is split into
  *                          float16 hi + lo parts and every product is three MMAs (hi*hi + hi*lo + lo*hi), float32
- *                          accumulation in registers, accurate tanh, float64 fitness sums (see rollout_tc2.cu)                */
+ *                          accumulation in registers, accurate tanh, float64 fitness sums (see rollout_tc2.cu)
+ *         The tensor-core modes cover obs(<=383 TC3, <=511 TC)-64-64-act(<=32) tanh MLPs (rollout_tc2.cu) and tanh MLPs
+ *         with 2 to 4 hidden layers of widths in {64, 128, 192, 256}, obs <= 256 and act <= 32 (rollout_tcw.cu; there
+ *         ES_ROLLOUT_TC needs T >= 4: episodes of 1 to 3 steps measured above its error bound); other shapes are refused
+ *         with ES_ERR_UNSUPPORTED.                                                              */
 #define ES_ROLLOUT_F32 0
 #define ES_ROLLOUT_TC  1
 #define ES_ROLLOUT_TC3 2
