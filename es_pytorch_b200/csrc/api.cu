@@ -295,6 +295,54 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
     return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
 }
 
+// the shapes es_rollout_closedloop's one-CTA kernel (rollout_closed.cu) covers: two hidden layers <= 64, act <= 64, obs <= 384
+static bool es_closed_one_cta_covers(const int* dims, int n_layers) {
+    return n_layers == 3 && dims[1] <= 64 && dims[2] <= 64 && dims[3] <= 64 && dims[0] <= 384;
+}
+
+int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int* cluster_size, int* clusters,
+                                   int64_t* smem_bytes) {
+    ES_ENTER(ctx);
+    ES_REQUIRE(layer_sizes && cluster_size && clusters && smem_bytes, "es_rollout_closedloop_mlp_plan: NULL pointer");
+    ES_REQUIRE(n_layers >= 1 && n_layers <= ES_MAX_LAYERS, "es_rollout_closedloop_mlp_plan: n_layers must be in [1,%d]", ES_MAX_LAYERS);
+    for (int l = 0; l <= n_layers; ++l) ES_REQUIRE(layer_sizes[l] > 0, "es_rollout_closedloop_mlp_plan: layer size <= 0");
+    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop_mlp_plan: band must be in [1, obs_dim]");
+    int C = 0;
+    size_t smem = 0;
+    const int rc = es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);
+    if (rc) return rc;
+    if (es_closed_one_cta_covers(layer_sizes, n_layers)) {
+        *cluster_size = 0; *clusters = ctx->sm_count; *smem_bytes = 0;
+        return ES_OK;
+    }
+    *cluster_size = C; *smem_bytes = (int64_t)smem;
+    return es_closedw_max_clusters(n_layers, C, smem, clusters);
+}
+
+int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
+                              int P, float sigma, const int* layer_sizes, int n_layers, const double* ob_mean, const double* ob_std,
+                              double ob_clip, const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
+                              int T, float pos_scale, const uint32_t* coin_words, double save_obs_chance, double* fit_pos,
+                              double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
+                              double* ob_count, void* stream) {
+    ES_ENTER(ctx);
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1};
+    int rc = es_rollout_check("es_rollout_closedloop_mlp", ob_mean && ob_std && obs0 && env_a && env_b, r);
+    if (rc) return rc;
+    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop_mlp: band must be in [1, obs_dim]");
+    ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
+               "es_rollout_closedloop_mlp: ob_sum/ob_sumsq/ob_count must all be set or NULL");
+    int C = 0;
+    size_t smem = 0;
+    rc = es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);      // coverage does not depend on n_pairs
+    if (rc) return rc;
+    if (n_pairs == 0) return ES_OK;
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    if (es_closed_one_cta_covers(layer_sizes, n_layers)) return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
+    return es_impl_rollout_closedw(ctx, r, env, (cudaStream_t)stream);
+}
+
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,
                   int n_per_stream, uint64_t upper_bound, int coins_per_eval, int normals_per_eval, double scale,
                   int64_t* idx_out, uint32_t* coin_out, float* noise_out, void* stream) {

@@ -1,0 +1,416 @@
+// rollout_closedw.cu -- the CLOSED-LOOP synthetic env (obs_{t+1} = tanh(A obs_t + B a_t)) for policies too wide for
+// rollout_closed.cu's one pair per CTA: tanh MLPs with 2 to 4 hidden layers of 1 .. 256 units, obs <= 384, act <= 64 -- every
+// shipped config's policy (15-256-256-3, 17/26/28-256-256-256-6/8, 28-128-256-256-128-8) and a Humanoid-shaped 376-256-256-17.
+//
+// Semantics are rollout_closed.cu's: theta +- sigma eps through es_pheno_pm (slices checked by es_checked_slice and the ctx's
+// error word), clip((o - mean) / std) in float64 (here an exact float64 division, as the reference), Linear + tanh after every
+// layer including the output (the same fast tanh as rollout_closed.cu, cw_tanh: absolute error ~1e-7), the reward as a
+// float32 dot in index order summed in float64 in step order, the position integrator, behaviour outputs with fit_stride, and
+// the ObStat increments (float32 column sums in step order, added in float64) of evaluations whose save_obs coin fell.  The env
+// step is the oracle's arithmetic exactly: one float32 accumulator, A's diagonals then B's columns in index order, every product
+// and sum rounded separately (rollout_closed.cu interleaves two FMA accumulators instead).
+//
+// Why a cluster: one evaluation's float32 weights are 276 KiB (15-256-256-3) to 651 KiB (376-256-256-17), more than one SM's
+// 227 KiB of shared memory, and re-reading them from L2 at every step would move ~1.3 PB per simple_conf generation.  So:
+//   * one thread-block cluster of C CTAs (C in {1, 2, 4, 8}, the smallest that holds the weights; a function of the shape
+//     only, es_closedw_plan) runs one evaluation (one sign of a pair) at a time, and clusters loop over the 2 n_pairs
+//     evaluations (persistent grid: cudaOccupancyMaxActiveClusters clusters -- a cluster lives inside one GPC and H100's GPCs
+//     do not all have the same SM count, so sm_count / C would overestimate);
+//   * row split: CTA q of the cluster owns the contiguous output rows [q R_l, (q + 1) R_l) of every layer l
+//     (R_l = ceil(d_{l+1} / C)) and keeps their weights and biases in its shared memory, rows [R_l][pad32(d_l)] zero padded;
+//   * one warp computes 4 rows at a time: lane s accumulates the elements k = 32 j + s of each row in j order (fmaf), and a
+//     transposing butterfly (7 shuffles) adds the 32 lane sums in the fixed xor-16, 8, 4, 2, 1 tree.  A row's value therefore
+//     depends on neither C, nor the warp that computes it, nor the grid, nor the order of the pairs;
+//   * activation exchange: the lane that holds a row's tanh stores it into the layer's activation buffer of EVERY CTA of the
+//     cluster (mapa + st.shared::cluster, its own included), then the cluster meets at barrier.cluster.arrive.release /
+//     wait.acquire.  Every layer has its own buffer (the input x, a_0 .. a_{L-1}, the last being the action), so that one
+//     barrier per layer (B_0 .. B_{L-1} of a step) orders all remote writes:
+//       - write-after-read: a_l is read by layer l + 1 of step t before the reader arrives at B_{l+1}(t) (for the action
+//         a_{L-1}: by the env step and the reward of step t, before the reader arrives at B_0(t + 1)); the next write of a_l
+//         comes from layer l of step t + 1, after the writer waited at B_{L-1}(t) >= B_{l+1}(t) (for the action: after it
+//         waited at B_0(t + 1), which precedes layer L - 1 because L >= 3).  With a single buffer the write of layer l + 1
+//         would race with the peers' reads of layer l, and a second barrier per layer would be needed;
+//       - read-after-write: the release / acquire pair of B_l orders every store of layer l before every read of layer l + 1;
+//   * env step: every CTA computes the whole step redundantly (thread i < obs owns observation i; A's diagonals and B in its
+//     own shared memory, the raw observation double buffered with a wrap-around halo), so the next input x needs no exchange,
+//     only a __syncthreads.  Rank 0's last warp (idle in the env step: obs <= 384 < 480) forms the reward and the position,
+//     and rank 0 keeps the ObStat column sums and writes the results;
+//   * other cluster barriers: START after the buffers are zeroed and before the first remote store (a peer's shared memory
+//     may only be written once that CTA runs), and REUSE at the end of every evaluation, before the cluster reloads its
+//     weights and restarts its buffers for the next one; the last REUSE is the EXIT barrier, so no CTA exits while a peer
+//     might still store into its shared memory;
+//   * arithmetic on float32 CUDA cores: each weight matrix meets one activation column per step, so a wgmma (N >= 8) would
+//     run at most 1/8 full.
+// Alternatives not built (so not measured): weights partly in registers (rollout_closed.cu's layer 1), and a pair (both signs)
+// per cluster, which doubles the footprint to save only the load-time reads of eps.
+#include <math.h>
+#include "common.cuh"
+#include "mt19937.cuh"
+
+namespace {
+
+constexpr int CW_THREADS = 512;
+constexpr int CW_WARPS = CW_THREADS / 32;
+constexpr int CW_MAX_LAYERS = 5;           // 2 to 4 hidden layers
+constexpr int CW_MAX_WIDTH = 256;
+constexpr int CW_MAX_OBS = 384;
+constexpr int CW_MAX_ACT = 64;
+constexpr int CW_HALO = 16;                // band <= 16
+constexpr int CW_SMEM_MAX = 227 * 1024 - 1024;    // dynamic shared memory per CTA: 227 KiB less 1 KiB for the static cw_layers
+
+struct CwParams {
+    const float* table; long long table_len; const int64_t* idx; int n_pairs;
+    const float* theta; float sigma;
+    int n_layers, T, n_params;
+    int dims[CW_MAX_LAYERS + 1];
+    int woff[CW_MAX_LAYERS], boff[CW_MAX_LAYERS];     // flat offsets of W_l [d_{l+1}][d_l] and b_l
+    const double* ob_mean; const double* ob_std; double ob_clip;
+    const float* obs0; const float* env_a; const float* env_b; int band;
+    const float* crew; float pos_scale;
+    const uint32_t* coins; double chance;
+    double* fit_pos; double* fit_neg; int fit_stride;
+    float* behv_pos; float* behv_neg;
+    double* ob_sum; double* ob_sumsq; double* ob_count;
+    int* err;
+};
+
+__host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
+__host__ __device__ inline int cw_pad4(int n) { return (n + 3) & ~3; }
+
+struct CwLayout {                          // offsets in floats into dynamic shared memory (all multiples of 4)
+    int norm, racc, x, prod, stat, o2, o2_stride, env_a, env_b, total;
+    int act[CW_MAX_LAYERS], w[CW_MAX_LAYERS], bias[CW_MAX_LAYERS], rows[CW_MAX_LAYERS], stride[CW_MAX_LAYERS];
+};
+__host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int C, int band) {
+    CwLayout L;
+    const int obs = dims[0], act = dims[n_layers];
+    int at = 0;
+    L.norm = at; at += 4 * obs;                            // double mean[obs], double std[obs]  (first: 8-byte aligned)
+    L.racc = at; at += 8;                                  // double fitness, float position[3]
+    L.x = at; at += cw_pad32(obs);                         // the normalised observation, zero padded
+    for (int l = 0; l < n_layers; ++l) { L.act[l] = at; at += cw_pad32(dims[l + 1]); }    // a_l, zero padded
+    for (int l = 0; l < n_layers; ++l) {
+        L.rows[l] = (dims[l + 1] + C - 1) / C;
+        L.stride[l] = cw_pad32(dims[l]);
+        L.w[l] = at; at += cw_pad4(L.rows[l]) * L.stride[l];
+        L.bias[l] = at; at += cw_pad4(L.rows[l]);
+    }
+    L.prod = at; at += cw_pad4(act);
+    L.stat = at; at += 2 * obs;                            // float2 (sum, sumsq) of the post-step observations
+    L.o2_stride = cw_pad4(obs + CW_HALO);
+    L.o2 = at; at += 2 * L.o2_stride;                      // [2 buffers] raw observations with halo
+    L.env_a = at; at += cw_pad4(band * obs);
+    L.env_b = at; at += cw_pad4(act * obs);
+    L.total = at;
+    return L;
+}
+
+__device__ __forceinline__ float cw_normalise(float o, double mean, double std, double clip) {
+    double x = ((double)o - mean) / std;
+    x = fmin(fmax(x, -clip), clip);
+    return (float)x;
+}
+// rollout_closed.cu's cl_tanh: tanh(x) = 1 - 2 / (1 + e^2x) with the fast exponential and division, absolute error ~1e-7
+__device__ __forceinline__ float cw_tanh(float x) {
+    const float e = __expf(2.f * x);
+    return 1.f - __fdividef(2.f, 1.f + e);
+}
+// the warp-wide sums of v[0..3] in 7 shuffles (transposing butterfly, the xor-16, 8, 4, 2, 1 tree for every row): lane L
+// returns the sum over the lanes of v[L / 8]
+__device__ __forceinline__ float cw_warp_sum4(const float (&v)[4], int lane) {
+    const bool h16 = lane & 16, h8 = lane & 8;
+    float a[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) a[i] = (h16 ? v[i + 2] : v[i]) + __shfl_xor_sync(0xffffffffu, h16 ? v[i] : v[i + 2], 16);
+    float c = (h8 ? a[1] : a[0]) + __shfl_xor_sync(0xffffffffu, h8 ? a[0] : a[1], 8);
+    c += __shfl_xor_sync(0xffffffffu, c, 4);
+    c += __shfl_xor_sync(0xffffffffu, c, 2);
+    c += __shfl_xor_sync(0xffffffffu, c, 1);
+    return c;
+}
+// all threads of all CTAs of the cluster; orders every earlier shared-memory access (local and remote) before every later one
+__device__ __forceinline__ void cw_cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ unsigned cw_cluster_rank() {
+    unsigned r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ unsigned cw_cluster_nctas() {
+    unsigned r;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+    return r;
+}
+// v into the same shared-memory word of CTA `rank` of the cluster
+__device__ __forceinline__ void cw_store_remote(float* local, unsigned rank, float v) {
+    const unsigned a = (unsigned)__cvta_generic_to_shared(local);
+    unsigned r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(r), "f"(v) : "memory");
+}
+
+// one layer of this CTA in the step loop (read from shared memory: a per-layer index into registers would go to local memory)
+struct CwLayer { int in, nr, S, r0, w, bias, xin, out, woff, boff; };
+
+template <int NL>
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) {
+    extern __shared__ __align__(16) float cw_smem[];
+    __shared__ CwLayer cw_layers[NL];
+    const unsigned C = cw_cluster_nctas(), rank = cw_cluster_rank();
+    const int n_clusters = gridDim.x / C, cluster = blockIdx.x / C;
+    const int obs = p.dims[0], act = p.dims[NL], T = p.T, band = p.band, half = p.band >> 1;
+    const CwLayout L = cw_layout(NL, p.dims, (int)C, band);
+    double* __restrict__ nmean = reinterpret_cast<double*>(cw_smem + L.norm);
+    double* __restrict__ nstd = nmean + obs;
+    double* __restrict__ rfit = reinterpret_cast<double*>(cw_smem + L.racc);
+    float* __restrict__ rpos = cw_smem + L.racc + 2;
+    float* __restrict__ x = cw_smem + L.x;
+    float* __restrict__ prod = cw_smem + L.prod;
+    float2* __restrict__ stat = reinterpret_cast<float2*>(cw_smem + L.stat);
+    float* __restrict__ o2 = cw_smem + L.o2;
+    const float* __restrict__ envA = cw_smem + L.env_a;
+    const float* __restrict__ envB = cw_smem + L.env_b;
+    const float* __restrict__ action = cw_smem + L.act[NL - 1];
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const bool rew_warp = rank == 0 && warp == CW_WARPS - 1;
+
+    for (int i = tid; i < band * obs; i += CW_THREADS) cw_smem[L.env_a + i] = p.env_a[i];
+    for (int i = tid; i < act * obs; i += CW_THREADS) cw_smem[L.env_b + i] = p.env_b[i];
+    for (int i = tid; i < obs; i += CW_THREADS) { nmean[i] = p.ob_mean[i]; nstd[i] = p.ob_std[i]; }
+    for (int i = tid; i < L.w[0] - L.x; i += CW_THREADS) cw_smem[L.x + i] = 0.f;     // x and every a_l, padding included
+    if (tid == 0) {
+#pragma unroll
+        for (int l = 0; l < NL; ++l) {                      // this CTA owns rows [r0, r0 + nr) of layer l (nr may be <= 0)
+            const int r0 = (int)rank * L.rows[l];
+            cw_layers[l] = {p.dims[l], min(L.rows[l], p.dims[l + 1] - r0), L.stride[l], r0, L.w[l], L.bias[l],
+                            l ? L.act[l - 1] : L.x, L.act[l], p.woff[l], p.boff[l]};
+        }
+    }
+    cw_cluster_sync();                                      // START: every CTA of the cluster runs and has zeroed its buffers
+
+    auto put_obs = [&](float* __restrict__ buf, int i, float v) {   // slot q = k + half for k in [-half, obs + band - half)
+        buf[i + half] = v;
+        if (i >= obs - half) buf[i - obs + half] = v;
+        if (i < band - half) buf[i + obs + half] = v;
+    };
+
+    for (int ev = cluster; ev < 2 * p.n_pairs; ev += n_clusters) {
+        const int pair = ev >> 1, neg = ev & 1;
+        const long long base = es_checked_slice(p.idx[pair], p.n_params, p.table_len, p.err);
+        const float* __restrict__ eps = p.table + base;
+        const float* __restrict__ th = p.theta;
+        const float sg = p.sigma;
+        auto w_at = [&](int at) {                           // theta + sigma eps or theta - sigma eps
+            float wp, wm;
+            es_pheno_pm(sg, eps[at], th[at], wp, wm);
+            return neg ? wm : wp;
+        };
+#pragma unroll 1
+        for (int l = 0; l < NL; ++l) {                      // this CTA's rows of every layer, zero padded to a multiple of 4
+            const CwLayer ly = cw_layers[l];
+            const int R4 = cw_pad4(max(ly.nr, 0)), in = ly.in, S = ly.S;
+            float* __restrict__ W = cw_smem + ly.w;
+            for (int r = warp; r < R4; r += CW_WARPS)
+                for (int k = lane; k < S; k += 32)
+                    W[r * S + k] = (r < ly.nr && k < in) ? w_at(ly.woff + (ly.r0 + r) * in + k) : 0.f;
+            for (int r = tid; r < R4; r += CW_THREADS) cw_smem[ly.bias + r] = r < ly.nr ? w_at(ly.boff + ly.r0 + r) : 0.f;
+        }
+        for (int i = tid; i < obs; i += CW_THREADS) {
+            const float v = p.obs0[i];
+            put_obs(o2, i, v);
+            x[i] = cw_normalise(v, nmean[i], nstd[i], p.ob_clip);
+            stat[i] = make_float2(0.f, 0.f);
+        }
+        if (tid == 0) { rfit[0] = 0.0; rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
+        bool save = false;                                  // the evaluation's save_obs coin (legacy random_sample < chance)
+        if (p.coins) {
+            const uint32_t* c = p.coins + (size_t)pair * 4 + 2 * neg;
+            save = mt19937_random_sample(c[0], c[1]) < p.chance;
+        }
+        const bool keep_stat = rank == 0 && p.ob_sum && save;
+        __syncthreads();
+
+        for (int t = 0; t < T; ++t) {
+            const int cur = t & 1;
+            float crow0 = 0.f, crow1 = 0.f;
+            if (rew_warp) {                                 // this step's reward coefficients: in flight under the layers
+                const float* __restrict__ c = p.crew + (size_t)t * act;
+                if (lane < act) crow0 = __ldg(c + lane);
+                if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
+            }
+            // ---- the layers: 4 rows per warp and pass, each row's tanh stored into every CTA's a_l, then B_l ----
+#pragma unroll 1
+            for (int l = 0; l < NL; ++l) {
+                const CwLayer ly = cw_layers[l];
+                const int S = ly.S, r0 = ly.r0, nr = ly.nr, nj = S >> 5;
+                const float* __restrict__ xin = cw_smem + ly.xin + lane;
+                const float* __restrict__ W = cw_smem + ly.w + lane;
+                const float* __restrict__ bias = cw_smem + ly.bias;
+                float* __restrict__ out = cw_smem + ly.out;
+                for (int g = 4 * warp; g < nr; g += 4 * CW_WARPS) {
+                    float z[4] = {0.f, 0.f, 0.f, 0.f};
+                    const float* __restrict__ wr = W + g * S;
+#pragma unroll 4
+                    for (int j = 0; j < nj; ++j) {
+                        const float xv = xin[32 * j];
+#pragma unroll
+                        for (int r = 0; r < 4; ++r) z[r] = fmaf(wr[r * S + 32 * j], xv, z[r]);
+                    }
+                    const float s = cw_warp_sum4(z, lane);
+                    const int r = g + (lane >> 3);
+                    if ((lane & 7) == 0 && r < nr) {
+                        const float y = cw_tanh(s + bias[r]);
+                        for (unsigned q = 0; q < C; ++q) cw_store_remote(out + r0 + r, q, y);
+                    }
+                }
+                cw_cluster_sync();                          // B_l
+            }
+            // ---- env step, redundantly in every CTA: thread i owns observation i ----
+            if (tid < obs) {
+                const float* __restrict__ oc = o2 + cur * L.o2_stride;
+                const int i = tid;
+                float acc = 0.f;
+                for (int d = 0; d < band; ++d) acc = __fadd_rn(acc, __fmul_rn(envA[d * obs + i], oc[i + d]));
+                for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, __fmul_rn(envB[j * obs + i], action[j]));
+                const float nv = cw_tanh(acc);
+                put_obs(o2 + (cur ^ 1) * L.o2_stride, i, nv);
+                x[i] = cw_normalise(nv, nmean[i], nstd[i], p.ob_clip);
+                if (keep_stat) {                            // float32 column sums in step order (numpy's axis-0 reduction)
+                    float2 st = stat[i];
+                    st.x = __fadd_rn(st.x, nv); st.y = __fadd_rn(st.y, __fmul_rn(nv, nv));
+                    stat[i] = st;
+                }
+            }
+            // ---- reward (float32 dot in index order, summed in float64) and position: rank 0's last warp ----
+            if (rew_warp) {
+                if (lane < act) prod[lane] = __fmul_rn(action[lane], crow0);
+                if (lane + 32 < act) prod[lane + 32] = __fmul_rn(action[lane + 32], crow1);
+                __syncwarp();
+                if (lane == 0) {
+                    float acc = 0.f;
+                    for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, prod[j]);
+                    rfit[0] += (double)acc;
+                    const float ps = p.pos_scale;
+                    rpos[0] = __fadd_rn(rpos[0], __fmul_rn(ps, action[0]));
+                    rpos[1] = __fadd_rn(rpos[1], __fmul_rn(ps, action[1 % act]));
+                    rpos[2] = __fadd_rn(rpos[2], __fmul_rn(ps, action[2 % act]));
+                }
+                __syncwarp();
+            }
+            __syncthreads();                                // x and the raw observation before the next step's layer 0
+        }
+        if (rew_warp && lane == 0) {
+            (neg ? p.fit_neg : p.fit_pos)[(size_t)pair * p.fit_stride] = rfit[0];
+            float* bv = neg ? p.behv_neg : p.behv_pos;
+            if (bv) { bv[(size_t)pair * 3 + 0] = rpos[0]; bv[(size_t)pair * 3 + 1] = rpos[1]; bv[(size_t)pair * 3 + 2] = rpos[2]; }
+        }
+        if (keep_stat) {
+            // ObStat.inc of a saved rollout: float32 column sums added in float64 (the order over rollouts is the atomics')
+            for (int i = tid; i < obs; i += CW_THREADS) {
+                const float2 st = stat[i];
+                atomicAdd(p.ob_sum + i, (double)st.x);
+                atomicAdd(p.ob_sumsq + i, (double)st.y);
+            }
+            if (tid == 0) { atomicAdd(p.ob_count, (double)T); atomicAdd(p.ob_count + 1, 1.0); }
+        }
+        cw_cluster_sync();                                  // REUSE (the last one: EXIT)
+    }
+}
+
+}  // namespace
+
+// the smallest cluster size that holds the shape, its shared memory per CTA, or an error message; no device work
+int es_closedw_plan(const int* dims, int n_layers, int band, int* cluster_size, size_t* smem_bytes) {
+    const int obs = dims[0], act = dims[n_layers];
+    if (n_layers < 3 || n_layers > CW_MAX_LAYERS) {
+        es_set_error("es_rollout_closedloop_mlp: 2 to 4 hidden layers (n_layers 3 to %d) supported, got n_layers %d", CW_MAX_LAYERS,
+                     n_layers);
+        return ES_ERR_UNSUPPORTED;
+    }
+    for (int l = 1; l < n_layers; ++l)
+        if (dims[l] > CW_MAX_WIDTH) {
+            es_set_error("es_rollout_closedloop_mlp: hidden widths up to %d supported, hidden layer %d has %d", CW_MAX_WIDTH, l, dims[l]);
+            return ES_ERR_UNSUPPORTED;
+        }
+    if (obs > CW_MAX_OBS || act > CW_MAX_ACT) {
+        es_set_error("es_rollout_closedloop_mlp: obs <= %d and act <= %d supported, got obs %d, act %d", CW_MAX_OBS, CW_MAX_ACT, obs, act);
+        return ES_ERR_UNSUPPORTED;
+    }
+    if ((band & 1) || band > CW_HALO || band > obs) {
+        es_set_error("es_rollout_closedloop_mlp: the band must be even, <= %d and <= obs (got band %d, obs %d)", CW_HALO, band, obs);
+        return ES_ERR_UNSUPPORTED;
+    }
+    size_t bytes = 0;
+    for (int C = 1; C <= 8; C *= 2) {
+        bytes = (size_t)cw_layout(n_layers, dims, C, band).total * sizeof(float);
+        if (bytes <= (size_t)CW_SMEM_MAX) {
+            *cluster_size = C;
+            *smem_bytes = bytes;
+            return ES_OK;
+        }
+    }
+    es_set_error("es_rollout_closedloop_mlp: the weights and env matrices need %zu bytes of shared memory per CTA in a cluster of "
+                 "8 CTAs, %d available", bytes, CW_SMEM_MAX);
+    return ES_ERR_UNSUPPORTED;
+}
+
+typedef void (*CwKernel)(const CwParams);
+static CwKernel cw_kernel(int n_layers) {
+    return n_layers == 3 ? rollout_closedw_kernel<3> : n_layers == 4 ? rollout_closedw_kernel<4> : rollout_closedw_kernel<5>;
+}
+// a launch of `clusters` clusters of C CTAs (attr: the cluster-dimension attribute the config points to)
+static cudaLaunchConfig_t cw_config(int C, size_t smem, int clusters, cudaStream_t stream, cudaLaunchAttribute* attr) {
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = C; attr->val.clusterDim.y = 1; attr->val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(clusters * C); cfg.blockDim = dim3(CW_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    return cfg;
+}
+
+// the number of clusters of the shape that can be resident at once (the persistent grid), 0 when none fits
+int es_closedw_max_clusters(int n_layers, int C, size_t smem, int* clusters) {
+    const CwKernel k = cw_kernel(n_layers);
+    ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = cw_config(C, smem, 1, nullptr, &attr);
+    ES_CHECK_CUDA(cudaOccupancyMaxActiveClusters(clusters, k, &cfg));
+    return ES_OK;
+}
+
+int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {
+    int C = 0, max_clusters = 0;
+    size_t smem = 0;
+    int rc = es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
+    if (rc) return rc;
+    rc = es_closedw_max_clusters(r.n_layers, C, smem, &max_clusters);
+    if (rc) return rc;
+    if (max_clusters < 1) {
+        es_set_error("es_rollout_closedloop_mlp: no cluster of %d CTAs with %zu bytes of shared memory each fits on this device", C, smem);
+        return ES_ERR_UNSUPPORTED;
+    }
+    CwParams p;
+    p.table = r.table; p.table_len = r.table_len; p.idx = r.idx; p.n_pairs = r.n_pairs; p.theta = r.theta; p.sigma = r.sigma;
+    p.n_layers = r.n_layers; p.T = r.T; p.n_params = r.P;
+    int at = 0;
+    for (int l = 0; l <= r.n_layers; ++l) p.dims[l] = r.layer_sizes[l];
+    for (int l = 0; l < r.n_layers; ++l) {                 // state-dict order: W_l [out][in], then b_l
+        p.woff[l] = at; at += p.dims[l] * p.dims[l + 1];
+        p.boff[l] = at; at += p.dims[l + 1];
+    }
+    p.ob_mean = env.ob_mean; p.ob_std = env.ob_std; p.ob_clip = env.ob_clip;
+    p.obs0 = env.obs0; p.env_a = env.env_a; p.env_b = env.env_b; p.band = env.band; p.crew = r.rew_vec; p.pos_scale = r.pos_scale;
+    p.coins = env.coins; p.chance = env.save_obs_chance;
+    p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.fit_stride = r.fit_stride; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
+    p.ob_sum = env.ob_sum; p.ob_sumsq = env.ob_sumsq; p.ob_count = env.ob_count;
+    p.err = r.err;
+    const long long evals = 2ll * r.n_pairs;
+    const int clusters = evals < max_clusters ? (int)evals : max_clusters;
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = cw_config(C, smem, clusters, stream, &attr);
+    ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cw_kernel(r.n_layers), p));
+    ES_LAUNCHED(ctx);
+    return ES_OK;
+}

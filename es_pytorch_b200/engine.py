@@ -342,6 +342,48 @@ class Engine:
                                              int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq),
                                              _ptr(ob_count), self.stream), 'es_rollout_closedloop')
 
+    def rollout_closed_mlp(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
+                           obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,
+                           behv_neg=None, coin_words=None, save_obs_chance: float = 0.0, ob_sum=None, ob_sumsq=None, ob_count=None):
+        """``rollout_closed`` (same arguments and checks) for every tanh MLP the closed loop covers: 2 to 4 hidden layers of
+        at most 256 units, obs <= 384, act <= 64.  The shapes ``rollout_closed`` takes run its kernel; the others one
+        thread-block cluster per evaluation (``closed_mlp_plan``)."""
+        d = self.device
+        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
+        _req(ob_mean, torch.float64, 'ob_mean', d); _req(ob_std, torch.float64, 'ob_std', d)
+        _req(obs0, torch.float32, 'obs0', d); _req(env_a, torch.float32, 'env_a', d); _req(env_b, torch.float32, 'env_b', d)
+        _req(rew_vec, torch.float32, 'rew_vec', d)
+        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
+        n, T, obs, act = idx.numel(), rew_vec.shape[0], int(layer_sizes[0]), int(layer_sizes[-1])
+        band = env_a.shape[0]
+        assert env_a.shape == (band, obs) and env_b.shape == (act, obs) and obs0.numel() == obs and rew_vec.shape == (T, act)
+        assert ob_mean.numel() == obs and ob_std.numel() == obs
+        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
+        if behv_pos is not None:
+            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
+            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
+        if coin_words is not None:
+            assert coin_words.dtype == torch.int32 and coin_words.numel() == 4 * n and coin_words.is_contiguous()
+        if ob_sum is not None:
+            _req(ob_sum, torch.float64, 'ob_sum', d); _req(ob_sumsq, torch.float64, 'ob_sumsq', d); _req(ob_count, torch.float64, 'ob_count', d)
+            assert ob_sum.numel() == obs and ob_sumsq.numel() == obs and ob_count.numel() == 2
+        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+        check(self.lib.es_rollout_closedloop_mlp(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
+                                                 float(sigma), ls, len(layer_sizes) - 1, _ptr(ob_mean), _ptr(ob_std), float(ob_clip),
+                                                 _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T, float(pos_scale),
+                                                 _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg),
+                                                 int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq),
+                                                 _ptr(ob_count), self.stream), 'es_rollout_closedloop_mlp')
+
+    def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int):
+        """How ``rollout_closed_mlp`` runs a shape: (CTAs per cluster, clusters resident at once, shared memory bytes per CTA);
+        (0, SM count, 0) for ``rollout_closed``'s one-CTA kernel.  Raises EsLibraryError for a shape it does not cover."""
+        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+        cs, nc, sm = C.c_int(0), C.c_int(0), C.c_int64(0)
+        check(self.lib.es_rollout_closedloop_mlp_plan(self._ctx, ls, len(layer_sizes) - 1, int(band), C.byref(cs), C.byref(nc),
+                                                      C.byref(sm)), 'es_rollout_closedloop_mlp_plan')
+        return cs.value, nc.value, sm.value
+
     # ------------------------------------------------------------------ a13
     def novelty(self, behv, archive, k: int, out, out_stride: int = 1):
         d = self.device

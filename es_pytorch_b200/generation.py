@@ -74,7 +74,7 @@ class DeviceGeneration:
                  engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1):
         self.eng = engine or get_engine()
         # closed-loop variant of the synthetic env (gym.synthetic_env.ClosedLoopEnv): (obs_0 [obs], A^T [band, obs], B^T [act, obs]);
-        # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop
+        # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop_mlp
         self.closed = closed
         self.ranker = ranker                            # a utils.rankers.Ranker; None = Centered / MultiObjective(moo_w)
         e = self.eng
@@ -212,13 +212,13 @@ class DeviceGeneration:
             self._gen_stats.zero_()
             obs0, env_a, env_b = self.closed
             with self._timed('rollout'):
-                e.rollout_closed(self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.ob_mean, self.ob_std,
-                                 self.ob_clip, obs0, env_a, env_b, self.rew_vec, self.pos_scale, fp, fn, self.n_obj,
-                                 None if self.behv is None else self.behv[0], None if self.behv is None else self.behv[1],
-                                 coin_words=self.extras if self.extra_words else None, save_obs_chance=self.save_obs_chance,
-                                 ob_sum=self.gen_sum if self.extra_words else None,
-                                 ob_sumsq=self.gen_sumsq if self.extra_words else None,
-                                 ob_count=self.gen_count if self.extra_words else None)
+                e.rollout_closed_mlp(self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.ob_mean, self.ob_std,
+                                     self.ob_clip, obs0, env_a, env_b, self.rew_vec, self.pos_scale, fp, fn, self.n_obj,
+                                     None if self.behv is None else self.behv[0], None if self.behv is None else self.behv[1],
+                                     coin_words=self.extras if self.extra_words else None, save_obs_chance=self.save_obs_chance,
+                                     ob_sum=self.gen_sum if self.extra_words else None,
+                                     ob_sumsq=self.gen_sumsq if self.extra_words else None,
+                                     ob_count=self.gen_count if self.extra_words else None)
             if self.n_obj == 2:
                 e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
         else:
@@ -309,8 +309,9 @@ class DeviceGeneration:
         fit0, behv0, idx0 = self._nl_bufs
         if self.closed is not None:
             obs0, env_a, env_b = self.closed
-            e.rollout_closed(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip, obs0,
-                             env_a, env_b, self.rew_vec, self.pos_scale, fit0[0:1], fit0[1:2], 1, behv0[0].view(-1), behv0[1].view(-1))
+            e.rollout_closed_mlp(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,
+                                 obs0, env_a, env_b, self.rew_vec, self.pos_scale, fit0[0:1], fit0[1:2], 1, behv0[0].view(-1),
+                                 behv0[1].view(-1))
             return fit0, behv0
         e.rollout(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.obsn, self.rew_vec, self.pos_scale,
                   fit0[0:1], fit0[1:2], 1, behv0[0].view(-1), behv0[1].view(-1), ES_ROLLOUT_F32)

@@ -79,7 +79,7 @@ class BatchedRollout:
                     rs.random()
         noise_rs = streams[0] if (use_ac_noise and streams is not None and len(streams)) else None
         closed = getattr(self.env, 'is_synthetic_closedloop', False)
-        if (closed and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp() and len(model.layer_sizes()) == 4
+        if (closed and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp() and self._closed_on_device(model.layer_sizes())
                 and not (noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0)):
             # the closed-loop episode as one launch (the observations are not returned: this result never carries them)
             from .gym_runner import _device_episode_closed
@@ -94,6 +94,22 @@ class BatchedRollout:
         if self.archive is None:
             return RewardResult(rews, behv, no_obs, steps)
         return NSRResult(rews, behv[-3:], no_obs, steps, self.archive, self.nov_k)
+
+    def _closed_on_device(self, sizes) -> bool:
+        """Whether a closed-loop episode of a tanh MLP runs as one launch (es_rollout_closedloop_mlp): two hidden layers always
+        do (a shape outside the kernels' coverage raises there); three or four when the kernels cover the shape; anything else
+        runs run_model's python loop."""
+        n_hidden = len(sizes) - 2
+        if n_hidden == 2:
+            return True
+        if n_hidden not in (3, 4):
+            return False
+        from ..engine import get_engine
+        try:
+            get_engine().closed_mlp_plan(sizes, self.env.band)
+        except _lib.EsLibraryError:
+            return False
+        return True
 
     def _run_episodes(self, model, rs, episodes: int):
         """obj.py:57-60 with action noise: ``episodes`` runs of run_model drawing from ``rs``, rewards summed per step in

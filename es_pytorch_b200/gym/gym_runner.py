@@ -69,7 +69,7 @@ def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
 
 
 def _device_episode_closed(model, env, max_steps: int):
-    """One noise-free episode on the closed-loop synthetic env as one launch of es_rollout_closedloop (sigma = 0)."""
+    """One noise-free episode on the closed-loop synthetic env as one launch of es_rollout_closedloop_mlp (sigma = 0)."""
     from ..engine import get_engine
     from ..core.policy import Policy
     eng = get_engine()
@@ -84,8 +84,8 @@ def _device_episode_closed(model, env, max_steps: int):
     idx = torch.zeros(1, dtype=torch.int64, device=eng.device)
     fit = torch.zeros(2, dtype=torch.float64, device=eng.device)
     behv = torch.zeros(2, 3, dtype=torch.float32, device=eng.device)
-    eng.rollout_closed(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), obs0, env_a, env_b, rew_dev[:T].contiguous(),
-                       env.pos_scale, fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1))
+    eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), obs0, env_a, env_b,
+                           rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1))
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 

@@ -161,6 +161,29 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
                           double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
                           double* ob_sum, double* ob_sumsq, double* ob_count, void* stream);
 
+/* The same rollout for every tanh MLP the closed loop covers, including the shipped configs' wide policies: the parameter
+ * list, arrays and semantics of es_rollout_closedloop, for layer_sizes [n_layers + 1] with
+ *   n_layers 3 to 5 (2 to 4 hidden layers), every hidden width in [1, 256], obs <= 384, act <= 64,
+ *   an even band <= 16 and <= obs, and the shape's weights and env matrices within a cluster of 8 CTAs' shared memory.
+ * Anything else returns ES_ERR_UNSUPPORTED (es_last_error() names the limit; for the cluster budget, the bytes needed per CTA)
+ * whatever n_pairs is.  The shapes es_rollout_closedloop covers (two hidden layers <= 64) run its kernel, bit for bit its
+ * results; every other covered shape runs rollout_closedw.cu: one thread-block cluster of 1, 2, 4 or 8 CTAs per evaluation
+ * holds the weights across its SMs and exchanges each layer's activations through distributed shared memory.  An evaluation's
+ * result depends neither on the cluster size nor on the grid or the order of the pairs.  One kernel launch per call.      */
+int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                              const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                              const double* ob_mean, const double* ob_std, double ob_clip,
+                              const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec, int T,
+                              float pos_scale, const uint32_t* coin_words, double save_obs_chance,
+                              double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                              double* ob_sum, double* ob_sumsq, double* ob_count, void* stream);
+
+/* How es_rollout_closedloop_mlp runs a shape, without running it: cluster_size 0 for es_rollout_closedloop's one-CTA kernel
+ * (clusters = the SM count, smem_bytes = 0), else the CTAs per cluster, the clusters resident at once (the persistent grid)
+ * and the dynamic shared memory per CTA.  ES_ERR_UNSUPPORTED with es_rollout_closedloop_mlp's message for an uncovered shape. */
+int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int* cluster_size, int* clusters,
+                                   int64_t* smem_bytes);
+
 /* ---- a2 + a4 with action noise: all draws of a generation in stream order ---------------------------------------------
  * When FeedForward._action_std != 0 every step of every rollout draws rs.randn(act_dim) from the SAME RandomState that
  * draws the noise indices and the save_obs coins (src/nn/nn.py:47-48, src/core/es.py:66-72, simple_example.py:37-40).  Per
