@@ -272,6 +272,64 @@ int es_rollout_openloop(es_ctx* ctx, const float* table, int64_t table_len, cons
                                      pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, mode, stream);
 }
 
+// the head arguments of the binned entry points: bins >= 2 (the reference divides by bins - 1), low / range set, the last layer
+// adim * bins <= 256 wide
+static int es_binned_check(const char* fn, const int* layer_sizes, int n_layers, int bins, const float* low, const float* range) {
+    ES_REQUIRE(bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, bins);
+    ES_REQUIRE(low && range, "%s: NULL low / range", fn);
+    const int out = layer_sizes[n_layers];
+    ES_REQUIRE(out % bins == 0, "%s: the last layer's %d outputs are not adim * bins for bins %d", fn, out, bins);
+    if (out > 256) {
+        es_set_error("%s: binned heads up to adim * bins = 256 outputs supported, got %d * %d", fn, out / bins, bins);
+        return ES_ERR_UNSUPPORTED;
+    }
+    return ES_OK;
+}
+
+int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                               const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
+                               const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
+                               float* behv_pos, float* behv_neg, int bins, const float* low, const float* range, int mode,
+                               void* stream) {
+    ES_ENTER(ctx);
+    EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
+                   fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
+    int rc = es_rollout_check("es_rollout_openloop_binned", obsn != nullptr, r);
+    if (rc) return rc;
+    rc = es_binned_check("es_rollout_openloop_binned", layer_sizes, n_layers, bins, low, range);
+    if (rc) return rc;
+    if (mode == ES_ROLLOUT_TC) {
+        es_set_error("es_rollout_openloop_binned: ES_ROLLOUT_TC refuses binned heads: an arg-max over float16-grade outputs is not "
+                     "parity grade; use ES_ROLLOUT_TC3 or ES_ROLLOUT_F32");
+        return ES_ERR_UNSUPPORTED;
+    }
+    if (mode == ES_ROLLOUT_TC3 && !es_tcw_covers_binned(r)) {
+        char why[96];                               // the part of the shape outside the coverage
+        if (n_layers < 3 || n_layers > 5) {
+            snprintf(why, sizeof why, "%d hidden layers", n_layers - 1);
+        } else if (layer_sizes[0] > 256) {
+            snprintf(why, sizeof why, "obs %d", layer_sizes[0]);
+        } else {
+            snprintf(why, sizeof why, "the shape");
+            for (int l = 1; l < n_layers; ++l)
+                if (layer_sizes[l] % 64 || layer_sizes[l] > 256) {
+                    snprintf(why, sizeof why, "hidden layer %d of width %d", l, layer_sizes[l]);
+                    break;
+                }
+        }
+        es_set_error("es_rollout_openloop_binned: ES_ROLLOUT_TC3 covers binned heads with 2 to 4 hidden layers of widths in {64, 128, "
+                     "192, 256} and obs <= 256, got %s; use ES_ROLLOUT_F32", why);
+        return ES_ERR_UNSUPPORTED;
+    }
+    if (mode != ES_ROLLOUT_F32 && mode != ES_ROLLOUT_TC3) {
+        es_set_error("es_rollout_openloop_binned: unknown mode %d", mode);
+        return ES_ERR_INVALID;
+    }
+    if (n_pairs == 0) return ES_OK;
+    if (mode == ES_ROLLOUT_TC3) return es_impl_rollout_tcw(ctx, r, 1, (cudaStream_t)stream);
+    return es_impl_rollout_f32(ctx, r, (cudaStream_t)stream);
+}
+
 int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
                           int P, float sigma, const int* layer_sizes, int n_layers, const double* ob_mean, const double* ob_std,
                           double ob_clip, const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
@@ -340,6 +398,50 @@ int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len
     if (n_pairs == 0) return ES_OK;
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
     if (es_closed_one_cta_covers(layer_sizes, n_layers)) return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
+    return es_impl_rollout_closedw(ctx, r, env, (cudaStream_t)stream);
+}
+
+int es_rollout_closedloop_mlp_binned_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size,
+                                          int* clusters, int64_t* smem_bytes) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_closedloop_mlp_binned_plan";
+    ES_REQUIRE(layer_sizes && cluster_size && clusters && smem_bytes, "%s: NULL pointer", fn);
+    ES_REQUIRE(n_layers >= 1 && n_layers <= ES_MAX_LAYERS, "%s: n_layers must be in [1,%d]", fn, ES_MAX_LAYERS);
+    for (int l = 0; l <= n_layers; ++l) ES_REQUIRE(layer_sizes[l] > 0, "%s: layer size <= 0", fn);
+    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
+    ES_REQUIRE(bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, bins);
+    int C = 0;
+    size_t smem = 0;
+    const int rc = es_closedw_binned_plan(layer_sizes, n_layers, band, bins, &C, &smem);
+    if (rc) return rc;
+    *cluster_size = C; *smem_bytes = (int64_t)smem;
+    return es_closedw_binned_max_clusters(n_layers, C, smem, clusters);
+}
+
+int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                     const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const double* ob_mean,
+                                     const double* ob_std, double ob_clip, const float* obs0, const float* env_a, int band,
+                                     const float* env_b, const float* rew_vec, int T, float pos_scale, const uint32_t* coin_words,
+                                     double save_obs_chance, double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos,
+                                     float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins, const float* low,
+                                     const float* range, void* stream) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_closedloop_mlp_binned";
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
+    int rc = es_rollout_check(fn, ob_mean && ob_std && obs0 && env_a && env_b, r);
+    if (rc) return rc;
+    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
+    ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
+               "%s: ob_sum/ob_sumsq/ob_count must all be set or NULL", fn);
+    rc = es_binned_check(fn, layer_sizes, n_layers, bins, low, range);
+    if (rc) return rc;
+    int C = 0;
+    size_t smem = 0;
+    rc = es_closedw_binned_plan(layer_sizes, n_layers, band, bins, &C, &smem);      // coverage does not depend on n_pairs
+    if (rc) return rc;
+    if (n_pairs == 0) return ES_OK;
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
     return es_impl_rollout_closedw(ctx, r, env, (cudaStream_t)stream);
 }
 

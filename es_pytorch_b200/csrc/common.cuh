@@ -105,6 +105,11 @@ struct EsRollout {
     const float* act_noise;     // open loop: scaled action noise [n_pairs][2][n_episodes][T][act] (mt_gauss.cu) or NULL
     int* err;                   // the ctx's error word (es_checked_slice)
     int n_episodes;             // episodes per evaluation, averaged per step (>= 1; 1 when act_noise is NULL)
+    // the policy head: bins == 0, the tanh outputs are the actions; bins >= 2, a binned-action policy (FFBinned): the last
+    // layer's adim * bins outputs become adim actions, low[j] + range[j] * (arg-max bin) / (bins - 1)
+    int bins;
+    const float* head_low;      // dev float [adim]
+    const float* head_range;    // dev float [adim]
 };
 // the closed-loop env, the observation normalisation and the ObStat increments of es_rollout_closedloop
 struct EsClosedEnv {
@@ -143,6 +148,9 @@ void es_tc2_free_shadows(es_ctx* ctx);
 // tanh MLPs with 2 to 4 hidden layers of widths in {64, 128, 192, 256}, obs <= 256, act <= 32, other than obs-64-64-act
 bool es_tcw_covers(const EsRollout&);
 int es_impl_rollout_tcw(es_ctx*, const EsRollout&, int split, cudaStream_t);
+// binned heads on ES_ROLLOUT_TC3: 2 to 4 hidden layers of widths in {64, 128, 192, 256} (obs-64-64-X included), obs <= 256,
+// adim * bins <= 256
+bool es_tcw_covers_binned(const EsRollout&);
 int es_impl_rollout_closed(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // the closed loop for tanh MLPs with 2 to 4 hidden layers of <= 256 units, obs <= 384, act <= 64, an even band <= 16, on a
 // thread-block cluster per evaluation (rollout_closedw.cu): the cluster size and shared memory per CTA of a shape (or
@@ -150,6 +158,9 @@ int es_impl_rollout_closed(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaSt
 int es_closedw_plan(const int* layer_sizes, int n_layers, int band, int* cluster_size, size_t* smem_bytes);
 int es_closedw_max_clusters(int n_layers, int cluster_size, size_t smem_bytes, int* clusters);
 int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
+// binned heads (EsRollout::bins >= 2): every shape es_closedw_plan covers with act = adim; the cluster kernel at every C
+int es_closedw_binned_plan(const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes);
+int es_closedw_binned_max_clusters(int n_layers, int cluster_size, size_t smem_bytes, int* clusters);
 // U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
 int es_launch_ubase(es_ctx*, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
                     float* ubase, cudaStream_t);

@@ -41,6 +41,12 @@
 //     might still store into its shared memory;
 //   * arithmetic on float32 CUDA cores: each weight matrix meets one activation column per step, so a wgmma (N >= 8) would
 //     run at most 1/8 full.
+// Binned-action policies (FFBinned, src/nn/nn.py:99-117; rollout_closedw_binned_kernel): the last layer has adim * bins outputs
+// and every CTA holds all of them after B_{L-1}, so each CTA forms the adim actions locally (threads j < adim: the first
+// maximal bin, as torch.argmax, mapped to low[j] + range[j] * idx / (bins - 1) in the reference's float32 operation order) into
+// a local action buffer, then a __syncthreads, before the env step.  The env's B, the reward and the position use adim.  That
+// buffer is written after B_{L-1}(t) and read within step t only, so the barrier argument above is unchanged.  Binned shapes
+// always run here (C = 1 included): rollout_closed.cu has no head.
 // Alternatives not built (so not measured): weights partly in registers (rollout_closed.cu's layer 1), and a pair (both signs)
 // per cluster, which doubles the footprint to save only the load-time reads of eps.
 #include <math.h>
@@ -72,18 +78,20 @@ struct CwParams {
     float* behv_pos; float* behv_neg;
     double* ob_sum; double* ob_sumsq; double* ob_count;
     int* err;
+    int adim, bins; float scale; const float* low; const float* range;      // binned head (rollout_closedw_binned_kernel only)
 };
 
 __host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
 __host__ __device__ inline int cw_pad4(int n) { return (n + 3) & ~3; }
 
 struct CwLayout {                          // offsets in floats into dynamic shared memory (all multiples of 4)
-    int norm, racc, x, prod, stat, o2, o2_stride, env_a, env_b, total;
+    int norm, racc, x, prod, abin, stat, o2, o2_stride, env_a, env_b, total;
     int act[CW_MAX_LAYERS], w[CW_MAX_LAYERS], bias[CW_MAX_LAYERS], rows[CW_MAX_LAYERS], stride[CW_MAX_LAYERS];
 };
-__host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int C, int band) {
+// act: the actions the env sees (dims[n_layers], or adim for a binned head, whose actions get their own buffer `abin`)
+__host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int C, int band, int act, bool binned) {
     CwLayout L;
-    const int obs = dims[0], act = dims[n_layers];
+    const int obs = dims[0];
     int at = 0;
     L.norm = at; at += 4 * obs;                            // double mean[obs], double std[obs]  (first: 8-byte aligned)
     L.racc = at; at += 8;                                  // double fitness, float position[3]
@@ -96,6 +104,7 @@ __host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int
         L.bias[l] = at; at += cw_pad4(L.rows[l]);
     }
     L.prod = at; at += cw_pad4(act);
+    L.abin = at; if (binned) at += cw_pad4(act);
     L.stat = at; at += 2 * obs;                            // float2 (sum, sumsq) of the post-step observations
     L.o2_stride = cw_pad4(obs + CW_HALO);
     L.o2 = at; at += 2 * L.o2_stride;                      // [2 buffers] raw observations with halo
@@ -103,6 +112,9 @@ __host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int
     L.env_b = at; at += cw_pad4(act * obs);
     L.total = at;
     return L;
+}
+__host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int C, int band) {
+    return cw_layout(n_layers, dims, C, band, dims[n_layers], false);
 }
 
 __device__ __forceinline__ float cw_normalise(float o, double mean, double std, double clip) {
@@ -153,14 +165,14 @@ __device__ __forceinline__ void cw_store_remote(float* local, unsigned rank, flo
 // one layer of this CTA in the step loop (read from shared memory: a per-layer index into registers would go to local memory)
 struct CwLayer { int in, nr, S, r0, w, bias, xin, out, woff, boff; };
 
-template <int NL>
-__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) {
+template <int NL, bool BINNED>
+__device__ __forceinline__ void cw_rollout(const CwParams& p) {
     extern __shared__ __align__(16) float cw_smem[];
     __shared__ CwLayer cw_layers[NL];
     const unsigned C = cw_cluster_nctas(), rank = cw_cluster_rank();
     const int n_clusters = gridDim.x / C, cluster = blockIdx.x / C;
-    const int obs = p.dims[0], act = p.dims[NL], T = p.T, band = p.band, half = p.band >> 1;
-    const CwLayout L = cw_layout(NL, p.dims, (int)C, band);
+    const int obs = p.dims[0], act = BINNED ? p.adim : p.dims[NL], T = p.T, band = p.band, half = p.band >> 1;
+    const CwLayout L = BINNED ? cw_layout(NL, p.dims, (int)C, band, act, true) : cw_layout(NL, p.dims, (int)C, band);
     double* __restrict__ nmean = reinterpret_cast<double*>(cw_smem + L.norm);
     double* __restrict__ nstd = nmean + obs;
     double* __restrict__ rfit = reinterpret_cast<double*>(cw_smem + L.racc);
@@ -171,7 +183,7 @@ __global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const Cw
     float* __restrict__ o2 = cw_smem + L.o2;
     const float* __restrict__ envA = cw_smem + L.env_a;
     const float* __restrict__ envB = cw_smem + L.env_b;
-    const float* __restrict__ action = cw_smem + L.act[NL - 1];
+    const float* __restrict__ action = cw_smem + (BINNED ? L.abin : L.act[NL - 1]);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const bool rew_warp = rank == 0 && warp == CW_WARPS - 1;
@@ -267,6 +279,20 @@ __global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const Cw
                 }
                 cw_cluster_sync();                          // B_l
             }
+            if (BINNED) {                                   // the actions from this CTA's copy of the last layer's outputs
+                if (tid < act) {
+                    const float* __restrict__ o = cw_smem + L.act[NL - 1] + tid * p.bins;
+                    int best = 0;
+                    float bv = o[0];
+                    for (int b = 1; b < p.bins && bv == bv; ++b) {      // first maximal bin; a NaN counts as the maximum
+                        const float v = o[b];
+                        if (v > bv || v != v) { bv = v; best = b; }
+                    }
+                    cw_smem[L.abin + tid] = __fadd_rn(__fmul_rn(__fmul_rn(p.scale, (float)best), __ldg(p.range + tid)),
+                                                      __ldg(p.low + tid));
+                }
+                __syncthreads();
+            }
             // ---- env step, redundantly in every CTA: thread i owns observation i ----
             if (tid < obs) {
                 const float* __restrict__ oc = o2 + cur * L.o2_stride;
@@ -319,45 +345,69 @@ __global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const Cw
     }
 }
 
+template <int NL>
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) { cw_rollout<NL, false>(p); }
+template <int NL>
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_binned_kernel(const CwParams p) { cw_rollout<NL, true>(p); }
+
 }  // namespace
 
-// the smallest cluster size that holds the shape, its shared memory per CTA, or an error message; no device work
-int es_closedw_plan(const int* dims, int n_layers, int band, int* cluster_size, size_t* smem_bytes) {
-    const int obs = dims[0], act = dims[n_layers];
+// the smallest cluster size that holds the shape (act: the env's actions; binned: a binned head), its shared memory per CTA, or
+// an error message naming `fn`; no device work
+static int cw_plan(const char* fn, const int* dims, int n_layers, int band, int act, bool binned, int* cluster_size,
+                   size_t* smem_bytes) {
+    const int obs = dims[0];
     if (n_layers < 3 || n_layers > CW_MAX_LAYERS) {
-        es_set_error("es_rollout_closedloop_mlp: 2 to 4 hidden layers (n_layers 3 to %d) supported, got n_layers %d", CW_MAX_LAYERS,
-                     n_layers);
+        es_set_error("%s: 2 to 4 hidden layers (n_layers 3 to %d) supported, got n_layers %d", fn, CW_MAX_LAYERS, n_layers);
         return ES_ERR_UNSUPPORTED;
     }
     for (int l = 1; l < n_layers; ++l)
         if (dims[l] > CW_MAX_WIDTH) {
-            es_set_error("es_rollout_closedloop_mlp: hidden widths up to %d supported, hidden layer %d has %d", CW_MAX_WIDTH, l, dims[l]);
+            es_set_error("%s: hidden widths up to %d supported, hidden layer %d has %d", fn, CW_MAX_WIDTH, l, dims[l]);
             return ES_ERR_UNSUPPORTED;
         }
     if (obs > CW_MAX_OBS || act > CW_MAX_ACT) {
-        es_set_error("es_rollout_closedloop_mlp: obs <= %d and act <= %d supported, got obs %d, act %d", CW_MAX_OBS, CW_MAX_ACT, obs, act);
+        es_set_error("%s: obs <= %d and act <= %d supported, got obs %d, act %d", fn, CW_MAX_OBS, CW_MAX_ACT, obs, act);
         return ES_ERR_UNSUPPORTED;
     }
     if ((band & 1) || band > CW_HALO || band > obs) {
-        es_set_error("es_rollout_closedloop_mlp: the band must be even, <= %d and <= obs (got band %d, obs %d)", CW_HALO, band, obs);
+        es_set_error("%s: the band must be even, <= %d and <= obs (got band %d, obs %d)", fn, CW_HALO, band, obs);
         return ES_ERR_UNSUPPORTED;
     }
     size_t bytes = 0;
     for (int C = 1; C <= 8; C *= 2) {
-        bytes = (size_t)cw_layout(n_layers, dims, C, band).total * sizeof(float);
+        bytes = (size_t)cw_layout(n_layers, dims, C, band, act, binned).total * sizeof(float);
         if (bytes <= (size_t)CW_SMEM_MAX) {
             *cluster_size = C;
             *smem_bytes = bytes;
             return ES_OK;
         }
     }
-    es_set_error("es_rollout_closedloop_mlp: the weights and env matrices need %zu bytes of shared memory per CTA in a cluster of "
-                 "8 CTAs, %d available", bytes, CW_SMEM_MAX);
+    es_set_error("%s: the weights and env matrices need %zu bytes of shared memory per CTA in a cluster of 8 CTAs, %d available",
+                 fn, bytes, CW_SMEM_MAX);
     return ES_ERR_UNSUPPORTED;
 }
 
+int es_closedw_plan(const int* dims, int n_layers, int band, int* cluster_size, size_t* smem_bytes) {
+    return cw_plan("es_rollout_closedloop_mlp", dims, n_layers, band, dims[n_layers], false, cluster_size, smem_bytes);
+}
+// binned heads: the last layer is adim * bins <= 256 wide (checked as a hidden width), the env sees adim <= 64 actions
+int es_closedw_binned_plan(const int* dims, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes) {
+    const char* fn = "es_rollout_closedloop_mlp_binned";
+    const int out = dims[n_layers];
+    if (bins < 2 || out % bins || out > CW_MAX_WIDTH) {
+        es_set_error("%s: the last layer must have adim * bins <= %d outputs with bins >= 2, got %d outputs, bins %d", fn,
+                     CW_MAX_WIDTH, out, bins);
+        return ES_ERR_UNSUPPORTED;
+    }
+    return cw_plan(fn, dims, n_layers, band, out / bins, true, cluster_size, smem_bytes);
+}
+
 typedef void (*CwKernel)(const CwParams);
-static CwKernel cw_kernel(int n_layers) {
+static CwKernel cw_kernel(int n_layers, bool binned = false) {
+    if (binned)
+        return n_layers == 3 ? rollout_closedw_binned_kernel<3> : n_layers == 4 ? rollout_closedw_binned_kernel<4>
+                                                                                 : rollout_closedw_binned_kernel<5>;
     return n_layers == 3 ? rollout_closedw_kernel<3> : n_layers == 4 ? rollout_closedw_kernel<4> : rollout_closedw_kernel<5>;
 }
 // a launch of `clusters` clusters of C CTAs (attr: the cluster-dimension attribute the config points to)
@@ -371,21 +421,28 @@ static cudaLaunchConfig_t cw_config(int C, size_t smem, int clusters, cudaStream
 }
 
 // the number of clusters of the shape that can be resident at once (the persistent grid), 0 when none fits
-int es_closedw_max_clusters(int n_layers, int C, size_t smem, int* clusters) {
-    const CwKernel k = cw_kernel(n_layers);
+static int cw_max_clusters(CwKernel k, int C, size_t smem, int* clusters) {
     ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cw_config(C, smem, 1, nullptr, &attr);
     ES_CHECK_CUDA(cudaOccupancyMaxActiveClusters(clusters, k, &cfg));
     return ES_OK;
 }
+int es_closedw_max_clusters(int n_layers, int C, size_t smem, int* clusters) {
+    return cw_max_clusters(cw_kernel(n_layers), C, smem, clusters);
+}
+int es_closedw_binned_max_clusters(int n_layers, int C, size_t smem, int* clusters) {
+    return cw_max_clusters(cw_kernel(n_layers, true), C, smem, clusters);
+}
 
 int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {
     int C = 0, max_clusters = 0;
     size_t smem = 0;
-    int rc = es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
+    const bool binned = r.bins != 0;
+    int rc = binned ? es_closedw_binned_plan(r.layer_sizes, r.n_layers, env.band, r.bins, &C, &smem)
+                    : es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
     if (rc) return rc;
-    rc = es_closedw_max_clusters(r.n_layers, C, smem, &max_clusters);
+    rc = cw_max_clusters(cw_kernel(r.n_layers, binned), C, smem, &max_clusters);
     if (rc) return rc;
     if (max_clusters < 1) {
         es_set_error("es_rollout_closedloop_mlp: no cluster of %d CTAs with %zu bytes of shared memory each fits on this device", C, smem);
@@ -406,11 +463,13 @@ int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& 
     p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.fit_stride = r.fit_stride; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
     p.ob_sum = env.ob_sum; p.ob_sumsq = env.ob_sumsq; p.ob_count = env.ob_count;
     p.err = r.err;
+    p.bins = r.bins; p.adim = binned ? r.layer_sizes[r.n_layers] / r.bins : 0; p.scale = binned ? (float)(1.0 / (r.bins - 1.0)) : 0.f;
+    p.low = r.head_low; p.range = r.head_range;
     const long long evals = 2ll * r.n_pairs;
     const int clusters = evals < max_clusters ? (int)evals : max_clusters;
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cw_config(C, smem, clusters, stream, &attr);
-    ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cw_kernel(r.n_layers), p));
+    ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cw_kernel(r.n_layers, binned), p));
     ES_LAUNCHED(ctx);
     return ES_OK;
 }

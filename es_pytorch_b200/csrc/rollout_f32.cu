@@ -103,15 +103,26 @@ rollout_f32_stage_kernel(const float* __restrict__ table, const int64_t* __restr
     rf_stage_weights(W, table + es_checked_slice(idx[blockIdx.x >> 1], d.P, d.table_len, d.err), theta, sigma, blockIdx.x & 1, d);
 }
 
-// GW: weights in the global scratch filled by rollout_f32_stage_kernel instead of shared memory
-template <bool GW>
-__global__ void __launch_bounds__(RF_THREADS, 1)
-rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ idx, const float* __restrict__ theta,
-                   float sigma, const __grid_constant__ RfDesc d, const float* __restrict__ obsn,
-                   const float* __restrict__ rew_vec, int T, float pos_scale, double* __restrict__ fit_pos,
-                   double* __restrict__ fit_neg, int fit_stride, float* __restrict__ behv_pos,
-                   float* __restrict__ behv_neg, double* __restrict__ part, unsigned* __restrict__ tickets,
-                   const float* __restrict__ wglobal, const float* __restrict__ act_noise, int n_eps) {
+// the policy head of a binned-action policy (FFBinned, src/nn/nn.py:99-117): the last layer has adim * bins outputs; the
+// action of dimension j is the first maximal of its bins outputs, idx, mapped to (scale * idx) * range[j] + low[j] with
+// scale = float32(1 / (bins - 1)), every operation rounded to float32 as the reference's torch expression does
+struct RfHead {
+    int adim, bins;
+    float scale;
+    const float* low;            // dev float [adim]
+    const float* range;          // dev float [adim]: high - low in float32
+};
+
+// GW: weights in the global scratch filled by rollout_f32_stage_kernel instead of shared memory.  BINNED: the head above;
+// else the tanh outputs are the actions (`h` unused)
+template <bool GW, bool BINNED>
+__device__ __forceinline__ void
+rf_rollout(const float* __restrict__ table, const int64_t* __restrict__ idx, const float* __restrict__ theta,
+           float sigma, const RfDesc& d, const float* __restrict__ obsn,
+           const float* __restrict__ rew_vec, int T, float pos_scale, double* __restrict__ fit_pos,
+           double* __restrict__ fit_neg, int fit_stride, float* __restrict__ behv_pos,
+           float* __restrict__ behv_neg, double* __restrict__ part, unsigned* __restrict__ tickets,
+           const float* __restrict__ wglobal, const float* __restrict__ act_noise, int n_eps, const RfHead& h) {
     extern __shared__ __align__(16) float smem[];
     float* Wsm = GW ? const_cast<float*>(wglobal) + (size_t)blockIdx.x * d.w_floats : smem;    // [w_floats]
     float* Xa = GW ? smem : smem + d.w_floats;          // [RF_TM][xpitch]
@@ -133,7 +144,7 @@ rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ 
     __syncthreads();
 
     const int obs_dim = d.in[0];
-    const int act_dim = d.out[d.n_layers - 1];
+    const int act_dim = BINNED ? h.adim : d.out[d.n_layers - 1];
     // time split (gridDim.y > 1, used when there are fewer policies than SMs): the open-loop episode has no state, so
     // CTA y evaluates a contiguous range of time tiles; the partial sums are combined in tile order by the last CTA
     const int n_tiles = (T + RF_TM - 1) / RF_TM;
@@ -159,6 +170,23 @@ rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ 
                     xout[(i / padw) * d.xpitch + d.out[l] + (i % padw)] = 0.f;
             }
             rf_dense(Wsm + d.sw_off[l], Wsm + d.sb_off[l], d.in4[l], d.pitch[l], d.out[l], xin, xout, d.xpitch);
+            __syncthreads();
+            float* tmp = xin; xin = xout; xout = tmp;
+        }
+        if (BINNED) {
+            // xin holds the [RF_TM][adim * bins] outputs: the actions go to xout (free), which then becomes xin.  The first
+            // maximal bin wins, as torch.argmax; a NaN output counts as the maximum, as in torch
+            for (int i = threadIdx.x; i < rows * act_dim; i += RF_THREADS) {
+                const int r = i / act_dim, j = i - r * act_dim;
+                const float* o = xin + r * d.xpitch + j * h.bins;
+                int best = 0;
+                float bv = o[0];
+                for (int b = 1; b < h.bins && bv == bv; ++b) {
+                    const float v = o[b];
+                    if (v > bv || v != v) { bv = v; best = b; }
+                }
+                xout[r * d.xpitch + j] = __fadd_rn(__fmul_rn(__fmul_rn(h.scale, (float)best), __ldg(h.range + j)), __ldg(h.low + j));
+            }
             __syncthreads();
             float* tmp = xin; xin = xout; xout = tmp;
         }
@@ -231,13 +259,32 @@ rollout_f32_kernel(const float* __restrict__ table, const int64_t* __restrict__ 
     }
 }
 
+#define RF_KERNEL_PARAMS                                                                                                   \
+    const float* __restrict__ table, const int64_t* __restrict__ idx, const float* __restrict__ theta, float sigma,      \
+    const __grid_constant__ RfDesc d, const float* __restrict__ obsn, const float* __restrict__ rew_vec, int T,           \
+    float pos_scale, double* __restrict__ fit_pos, double* __restrict__ fit_neg, int fit_stride,                          \
+    float* __restrict__ behv_pos, float* __restrict__ behv_neg, double* __restrict__ part, unsigned* __restrict__ tickets, \
+    const float* __restrict__ wglobal, const float* __restrict__ act_noise, int n_eps
+#define RF_KERNEL_ARGS table, idx, theta, sigma, d, obsn, rew_vec, T, pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, \
+    part, tickets, wglobal, act_noise, n_eps
+
+template <bool GW>
+__global__ void __launch_bounds__(RF_THREADS, 1) rollout_f32_kernel(RF_KERNEL_PARAMS) {
+    rf_rollout<GW, false>(RF_KERNEL_ARGS, RfHead{});
+}
+template <bool GW>
+__global__ void __launch_bounds__(RF_THREADS, 1) rollout_f32_binned_kernel(RF_KERNEL_PARAMS, const RfHead h) {
+    rf_rollout<GW, true>(RF_KERNEL_ARGS, h);
+}
+
 static int rf_round4(int x) { return (x + 3) & ~3; }
 
 int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     // obs-64-64-act networks with enough pairs to fill the GPU: the packed-FMA kernel of rollout_f32x.cu (one CTA per pair);
     // fewer pairs than half the SMs (single evaluations, es.step's noiseless evaluation) stay here, where the episode's time
-    // tiles are split over the idle SMs.  ES_F32_GENERAL=1 forces this kernel (tests compare the two).
-    if (2 * r.n_pairs >= ctx->sm_count && !getenv("ES_F32_GENERAL")) {
+    // tiles are split over the idle SMs.  ES_F32_GENERAL=1 forces this kernel (tests compare the two).  Binned heads always
+    // run here.
+    if (!r.bins && 2 * r.n_pairs >= ctx->sm_count && !getenv("ES_F32_GENERAL")) {
         const int rc = es_impl_rollout_f32x(ctx, r, stream);
         if (rc != ES_ERR_UNSUPPORTED) return rc;
     }
@@ -313,7 +360,19 @@ int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
         float* bn = r.behv_neg ? r.behv_neg + (size_t)p0 * 3 : nullptr;
         const int n_eps = r.act_noise ? r.n_episodes : 1;
         const float* an = r.act_noise ? r.act_noise + (size_t)p0 * 2 * n_eps * T * r.layer_sizes[n_layers] : nullptr;
-        if (gw) {
+        if (r.bins) {
+            const RfHead h = {r.layer_sizes[n_layers] / r.bins, r.bins, (float)(1.0 / (r.bins - 1.0)), r.head_low, r.head_range};
+            if (gw) {
+                rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, d, wglobal);
+                ES_LAUNCHED(ctx);
+            }
+            const size_t smem = gw ? act_smem : smem_w;
+            auto k = gw ? rollout_f32_binned_kernel<true> : rollout_f32_binned_kernel<false>;
+            ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            k<<<dim3(2 * np, n_splits), RF_THREADS, smem, stream>>>(
+                r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
+                wglobal, an, n_eps, h);
+        } else if (gw) {
             rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, d, wglobal);
             ES_LAUNCHED(ctx);
             ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)act_smem));

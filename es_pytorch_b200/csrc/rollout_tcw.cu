@@ -44,6 +44,16 @@
 //     once, the tanh and hi / lo values of a 256-wide layer did not fit beside the accumulators (the TC3 kernels spilled
 //     about 140 bytes per thread).
 //
+// Binned-action policies (FFBinned, src/nn/nn.py:99-117; ES_ROLLOUT_TC3 only, rollout_tcw_binned_kernel): the last layer is up
+// to four 64-wide N blocks (adim * bins <= 256), and obs-64-64-X binned shapes run here too.  Its tanh outputs go as float32 into
+// the warpgroup's rows of the activation buffer, which no MMA reads any more at that point (64 rows x 256 floats = the
+// warpgroup's 8 pieces of 8 KB: column n in piece n / 32, at word (n ^ row) mod 32 of its 128-byte row, so that the 32 rows a warp
+// reads at one column fall in 32 banks), rather than being reduced across the quads holding a row's columns
+// with shuffles: the buffer is free, and one thread per row then takes the arg-max of each dimension in bin order (the first
+// maximal bin, as torch.argmax) and forms the action and the float32 reward in index order as rollout_f32.cu does; only the
+// float64 sums over the rows and tiles are reassociated.  ES_ROLLOUT_TC refuses binned heads (api.cu): an arg-max over
+// float16-grade outputs is not parity grade.
+//
 // 12 warps (3 warpgroups): warpgroup 0 = warp 0 producer (the other three idle) -> setmaxnreg 24 registers;
 // warpgroups 1 and 2: consumers, rows 0-63 / 64-127 of every tile -> setmaxnreg 240 registers.
 #include <cuda_fp16.h>
@@ -98,6 +108,7 @@ struct TwParams {
     const float* act_noise;       // [n_evals][n_eps][T][act] or NULL
     double* part;                 // [n_evals][n_mtiles][8 consumer warps][4]: reward, position sums 0..2
     int n_evals, n_mtiles, obs, act, T, n_eps;
+    int bins; float scale; const float* low; const float* range;    // binned head (act = adim), rollout_tcw_binned_kernel only
 };
 
 template <bool SPLIT>
@@ -147,8 +158,8 @@ __device__ __forceinline__ void st_shared_u32(void* p, uint32_t v) {
 }
 __device__ __forceinline__ void wg_bar(int half) { asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory"); }
 
-template <bool SPLIT, bool NOISE>
-__global__ void __launch_bounds__(TW_THREADS, 1) rollout_tcw_kernel(const __grid_constant__ TwParams p) {
+template <bool SPLIT, bool NOISE, bool BINNED>
+__device__ __forceinline__ void tw_rollout(const TwParams& p) {
     using C = TwCfg<SPLIT>;
     constexpr int NP = C::NP, NSTAGE = C::NSTAGE;
     extern __shared__ uint8_t smem_raw[];
@@ -306,6 +317,43 @@ __global__ void __launch_bounds__(TW_THREADS, 1) rollout_tcw_kernel(const __grid
                     wg_bar(half);
                     return;
                 }
+                if (BINNED) {
+                    // ---- binned head: float32 tanh outputs -> the warpgroup's rows of the free activation buffer; then one
+                    //      thread per row: the arg-max bin of every dimension, the action, the float32 reward in index order ----
+                    wg_bar(half);                                // every warp's MMAs of this layer have read the buffer
+#pragma unroll
+                    for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+                        for (int c = 0; c < 8; ++c)
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                const int col = 64 * nb + 8 * c + 2 * q + (e & 1), row = rw + 8 * (e >> 1);
+                                *(float*)(act_wg + (size_t)(col >> 5) * C::PIECE + row * 128 + (((col ^ row) & 31) << 2)) =
+                                    tanh_acc(acc[nb][4 * c + e]);
+                            }
+                    wg_bar(half);
+                    const int t = t0 + wt;
+                    if (wt < 64 && t < p.T) {
+                        const uint8_t* rowp = act_wg + wt * 128;
+                        float r = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f;
+                        for (int j = 0; j < p.act; ++j) {
+                            int best = 0;
+                            float bv = 0.f;
+                            for (int b = 0; b < p.bins; ++b) {
+                                const int col = j * p.bins + b;
+                                const float v = *(const float*)(rowp + (size_t)(col >> 5) * C::PIECE + (((col ^ wt) & 31) << 2));
+                                if (b == 0 || (bv == bv && (v > bv || v != v))) { bv = v; best = b; }    // a NaN is the maximum
+                            }
+                            const float a = __fadd_rn(__fmul_rn(__fmul_rn(p.scale, (float)best), __ldg(p.range + j)), __ldg(p.low + j));
+                            r = __fadd_rn(r, __fmul_rn(a, __ldg(p.rew_vec + (size_t)t * p.act + j)));
+                            if (j == 0) a0 = a;
+                            if (j == 1) a1 = a;
+                            if (j == 2) a2 = a;
+                        }
+                        fitd = (double)r; q0s = a0; q1s = a1; q2s = a2;
+                    }
+                    return;
+                }
                 // ---- last layer: a = tanh(z) [+ action noise of each episode]; r_t = <a_t, c_t>; positions (act <= 32: N block 0,
                 //      columns 8 c + 2 q (+1) for c < 4) ----
                 const int ta = t0 + rw, tb = ta + 8;
@@ -352,6 +400,12 @@ __global__ void __launch_bounds__(TW_THREADS, 1) rollout_tcw_kernel(const __grid
             o[0] = f; o[1] = g0; o[2] = g1; o[3] = g2;
         }
     }
+}
+
+template <bool SPLIT, bool NOISE>
+__global__ void __launch_bounds__(TW_THREADS, 1) rollout_tcw_kernel(const __grid_constant__ TwParams p) { tw_rollout<SPLIT, NOISE, false>(p); }
+__global__ void __launch_bounds__(TW_THREADS, 1) rollout_tcw_binned_kernel(const __grid_constant__ TwParams p) {
+    tw_rollout<true, false, true>(p);
 }
 
 // the partial sums of every evaluation, tile by tile and warp by warp -> fitness and behaviour
@@ -417,7 +471,8 @@ int tw_run(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     if (rc) return rc;
     uint8_t* images = (uint8_t*)scratch;
     double* part = (double*)((uint8_t*)scratch + img_total);
-    const int act = L.out[r.n_layers - 1];
+    const int act = r.bins ? L.out[r.n_layers - 1] / r.bins : L.out[r.n_layers - 1];
+    if (r.bins) { p.bins = r.bins; p.scale = (float)(1.0 / (r.bins - 1.0)); p.low = r.head_low; p.range = r.head_range; }
     for (int p0 = 0; p0 < r.n_pairs; p0 += chunk) {
         const int np = (r.n_pairs - p0 < chunk) ? r.n_pairs - p0 : chunk;
         rollout_tcw_build_kernel<SPLIT><<<np, 256, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, r.table_len, r.P, r.err, L, images);
@@ -429,8 +484,18 @@ int tw_run(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
         p.n_evals = 2 * np; p.n_mtiles = n_mtiles; p.obs = L.in[0]; p.act = act; p.T = T; p.n_eps = n_eps;
         const int n_items = p.n_evals * n_mtiles;
         const int grid = n_items < ctx->sm_count ? n_items : ctx->sm_count;
-        rc = p.act_noise ? tw_launch_main<SPLIT, true>(ctx, p, grid, stream) : tw_launch_main<SPLIT, false>(ctx, p, grid, stream);
-        if (rc) return rc;
+        if constexpr (SPLIT) {
+            if (r.bins) {
+                constexpr size_t smem = TwCfg<true>::SMEM;
+                ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_tcw_binned_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                rollout_tcw_binned_kernel<<<grid, TW_THREADS, smem, stream>>>(p);
+                ES_LAUNCHED(ctx);
+            }
+        }
+        if (!r.bins) {
+            rc = p.act_noise ? tw_launch_main<SPLIT, true>(ctx, p, grid, stream) : tw_launch_main<SPLIT, false>(ctx, p, grid, stream);
+            if (rc) return rc;
+        }
         rollout_tcw_finish_kernel<<<es_div_up(2 * np, 128), 128, 0, stream>>>(
             part, 2 * np, n_mtiles, act, r.pos_scale, r.fit_pos + (size_t)p0 * r.fit_stride, r.fit_neg + (size_t)p0 * r.fit_stride,
             r.fit_stride, r.behv_pos ? r.behv_pos + (size_t)p0 * 3 : nullptr, r.behv_neg ? r.behv_neg + (size_t)p0 * 3 : nullptr);
@@ -446,6 +511,17 @@ bool es_tcw_covers(const EsRollout& r) {
     if (r.n_layers < 3 || r.n_layers > TW_MAX_LAYERS) return false;      // 2 to 4 hidden layers
     if (r.n_layers == 3 && ls[1] == 64 && ls[2] == 64) return false;    // obs-64-64-act: rollout_tc2.cu
     if (ls[0] < 1 || ls[0] > 256 || ls[r.n_layers] < 1 || ls[r.n_layers] > 32) return false;
+    for (int l = 1; l < r.n_layers; ++l)
+        if (ls[l] % 64 != 0 || ls[l] < 64 || ls[l] > 256) return false;
+    return true;
+}
+
+// binned heads (ES_ROLLOUT_TC3): 2 to 4 hidden layers of multiples of 64 in [64, 256] (obs-64-64-X included), obs <= 256 and
+// adim * bins <= 256 (up to four N blocks in the last layer)
+bool es_tcw_covers_binned(const EsRollout& r) {
+    const int* ls = r.layer_sizes;
+    if (r.n_layers < 3 || r.n_layers > TW_MAX_LAYERS) return false;
+    if (ls[0] < 1 || ls[0] > 256 || ls[r.n_layers] < 1 || ls[r.n_layers] > 256) return false;
     for (int l = 1; l < r.n_layers; ++l)
         if (ls[l] % 64 != 0 || ls[l] < 64 || ls[l] > 256) return false;
     return true;

@@ -272,11 +272,17 @@ class Engine:
     # ------------------------------------------------------------------ a3+a4+a5
     def rollout(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], obsn, rew_vec, pos_scale: float,
                 fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None, behv_neg=None, mode: int = ES_ROLLOUT_F32,
-                act_noise=None, episodes: int = 1):
+                act_noise=None, episodes: int = 1, head=None):
         """``act_noise``: float32 [n_pairs, 2, episodes, T, act] scaled action noise (``draw_noisy``), added to every action.
         ``episodes`` > 1 (obj.py:54-63's eps_per_policy): every evaluation is the per-step mean of that many episodes, each
         with its own noise rows; behaviour is the last episode's.  Without ``act_noise`` the episodes are identical and the
-        result is the single episode's."""
+        result is the single episode's.
+        ``head``: None or ``'tanh'`` (the outputs are the actions), or an ``nn.BinnedHead`` (FFBinned:
+        es_rollout_openloop_binned; ``layer_sizes[-1]`` is adim * bins, ``rew_vec`` [T, adim]; no action noise; modes F32 and
+        TC3)."""
+        if head is not None and head != 'tanh':
+            return self._rollout_binned(table, idx, theta, sigma, layer_sizes, obsn, rew_vec, pos_scale, fit_pos, fit_neg,
+                                        fit_stride, behv_pos, behv_neg, mode, act_noise, episodes, head)
         d = self.device
         _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
         _req(obsn, torch.float32, 'obsn', d); _req(rew_vec, torch.float32, 'rew_vec', d)
@@ -307,6 +313,39 @@ class Engine:
                                                     _ptr(rew_vec), T, float(pos_scale), _ptr(fit_pos), _ptr(fit_neg),
                                                     int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(act_noise),
                                                     episodes, int(mode), self.stream), 'es_rollout_openloop')
+
+    def _rollout_binned(self, table, idx, theta, sigma, layer_sizes, obsn, rew_vec, pos_scale, fit_pos, fit_neg, fit_stride,
+                        behv_pos, behv_neg, mode, act_noise, episodes, head):
+        d = self.device
+        if act_noise is not None or int(episodes) != 1:
+            raise ValueError('a binned head draws no action noise: act_noise must be None and episodes 1')
+        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
+        _req(obsn, torch.float32, 'obsn', d); _req(rew_vec, torch.float32, 'rew_vec', d)
+        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
+        n, T = idx.numel(), obsn.shape[0]
+        assert obsn.shape[1] == layer_sizes[0] and rew_vec.shape == (T, head.adim)
+        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
+        if behv_pos is not None:
+            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
+            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
+        low, rng = self._head_arrays(head)
+        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+        check(self.lib.es_rollout_openloop_binned(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
+                                                  float(sigma), ls, len(layer_sizes) - 1, _ptr(obsn), _ptr(rew_vec), T,
+                                                  float(pos_scale), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride), _ptr(behv_pos),
+                                                  _ptr(behv_neg), int(head.bins), _ptr(low), _ptr(rng), int(mode), self.stream),
+              'es_rollout_openloop_binned')
+
+    def _head_arrays(self, head):
+        """A binned head's (low, high - low) float32 device tensors, uploaded once per head (the last few heads are kept)."""
+        cache = self.__dict__.setdefault('_heads', {})
+        key = head.key()
+        arrs = cache.get(key)
+        if arrs is None:
+            if len(cache) >= 8:
+                cache.pop(next(iter(cache)))            # the oldest: scripts use one head per run
+            arrs = cache[key] = head.device_arrays(self)
+        return arrs
 
     def rollout_closed(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
                        obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,
@@ -344,17 +383,21 @@ class Engine:
 
     def rollout_closed_mlp(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
                            obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,
-                           behv_neg=None, coin_words=None, save_obs_chance: float = 0.0, ob_sum=None, ob_sumsq=None, ob_count=None):
+                           behv_neg=None, coin_words=None, save_obs_chance: float = 0.0, ob_sum=None, ob_sumsq=None, ob_count=None,
+                           head=None):
         """``rollout_closed`` (same arguments and checks) for every tanh MLP the closed loop covers: 2 to 4 hidden layers of
         at most 256 units, obs <= 384, act <= 64.  The shapes ``rollout_closed`` takes run its kernel; the others one
-        thread-block cluster per evaluation (``closed_mlp_plan``)."""
+        thread-block cluster per evaluation (``closed_mlp_plan``).  ``head``: as ``rollout``; a binned head
+        (es_rollout_closedloop_mlp_binned) always runs the cluster kernel, ``env_b`` [adim, obs] and ``rew_vec`` [T, adim]."""
+        binned = head is not None and head != 'tanh'
         d = self.device
         _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
         _req(ob_mean, torch.float64, 'ob_mean', d); _req(ob_std, torch.float64, 'ob_std', d)
         _req(obs0, torch.float32, 'obs0', d); _req(env_a, torch.float32, 'env_a', d); _req(env_b, torch.float32, 'env_b', d)
         _req(rew_vec, torch.float32, 'rew_vec', d)
         _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
-        n, T, obs, act = idx.numel(), rew_vec.shape[0], int(layer_sizes[0]), int(layer_sizes[-1])
+        n, T, obs = idx.numel(), rew_vec.shape[0], int(layer_sizes[0])
+        act = head.adim if binned else int(layer_sizes[-1])
         band = env_a.shape[0]
         assert env_a.shape == (band, obs) and env_b.shape == (act, obs) and obs0.numel() == obs and rew_vec.shape == (T, act)
         assert ob_mean.numel() == obs and ob_std.numel() == obs
@@ -368,6 +411,15 @@ class Engine:
             _req(ob_sum, torch.float64, 'ob_sum', d); _req(ob_sumsq, torch.float64, 'ob_sumsq', d); _req(ob_count, torch.float64, 'ob_count', d)
             assert ob_sum.numel() == obs and ob_sumsq.numel() == obs and ob_count.numel() == 2
         ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+        if binned:
+            low, rng = self._head_arrays(head)
+            check(self.lib.es_rollout_closedloop_mlp_binned(
+                self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
+                _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T,
+                float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
+                _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), int(head.bins), _ptr(low), _ptr(rng),
+                self.stream), 'es_rollout_closedloop_mlp_binned')
+            return
         check(self.lib.es_rollout_closedloop_mlp(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
                                                  float(sigma), ls, len(layer_sizes) - 1, _ptr(ob_mean), _ptr(ob_std), float(ob_clip),
                                                  _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T, float(pos_scale),
@@ -375,11 +427,17 @@ class Engine:
                                                  int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq),
                                                  _ptr(ob_count), self.stream), 'es_rollout_closedloop_mlp')
 
-    def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int):
+    def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int, head=None):
         """How ``rollout_closed_mlp`` runs a shape: (CTAs per cluster, clusters resident at once, shared memory bytes per CTA);
-        (0, SM count, 0) for ``rollout_closed``'s one-CTA kernel.  Raises EsLibraryError for a shape it does not cover."""
+        (0, SM count, 0) for ``rollout_closed``'s one-CTA kernel.  Raises EsLibraryError for a shape it does not cover.
+        ``head``: as ``rollout_closed_mlp`` (a binned head's plan is always a cluster of >= 1 CTA)."""
         ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
         cs, nc, sm = C.c_int(0), C.c_int(0), C.c_int64(0)
+        if head is not None and head != 'tanh':
+            check(self.lib.es_rollout_closedloop_mlp_binned_plan(self._ctx, ls, len(layer_sizes) - 1, int(band), int(head.bins),
+                                                                 C.byref(cs), C.byref(nc), C.byref(sm)),
+                  'es_rollout_closedloop_mlp_binned_plan')
+            return cs.value, nc.value, sm.value
         check(self.lib.es_rollout_closedloop_mlp_plan(self._ctx, ls, len(layer_sizes) - 1, int(band), C.byref(cs), C.byref(nc),
                                                       C.byref(sm)), 'es_rollout_closedloop_mlp_plan')
         return cs.value, nc.value, sm.value

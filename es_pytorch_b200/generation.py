@@ -71,7 +71,7 @@ class DeviceGeneration:
                  optim: Optimizer, ob_clip: float = 5.0, pos_scale: float = 0.05, coins_per_eval: int = 0,
                  save_obs_chance: float = 0.0, archive: Optional[torch.Tensor] = None, nov_k: int = 10,
                  moo_w: float = 1.0, rollout_mode: int = ES_ROLLOUT_F32, comm: Optional[dist.Comm] = None,
-                 engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1):
+                 engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1, head=None):
         self.eng = engine or get_engine()
         # closed-loop variant of the synthetic env (gym.synthetic_env.ClosedLoopEnv): (obs_0 [obs], A^T [band, obs], B^T [act, obs]);
         # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop_mlp
@@ -83,7 +83,12 @@ class DeviceGeneration:
         self.theta = theta
         self.P = theta.numel()
         self.layer_sizes = [int(x) for x in layer_sizes]
-        self.obs_dim, self.act_dim = self.layer_sizes[0], self.layer_sizes[-1]
+        # the policy head (nn.BaseNet.head): None / 'tanh', the outputs are the actions; an nn.BinnedHead (FFBinned), the last
+        # layer's adim * bins outputs become the env's adim actions
+        self.head = None if head == 'tanh' else head
+        self.head_key = None if self.head is None else self.head.key()       # what a cached generation is valid for
+        self.obs_dim = self.layer_sizes[0]
+        self.act_dim = self.head.adim if self.head is not None else self.layer_sizes[-1]
         self.obs_stream = obs_stream                    # [T+1, obs_dim]
         self.rew_vec = rew_vec                          # [T, act_dim]
         self.T = rew_vec.shape[0]
@@ -103,6 +108,8 @@ class DeviceGeneration:
         self.episodes = int(episodes)
         assert self.episodes >= 1
         assert self.coins_per_eval in (0, 1), 'fit_fns draw at most one save_obs coin per evaluation'
+        if self.head is not None and self.ac_std != 0.0:
+            raise ValueError('a binned head draws no action noise (FFBinned.forward ignores rs): ac_std must be 0')
 
         # per-rank MT19937 streams, resident on the device between generations
         self.n_streams = len(rank_states)
@@ -218,7 +225,7 @@ class DeviceGeneration:
                                      coin_words=self.extras if self.extra_words else None, save_obs_chance=self.save_obs_chance,
                                      ob_sum=self.gen_sum if self.extra_words else None,
                                      ob_sumsq=self.gen_sumsq if self.extra_words else None,
-                                     ob_count=self.gen_count if self.extra_words else None)
+                                     ob_count=self.gen_count if self.extra_words else None, head=self.head)
             if self.n_obj == 2:
                 e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
         else:
@@ -245,7 +252,7 @@ class DeviceGeneration:
                       self.pos_scale, fp, fn, self.n_obj, None if self.behv is None else self.behv[0],
                       None if self.behv is None else self.behv[1], self.rollout_mode,
                       act_noise=self.act_noise if self.ac_std != 0.0 else None,
-                      episodes=self.episodes if self.ac_std != 0.0 else 1)
+                      episodes=self.episodes if self.ac_std != 0.0 else 1, head=self.head)
         if self.n_obj == 2:
             # second objective column = novelty of the final (x, y) (training_result.py:95-97)
             e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
@@ -311,10 +318,10 @@ class DeviceGeneration:
             obs0, env_a, env_b = self.closed
             e.rollout_closed_mlp(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,
                                  obs0, env_a, env_b, self.rew_vec, self.pos_scale, fit0[0:1], fit0[1:2], 1, behv0[0].view(-1),
-                                 behv0[1].view(-1))
+                                 behv0[1].view(-1), head=self.head)
             return fit0, behv0
         e.rollout(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.obsn, self.rew_vec, self.pos_scale,
-                  fit0[0:1], fit0[1:2], 1, behv0[0].view(-1), behv0[1].view(-1), ES_ROLLOUT_F32)
+                  fit0[0:1], fit0[1:2], 1, behv0[0].view(-1), behv0[1].view(-1), ES_ROLLOUT_F32, head=self.head)
         return fit0, behv0
 
     def skip_eval_coins(self, n_evals: int = 1):

@@ -79,7 +79,8 @@ class BatchedRollout:
                     rs.random()
         noise_rs = streams[0] if (use_ac_noise and streams is not None and len(streams)) else None
         closed = getattr(self.env, 'is_synthetic_closedloop', False)
-        if (closed and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp() and self._closed_on_device(model.layer_sizes())
+        head = model.head() if hasattr(model, 'head') else None
+        if (closed and head is not None and self._closed_on_device(model.layer_sizes(), head)
                 and not (noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0)):
             # the closed-loop episode as one launch (the observations are not returned: this result never carries them)
             from .gym_runner import _device_episode_closed
@@ -95,18 +96,19 @@ class BatchedRollout:
             return RewardResult(rews, behv, no_obs, steps)
         return NSRResult(rews, behv[-3:], no_obs, steps, self.archive, self.nov_k)
 
-    def _closed_on_device(self, sizes) -> bool:
+    def _closed_on_device(self, sizes, head='tanh') -> bool:
         """Whether a closed-loop episode of a tanh MLP runs as one launch (es_rollout_closedloop_mlp): two hidden layers always
         do (a shape outside the kernels' coverage raises there); three or four when the kernels cover the shape; anything else
-        runs run_model's python loop."""
+        runs run_model's python loop.  A binned head (es_rollout_closedloop_mlp_binned) runs as one launch when the cluster
+        kernel covers the shape."""
         n_hidden = len(sizes) - 2
-        if n_hidden == 2:
+        if n_hidden == 2 and head == 'tanh':
             return True
-        if n_hidden not in (3, 4):
+        if n_hidden not in (2, 3, 4):
             return False
         from ..engine import get_engine
         try:
-            get_engine().closed_mlp_plan(sizes, self.env.band)
+            get_engine().closed_mlp_plan(sizes, self.env.band, head)
         except _lib.EsLibraryError:
             return False
         return True

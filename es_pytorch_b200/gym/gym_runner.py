@@ -1,7 +1,7 @@
 """Rollout runner (mirror of src/gym/gym_runner.py:33-67).
 
 ``run_model`` keeps the reference signature.  When the env is the synthetic open-loop env
-and the model is a tanh ``FeedForward``, the whole episode is ONE launch of the fused rollout
+and the model is a tanh ``FeedForward`` or a tanh ``FFBinned`` (``BaseNet.head``), the whole episode is ONE launch of the fused rollout
 kernel (per-policy compatibility path: theta' is the module's current weights, sigma = 0;
 action noise, nn.py:47-48, is drawn from ``rs`` for the whole episode at once and added on
 the device); any other env is stepped in the reference's python loop with the module's own
@@ -64,7 +64,7 @@ def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
     else:
         episodes = 1
     eng.rollout(table, idx, theta, 0.0, sizes, obsn, rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1,
-                behv[0:1].view(-1), behv[1:2].view(-1), act_noise=noise, episodes=episodes)
+                behv[0:1].view(-1), behv[1:2].view(-1), act_noise=noise, episodes=episodes, head=model.head())
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 
@@ -85,14 +85,15 @@ def _device_episode_closed(model, env, max_steps: int):
     fit = torch.zeros(2, dtype=torch.float64, device=eng.device)
     behv = torch.zeros(2, 3, dtype=torch.float32, device=eng.device)
     eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), obs0, env_a, env_b,
-                           rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1))
+                           rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1),
+                           head=model.head())
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 
 def run_model(model: torch.nn.Module, env, max_steps: int, rs: np.random.RandomState = None, render: bool = False,
               get_pos_fn: Callable = pybullet_gym_pos) -> Tuple[List[float], List[float], np.ndarray, int]:
     """(rewards, positions padded to max_steps triples, post-step observations, last loop index)."""
-    fused = (getattr(env, 'is_synthetic_openloop', False) and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp()
+    fused = (getattr(env, 'is_synthetic_openloop', False) and hasattr(model, 'head') and model.head() is not None
              and not render)
     if fused:
         total, pos, T = _device_episode(model, env, max_steps, rs)

@@ -10,11 +10,36 @@ an arbitrary gym env itself.
 from __future__ import annotations
 
 from abc import ABC
-from typing import List
+from typing import List, NamedTuple, Optional, Union
 
 import numpy as np
 import torch
 from torch import nn, Tensor
+
+
+_BINNED_MAX_OUT = 256          # adim * bins the binned kernels take (es_rollout_openloop_binned, es_rollout_closedloop_mlp_binned)
+
+
+class BinnedHead(NamedTuple):
+    """FFBinned's head as the fused rollouts take it: ``bins`` outputs per action dimension, the action
+    ``1 / (bins - 1) * argmax * (high - low) + low`` in float32 (nn.py:114-117)."""
+    bins: int
+    low: np.ndarray                 # float32 [adim]
+    high: np.ndarray                # float32 [adim]
+
+    @property
+    def adim(self) -> int:
+        return int(self.low.shape[0])
+
+    def key(self) -> tuple:
+        """What identifies the head's arithmetic (a cache key)."""
+        return ('binned', self.bins, self.low.tobytes(), self.high.tobytes())
+
+    def device_arrays(self, engine):
+        """(low, high - low) as float32 device tensors; ``high - low`` is rounded to float32 as FFBinned.forward's ac_range."""
+        low = np.ascontiguousarray(self.low, dtype=np.float32)
+        rng = np.ascontiguousarray(np.asarray(self.high, dtype=np.float32) - low, dtype=np.float32)
+        return engine.to_device(low), engine.to_device(rng)
 
 
 class BaseNet(nn.Module, ABC):
@@ -40,9 +65,36 @@ class BaseNet(nn.Module, ABC):
         are stepped through their own forward)."""
         if type(self).forward is not FeedForward.forward:
             return False
+        return self._tanh_stack()
+
+    def _tanh_stack(self) -> bool:
         mods = list(self.model)
         return (len(mods) % 2 == 0 and all(isinstance(m, nn.Linear) for m in mods[0::2])
                 and all(isinstance(m, nn.Tanh) for m in mods[1::2]))
+
+    def head(self) -> Optional[Union[str, BinnedHead]]:
+        """How the fused rollout kernels turn this network's outputs into actions: ``'tanh'`` for the tanh MLPs of
+        ``is_tanh_mlp`` (the outputs are the actions), a ``BinnedHead`` for an FFBinned the kernels evaluate exactly as its
+        forward does, None for anything else (stepped through the module's own forward, as the reference does).
+
+        An FFBinned is fused when it is a Linear + Tanh stack, its action bounds are float32 arrays of shape [adim] (with
+        float64 bounds FFBinned.forward computes the action in float64 and rounds once; the kernels round every operation
+        to float32), ``bins >= 2`` (the reference divides by ``bins - 1``), ``adim * bins <= 256`` outputs and every layer
+        fits the float32 kernel's activation tiles (the limit ``es_rollout_openloop_binned`` refuses beyond)."""
+        if self.is_tanh_mlp():
+            return 'tanh'
+        if type(self).forward is not FFBinned.forward or not self._tanh_stack():
+            return None
+        low, high = np.asarray(self.alow), np.asarray(self.ahigh)
+        adim, bins = int(self.adim), int(self.bins)
+        if low.dtype != np.float32 or high.dtype != np.float32 or low.shape != (adim,) or high.shape != (adim,):
+            return None
+        sizes = self.layer_sizes()
+        if bins < 2 or sizes[-1] != adim * bins or sizes[-1] > _BINNED_MAX_OUT:
+            return None
+        if 2 * 32 * max((s + 3) & ~3 for s in sizes) * 4 + 32 * 8 > 227 * 1024:       # rollout_f32.cu's activation tiles
+            return None
+        return BinnedHead(bins, low.copy(), high.copy())
 
 
 class FeedForward(BaseNet):

@@ -140,6 +140,24 @@ int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_
                                  double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
                                  const float* act_noise, int n_episodes, int mode, void* stream);
 
+/* The same open-loop rollout for a binned-action policy (FFBinned, src/nn/nn.py:99-117): layer_sizes ends in adim * bins
+ * tanh outputs; per step and action dimension j the action is the first maximal of its bins outputs (torch.argmax), idx,
+ * mapped to float32 ((scale * idx) * range[j]) + low[j] with scale = float32(1 / (bins - 1)), each operation rounded to float32
+ * as FFBinned.forward's torch expression.  Reward (a float32 dot in index order) and position use the adim actions; rew_vec is
+ * [T][adim].  No action noise: FFBinned draws none.
+ *   bins >= 2 (ES_ERR_INVALID otherwise), adim * bins <= 256 (ES_ERR_UNSUPPORTED otherwise)
+ *   low, range dev float [adim]: action_space.low and float32(high - low)
+ *   mode: ES_ROLLOUT_F32 = the general float32 kernel (rollout_f32.cu, with its time split for fewer pairs than SMs; never the
+ *                          packed-FMA kernel);
+ *         ES_ROLLOUT_TC3 = rollout_tcw.cu for 2 to 4 hidden layers of widths in {64, 128, 192, 256} (obs-64-64-X included) and
+ *                          obs <= 256, ES_ERR_UNSUPPORTED otherwise;
+ *         ES_ROLLOUT_TC  = ES_ERR_UNSUPPORTED: an arg-max over float16-grade outputs is not parity grade.                  */
+int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                               const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                               const float* obsn, const float* rew_vec, int T, float pos_scale,
+                               double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                               int bins, const float* low, const float* range, int mode, void* stream);
+
 /* ---- a3 + a4 + a5 on the CLOSED-LOOP synthetic env (SURVEY.md section 8d's optional variant; never part of the headline) --
  * obs_{t+1} = tanh(A obs_t + B a_t): the observation depends on the policy's own actions, so the episode runs step by step
  * with one pair's perturbed weights resident on chip (rollout_closed.cu).  Replaces the same reference loop as
@@ -183,6 +201,23 @@ int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len
  * and the dynamic shared memory per CTA.  ES_ERR_UNSUPPORTED with es_rollout_closedloop_mlp's message for an uncovered shape. */
 int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int* cluster_size, int* clusters,
                                    int64_t* smem_bytes);
+
+/* es_rollout_closedloop_mlp for a binned-action policy, the head as in es_rollout_openloop_binned: layer_sizes ends in
+ * adim * bins <= 256 outputs, env_b is [adim][obs], rew_vec [T][adim].  Every covered shape (the hidden layers, obs, band and
+ * shared-memory limits of es_rollout_closedloop_mlp, adim <= 64) runs rollout_closedw.cu's cluster kernel, a cluster of one
+ * CTA included; each CTA forms the actions from its copy of the output layer.  One kernel launch per call.             */
+int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                     const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                     const double* ob_mean, const double* ob_std, double ob_clip,
+                                     const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
+                                     int T, float pos_scale, const uint32_t* coin_words, double save_obs_chance,
+                                     double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                                     double* ob_sum, double* ob_sumsq, double* ob_count, int bins, const float* low,
+                                     const float* range, void* stream);
+/* es_rollout_closedloop_mlp_plan for es_rollout_closedloop_mlp_binned: the cluster size (>= 1), resident clusters and
+ * dynamic shared memory per CTA of a binned shape, or its refusal.                                                   */
+int es_rollout_closedloop_mlp_binned_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int bins,
+                                          int* cluster_size, int* clusters, int64_t* smem_bytes);
 
 /* ---- a2 + a4 with action noise: all draws of a generation in stream order ---------------------------------------------
  * When FeedForward._action_std != 0 every step of every rollout draws rs.randn(act_dim) from the SAME RandomState that
