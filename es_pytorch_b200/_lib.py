@@ -44,7 +44,10 @@ SIGNATURES = {
                                      _vp, _vp, _i32, _f32, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     'es_rollout_closedloop_mlp': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64, _vp, _vp,
                                          _i32, _vp, _vp, _i32, _f32, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'es_rollout_closedloop_mlp_plan': (_i32, [_vp, C.POINTER(_i32), _i32, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i64)]),
+    'es_rollout_closedloop_mlp_episodes': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64,
+                                                  _vp, _vp, _i32, _vp, _vp, _i32, _f32, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _vp,
+                                                  _vp, _vp, _vp, _i32, _vp]),
+    'es_rollout_closedloop_mlp_plan':(_i32, [_vp, C.POINTER(_i32), _i32, _i32, C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i64)]),
     'es_rollout_openloop_binned': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _i32,
                                           _f32, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _i32, _vp]),
     'es_rollout_closedloop_mlp_binned': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64, _vp,

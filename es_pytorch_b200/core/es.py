@@ -196,7 +196,7 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
                                archive=archive, nov_k=fit_fn.nov_k, rollout_mode=fit_fn.rollout_mode, engine=eng,
                                ac_std=float(getattr(policy._module, '_action_std', 0.0) or 0.0),
                                closed=env.device_closed(eng) if getattr(env, 'is_synthetic_closedloop', False) else None,
-                               episodes=fit_fn.episodes, head=head)
+                               episodes=fit_fn.episodes, head=head, closed_act_noise=True)
         fit_fn._gen = gen
     else:
         gen.load_states(streams)

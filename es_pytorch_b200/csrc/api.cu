@@ -377,15 +377,18 @@ int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_la
     return es_closedw_max_clusters(n_layers, C, smem, clusters);
 }
 
-int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
-                              int P, float sigma, const int* layer_sizes, int n_layers, const double* ob_mean, const double* ob_std,
-                              double ob_clip, const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
-                              int T, float pos_scale, const uint32_t* coin_words, double save_obs_chance, double* fit_pos,
-                              double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
-                              double* ob_count, void* stream) {
+int es_rollout_closedloop_mlp_episodes(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                       const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                       const double* ob_mean, const double* ob_std, double ob_clip, const float* obs0,
+                                       const float* env_a, int band, const float* env_b, const float* rew_vec, int T, float pos_scale,
+                                       const uint32_t* coin_words, double save_obs_chance, double* fit_pos, double* fit_neg,
+                                       int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
+                                       double* ob_count, const float* act_noise, int n_episodes, void* stream) {
     ES_ENTER(ctx);
+    ES_REQUIRE(n_episodes >= 1, "es_rollout_closedloop_mlp: n_episodes must be >= 1, got %d", n_episodes);
+    // without action noise the episodes are identical: the noise-free kernels run one (as es_rollout_openloop_episodes)
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1};
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
     int rc = es_rollout_check("es_rollout_closedloop_mlp", ob_mean && ob_std && obs0 && env_a && env_b, r);
     if (rc) return rc;
     ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop_mlp: band must be in [1, obs_dim]");
@@ -396,9 +399,27 @@ int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len
     rc = es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);      // coverage does not depend on n_pairs
     if (rc) return rc;
     if (n_pairs == 0) return ES_OK;
-    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    if (r.n_episodes > 1) {
+        void* rows = nullptr;
+        rc = es_ctx_scratch(ctx, (size_t)2 * ctx->sm_count * T * sizeof(double), &rows);
+        if (rc) return rc;
+        env.ep_rows = (double*)rows;
+    }
     if (es_closed_one_cta_covers(layer_sizes, n_layers)) return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
     return es_impl_rollout_closedw(ctx, r, env, (cudaStream_t)stream);
+}
+
+int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
+                              int P, float sigma, const int* layer_sizes, int n_layers, const double* ob_mean, const double* ob_std,
+                              double ob_clip, const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
+                              int T, float pos_scale, const uint32_t* coin_words, double save_obs_chance, double* fit_pos,
+                              double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
+                              double* ob_count, void* stream) {
+    return es_rollout_closedloop_mlp_episodes(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, ob_mean,
+                                              ob_std, ob_clip, obs0, env_a, band, env_b, rew_vec, T, pos_scale, coin_words,
+                                              save_obs_chance, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, ob_sum, ob_sumsq,
+                                              ob_count, nullptr, 1, stream);
 }
 
 int es_rollout_closedloop_mlp_binned_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size,

@@ -102,7 +102,7 @@ struct EsRollout {
     int fit_stride;
     float* behv_pos;            // [n_pairs][3] or NULL
     float* behv_neg;
-    const float* act_noise;     // open loop: scaled action noise [n_pairs][2][n_episodes][T][act] (mt_gauss.cu) or NULL
+    const float* act_noise;     // scaled action noise [n_pairs][2][n_episodes][T][act] (mt_gauss.cu) or NULL
     int* err;                   // the ctx's error word (es_checked_slice)
     int n_episodes;             // episodes per evaluation, averaged per step (>= 1; 1 when act_noise is NULL)
     // the policy head: bins == 0, the tanh outputs are the actions; bins >= 2, a binned-action policy (FFBinned): the last
@@ -125,6 +125,9 @@ struct EsClosedEnv {
     double* ob_sum;             // [obs], or NULL with ob_sumsq and ob_count
     double* ob_sumsq;
     double* ob_count;           // [2]
+    // with action noise and n_episodes > 1: the per-step float64 episode sums, [2 sm_count][T] (a [2][T] pair per CTA of
+    // rollout_closed.cu, a [T] row per cluster of rollout_closedw.cu; either grid has at most sm_count CTAs / clusters)
+    double* ep_rows;
 };
 
 // ---- entry points implemented one per .cu file (called from api.cu) -------------------------

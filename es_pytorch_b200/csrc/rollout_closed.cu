@@ -20,6 +20,13 @@
 //     post-step observations for the ObStat of a rollout whose save_obs coin fell;
 //   * reward (float32 dot in index order, summed in float64 like python's sum) and position by the last warp.
 // Four barriers per step.
+//
+// Action noise and episodes (rollout_closed_noisy_kernel, es_rollout_closedloop_mlp_episodes): FeedForward.forward adds
+// rs.randn(act) * ac_std to the action (src/nn/nn.py:47-48) and obj.py:54-63 averages E episodes per evaluation.  The lane
+// that writes a row of layer 3 adds its (+ or -) noise value, loaded at the top of the step like the reward coefficients, so
+// the env step, the reward and the position all see the noisy action.  Each episode restarts the env from obs_0 with the
+// weights left in place; the per-step float64 sums of episodes 0 .. E - 2 go to a [2][T] row per CTA in global memory, and the
+// last episode adds (row[t] + r) / E to the fitness and keeps the behaviour and the ObStat sums.
 #include <math.h>
 #include "common.cuh"
 #include "mt19937.cuh"
@@ -45,6 +52,8 @@ struct ClParams {
     float* behv_pos; float* behv_neg;
     double* ob_sum; double* ob_sumsq; double* ob_count;
     int* err;
+    const float* act_noise; int n_eps;      // [n_pairs][2][n_eps][T][act] (rollout_closed_noisy_kernel only)
+    double* ep_row;                         // [gridDim.x][2][T] per-step episode sums (n_eps > 1)
 };
 
 struct ClLayout {                          // offsets in floats into dynamic shared memory
@@ -89,20 +98,23 @@ __device__ __forceinline__ float cl_tanh(float x) {
 }
 // the float32 pairs (es_f32x2) of this kernel hold (+, -) of a weight times (x+, x-) of an input
 // the four rows of a warp: z[r] (+, -) -> tanh(z + bias) of row 4 w + r, written by the lane that ends up with that sum
+// (lanes 4 q: row 4 w + q / 2, sign q & 1); NZ: plus that lane's action noise nz
+template <bool NZ = false>
 __device__ __forceinline__ void cl_finish_rows(const es_f32x2 (&z)[4], int warp, int lane, int rows, const float* __restrict__ bias_p,
-                                               const float* __restrict__ bias_m, float* __restrict__ out2) {
+                                               const float* __restrict__ bias_m, float* __restrict__ out2, float nz = 0.f) {
     float v[8];
 #pragma unroll
     for (int r = 0; r < 4; ++r) es_unpack2(z[r], v[2 * r], v[2 * r + 1]);
     const float c = es_warp_sum8(v, lane);
     if ((lane & 3) == 0) {
         const int q = lane >> 2, o = 4 * warp + (q >> 1), sg = q & 1;
-        out2[2 * o + sg] = (o < rows) ? cl_tanh(c + (sg ? bias_m : bias_p)[o]) : 0.f;
+        out2[2 * o + sg] = (o < rows) ? (NZ ? __fadd_rn(cl_tanh(c + (sg ? bias_m : bias_p)[o]), nz)
+                                            : cl_tanh(c + (sg ? bias_m : bias_p)[o])) : 0.f;
     }
 }
 
-template <int JL>
-__global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClParams p) {
+template <int JL, bool NOISY>
+__device__ __forceinline__ void cl_rollout(const ClParams& p) {
     extern __shared__ __align__(16) float cl_smem[];
     const ClLayout L = cl_layout(JL, p.obs, p.act, p.band);
     double* __restrict__ nmean = reinterpret_cast<double*>(cl_smem + L.norm);
@@ -182,13 +194,16 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
             es_unpack2(tid < act ? wpm(off.b3 + tid) : 0ull, a, b);
             bias[4 * CL_H + tid] = a; bias[5 * CL_H + tid] = b;
         }
-        for (int i = tid; i < obs; i += CL_THREADS) {
-            const float v = p.obs0[i];
-            put_obs(o2, i, make_float2(v, v));
-            const float xn = cl_normalise(v, nmean[i], nrstd[i], p.ob_clip);
-            x2[i] = make_float2(xn, xn);
-            stat[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
+        auto start_episode = [&]() {                                // a fresh env: obs_0, position 0
+            for (int i = tid; i < obs; i += CL_THREADS) {
+                const float v = p.obs0[i];
+                put_obs(o2, i, make_float2(v, v));
+                const float xn = cl_normalise(v, nmean[i], nrstd[i], p.ob_clip);
+                x2[i] = make_float2(xn, xn);
+                stat[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+        };
+        start_episode();
         if (tid < 2) rfit[tid] = 0.0;
         if (tid < 6) rpos[tid] = 0.f;
         // the save_obs coins of the pair's two evaluations (legacy random_sample < chance)
@@ -201,109 +216,139 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
         const bool keep_stat = p.ob_sum && (save_p || save_m);
         __syncthreads();
 
-        for (int t = 0; t < T; ++t) {
-            const int cur = t & 1;
-            float crow0 = 0.f, crow1 = 0.f;
-            if (rew_warp) {                                         // this step's reward coefficients: in flight under the layers
-                const float* __restrict__ c = p.crew + (size_t)t * act;
-                if (lane < act) crow0 = __ldg(c + lane);
-                if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
+        const int n_eps = NOISY ? p.n_eps : 1;
+        for (int ep = 0; ep < n_eps; ++ep) {
+            const bool last_ep = ep == n_eps - 1;
+            const bool add_stat = keep_stat && last_ep;                 // behaviour and ObStat: the last episode's
+            if (NOISY && ep > 0) {
+                start_episode();
+                if (tid < 6) rpos[tid] = 0.f;
+                __syncthreads();
             }
-            // ---- layer 1: 4 rows x JL elements per lane, weights in registers, every input read once per warp ----
-            {
-                es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
-                const es_f32x2* __restrict__ xv = reinterpret_cast<const es_f32x2*>(x2) + lane;
-#pragma unroll
-                for (int j = 0; j < JL; ++j) {
-                    const es_f32x2 x = xv[32 * j];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) z[r] = es_fma2(w1[r][j], x, z[r]);
-                }
-                cl_finish_rows(z, warp, lane, h1, bias, bias + CL_H, reinterpret_cast<float*>(h1v));
+
+            // this CTA's episode sums of the + / - evaluation, and the noise of the episode (row o of sign sg at lanes 4 q of the
+            // warps that hold layer 3's rows, as cl_finish_rows writes them)
+            double* __restrict__ erow = NOISY ? p.ep_row + (size_t)blockIdx.x * 2 * T : nullptr;
+            const float* __restrict__ nzp = nullptr;
+            if (NOISY && l3_warp && (lane & 3) == 0) {
+                const int q = lane >> 2, o = 4 * warp + (q >> 1), sg = q & 1;
+                if (o < act) nzp = p.act_noise + (((size_t)pair * 2 + sg) * n_eps + ep) * T * act + o;
             }
-            __syncthreads();
-            // ---- layer 2 ----
-            {
-                es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
-                const es_f32x2* __restrict__ hv = reinterpret_cast<const es_f32x2*>(h1v) + lane;
-                const es_f32x2* __restrict__ wr = W2 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
-#pragma unroll
-                for (int j = 0; j < CL_J23; ++j) {
-                    const es_f32x2 x = hv[32 * j];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) z[r] = es_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
+
+            for (int t = 0; t < T; ++t) {
+                const int cur = t & 1;
+                float crow0 = 0.f, crow1 = 0.f;
+                double esum = 0.0;                                      // the earlier episodes' rewards of this step
+                if (rew_warp) {                                         // this step's reward coefficients: in flight under the layers
+                    const float* __restrict__ c = p.crew + (size_t)t * act;
+                    if (lane < act) crow0 = __ldg(c + lane);
+                    if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
+                    if (NOISY && lane < 2 && ep > 0) esum = erow[(size_t)lane * T + t];
                 }
-                cl_finish_rows(z, warp, lane, h2, bias + 2 * CL_H, bias + 3 * CL_H, reinterpret_cast<float*>(h2v));
-            }
-            __syncthreads();
-            // ---- layer 3 (only the warps that hold its rows) ----
-            if (l3_warp) {
-                es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
-                const es_f32x2* __restrict__ hv = reinterpret_cast<const es_f32x2*>(h2v) + lane;
-                const es_f32x2* __restrict__ wr = W3 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
-#pragma unroll
-                for (int j = 0; j < CL_J23; ++j) {
-                    const es_f32x2 x = hv[32 * j];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) z[r] = es_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
-                }
-                cl_finish_rows(z, warp, lane, act, bias + 4 * CL_H, bias + 5 * CL_H, reinterpret_cast<float*>(a2));
-            }
-            __syncthreads();
-            // ---- env step: thread i owns observation i; the raw observations carry a wrap-around halo, so the band is a
-            //      linear read ----
-            if (tid < obs) {
-                const float2* __restrict__ oc = o2 + cur * o2s;
-                const int i = tid;
-                float ap = 0.f, am = 0.f, ap1 = 0.f, am1 = 0.f;
-#pragma unroll 4
-                for (int d = 0; d < band; d += 2) {                 // (band is even, checked on the host)
-                    const float w0 = envA[d * obs + i], w1_ = envA[(d + 1) * obs + i];
-                    const float2 u0 = oc[i + d], u1 = oc[i + d + 1];
-                    ap = fmaf(w0, u0.x, ap); am = fmaf(w0, u0.y, am);
-                    ap1 = fmaf(w1_, u1.x, ap1); am1 = fmaf(w1_, u1.y, am1);
-                }
-#pragma unroll 2
-                for (int j = 0; j < act_pad; j += 2) {
-                    const float w0 = envB[j * obs + i], w1_ = envB[(j + 1) * obs + i];
-                    const float4 av = *reinterpret_cast<const float4*>(a2 + j);
-                    ap = fmaf(w0, av.x, ap); am = fmaf(w0, av.y, am);
-                    ap1 = fmaf(w1_, av.z, ap1); am1 = fmaf(w1_, av.w, am1);
-                }
-                const float np_ = cl_tanh(ap + ap1), nm = cl_tanh(am + am1);
-                put_obs(o2 + (cur ^ 1) * o2s, i, make_float2(np_, nm));
-                const double mu = nmean[i], rs_ = nrstd[i];
-                x2[i] = make_float2(cl_normalise(np_, mu, rs_, p.ob_clip), cl_normalise(nm, mu, rs_, p.ob_clip));
-                if (keep_stat) {                                    // float32 column sums in step order (numpy's axis-0 reduction)
-                    float4 st = stat[i];
-                    st.x = __fadd_rn(st.x, np_); st.y = __fadd_rn(st.y, __fmul_rn(np_, np_));
-                    st.z = __fadd_rn(st.z, nm);  st.w = __fadd_rn(st.w, __fmul_rn(nm, nm));
-                    stat[i] = st;
-                }
-            }
-            // ---- reward and position: the last warp's lanes form the products, lanes 0 / 1 add them in index order (the env's
-            //      float32 dot) for the + / - evaluation ----
-            if (rew_warp) {
-                if (lane < act) { const float2 av = a2[lane]; prod[lane] = make_float2(__fmul_rn(av.x, crow0), __fmul_rn(av.y, crow0)); }
-                if (lane + 32 < act) { const float2 av = a2[lane + 32]; prod[lane + 32] = make_float2(__fmul_rn(av.x, crow1), __fmul_rn(av.y, crow1)); }
-                __syncwarp();
-                if (lane < 2) {
-                    float acc = 0.f;
-#pragma unroll 8
-                    for (int j = 0; j < act; ++j) {
-                        const float2 pv = prod[j];
-                        acc = __fadd_rn(acc, lane ? pv.y : pv.x);
+                float nz = 0.f;                                         // this lane's action noise: in flight under layers 1 / 2
+                if (NOISY && nzp) nz = __ldg(nzp + (size_t)t * act);
+                // ---- layer 1: 4 rows x JL elements per lane, weights in registers, every input read once per warp ----
+                {
+                    es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
+                    const es_f32x2* __restrict__ xv = reinterpret_cast<const es_f32x2*>(x2) + lane;
+    #pragma unroll
+                    for (int j = 0; j < JL; ++j) {
+                        const es_f32x2 x = xv[32 * j];
+    #pragma unroll
+                        for (int r = 0; r < 4; ++r) z[r] = es_fma2(w1[r][j], x, z[r]);
                     }
-                    rfit[lane] += (double)acc;
-                    const float ps = p.pos_scale;
-                    const float2 q0 = a2[0], q1 = a2[1 % act], q2 = a2[2 % act];
-                    rpos[lane * 3 + 0] = __fadd_rn(rpos[lane * 3 + 0], __fmul_rn(ps, lane ? q0.y : q0.x));
-                    rpos[lane * 3 + 1] = __fadd_rn(rpos[lane * 3 + 1], __fmul_rn(ps, lane ? q1.y : q1.x));
-                    rpos[lane * 3 + 2] = __fadd_rn(rpos[lane * 3 + 2], __fmul_rn(ps, lane ? q2.y : q2.x));
+                    cl_finish_rows(z, warp, lane, h1, bias, bias + CL_H, reinterpret_cast<float*>(h1v));
                 }
-                __syncwarp();
+                __syncthreads();
+                // ---- layer 2 ----
+                {
+                    es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
+                    const es_f32x2* __restrict__ hv = reinterpret_cast<const es_f32x2*>(h1v) + lane;
+                    const es_f32x2* __restrict__ wr = W2 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
+    #pragma unroll
+                    for (int j = 0; j < CL_J23; ++j) {
+                        const es_f32x2 x = hv[32 * j];
+    #pragma unroll
+                        for (int r = 0; r < 4; ++r) z[r] = es_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
+                    }
+                    cl_finish_rows(z, warp, lane, h2, bias + 2 * CL_H, bias + 3 * CL_H, reinterpret_cast<float*>(h2v));
+                }
+                __syncthreads();
+                // ---- layer 3 (only the warps that hold its rows) ----
+                if (l3_warp) {
+                    es_f32x2 z[4] = {0ull, 0ull, 0ull, 0ull};
+                    const es_f32x2* __restrict__ hv = reinterpret_cast<const es_f32x2*>(h2v) + lane;
+                    const es_f32x2* __restrict__ wr = W3 + (size_t)(4 * warp) * CL_J23 * 32 + lane;
+    #pragma unroll
+                    for (int j = 0; j < CL_J23; ++j) {
+                        const es_f32x2 x = hv[32 * j];
+    #pragma unroll
+                        for (int r = 0; r < 4; ++r) z[r] = es_fma2(wr[(r * CL_J23 + j) * 32], x, z[r]);
+                    }
+                    cl_finish_rows<NOISY>(z, warp, lane, act, bias + 4 * CL_H, bias + 5 * CL_H, reinterpret_cast<float*>(a2), nz);
+                }
+                __syncthreads();
+                // ---- env step: thread i owns observation i; the raw observations carry a wrap-around halo, so the band is a
+                //      linear read ----
+                if (tid < obs) {
+                    const float2* __restrict__ oc = o2 + cur * o2s;
+                    const int i = tid;
+                    float ap = 0.f, am = 0.f, ap1 = 0.f, am1 = 0.f;
+    #pragma unroll 4
+                    for (int d = 0; d < band; d += 2) {                 // (band is even, checked on the host)
+                        const float w0 = envA[d * obs + i], w1_ = envA[(d + 1) * obs + i];
+                        const float2 u0 = oc[i + d], u1 = oc[i + d + 1];
+                        ap = fmaf(w0, u0.x, ap); am = fmaf(w0, u0.y, am);
+                        ap1 = fmaf(w1_, u1.x, ap1); am1 = fmaf(w1_, u1.y, am1);
+                    }
+    #pragma unroll 2
+                    for (int j = 0; j < act_pad; j += 2) {
+                        const float w0 = envB[j * obs + i], w1_ = envB[(j + 1) * obs + i];
+                        const float4 av = *reinterpret_cast<const float4*>(a2 + j);
+                        ap = fmaf(w0, av.x, ap); am = fmaf(w0, av.y, am);
+                        ap1 = fmaf(w1_, av.z, ap1); am1 = fmaf(w1_, av.w, am1);
+                    }
+                    const float np_ = cl_tanh(ap + ap1), nm = cl_tanh(am + am1);
+                    put_obs(o2 + (cur ^ 1) * o2s, i, make_float2(np_, nm));
+                    const double mu = nmean[i], rs_ = nrstd[i];
+                    x2[i] = make_float2(cl_normalise(np_, mu, rs_, p.ob_clip), cl_normalise(nm, mu, rs_, p.ob_clip));
+                    if (add_stat) {                                     // float32 column sums in step order (numpy's axis-0 reduction)
+                        float4 st = stat[i];
+                        st.x = __fadd_rn(st.x, np_); st.y = __fadd_rn(st.y, __fmul_rn(np_, np_));
+                        st.z = __fadd_rn(st.z, nm);  st.w = __fadd_rn(st.w, __fmul_rn(nm, nm));
+                        stat[i] = st;
+                    }
+                }
+                // ---- reward and position: the last warp's lanes form the products, lanes 0 / 1 add them in index order (the env's
+                //      float32 dot) for the + / - evaluation ----
+                if (rew_warp) {
+                    if (lane < act) { const float2 av = a2[lane]; prod[lane] = make_float2(__fmul_rn(av.x, crow0), __fmul_rn(av.y, crow0)); }
+                    if (lane + 32 < act) { const float2 av = a2[lane + 32]; prod[lane + 32] = make_float2(__fmul_rn(av.x, crow1), __fmul_rn(av.y, crow1)); }
+                    __syncwarp();
+                    if (lane < 2) {
+                        float acc = 0.f;
+    #pragma unroll 8
+                        for (int j = 0; j < act; ++j) {
+                            const float2 pv = prod[j];
+                            acc = __fadd_rn(acc, lane ? pv.y : pv.x);
+                        }
+                        if (!NOISY) {
+                            rfit[lane] += (double)acc;
+                        } else if (!last_ep) {                          // the float64 per-step sum over the episodes, in their order
+                            erow[(size_t)lane * T + t] = esum + (double)acc;
+                        } else {                                        // ... and its mean (obj.py:57-61)
+                            rfit[lane] += (esum + (double)acc) / n_eps;
+                        }
+                        const float ps = p.pos_scale;
+                        const float2 q0 = a2[0], q1 = a2[1 % act], q2 = a2[2 % act];
+                        rpos[lane * 3 + 0] = __fadd_rn(rpos[lane * 3 + 0], __fmul_rn(ps, lane ? q0.y : q0.x));
+                        rpos[lane * 3 + 1] = __fadd_rn(rpos[lane * 3 + 1], __fmul_rn(ps, lane ? q1.y : q1.x));
+                        rpos[lane * 3 + 2] = __fadd_rn(rpos[lane * 3 + 2], __fmul_rn(ps, lane ? q2.y : q2.x));
+                    }
+                    __syncwarp();
+                }
+                __syncthreads();
             }
-            __syncthreads();
         }
         if (rew_warp && lane < 2) {
             (lane ? p.fit_neg : p.fit_pos)[(size_t)pair * p.fit_stride] = rfit[lane];
@@ -329,6 +374,11 @@ __global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClP
 }
 
 template <int JL>
+__global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_kernel(const ClParams p) { cl_rollout<JL, false>(p); }
+template <int JL>
+__global__ void __launch_bounds__(CL_THREADS, 1) rollout_closed_noisy_kernel(const ClParams p) { cl_rollout<JL, true>(p); }
+
+template <int JL>
 int cl_launch(es_ctx* ctx, const ClParams& p, cudaStream_t stream) {
     const ClLayout L = cl_layout(JL, p.obs, p.act, p.band);
     const size_t smem = (size_t)L.total * sizeof(float);
@@ -337,9 +387,14 @@ int cl_launch(es_ctx* ctx, const ClParams& p, cudaStream_t stream) {
                      p.act, p.band);
         return ES_ERR_UNSUPPORTED;
     }
-    ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_closed_kernel<JL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int grid = p.n_pairs < ctx->sm_count ? p.n_pairs : ctx->sm_count;
-    rollout_closed_kernel<JL><<<grid, CL_THREADS, smem, stream>>>(p);
+    if (p.act_noise) {
+        ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_closed_noisy_kernel<JL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        rollout_closed_noisy_kernel<JL><<<grid, CL_THREADS, smem, stream>>>(p);
+    } else {
+        ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_closed_kernel<JL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        rollout_closed_kernel<JL><<<grid, CL_THREADS, smem, stream>>>(p);
+    }
     ES_LAUNCHED(ctx);
     return ES_OK;
 }
@@ -357,6 +412,7 @@ int es_impl_rollout_closed(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& e
     p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.fit_stride = r.fit_stride; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
     p.ob_sum = env.ob_sum; p.ob_sumsq = env.ob_sumsq; p.ob_count = env.ob_count;
     p.err = r.err;
+    p.act_noise = r.act_noise; p.n_eps = r.act_noise ? r.n_episodes : 1; p.ep_row = env.ep_rows;
     if (p.h1 > CL_H || p.h2 > CL_H || p.act > CL_A || p.obs > 384 || p.band > CL_HALO || p.obs < p.band || (p.band & 1)) {
         es_set_error("es_rollout_closedloop: supports even band <= obs <= 384, hidden <= %d, act <= %d, band <= %d (got %d-%d-%d-%d, band %d)",
                      CL_H, CL_A, CL_HALO, p.obs, p.h1, p.h2, p.act, p.band);

@@ -22,7 +22,8 @@
 //     transposing butterfly (7 shuffles) adds the 32 lane sums in the fixed xor-16, 8, 4, 2, 1 tree.  A row's value therefore
 //     depends on neither C, nor the warp that computes it, nor the grid, nor the order of the pairs;
 //   * activation exchange: the lane that holds a row's tanh stores it into the layer's activation buffer of EVERY CTA of the
-//     cluster (mapa + st.shared::cluster, its own included), then the cluster meets at barrier.cluster.arrive.release /
+//     cluster (mapa + st.shared::cluster, its own included; for the output layer with action noise, the tanh plus the row's
+//     noise, so every CTA receives the noisy action), then the cluster meets at barrier.cluster.arrive.release /
 //     wait.acquire.  Every layer has its own buffer (the input x, a_0 .. a_{L-1}, the last being the action), so that one
 //     barrier per layer (B_0 .. B_{L-1} of a step) orders all remote writes:
 //       - write-after-read: a_l is read by layer l + 1 of step t before the reader arrives at B_{l+1}(t) (for the action
@@ -47,6 +48,14 @@
 // a local action buffer, then a __syncthreads, before the env step.  The env's B, the reward and the position use adim.  That
 // buffer is written after B_{L-1}(t) and read within step t only, so the barrier argument above is unchanged.  Binned shapes
 // always run here (C = 1 included): rollout_closed.cu has no head.
+// Action noise and episodes (rollout_closedw_noisy_kernel, es_rollout_closedloop_mlp_episodes; tanh heads only): the lane that
+// owns an output row adds its noise value (loaded at the top of the step: a CTA owns <= 64 output rows, so one pass of its 16
+// warps covers them) before the remote stores above, which is the only change inside a step, so the barrier argument holds as
+// it is.  The E episodes of an evaluation run in sequence in its cluster, the weights left in place: each restarts x, the raw
+// observation and the position locally (a step boundary as far as the barriers are concerned); rank 0's reward lane keeps the
+// float64 per-step sums of episodes 0 .. E - 2 in a [T] row per cluster in global memory, and the last episode adds
+// (row[t] + r) / E to the fitness and keeps the behaviour and the ObStat sums.  Spreading the episodes over clusters would
+// only help with fewer evaluations than resident clusters, and would make the result depend on the grid.
 // Alternatives not built (so not measured): weights partly in registers (rollout_closed.cu's layer 1), and a pair (both signs)
 // per cluster, which doubles the footprint to save only the load-time reads of eps.
 #include <math.h>
@@ -79,6 +88,8 @@ struct CwParams {
     double* ob_sum; double* ob_sumsq; double* ob_count;
     int* err;
     int adim, bins; float scale; const float* low; const float* range;      // binned head (rollout_closedw_binned_kernel only)
+    const float* act_noise; int n_eps;      // [n_pairs][2][n_eps][T][act] (rollout_closedw_noisy_kernel only)
+    double* ep_row;                         // [clusters][T] per-step episode sums (n_eps > 1)
 };
 
 __host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
@@ -165,7 +176,7 @@ __device__ __forceinline__ void cw_store_remote(float* local, unsigned rank, flo
 // one layer of this CTA in the step loop (read from shared memory: a per-layer index into registers would go to local memory)
 struct CwLayer { int in, nr, S, r0, w, bias, xin, out, woff, boff; };
 
-template <int NL, bool BINNED>
+template <int NL, bool BINNED, bool NOISY>
 __device__ __forceinline__ void cw_rollout(const CwParams& p) {
     extern __shared__ __align__(16) float cw_smem[];
     __shared__ CwLayer cw_layers[NL];
@@ -229,12 +240,15 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                     W[r * S + k] = (r < ly.nr && k < in) ? w_at(ly.woff + (ly.r0 + r) * in + k) : 0.f;
             for (int r = tid; r < R4; r += CW_THREADS) cw_smem[ly.bias + r] = r < ly.nr ? w_at(ly.boff + ly.r0 + r) : 0.f;
         }
-        for (int i = tid; i < obs; i += CW_THREADS) {
-            const float v = p.obs0[i];
-            put_obs(o2, i, v);
-            x[i] = cw_normalise(v, nmean[i], nstd[i], p.ob_clip);
-            stat[i] = make_float2(0.f, 0.f);
-        }
+        auto start_episode = [&]() {                        // a fresh env: obs_0, position 0
+            for (int i = tid; i < obs; i += CW_THREADS) {
+                const float v = p.obs0[i];
+                put_obs(o2, i, v);
+                x[i] = cw_normalise(v, nmean[i], nstd[i], p.ob_clip);
+                stat[i] = make_float2(0.f, 0.f);
+            }
+        };
+        start_episode();
         if (tid == 0) { rfit[0] = 0.0; rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
         bool save = false;                                  // the evaluation's save_obs coin (legacy random_sample < chance)
         if (p.coins) {
@@ -244,88 +258,119 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
         const bool keep_stat = rank == 0 && p.ob_sum && save;
         __syncthreads();
 
-        for (int t = 0; t < T; ++t) {
-            const int cur = t & 1;
-            float crow0 = 0.f, crow1 = 0.f;
-            if (rew_warp) {                                 // this step's reward coefficients: in flight under the layers
-                const float* __restrict__ c = p.crew + (size_t)t * act;
-                if (lane < act) crow0 = __ldg(c + lane);
-                if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
-            }
-            // ---- the layers: 4 rows per warp and pass, each row's tanh stored into every CTA's a_l, then B_l ----
-#pragma unroll 1
-            for (int l = 0; l < NL; ++l) {
-                const CwLayer ly = cw_layers[l];
-                const int S = ly.S, r0 = ly.r0, nr = ly.nr, nj = S >> 5;
-                const float* __restrict__ xin = cw_smem + ly.xin + lane;
-                const float* __restrict__ W = cw_smem + ly.w + lane;
-                const float* __restrict__ bias = cw_smem + ly.bias;
-                float* __restrict__ out = cw_smem + ly.out;
-                for (int g = 4 * warp; g < nr; g += 4 * CW_WARPS) {
-                    float z[4] = {0.f, 0.f, 0.f, 0.f};
-                    const float* __restrict__ wr = W + g * S;
-#pragma unroll 4
-                    for (int j = 0; j < nj; ++j) {
-                        const float xv = xin[32 * j];
-#pragma unroll
-                        for (int r = 0; r < 4; ++r) z[r] = fmaf(wr[r * S + 32 * j], xv, z[r]);
-                    }
-                    const float s = cw_warp_sum4(z, lane);
-                    const int r = g + (lane >> 3);
-                    if ((lane & 7) == 0 && r < nr) {
-                        const float y = cw_tanh(s + bias[r]);
-                        for (unsigned q = 0; q < C; ++q) cw_store_remote(out + r0 + r, q, y);
-                    }
-                }
-                cw_cluster_sync();                          // B_l
-            }
-            if (BINNED) {                                   // the actions from this CTA's copy of the last layer's outputs
-                if (tid < act) {
-                    const float* __restrict__ o = cw_smem + L.act[NL - 1] + tid * p.bins;
-                    int best = 0;
-                    float bv = o[0];
-                    for (int b = 1; b < p.bins && bv == bv; ++b) {      // first maximal bin; a NaN counts as the maximum
-                        const float v = o[b];
-                        if (v > bv || v != v) { bv = v; best = b; }
-                    }
-                    cw_smem[L.abin + tid] = __fadd_rn(__fmul_rn(__fmul_rn(p.scale, (float)best), __ldg(p.range + tid)),
-                                                      __ldg(p.low + tid));
-                }
+        const int n_eps = NOISY ? p.n_eps : 1;
+        for (int ep = 0; ep < n_eps; ++ep) {
+            const bool last_ep = ep == n_eps - 1;
+            const bool add_stat = keep_stat && last_ep;     // behaviour and ObStat: the last episode's
+            if (NOISY && ep > 0) {
+                start_episode();
+                if (tid == 0) { rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
                 __syncthreads();
             }
-            // ---- env step, redundantly in every CTA: thread i owns observation i ----
-            if (tid < obs) {
-                const float* __restrict__ oc = o2 + cur * L.o2_stride;
-                const int i = tid;
-                float acc = 0.f;
-                for (int d = 0; d < band; ++d) acc = __fadd_rn(acc, __fmul_rn(envA[d * obs + i], oc[i + d]));
-                for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, __fmul_rn(envB[j * obs + i], action[j]));
-                const float nv = cw_tanh(acc);
-                put_obs(o2 + (cur ^ 1) * L.o2_stride, i, nv);
-                x[i] = cw_normalise(nv, nmean[i], nstd[i], p.ob_clip);
-                if (keep_stat) {                            // float32 column sums in step order (numpy's axis-0 reduction)
-                    float2 st = stat[i];
-                    st.x = __fadd_rn(st.x, nv); st.y = __fadd_rn(st.y, __fmul_rn(nv, nv));
-                    stat[i] = st;
-                }
+
+            // this cluster's episode sums, and the noise of the output row this lane owns (row 4 warp + lane / 8 of the last
+            // layer's pass, lanes 8 i)
+            double* __restrict__ erow = NOISY ? p.ep_row + (size_t)cluster * T : nullptr;
+            const float* __restrict__ nzp = nullptr;
+            if (NOISY && (lane & 7) == 0) {
+                const CwLayer& lo = cw_layers[NL - 1];
+                const int r = 4 * warp + (lane >> 3);
+                if (r < lo.nr) nzp = p.act_noise + (((size_t)pair * 2 + neg) * n_eps + ep) * T * act + lo.r0 + r;
             }
-            // ---- reward (float32 dot in index order, summed in float64) and position: rank 0's last warp ----
-            if (rew_warp) {
-                if (lane < act) prod[lane] = __fmul_rn(action[lane], crow0);
-                if (lane + 32 < act) prod[lane + 32] = __fmul_rn(action[lane + 32], crow1);
-                __syncwarp();
-                if (lane == 0) {
+
+            for (int t = 0; t < T; ++t) {
+                const int cur = t & 1;
+                float crow0 = 0.f, crow1 = 0.f;
+                double esum = 0.0;                              // the earlier episodes' rewards of this step
+                if (rew_warp) {                                 // this step's reward coefficients: in flight under the layers
+                    const float* __restrict__ c = p.crew + (size_t)t * act;
+                    if (lane < act) crow0 = __ldg(c + lane);
+                    if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
+                    if (NOISY && lane == 0 && ep > 0) esum = erow[t];
+                }
+                float nz = 0.f;                                 // this lane's action noise: in flight under the layers
+                if (NOISY && nzp) nz = __ldg(nzp + (size_t)t * act);
+                // ---- the layers: 4 rows per warp and pass, each row's tanh stored into every CTA's a_l, then B_l ----
+#pragma unroll 1
+                for (int l = 0; l < NL; ++l) {
+                    const CwLayer ly = cw_layers[l];
+                    const int S = ly.S, r0 = ly.r0, nr = ly.nr, nj = S >> 5;
+                    const float* __restrict__ xin = cw_smem + ly.xin + lane;
+                    const float* __restrict__ W = cw_smem + ly.w + lane;
+                    const float* __restrict__ bias = cw_smem + ly.bias;
+                    float* __restrict__ out = cw_smem + ly.out;
+                    for (int g = 4 * warp; g < nr; g += 4 * CW_WARPS) {
+                        float z[4] = {0.f, 0.f, 0.f, 0.f};
+                        const float* __restrict__ wr = W + g * S;
+#pragma unroll 4
+                        for (int j = 0; j < nj; ++j) {
+                            const float xv = xin[32 * j];
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) z[r] = fmaf(wr[r * S + 32 * j], xv, z[r]);
+                        }
+                        const float s = cw_warp_sum4(z, lane);
+                        const int r = g + (lane >> 3);
+                        if ((lane & 7) == 0 && r < nr) {
+                            const float y = (NOISY && l == NL - 1) ? __fadd_rn(cw_tanh(s + bias[r]), nz) : cw_tanh(s + bias[r]);
+                            for (unsigned q = 0; q < C; ++q) cw_store_remote(out + r0 + r, q, y);
+                        }
+                    }
+                    cw_cluster_sync();                          // B_l
+                }
+                if (BINNED) {                                   // the actions from this CTA's copy of the last layer's outputs
+                    if (tid < act) {
+                        const float* __restrict__ o = cw_smem + L.act[NL - 1] + tid * p.bins;
+                        int best = 0;
+                        float bv = o[0];
+                        for (int b = 1; b < p.bins && bv == bv; ++b) {      // first maximal bin; a NaN counts as the maximum
+                            const float v = o[b];
+                            if (v > bv || v != v) { bv = v; best = b; }
+                        }
+                        cw_smem[L.abin + tid] = __fadd_rn(__fmul_rn(__fmul_rn(p.scale, (float)best), __ldg(p.range + tid)),
+                                                          __ldg(p.low + tid));
+                    }
+                    __syncthreads();
+                }
+                // ---- env step, redundantly in every CTA: thread i owns observation i ----
+                if (tid < obs) {
+                    const float* __restrict__ oc = o2 + cur * L.o2_stride;
+                    const int i = tid;
                     float acc = 0.f;
-                    for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, prod[j]);
-                    rfit[0] += (double)acc;
-                    const float ps = p.pos_scale;
-                    rpos[0] = __fadd_rn(rpos[0], __fmul_rn(ps, action[0]));
-                    rpos[1] = __fadd_rn(rpos[1], __fmul_rn(ps, action[1 % act]));
-                    rpos[2] = __fadd_rn(rpos[2], __fmul_rn(ps, action[2 % act]));
+                    for (int d = 0; d < band; ++d) acc = __fadd_rn(acc, __fmul_rn(envA[d * obs + i], oc[i + d]));
+                    for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, __fmul_rn(envB[j * obs + i], action[j]));
+                    const float nv = cw_tanh(acc);
+                    put_obs(o2 + (cur ^ 1) * L.o2_stride, i, nv);
+                    x[i] = cw_normalise(nv, nmean[i], nstd[i], p.ob_clip);
+                    if (add_stat) {                             // float32 column sums in step order (numpy's axis-0 reduction)
+                        float2 st = stat[i];
+                        st.x = __fadd_rn(st.x, nv); st.y = __fadd_rn(st.y, __fmul_rn(nv, nv));
+                        stat[i] = st;
+                    }
                 }
-                __syncwarp();
+                // ---- reward (float32 dot in index order, summed in float64) and position: rank 0's last warp ----
+                if (rew_warp) {
+                    if (lane < act) prod[lane] = __fmul_rn(action[lane], crow0);
+                    if (lane + 32 < act) prod[lane + 32] = __fmul_rn(action[lane + 32], crow1);
+                    __syncwarp();
+                    if (lane == 0) {
+                        float acc = 0.f;
+                        for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, prod[j]);
+                        if (!NOISY) {
+                            rfit[0] += (double)acc;
+                        } else if (!last_ep) {                  // the float64 per-step sum over the episodes, in their order
+                            erow[t] = esum + (double)acc;
+                        } else {                                // ... and its mean (obj.py:57-61)
+                            rfit[0] += (esum + (double)acc) / n_eps;
+                        }
+                        const float ps = p.pos_scale;
+                        rpos[0] = __fadd_rn(rpos[0], __fmul_rn(ps, action[0]));
+                        rpos[1] = __fadd_rn(rpos[1], __fmul_rn(ps, action[1 % act]));
+                        rpos[2] = __fadd_rn(rpos[2], __fmul_rn(ps, action[2 % act]));
+                    }
+                    __syncwarp();
+                }
+                __syncthreads();                                // x and the raw observation before the next step's layer 0
             }
-            __syncthreads();                                // x and the raw observation before the next step's layer 0
         }
         if (rew_warp && lane == 0) {
             (neg ? p.fit_neg : p.fit_pos)[(size_t)pair * p.fit_stride] = rfit[0];
@@ -346,9 +391,11 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
 }
 
 template <int NL>
-__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) { cw_rollout<NL, false>(p); }
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) { cw_rollout<NL, false, false>(p); }
 template <int NL>
-__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_binned_kernel(const CwParams p) { cw_rollout<NL, true>(p); }
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_binned_kernel(const CwParams p) { cw_rollout<NL, true, false>(p); }
+template <int NL>
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_noisy_kernel(const CwParams p) { cw_rollout<NL, false, true>(p); }
 
 }  // namespace
 
@@ -404,7 +451,10 @@ int es_closedw_binned_plan(const int* dims, int n_layers, int band, int bins, in
 }
 
 typedef void (*CwKernel)(const CwParams);
-static CwKernel cw_kernel(int n_layers, bool binned = false) {
+static CwKernel cw_kernel(int n_layers, bool binned = false, bool noisy = false) {
+    if (noisy)
+        return n_layers == 3 ? rollout_closedw_noisy_kernel<3> : n_layers == 4 ? rollout_closedw_noisy_kernel<4>
+                                                                                : rollout_closedw_noisy_kernel<5>;
     if (binned)
         return n_layers == 3 ? rollout_closedw_binned_kernel<3> : n_layers == 4 ? rollout_closedw_binned_kernel<4>
                                                                                  : rollout_closedw_binned_kernel<5>;
@@ -438,11 +488,12 @@ int es_closedw_binned_max_clusters(int n_layers, int C, size_t smem, int* cluste
 int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {
     int C = 0, max_clusters = 0;
     size_t smem = 0;
-    const bool binned = r.bins != 0;
+    const bool binned = r.bins != 0, noisy = r.act_noise != nullptr;       // (never both: the binned entry passes no noise)
     int rc = binned ? es_closedw_binned_plan(r.layer_sizes, r.n_layers, env.band, r.bins, &C, &smem)
                     : es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
     if (rc) return rc;
-    rc = cw_max_clusters(cw_kernel(r.n_layers, binned), C, smem, &max_clusters);
+    const CwKernel kernel = cw_kernel(r.n_layers, binned, noisy);
+    rc = cw_max_clusters(kernel, C, smem, &max_clusters);
     if (rc) return rc;
     if (max_clusters < 1) {
         es_set_error("es_rollout_closedloop_mlp: no cluster of %d CTAs with %zu bytes of shared memory each fits on this device", C, smem);
@@ -467,9 +518,10 @@ int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& 
     p.low = r.head_low; p.range = r.head_range;
     const long long evals = 2ll * r.n_pairs;
     const int clusters = evals < max_clusters ? (int)evals : max_clusters;
+    p.act_noise = r.act_noise; p.n_eps = noisy ? r.n_episodes : 1; p.ep_row = env.ep_rows;
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cw_config(C, smem, clusters, stream, &attr);
-    ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, cw_kernel(r.n_layers, binned), p));
+    ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
     ES_LAUNCHED(ctx);
     return ES_OK;
 }

@@ -384,12 +384,20 @@ class Engine:
     def rollout_closed_mlp(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
                            obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,
                            behv_neg=None, coin_words=None, save_obs_chance: float = 0.0, ob_sum=None, ob_sumsq=None, ob_count=None,
-                           head=None):
+                           head=None, act_noise=None, episodes: int = 1):
         """``rollout_closed`` (same arguments and checks) for every tanh MLP the closed loop covers: 2 to 4 hidden layers of
         at most 256 units, obs <= 384, act <= 64.  The shapes ``rollout_closed`` takes run its kernel; the others one
         thread-block cluster per evaluation (``closed_mlp_plan``).  ``head``: as ``rollout``; a binned head
-        (es_rollout_closedloop_mlp_binned) always runs the cluster kernel, ``env_b`` [adim, obs] and ``rew_vec`` [T, adim]."""
+        (es_rollout_closedloop_mlp_binned) always runs the cluster kernel, ``env_b`` [adim, obs] and ``rew_vec`` [T, adim].
+        ``act_noise`` / ``episodes``: as ``rollout`` (es_rollout_closedloop_mlp_episodes): every episode restarts the env and
+        steps it with the noisy actions; behaviour and ObStat are the last episode's.  Without ``act_noise`` the episodes are
+        identical and the library runs one on the noise-free kernels."""
         binned = head is not None and head != 'tanh'
+        episodes = int(episodes)
+        if episodes < 1:
+            raise ValueError(f'episodes must be >= 1, got {episodes}')
+        if binned and act_noise is not None:
+            raise ValueError('a binned head draws no action noise (FFBinned.forward ignores rs): act_noise must be None')
         d = self.device
         _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
         _req(ob_mean, torch.float64, 'ob_mean', d); _req(ob_std, torch.float64, 'ob_std', d)
@@ -419,6 +427,17 @@ class Engine:
                 float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
                 _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), int(head.bins), _ptr(low), _ptr(rng),
                 self.stream), 'es_rollout_closedloop_mlp_binned')
+            return
+        if act_noise is not None or episodes != 1:
+            if act_noise is not None:
+                _req(act_noise, torch.float32, 'act_noise', d)
+                assert act_noise.numel() == n * 2 * episodes * T * act
+            check(self.lib.es_rollout_closedloop_mlp_episodes(
+                self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
+                _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T,
+                float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
+                _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), _ptr(act_noise), episodes,
+                self.stream), 'es_rollout_closedloop_mlp_episodes')
             return
         check(self.lib.es_rollout_closedloop_mlp(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
                                                  float(sigma), ls, len(layer_sizes) - 1, _ptr(ob_mean), _ptr(ob_std), float(ob_clip),

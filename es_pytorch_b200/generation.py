@@ -71,11 +71,15 @@ class DeviceGeneration:
                  optim: Optimizer, ob_clip: float = 5.0, pos_scale: float = 0.05, coins_per_eval: int = 0,
                  save_obs_chance: float = 0.0, archive: Optional[torch.Tensor] = None, nov_k: int = 10,
                  moo_w: float = 1.0, rollout_mode: int = ES_ROLLOUT_F32, comm: Optional[dist.Comm] = None,
-                 engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1, head=None):
+                 engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1, head=None,
+                 closed_act_noise: bool = False):
         self.eng = engine or get_engine()
         # closed-loop variant of the synthetic env (gym.synthetic_env.ClosedLoopEnv): (obs_0 [obs], A^T [band, obs], B^T [act, obs]);
-        # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop_mlp
+        # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop_mlp.  With ac_std != 0 the
+        # closed loop rolls out with the action noise (es_rollout_closedloop_mlp_episodes) when closed_act_noise is True, and
+        # evaluate() refuses it otherwise
         self.closed = closed
+        self.closed_act_noise = bool(closed_act_noise)
         self.ranker = ranker                            # a utils.rankers.Ranker; None = Centered / MultiObjective(moo_w)
         e = self.eng
         self.comm = comm or dist.world()
@@ -213,9 +217,10 @@ class DeviceGeneration:
                                self.idx, self.extras)
         fp, fn = self.fit_local[0], self.fit_local[1]
         if self.closed is not None:
-            if self.ac_std != 0.0:
-                raise NotImplementedError('the closed-loop variant of the synthetic env is defined without action noise: set the '
-                                          'network\'s ac_std to 0 (the open-loop env supports ac_std != 0 on the device)')
+            if self.ac_std != 0.0 and not self.closed_act_noise:
+                raise NotImplementedError('this generation was built without closed_act_noise: pass closed_act_noise=True to roll '
+                                          'out the closed-loop env with action noise, or set the network\'s ac_std to 0')
+            noisy = self.ac_std != 0.0
             self._gen_stats.zero_()
             obs0, env_a, env_b = self.closed
             with self._timed('rollout'):
@@ -225,7 +230,8 @@ class DeviceGeneration:
                                      coin_words=self.extras if self.extra_words else None, save_obs_chance=self.save_obs_chance,
                                      ob_sum=self.gen_sum if self.extra_words else None,
                                      ob_sumsq=self.gen_sumsq if self.extra_words else None,
-                                     ob_count=self.gen_count if self.extra_words else None, head=self.head)
+                                     ob_count=self.gen_count if self.extra_words else None, head=self.head,
+                                     act_noise=self.act_noise if noisy else None, episodes=self.episodes if noisy else 1)
             if self.n_obj == 2:
                 e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
         else:

@@ -80,13 +80,14 @@ class BatchedRollout:
         noise_rs = streams[0] if (use_ac_noise and streams is not None and len(streams)) else None
         closed = getattr(self.env, 'is_synthetic_closedloop', False)
         head = model.head() if hasattr(model, 'head') else None
-        if (closed and head is not None and self._closed_on_device(model.layer_sizes(), head)
-                and not (noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0)):
-            # the closed-loop episode as one launch (the observations are not returned: this result never carries them)
+        noisy = noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0
+        episodes = self.episodes if noisy else 1
+        if closed and head is not None and self._closed_on_device(model.layer_sizes(), head):
+            # the closed-loop evaluation, all its episodes, as one launch (the observations are not returned: this result never
+            # carries them)
             from .gym_runner import _device_episode_closed
-            total, pos, _ = _device_episode_closed(model, self.env, self.max_steps)
+            total, pos, _ = _device_episode_closed(model, self.env, self.max_steps, noise_rs if noisy else None, episodes)
             return self.result_from_device(total, pos)
-        episodes = self.episodes if (noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0) else 1
         if episodes > 1:
             rews, behv, steps = self._run_episodes(model, noise_rs, episodes)
         else:
@@ -116,7 +117,8 @@ class BatchedRollout:
     def _run_episodes(self, model, rs, episodes: int):
         """obj.py:57-60 with action noise: ``episodes`` runs of run_model drawing from ``rs``, rewards summed per step in
         float64 in episode order and divided by the count.  A tanh MLP on the open-loop env runs all episodes as one launch
-        (one forward, the episodes' noise rows back to back) and reports the total of the per-step means."""
+        (one forward, the episodes' noise rows back to back) and reports the total of the per-step means.  (The closed-loop
+        env's device path is ``__call__``'s ``_device_episode_closed``.)"""
         from .gym_runner import _device_episode
         if getattr(self.env, 'is_synthetic_openloop', False) and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp():
             total, pos, T = _device_episode(model, self.env, self.max_steps, rs, episodes)

@@ -68,8 +68,10 @@ def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 
-def _device_episode_closed(model, env, max_steps: int):
-    """One noise-free episode on the closed-loop synthetic env as one launch of es_rollout_closedloop_mlp (sigma = 0)."""
+def _device_episode_closed(model, env, max_steps: int, rs=None, episodes: int = 1):
+    """One evaluation on the closed-loop synthetic env as one launch of es_rollout_closedloop_mlp (sigma = 0).  With ``rs`` and
+    a tanh model's ac_std != 0: the action noise of ``episodes`` episodes drawn back to back from ``rs`` (as ``_device_episode``),
+    the per-step mean over the episodes, the last episode's final position."""
     from ..engine import get_engine
     from ..core.policy import Policy
     eng = get_engine()
@@ -84,9 +86,19 @@ def _device_episode_closed(model, env, max_steps: int):
     idx = torch.zeros(1, dtype=torch.int64, device=eng.device)
     fit = torch.zeros(2, dtype=torch.float64, device=eng.device)
     behv = torch.zeros(2, 3, dtype=torch.float32, device=eng.device)
+    head = model.head()
+    noise = None
+    ac_std = float(getattr(model, '_action_std', 0) or 0)
+    if rs is not None and ac_std != 0 and head == 'tanh':
+        # the closed loop's noise does not depend on the state: one rs.randn(episodes * T * act) call consumes the stream as
+        # the episodes' T calls of rs.randn(act) each (nn.py:47-48); both signs of the sigma = 0 "pair" see it, only + is used
+        nz = (rs.randn(episodes * T * sizes[-1]) * ac_std).astype(np.float32)
+        noise = eng.to_device(np.stack([nz, nz]).reshape(1, 2, -1))
+    else:
+        episodes = 1
     eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), obs0, env_a, env_b,
                            rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1),
-                           head=model.head())
+                           head=head, act_noise=noise, episodes=episodes)
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 

@@ -196,6 +196,26 @@ int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len
                               double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
                               double* ob_sum, double* ob_sumsq, double* ob_count, void* stream);
 
+/* es_rollout_closedloop_mlp with action noise and E = n_episodes episodes per evaluation (FeedForward._action_std != 0,
+ * src/nn/nn.py:47-48; obj.py:54-63's eps_per_policy).  act_noise dev float [n_pairs][2 (+,-)][E][T][act_dim], as
+ * es_draw_noisy writes it with normals_per_eval = E * T * act_dim, or NULL.  Episode e of an evaluation starts from a fresh env
+ * (obs_0, position 0) with the same perturbed weights; at step t the float32 action noise[e][t] is added to the tanh output
+ * (float32 add) and the env step, the reward and the position all use the noisy action.  Per step the float32 rewards r_{e,t}
+ * are summed over the episodes in float64 in episode order and divided by E; fitness is the float64 sum of these means in step
+ * order (E = 1: the plain float64 sum).  behv_pos/behv_neg and the ObStat increments of saved evaluations are the LAST
+ * episode's (count += T and one rollout per saved evaluation).  act_noise == NULL: the episodes are identical and any
+ * n_episodes >= 1 gives es_rollout_closedloop_mlp's result bit for bit.  Covers es_rollout_closedloop_mlp's shapes with the
+ * same kernels (rollout_closed.cu for two hidden layers <= 64, else rollout_closedw.cu); results do not depend on the grid.
+ * E > 1 keeps a float64 [T] row per evaluation in flight in the ctx scratch.  One kernel launch per call.              */
+int es_rollout_closedloop_mlp_episodes(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                       const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                       const double* ob_mean, const double* ob_std, double ob_clip,
+                                       const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
+                                       int T, float pos_scale, const uint32_t* coin_words, double save_obs_chance,
+                                       double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                                       double* ob_sum, double* ob_sumsq, double* ob_count, const float* act_noise,
+                                       int n_episodes, void* stream);
+
 /* How es_rollout_closedloop_mlp runs a shape, without running it: cluster_size 0 for es_rollout_closedloop's one-CTA kernel
  * (clusters = the SM count, smem_bytes = 0), else the CTAs per cluster, the clusters resident at once (the persistent grid)
  * and the dynamic shared memory per CTA.  ES_ERR_UNSUPPORTED with es_rollout_closedloop_mlp's message for an uncovered shape. */
