@@ -17,6 +17,7 @@ ES_ROLLOUT_F32 = 0
 ES_ROLLOUT_TC = 1
 ES_ROLLOUT_TC3 = 2
 ES_MT_N = 624
+ES_OBJ_MEAN_REWARD, ES_OBJ_DIST, ES_OBJ_XDIST = 1, 2, 3
 
 _vp, _i32, _i64, _u64, _f32, _f64 = C.c_void_p, C.c_int, C.c_int64, C.c_uint64, C.c_float, C.c_double
 
@@ -59,6 +60,7 @@ SIGNATURES = {
     'es_randn': (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
     'es_randn_plan': (_i32, [_vp, _i64, C.POINTER(C.c_size_t), C.POINTER(_i32)]),
     'es_novelty': (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _vp, _i32, _vp]),
+    'es_fitness_objective': (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _i32, _vp]),
     'es_centered_rank': (_i32, [_vp, _vp, _vp, _i32, _i32, _f32, _f32, _i32, _i32, _vp, _vp, _vp]),
     'es_rank_transform': (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _f64, _f64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp]),

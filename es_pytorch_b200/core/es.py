@@ -176,6 +176,10 @@ def _step_fused(cfg, comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: O
 
 
 def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> DeviceGeneration:
+    objective = getattr(fit_fn, 'objective', 'reward')
+    if objective == 'mean_reward' and fit_fn.max_steps - 1 == 0:
+        # MeanRewardResult.get_result divides by steps, the last loop index: 0 for a one-step episode (training_result.py:69)
+        raise ZeroDivisionError('MeanRewardResult of a one-step episode: the reward is divided by steps = 0')
     eng = get_engine()
     gen = fit_fn._gen
     theta = policy.theta_dev(eng)
@@ -184,7 +188,7 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
     if (gen is None or gen.theta is not theta or gen.n_streams != len(streams) or gen.table is not nt.device_table(eng)
             or gen.coins_per_eval != int(fit_fn.coins_per_eval) or gen.rollout_mode != fit_fn.rollout_mode
             or (gen.archive is None) != (fit_fn.archive is None) or gen.episodes != fit_fn.episodes
-            or gen.head_key != head_key):
+            or gen.head_key != head_key or gen.objective != objective):
         env = fit_fn.env
         obs_dev, rew_dev = env.device_arrays(eng)
         T = fit_fn.max_steps
@@ -196,7 +200,7 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
                                archive=archive, nov_k=fit_fn.nov_k, rollout_mode=fit_fn.rollout_mode, engine=eng,
                                ac_std=float(getattr(policy._module, '_action_std', 0.0) or 0.0),
                                closed=env.device_closed(eng) if getattr(env, 'is_synthetic_closedloop', False) else None,
-                               episodes=fit_fn.episodes, head=head, closed_act_noise=True)
+                               episodes=fit_fn.episodes, head=head, closed_act_noise=True, objective=objective)
         fit_fn._gen = gen
     else:
         gen.load_states(streams)

@@ -507,6 +507,19 @@ int es_novelty(es_ctx* ctx, const float* behv, int n, const double* archive, int
     return es_impl_novelty(ctx, behv, n, archive, A, k, out, out_stride, (cudaStream_t)stream);
 }
 
+int es_fitness_objective(es_ctx* ctx, int kind, double* fit, int fit_stride, const float* behv, int n, int steps,
+                         void* stream) {
+    ES_ENTER(ctx);
+    ES_REQUIRE(kind == ES_OBJ_MEAN_REWARD || kind == ES_OBJ_DIST || kind == ES_OBJ_XDIST,
+               "es_fitness_objective: unknown kind %d", kind);
+    ES_REQUIRE(n >= 0 && fit_stride >= 1, "es_fitness_objective: bad sizes");
+    ES_REQUIRE(kind != ES_OBJ_MEAN_REWARD || steps > 0,
+               "es_fitness_objective: the mean reward of an episode with steps = %d (MeanRewardResult divides by zero)", steps);
+    if (n == 0) return ES_OK;
+    ES_REQUIRE(fit && (kind == ES_OBJ_MEAN_REWARD || behv), "es_fitness_objective: NULL pointer");
+    return es_impl_fitness_objective(ctx, kind, fit, fit_stride, behv, n, steps, (cudaStream_t)stream);
+}
+
 int es_centered_rank(es_ctx* ctx, const double* fpos, const double* fneg, int K, int n_obj, float w0, float w1,
                      int k_begin, int k_count, float* weights_out, int32_t* ranks_out, void* stream) {
     ES_ENTER(ctx);

@@ -168,6 +168,7 @@ int es_closedw_binned_max_clusters(int n_layers, int cluster_size, size_t smem_b
 int es_launch_ubase(es_ctx*, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
                     float* ubase, cudaStream_t);
 int es_impl_novelty(es_ctx*, const float*, int, const double*, int, int, double*, int, cudaStream_t);
+int es_impl_fitness_objective(es_ctx*, int, double*, int, const float*, int, int, cudaStream_t);
 int es_impl_rank_transform(es_ctx*, const double*, const double*, int, int, int, double, double, int, int, int,
                            const int64_t*, float*, double*, int32_t*, double*, int32_t*, int64_t*, cudaStream_t);
 int es_impl_grad_reconstruct(es_ctx*, const float*, int64_t, const int64_t*, const float*, int, int, float*,

@@ -471,6 +471,19 @@ class Engine:
         check(self.lib.es_novelty(self._ctx, _ptr(behv), n, _ptr(archive), A, int(k), _ptr(out), int(out_stride),
                                   self.stream), 'es_novelty')
 
+    def fitness_objective(self, kind: int, fit, fit_stride: int, behv, n: int, steps: int):
+        """Column 0 of ``n`` evaluations' fitness rows (element e * fit_stride of ``fit``), rewritten in place from the episode
+        total there and the final position ``behv`` [n][3] as ES_OBJ_MEAN_REWARD / ES_OBJ_DIST / ES_OBJ_XDIST
+        (MeanRewardResult / DistResult / XDistResult, training_result.py:67-79).  ``behv`` may be None for the mean reward."""
+        d = self.device
+        _req(fit, torch.float64, 'fit', d)
+        assert n == 0 or fit.numel() >= (n - 1) * fit_stride + 1
+        if behv is not None:
+            _req(behv, torch.float32, 'behv', d)
+            assert behv.numel() >= 3 * n
+        check(self.lib.es_fitness_objective(self._ctx, int(kind), _ptr(fit), int(fit_stride), _ptr(behv), int(n), int(steps),
+                                            self.stream), 'es_fitness_objective')
+
     # ------------------------------------------------------------------ a8/a9
     def centered_rank(self, fpos, fneg, w0: float = 1.0, w1: float = 0.0, k_begin: int = 0,
                       k_count: Optional[int] = None, want_ranks: bool = False):

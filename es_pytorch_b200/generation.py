@@ -10,7 +10,8 @@ replaces ``es.test_params`` -> ``Ranker.rank`` -> ``es.approx_grad`` of the refe
     normalise obs stream      es_normalise_obs       (nn.py:45)
     theta +- sigma*eps, MLP rollout, fitness
                               es_rollout_openloop    (policy.py:61-64, nn.py:42-50, gym_runner.py:33-67)
-    [novelty column]          es_novelty             (novelty.py:16-18)            NSRA only
+    [novelty column]          es_novelty             (novelty.py:16-18)            NSRA / NSResult only
+    [objective column]        es_fitness_objective   (training_result.py:67-79)    MeanRewardResult / DistResult / XDistResult
     [obs statistics]          es_obs_colsum + es_obstat_accumulate_coins           (es.py:73-74)
     allgather fitness         NCCL (only when world size > 1)                       (es.py:84-95)
     rank shaping -> weights   es_centered_rank / es_rank_transform  (rankers.py:9-120)
@@ -31,7 +32,7 @@ import numpy as np
 import torch
 
 from . import dist
-from ._lib import ES_MT_N, ES_ROLLOUT_F32
+from ._lib import ES_MT_N, ES_OBJ_DIST, ES_OBJ_MEAN_REWARD, ES_OBJ_XDIST, ES_ROLLOUT_F32
 from .engine import Engine, get_engine
 from .nn.optimizers import Optimizer
 
@@ -45,6 +46,13 @@ class _NoTimer:
 
 
 _NO_TIMER = _NoTimer()
+
+# what column 0 of an evaluation's fitness row holds (the TrainingResult adaptor it stands for, training_result.py:62-97):
+#   'reward'       the episode total (RewardResult; with an archive, NSRResult: reward then novelty, two columns)
+#   'mean_reward'  total / (T - 1) (MeanRewardResult)        'dist'  ||final (x, y)|| (DistResult)
+#   'xdist'        final x (XDistResult)                      'novelty'  novelty of the final (x, y) alone (NSResult)
+OBJECTIVES = ('reward', 'mean_reward', 'dist', 'xdist', 'novelty')
+_OBJ_KINDS = {'mean_reward': ES_OBJ_MEAN_REWARD, 'dist': ES_OBJ_DIST, 'xdist': ES_OBJ_XDIST}
 
 
 class _Timed:
@@ -72,8 +80,17 @@ class DeviceGeneration:
                  save_obs_chance: float = 0.0, archive: Optional[torch.Tensor] = None, nov_k: int = 10,
                  moo_w: float = 1.0, rollout_mode: int = ES_ROLLOUT_F32, comm: Optional[dist.Comm] = None,
                  engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1, head=None,
-                 closed_act_noise: bool = False):
+                 closed_act_noise: bool = False, objective: str = 'reward'):
         self.eng = engine or get_engine()
+        if objective not in OBJECTIVES:
+            raise ValueError(f'objective must be one of {OBJECTIVES}, got {objective!r}')
+        if objective == 'novelty' and archive is None:
+            raise ValueError('the novelty objective needs an archive')
+        if archive is not None and objective not in ('reward', 'novelty'):
+            raise ValueError(f'an archive scores reward and novelty (NSRResult) or novelty alone (NSResult), not {objective!r}')
+        if objective == 'mean_reward' and rew_vec.shape[0] - 1 == 0:
+            raise ZeroDivisionError('the mean reward of a one-step episode divides by steps = 0 (MeanRewardResult)')
+        self.objective = objective
         # closed-loop variant of the synthetic env (gym.synthetic_env.ClosedLoopEnv): (obs_0 [obs], A^T [band, obs], B^T [act, obs]);
         # row 0 of obs_stream is then the only one read and the rollout is es_rollout_closedloop_mlp.  With ac_std != 0 the
         # closed loop rolls out with the action noise (es_rollout_closedloop_mlp_episodes) when closed_act_noise is True, and
@@ -101,7 +118,7 @@ class DeviceGeneration:
         self.ob_clip, self.pos_scale = float(ob_clip), float(pos_scale)
         self.coins_per_eval, self.save_obs_chance = int(coins_per_eval), float(save_obs_chance)
         self.archive, self.nov_k, self.moo_w = archive, int(nov_k), float(moo_w)
-        self.n_obj = 1 if archive is None else 2
+        self.n_obj = 2 if (archive is not None and objective == 'reward') else 1
         self.rollout_mode = rollout_mode
         # FeedForward._action_std (nn.py:47-48): != 0 -> every step adds rs.randn(act) * ac_std, drawn from the rank streams
         self.ac_std = float(ac_std or 0.0)
@@ -180,7 +197,9 @@ class DeviceGeneration:
         self.fpos_all = e.empty((self.K, self.n_obj), f64) if G > 1 else None
         self.fneg_all = e.empty((self.K, self.n_obj), f64) if G > 1 else None
         self.idx_all = e.empty((self.K,), i64) if G > 1 else None             # every process's indices, rank-major
-        self.behv = e.empty((2, self.k_local, 3), f32) if self.n_obj == 2 else None
+        # the final positions, where an objective reads them (novelty, distance)
+        reads_pos = self.archive is not None or self.objective in ('dist', 'xdist')
+        self.behv = e.empty((2, self.k_local, 3), f32) if reads_pos else None
         self.weights = None
         self._bufs_for = n_per_stream
 
@@ -232,8 +251,7 @@ class DeviceGeneration:
                                      ob_sumsq=self.gen_sumsq if self.extra_words else None,
                                      ob_count=self.gen_count if self.extra_words else None, head=self.head,
                                      act_noise=self.act_noise if noisy else None, episodes=self.episodes if noisy else 1)
-            if self.n_obj == 2:
-                e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
+            self._score()
         else:
             self._evaluate_openloop(fp, fn)
         if self.comm.size > 1:
@@ -259,9 +277,7 @@ class DeviceGeneration:
                       None if self.behv is None else self.behv[1], self.rollout_mode,
                       act_noise=self.act_noise if self.ac_std != 0.0 else None,
                       episodes=self.episodes if self.ac_std != 0.0 else 1, head=self.head)
-        if self.n_obj == 2:
-            # second objective column = novelty of the final (x, y) (training_result.py:95-97)
-            e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, self.fit_local.view(-1)[1:], 2)
+        self._score()
         self._gen_stats.zero_()
         if self.extra_words:
             # column sums of the post-step observations of a rollout: the open-loop stream is the same for every rollout and
@@ -273,6 +289,19 @@ class DeviceGeneration:
             s, q = self._colsum
             e.obstat_accumulate_coins(self.gen_sum, self.gen_sumsq, self.gen_count, s, q, self.T,
                                       self.extras.view(-1, 2), self.save_obs_chance)
+
+    def _score(self):
+        """The objective columns of both signs' fitness rows, from the episode totals and final positions the rollout left:
+        NSRResult's second column and NSResult's only one are the novelty of the final (x, y) (training_result.py:82-97), the
+        other single-objective adaptors rewrite the total in column 0 (es_fitness_objective); RewardResult keeps it."""
+        e, fit = self.eng, self.fit_local.view(-1)
+        if self.n_obj == 2:
+            e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, fit[1:], 2)
+        elif self.objective == 'novelty':
+            e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, fit, 1)
+        elif self.objective != 'reward':
+            # steps = T - 1: the last loop index run_model returns (gym_runner.py:50,67)
+            e.fitness_objective(_OBJ_KINDS[self.objective], fit, 1, self.behv, 2 * self.k_local, self.T - 1)
 
     def _alloc_act_noise(self, nrm: int) -> torch.Tensor:
         """The [k_local, 2, episodes * T * act] float32 buffer of the generation's action noise."""

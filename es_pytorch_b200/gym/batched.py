@@ -13,6 +13,10 @@ the generation can run on the device with the same RNG consumption and the same 
 in order), with the last episode's behaviour.  With action noise every episode draws its own
 T x act gaussians from the stream; without it the episodes are identical and the mean is
 exactly the single episode (E copies of a float32 sum exactly in float64, and (E r) / E == r).
+
+``result`` is the TrainingResult adaptor the script's fit_fn builds (training_result.py:62-97): RewardResult (the default
+without an archive), MeanRewardResult, DistResult, XDistResult, NSResult (novelty alone) or NSRResult (reward and novelty,
+the default with an archive).  The fused generation computes the same column(s) on the device.
 """
 from __future__ import annotations
 
@@ -22,7 +26,11 @@ import numpy as np
 
 from .. import _lib
 from .gym_runner import run_model
-from .training_result import NSRResult, RewardResult, TrainingResult
+from .training_result import DistResult, MeanRewardResult, NSResult, NSRResult, RewardResult, TrainingResult, XDistResult
+
+# adaptor -> DeviceGeneration's objective (NSRResult is the reward column plus the novelty column of an archive)
+_OBJECTIVES = {RewardResult: 'reward', MeanRewardResult: 'mean_reward', DistResult: 'dist', XDistResult: 'xdist',
+               NSResult: 'novelty', NSRResult: 'reward'}
 
 
 class BatchedRollout:
@@ -31,7 +39,7 @@ class BatchedRollout:
     def __init__(self, env, max_steps: int, coins_per_eval: int = 1, save_obs_chance: float = 0.0,
                  archive: Optional[np.ndarray] = None, nov_k: int = 10,
                  rank_streams: Optional[Sequence[np.random.RandomState]] = None,
-                 rollout_mode: int = _lib.ES_ROLLOUT_F32, episodes: int = 1):
+                 rollout_mode: int = _lib.ES_ROLLOUT_F32, episodes: int = 1, result: Optional[type] = None):
         if not (getattr(env, 'is_synthetic_openloop', False) or getattr(env, 'is_synthetic_closedloop', False)):
             raise TypeError('BatchedRollout needs a synthetic env (es_pytorch_b200.gym.synthetic_env: open- or closed-loop)')
         self.env = env
@@ -47,6 +55,17 @@ class BatchedRollout:
         if episodes < 0:
             raise ValueError(f'episodes must be >= 0 (0 means 1, as max(1, eps_per_policy) in obj.py), got {episodes}')
         self.episodes = max(1, int(episodes))
+        if result is None:
+            result = RewardResult if self.archive is None else NSRResult
+        if not any(result is c for c in _OBJECTIVES):
+            raise ValueError(f'result must be one of {", ".join(c.__name__ for c in _OBJECTIVES)}, got {result!r}')
+        novelty = result in (NSResult, NSRResult)
+        if novelty and self.archive is None:
+            raise ValueError(f'{result.__name__} scores the novelty of the final position: it needs an archive')
+        if self.archive is not None and not novelty:
+            raise ValueError(f'an archive is the novelty search\'s: {result.__name__} does not read it (use NSResult or NSRResult)')
+        self.result = result
+        self.objective = _OBJECTIVES[result]
         if self.episodes > 1 and self.archive is not None:
             raise ValueError('episodes > 1 with a novelty archive: no reference script averages episodes for novelty search')
         self._gen = None            # cached DeviceGeneration (see core.es)
@@ -55,7 +74,13 @@ class BatchedRollout:
 
     @property
     def n_obj(self) -> int:
-        return 1 if self.archive is None else 2
+        return 2 if self.result is NSRResult else 1
+
+    def _result(self, rews, behv, obs, steps) -> TrainingResult:
+        """The adaptor as the scripts build it (nsra.py:93 hands the novelty adaptors the last position only)."""
+        if self.result in (NSResult, NSRResult):
+            return self.result(rews, behv[-3:], obs, steps, self.archive, self.nov_k)
+        return self.result(rews, behv, obs, steps)
 
     def result_from_device(self, total: float, pos) -> TrainingResult:
         """The TrainingResult ``__call__`` would build, from an episode total and final position computed on the device."""
@@ -63,9 +88,7 @@ class BatchedRollout:
         behv = [float(pos[0]), float(pos[1]), float(pos[2])] * int(self.max_steps)
         no_obs = np.array([np.zeros(self.env.observation_space.shape)])
         steps = self.max_steps - 1                              # run_model returns the last loop index (gym_runner.py:50,67)
-        if self.archive is None:
-            return RewardResult(rews, behv, no_obs, steps)
-        return NSRResult(rews, behv[-3:], no_obs, steps, self.archive, self.nov_k)
+        return self._result(rews, behv, no_obs, steps)
 
     def __call__(self, model, use_ac_noise=True) -> TrainingResult:
         """Single-policy evaluation with the reference's fit_fn contract.  Like the scripts' fit_fn (simple_example.py:38,
@@ -93,9 +116,7 @@ class BatchedRollout:
         else:
             rews, behv, obs, steps = run_model(model, self.env, self.max_steps, noise_rs)
         no_obs = np.array([np.zeros(self.env.observation_space.shape)])
-        if self.archive is None:
-            return RewardResult(rews, behv, no_obs, steps)
-        return NSRResult(rews, behv[-3:], no_obs, steps, self.archive, self.nov_k)
+        return self._result(rews, behv, no_obs, steps)
 
     def _closed_on_device(self, sizes, head='tanh') -> bool:
         """Whether a closed-loop episode of a tanh MLP runs as one launch (es_rollout_closedloop_mlp): two hidden layers always

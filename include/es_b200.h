@@ -284,6 +284,20 @@ int es_noise_table_changed(es_ctx* ctx);
 int es_novelty(es_ctx* ctx, const float* behv, int n, const double* archive, int A, int k, double* out,
                int out_stride, void* stream);
 
+/* ---- the single-objective fitness adaptors -------------------------------------------------
+ * Rewrites fit[e * fit_stride], e in [0, n), in place from the float64 episode total a rollout left there and the float32
+ * final position behv[e][0..2] it wrote, as the adaptor of src/gym/training_result.py computes get_result:
+ *   ES_OBJ_MEAN_REWARD  total / steps (IEEE division)        MeanRewardResult  (training_result.py:67-69)
+ *   ES_OBJ_DIST         sqrt((double)x*x + (double)y*y)      DistResult        np.linalg.norm(positions[-3:-1])  (:72-74)
+ *   ES_OBJ_XDIST        (double)x                            XDistResult       positions[-3]                      (:77-79)
+ * Bit-exact with the host classes on the same numbers (the argument is in csrc/objective.cu).  steps is the last loop index
+ * run_model returns (gym_runner.py:50,67); MEAN_REWARD with steps <= 0 is refused (the reference raises ZeroDivisionError).
+ * NSResult (novelty alone) needs no adaptor: es_novelty writes column 0 with out_stride 1.
+ *   fit dev double, element e*fit_stride, in/out; behv dev float [n][3] (read by DIST / XDIST only, may be NULL otherwise) */
+enum { ES_OBJ_MEAN_REWARD = 1, ES_OBJ_DIST = 2, ES_OBJ_XDIST = 3 };
+int es_fitness_objective(es_ctx* ctx, int kind, double* fit, int fit_stride, const float* behv, int n, int steps,
+                         void* stream);
+
 /* ---- a8/a9: centered rank -> antithetic weights -------------------------------------------
  * Replaces Ranker.rank with CenteredRanker (src/utils/rankers.py:9-17,37-58) and, for
  * n_obj == 2, MultiObjectiveRanker (rankers.py:106-120): ranks over all 2K fitnesses
