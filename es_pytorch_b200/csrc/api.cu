@@ -233,6 +233,70 @@ static int es_rollout_check(const char* fn, bool ptrs, const EsRollout& r) {
     return ES_OK;
 }
 
+// the head arguments of the binned entry points: bins >= 2 (the reference divides by bins - 1), low / range set, the last layer
+// adim * bins <= 256 wide
+static int es_binned_check(const char* fn, const EsRollout& r) {
+    ES_REQUIRE(r.bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, r.bins);
+    ES_REQUIRE(r.head_low && r.head_range, "%s: NULL low / range", fn);
+    const int out = r.layer_sizes[r.n_layers];
+    ES_REQUIRE(out % r.bins == 0, "%s: the last layer's %d outputs are not adim * bins for bins %d", fn, out, r.bins);
+    if (out > 256) {
+        es_set_error("%s: binned heads up to adim * bins = 256 outputs supported, got %d * %d", fn, out / r.bins, r.bins);
+        return ES_ERR_UNSUPPORTED;
+    }
+    return ES_OK;
+}
+
+// the policies an entry point takes: tanh MLPs, binned heads (EsRollout::bins, which es_binned_check refuses below 2), or
+// es_rollout_closedloop's tanh MLPs (two hidden layers, rollout_closed.cu only)
+enum EsHead { ES_HEAD_TANH, ES_HEAD_BINNED, ES_HEAD_TANH_ONE_CTA };
+
+// an open-loop entry point after ES_ENTER: its checks in order, then the mode's kernel; `fn` names it in every message
+static int es_openloop(es_ctx* ctx, const char* fn, const EsRollout& r, EsHead head, int mode, cudaStream_t stream) {
+    int rc = es_rollout_check(fn, r.obsn != nullptr, r);
+    if (rc) return rc;
+    if (head == ES_HEAD_BINNED) {
+        rc = es_binned_check(fn, r);
+        if (rc) return rc;
+        if (mode == ES_ROLLOUT_TC) {
+            es_set_error("%s: ES_ROLLOUT_TC refuses binned heads: an arg-max over float16-grade outputs is not parity grade; use "
+                         "ES_ROLLOUT_TC3 or ES_ROLLOUT_F32", fn);
+            return ES_ERR_UNSUPPORTED;
+        }
+        if (mode == ES_ROLLOUT_TC3 && !es_tcw_covers_binned(r)) {
+            const int* dims = r.layer_sizes;
+            char why[96];                               // the part of the shape outside the coverage
+            if (r.n_layers < 3 || r.n_layers > 5) {
+                snprintf(why, sizeof why, "%d hidden layers", r.n_layers - 1);
+            } else if (dims[0] > 256) {
+                snprintf(why, sizeof why, "obs %d", dims[0]);
+            } else {
+                snprintf(why, sizeof why, "the shape");
+                for (int l = 1; l < r.n_layers; ++l)
+                    if (dims[l] % 64 || dims[l] > 256) {
+                        snprintf(why, sizeof why, "hidden layer %d of width %d", l, dims[l]);
+                        break;
+                    }
+            }
+            es_set_error("%s: ES_ROLLOUT_TC3 covers binned heads with 2 to 4 hidden layers of widths in {64, 128, 192, 256} and obs "
+                         "<= 256, got %s; use ES_ROLLOUT_F32", fn, why);
+            return ES_ERR_UNSUPPORTED;
+        }
+    } else if (r.n_pairs == 0) {
+        return ES_OK;                               // a tanh head returns before it looks at the mode, a binned head after
+    }
+    if (mode != ES_ROLLOUT_F32 && mode != ES_ROLLOUT_TC && mode != ES_ROLLOUT_TC3) {
+        es_set_error("%s: unknown mode %d", fn, mode);
+        return ES_ERR_INVALID;
+    }
+    if (r.n_pairs == 0) return ES_OK;
+    if (mode == ES_ROLLOUT_F32) return es_impl_rollout_f32(ctx, r, stream);
+    // tensor cores: binned heads and the shipped configs' wide policies on rollout_tcw.cu; obs-64-64-act and everything else on
+    // rollout_tc2.cu
+    if (head == ES_HEAD_BINNED || es_tcw_covers(r)) return es_impl_rollout_tcw(ctx, r, mode == ES_ROLLOUT_TC3, stream);
+    return es_impl_rollout_tc2(ctx, r, mode == ES_ROLLOUT_TC3, stream);
+}
+
 int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
                                  const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
                                  const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
@@ -243,17 +307,7 @@ int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_
     // sum exactly in float64, and (E r) / E == r)
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
-    const int rc = es_rollout_check("es_rollout_openloop", obsn != nullptr, r);
-    if (rc) return rc;
-    if (n_pairs == 0) return ES_OK;
-    if (mode == ES_ROLLOUT_F32) return es_impl_rollout_f32(ctx, r, (cudaStream_t)stream);
-    if (mode == ES_ROLLOUT_TC || mode == ES_ROLLOUT_TC3) {
-        // the shipped configs' wide policies (rollout_tcw.cu); obs-64-64-act and everything else: rollout_tc2.cu
-        if (es_tcw_covers(r)) return es_impl_rollout_tcw(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
-        return es_impl_rollout_tc2(ctx, r, mode == ES_ROLLOUT_TC3, (cudaStream_t)stream);
-    }
-    es_set_error("es_rollout_openloop: unknown mode %d", mode);
-    return ES_ERR_INVALID;
+    return es_openloop(ctx, "es_rollout_openloop", r, ES_HEAD_TANH, mode, (cudaStream_t)stream);
 }
 
 int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
@@ -272,62 +326,54 @@ int es_rollout_openloop(es_ctx* ctx, const float* table, int64_t table_len, cons
                                      pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, mode, stream);
 }
 
-// the head arguments of the binned entry points: bins >= 2 (the reference divides by bins - 1), low / range set, the last layer
-// adim * bins <= 256 wide
-static int es_binned_check(const char* fn, const int* layer_sizes, int n_layers, int bins, const float* low, const float* range) {
-    ES_REQUIRE(bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, bins);
-    ES_REQUIRE(low && range, "%s: NULL low / range", fn);
-    const int out = layer_sizes[n_layers];
-    ES_REQUIRE(out % bins == 0, "%s: the last layer's %d outputs are not adim * bins for bins %d", fn, out, bins);
-    if (out > 256) {
-        es_set_error("%s: binned heads up to adim * bins = 256 outputs supported, got %d * %d", fn, out / bins, bins);
-        return ES_ERR_UNSUPPORTED;
-    }
-    return ES_OK;
-}
-
 int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
                                const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
                                const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
                                float* behv_pos, float* behv_neg, int bins, const float* low, const float* range, int mode,
                                void* stream) {
     ES_ENTER(ctx);
-    EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
-                   fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
-    int rc = es_rollout_check("es_rollout_openloop_binned", obsn != nullptr, r);
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
+                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
+    return es_openloop(ctx, "es_rollout_openloop_binned", r, ES_HEAD_BINNED, mode, (cudaStream_t)stream);
+}
+
+// the shapes es_rollout_closedloop's one-CTA kernel (rollout_closed.cu) covers: two hidden layers <= 64, act <= 64, obs <= 384
+static bool es_closed_one_cta_covers(const int* dims, int n_layers) {
+    return n_layers == 3 && dims[1] <= 64 && dims[2] <= 64 && dims[3] <= 64 && dims[0] <= 384;
+}
+
+// a closed-loop entry point after ES_ENTER: its checks in order (the cluster plan refuses a shape whatever n_pairs is;
+// rollout_closed.cu checks its own coverage when it runs), the scratch rows of E > 1 episodes, then the kernel; `fn` names it in
+// every message
+static int es_closedloop(es_ctx* ctx, const char* fn, const EsRollout& r, EsClosedEnv env, EsHead head, cudaStream_t stream) {
+    int rc = es_rollout_check(fn, env.ob_mean && env.ob_std && env.obs0 && env.env_a && env.env_b, r);
     if (rc) return rc;
-    rc = es_binned_check("es_rollout_openloop_binned", layer_sizes, n_layers, bins, low, range);
-    if (rc) return rc;
-    if (mode == ES_ROLLOUT_TC) {
-        es_set_error("es_rollout_openloop_binned: ES_ROLLOUT_TC refuses binned heads: an arg-max over float16-grade outputs is not "
-                     "parity grade; use ES_ROLLOUT_TC3 or ES_ROLLOUT_F32");
+    if (head == ES_HEAD_TANH_ONE_CTA && r.n_layers != 3) {
+        es_set_error("%s: two hidden layers (n_layers == 3) supported, got %d", fn, r.n_layers);
         return ES_ERR_UNSUPPORTED;
     }
-    if (mode == ES_ROLLOUT_TC3 && !es_tcw_covers_binned(r)) {
-        char why[96];                               // the part of the shape outside the coverage
-        if (n_layers < 3 || n_layers > 5) {
-            snprintf(why, sizeof why, "%d hidden layers", n_layers - 1);
-        } else if (layer_sizes[0] > 256) {
-            snprintf(why, sizeof why, "obs %d", layer_sizes[0]);
-        } else {
-            snprintf(why, sizeof why, "the shape");
-            for (int l = 1; l < n_layers; ++l)
-                if (layer_sizes[l] % 64 || layer_sizes[l] > 256) {
-                    snprintf(why, sizeof why, "hidden layer %d of width %d", l, layer_sizes[l]);
-                    break;
-                }
-        }
-        es_set_error("es_rollout_openloop_binned: ES_ROLLOUT_TC3 covers binned heads with 2 to 4 hidden layers of widths in {64, 128, "
-                     "192, 256} and obs <= 256, got %s; use ES_ROLLOUT_F32", why);
-        return ES_ERR_UNSUPPORTED;
+    ES_REQUIRE(env.band >= 1 && env.band <= r.layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
+    ES_REQUIRE((env.ob_sum == nullptr) == (env.ob_sumsq == nullptr) && (env.ob_sum == nullptr) == (env.ob_count == nullptr),
+               "%s: ob_sum/ob_sumsq/ob_count must all be set or NULL", fn);
+    int C = 0;
+    size_t smem = 0;
+    if (head == ES_HEAD_BINNED) {
+        rc = es_binned_check(fn, r);
+        if (!rc) rc = es_closedw_binned_plan(r.layer_sizes, r.n_layers, env.band, r.bins, &C, &smem);
+    } else if (head == ES_HEAD_TANH) {
+        rc = es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
     }
-    if (mode != ES_ROLLOUT_F32 && mode != ES_ROLLOUT_TC3) {
-        es_set_error("es_rollout_openloop_binned: unknown mode %d", mode);
-        return ES_ERR_INVALID;
+    if (rc) return rc;
+    if (r.n_pairs == 0) return ES_OK;
+    if (r.n_episodes > 1) {
+        void* rows = nullptr;
+        rc = es_ctx_scratch(ctx, (size_t)2 * ctx->sm_count * r.T * sizeof(double), &rows);
+        if (rc) return rc;
+        env.ep_rows = (double*)rows;
     }
-    if (n_pairs == 0) return ES_OK;
-    if (mode == ES_ROLLOUT_TC3) return es_impl_rollout_tcw(ctx, r, 1, (cudaStream_t)stream);
-    return es_impl_rollout_f32(ctx, r, (cudaStream_t)stream);
+    if (head == ES_HEAD_TANH_ONE_CTA || (head == ES_HEAD_TANH && es_closed_one_cta_covers(r.layer_sizes, r.n_layers)))
+        return es_impl_rollout_closed(ctx, r, env, stream);
+    return es_impl_rollout_closedw(ctx, r, env, stream);
 }
 
 int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
@@ -339,42 +385,37 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
     ES_ENTER(ctx);
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1};
-    const int rc = es_rollout_check("es_rollout_closedloop", ob_mean && ob_std && obs0 && env_a && env_b, r);
-    if (rc) return rc;
-    if (n_layers != 3) {
-        es_set_error("es_rollout_closedloop: two hidden layers (n_layers == 3) supported, got %d", n_layers);
-        return ES_ERR_UNSUPPORTED;
-    }
-    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop: band must be in [1, obs_dim]");
-    ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
-               "es_rollout_closedloop: ob_sum/ob_sumsq/ob_count must all be set or NULL");
-    if (n_pairs == 0) return ES_OK;
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
+    return es_closedloop(ctx, "es_rollout_closedloop", r, env, ES_HEAD_TANH_ONE_CTA, (cudaStream_t)stream);
 }
 
-// the shapes es_rollout_closedloop's one-CTA kernel (rollout_closed.cu) covers: two hidden layers <= 64, act <= 64, obs <= 384
-static bool es_closed_one_cta_covers(const int* dims, int n_layers) {
-    return n_layers == 3 && dims[1] <= 64 && dims[2] <= 64 && dims[3] <= 64 && dims[0] <= 384;
+// both plan entry points after ES_ENTER (`bins`: a binned head's, 0 for a tanh head)
+static int es_closedloop_plan(es_ctx* ctx, const char* fn, const int* layer_sizes, int n_layers, int band, EsHead head, int bins,
+                              int* cluster_size, int* clusters, int64_t* smem_bytes) {
+    ES_REQUIRE(layer_sizes && cluster_size && clusters && smem_bytes, "%s: NULL pointer", fn);
+    ES_REQUIRE(n_layers >= 1 && n_layers <= ES_MAX_LAYERS, "%s: n_layers must be in [1,%d]", fn, ES_MAX_LAYERS);
+    for (int l = 0; l <= n_layers; ++l) ES_REQUIRE(layer_sizes[l] > 0, "%s: layer size <= 0", fn);
+    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
+    const bool binned = head == ES_HEAD_BINNED;
+    ES_REQUIRE(!binned || bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, bins);
+    int C = 0;
+    size_t smem = 0;
+    const int rc = binned ? es_closedw_binned_plan(layer_sizes, n_layers, band, bins, &C, &smem)
+                          : es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);
+    if (rc) return rc;
+    if (!binned && es_closed_one_cta_covers(layer_sizes, n_layers)) {
+        *cluster_size = 0; *clusters = ctx->sm_count; *smem_bytes = 0;
+        return ES_OK;
+    }
+    *cluster_size = C; *smem_bytes = (int64_t)smem;
+    return es_closedw_max_clusters(n_layers, bins, C, smem, clusters);
 }
 
 int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int* cluster_size, int* clusters,
                                    int64_t* smem_bytes) {
     ES_ENTER(ctx);
-    ES_REQUIRE(layer_sizes && cluster_size && clusters && smem_bytes, "es_rollout_closedloop_mlp_plan: NULL pointer");
-    ES_REQUIRE(n_layers >= 1 && n_layers <= ES_MAX_LAYERS, "es_rollout_closedloop_mlp_plan: n_layers must be in [1,%d]", ES_MAX_LAYERS);
-    for (int l = 0; l <= n_layers; ++l) ES_REQUIRE(layer_sizes[l] > 0, "es_rollout_closedloop_mlp_plan: layer size <= 0");
-    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop_mlp_plan: band must be in [1, obs_dim]");
-    int C = 0;
-    size_t smem = 0;
-    const int rc = es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);
-    if (rc) return rc;
-    if (es_closed_one_cta_covers(layer_sizes, n_layers)) {
-        *cluster_size = 0; *clusters = ctx->sm_count; *smem_bytes = 0;
-        return ES_OK;
-    }
-    *cluster_size = C; *smem_bytes = (int64_t)smem;
-    return es_closedw_max_clusters(n_layers, C, smem, clusters);
+    return es_closedloop_plan(ctx, "es_rollout_closedloop_mlp_plan", layer_sizes, n_layers, band, ES_HEAD_TANH, 0, cluster_size,
+                              clusters, smem_bytes);
 }
 
 int es_rollout_closedloop_mlp_episodes(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
@@ -389,25 +430,8 @@ int es_rollout_closedloop_mlp_episodes(es_ctx* ctx, const float* table, int64_t 
     // without action noise the episodes are identical: the noise-free kernels run one (as es_rollout_openloop_episodes)
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
-    int rc = es_rollout_check("es_rollout_closedloop_mlp", ob_mean && ob_std && obs0 && env_a && env_b, r);
-    if (rc) return rc;
-    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "es_rollout_closedloop_mlp: band must be in [1, obs_dim]");
-    ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
-               "es_rollout_closedloop_mlp: ob_sum/ob_sumsq/ob_count must all be set or NULL");
-    int C = 0;
-    size_t smem = 0;
-    rc = es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);      // coverage does not depend on n_pairs
-    if (rc) return rc;
-    if (n_pairs == 0) return ES_OK;
-    EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    if (r.n_episodes > 1) {
-        void* rows = nullptr;
-        rc = es_ctx_scratch(ctx, (size_t)2 * ctx->sm_count * T * sizeof(double), &rows);
-        if (rc) return rc;
-        env.ep_rows = (double*)rows;
-    }
-    if (es_closed_one_cta_covers(layer_sizes, n_layers)) return es_impl_rollout_closed(ctx, r, env, (cudaStream_t)stream);
-    return es_impl_rollout_closedw(ctx, r, env, (cudaStream_t)stream);
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    return es_closedloop(ctx, "es_rollout_closedloop_mlp", r, env, ES_HEAD_TANH, (cudaStream_t)stream);
 }
 
 int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
@@ -425,18 +449,8 @@ int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len
 int es_rollout_closedloop_mlp_binned_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size,
                                           int* clusters, int64_t* smem_bytes) {
     ES_ENTER(ctx);
-    const char* fn = "es_rollout_closedloop_mlp_binned_plan";
-    ES_REQUIRE(layer_sizes && cluster_size && clusters && smem_bytes, "%s: NULL pointer", fn);
-    ES_REQUIRE(n_layers >= 1 && n_layers <= ES_MAX_LAYERS, "%s: n_layers must be in [1,%d]", fn, ES_MAX_LAYERS);
-    for (int l = 0; l <= n_layers; ++l) ES_REQUIRE(layer_sizes[l] > 0, "%s: layer size <= 0", fn);
-    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
-    ES_REQUIRE(bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, bins);
-    int C = 0;
-    size_t smem = 0;
-    const int rc = es_closedw_binned_plan(layer_sizes, n_layers, band, bins, &C, &smem);
-    if (rc) return rc;
-    *cluster_size = C; *smem_bytes = (int64_t)smem;
-    return es_closedw_binned_max_clusters(n_layers, C, smem, clusters);
+    return es_closedloop_plan(ctx, "es_rollout_closedloop_mlp_binned_plan", layer_sizes, n_layers, band, ES_HEAD_BINNED, bins,
+                              cluster_size, clusters, smem_bytes);
 }
 
 int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
@@ -447,23 +461,10 @@ int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t ta
                                      float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins, const float* low,
                                      const float* range, void* stream) {
     ES_ENTER(ctx);
-    const char* fn = "es_rollout_closedloop_mlp_binned";
     const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
-    int rc = es_rollout_check(fn, ob_mean && ob_std && obs0 && env_a && env_b, r);
-    if (rc) return rc;
-    ES_REQUIRE(band >= 1 && band <= layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
-    ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
-               "%s: ob_sum/ob_sumsq/ob_count must all be set or NULL", fn);
-    rc = es_binned_check(fn, layer_sizes, n_layers, bins, low, range);
-    if (rc) return rc;
-    int C = 0;
-    size_t smem = 0;
-    rc = es_closedw_binned_plan(layer_sizes, n_layers, band, bins, &C, &smem);      // coverage does not depend on n_pairs
-    if (rc) return rc;
-    if (n_pairs == 0) return ES_OK;
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    return es_impl_rollout_closedw(ctx, r, env, (cudaStream_t)stream);
+    return es_closedloop(ctx, "es_rollout_closedloop_mlp_binned", r, env, ES_HEAD_BINNED, (cudaStream_t)stream);
 }
 
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,

@@ -157,13 +157,13 @@ bool es_tcw_covers_binned(const EsRollout&);
 int es_impl_rollout_closed(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // the closed loop for tanh MLPs with 2 to 4 hidden layers of <= 256 units, obs <= 384, act <= 64, an even band <= 16, on a
 // thread-block cluster per evaluation (rollout_closedw.cu): the cluster size and shared memory per CTA of a shape (or
-// ES_ERR_UNSUPPORTED with the limit in es_last_error()), the clusters resident at once, and the rollout
+// ES_ERR_UNSUPPORTED with the limit in es_last_error()), the clusters resident at once (bins: 0 for a tanh head, else the
+// binned head's), and the rollout
 int es_closedw_plan(const int* layer_sizes, int n_layers, int band, int* cluster_size, size_t* smem_bytes);
-int es_closedw_max_clusters(int n_layers, int cluster_size, size_t smem_bytes, int* clusters);
+int es_closedw_max_clusters(int n_layers, int bins, int cluster_size, size_t smem_bytes, int* clusters);
 int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // binned heads (EsRollout::bins >= 2): every shape es_closedw_plan covers with act = adim; the cluster kernel at every C
 int es_closedw_binned_plan(const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes);
-int es_closedw_binned_max_clusters(int n_layers, int cluster_size, size_t smem_bytes, int* clusters);
 // U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
 int es_launch_ubase(es_ctx*, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
                     float* ubase, cudaStream_t);

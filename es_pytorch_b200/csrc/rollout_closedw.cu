@@ -478,11 +478,8 @@ static int cw_max_clusters(CwKernel k, int C, size_t smem, int* clusters) {
     ES_CHECK_CUDA(cudaOccupancyMaxActiveClusters(clusters, k, &cfg));
     return ES_OK;
 }
-int es_closedw_max_clusters(int n_layers, int C, size_t smem, int* clusters) {
-    return cw_max_clusters(cw_kernel(n_layers), C, smem, clusters);
-}
-int es_closedw_binned_max_clusters(int n_layers, int C, size_t smem, int* clusters) {
-    return cw_max_clusters(cw_kernel(n_layers, true), C, smem, clusters);
+int es_closedw_max_clusters(int n_layers, int bins, int C, size_t smem, int* clusters) {
+    return cw_max_clusters(cw_kernel(n_layers, bins != 0), C, smem, clusters);
 }
 
 int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {

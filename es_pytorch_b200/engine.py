@@ -270,6 +270,19 @@ class Engine:
               'es_obstat_accumulate_coins')
 
     # ------------------------------------------------------------------ a3+a4+a5
+    def _check_rollout(self, table, idx, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg):
+        """The arguments every rollout takes: table, pair indices and parameters, ``fit_stride`` fitness rows and (or None) the
+        behaviour rows of every pair.  Returns (pairs, layer sizes as a C array)."""
+        d = self.device
+        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
+        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
+        n = idx.numel()
+        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
+        if behv_pos is not None:
+            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
+            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
+        return n, (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+
     def rollout(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], obsn, rew_vec, pos_scale: float,
                 fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None, behv_neg=None, mode: int = ES_ROLLOUT_F32,
                 act_noise=None, episodes: int = 1, head=None):
@@ -280,27 +293,28 @@ class Engine:
         ``head``: None or ``'tanh'`` (the outputs are the actions), or an ``nn.BinnedHead`` (FFBinned:
         es_rollout_openloop_binned; ``layer_sizes[-1]`` is adim * bins, ``rew_vec`` [T, adim]; no action noise; modes F32 and
         TC3)."""
-        if head is not None and head != 'tanh':
-            return self._rollout_binned(table, idx, theta, sigma, layer_sizes, obsn, rew_vec, pos_scale, fit_pos, fit_neg,
-                                        fit_stride, behv_pos, behv_neg, mode, act_noise, episodes, head)
+        binned = head is not None and head != 'tanh'
+        if binned and (act_noise is not None or int(episodes) != 1):
+            raise ValueError('a binned head draws no action noise: act_noise must be None and episodes 1')
+        n, ls = self._check_rollout(table, idx, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg)
         d = self.device
-        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
         _req(obsn, torch.float32, 'obsn', d); _req(rew_vec, torch.float32, 'rew_vec', d)
-        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
-        n = idx.numel()
-        T = obsn.shape[0]
-        assert obsn.shape[1] == layer_sizes[0] and rew_vec.shape == (T, layer_sizes[-1])
-        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
-        if behv_pos is not None:
-            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
-            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
+        T, act = obsn.shape[0], head.adim if binned else layer_sizes[-1]
+        assert obsn.shape[1] == layer_sizes[0] and rew_vec.shape == (T, act)
         episodes = int(episodes)
         if episodes < 1:
             raise ValueError(f'episodes must be >= 1, got {episodes}')
         if act_noise is not None:
             _req(act_noise, torch.float32, 'act_noise', d)
-            assert act_noise.numel() == n * 2 * episodes * T * layer_sizes[-1]
-        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+            assert act_noise.numel() == n * 2 * episodes * T * act
+        args = (self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
+                _ptr(obsn), _ptr(rew_vec), T, float(pos_scale), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride), _ptr(behv_pos),
+                _ptr(behv_neg))
+        if binned:
+            low, rng = self._head_arrays(head)
+            check(self.lib.es_rollout_openloop_binned(*args, int(head.bins), _ptr(low), _ptr(rng), int(mode), self.stream),
+                  'es_rollout_openloop_binned')
+            return
         if mode in (ES_ROLLOUT_TC, ES_ROLLOUT_TC3):
             # the library keeps a bf16 shadow of the table keyed by (pointer, length); a different tensor object (the
             # caching allocator reuses addresses) or an in-place torch write (version counter) invalidates it
@@ -308,33 +322,7 @@ class Engine:
             if ref is None or ref() is not table or ver != table._version:
                 check(self.lib.es_noise_table_changed(self._ctx), 'es_noise_table_changed')
                 self._tc_table = (weakref.ref(table), table._version)
-        check(self.lib.es_rollout_openloop_episodes(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta),
-                                                    theta.numel(), float(sigma), ls, len(layer_sizes) - 1, _ptr(obsn),
-                                                    _ptr(rew_vec), T, float(pos_scale), _ptr(fit_pos), _ptr(fit_neg),
-                                                    int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(act_noise),
-                                                    episodes, int(mode), self.stream), 'es_rollout_openloop')
-
-    def _rollout_binned(self, table, idx, theta, sigma, layer_sizes, obsn, rew_vec, pos_scale, fit_pos, fit_neg, fit_stride,
-                        behv_pos, behv_neg, mode, act_noise, episodes, head):
-        d = self.device
-        if act_noise is not None or int(episodes) != 1:
-            raise ValueError('a binned head draws no action noise: act_noise must be None and episodes 1')
-        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
-        _req(obsn, torch.float32, 'obsn', d); _req(rew_vec, torch.float32, 'rew_vec', d)
-        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
-        n, T = idx.numel(), obsn.shape[0]
-        assert obsn.shape[1] == layer_sizes[0] and rew_vec.shape == (T, head.adim)
-        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
-        if behv_pos is not None:
-            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
-            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
-        low, rng = self._head_arrays(head)
-        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
-        check(self.lib.es_rollout_openloop_binned(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
-                                                  float(sigma), ls, len(layer_sizes) - 1, _ptr(obsn), _ptr(rew_vec), T,
-                                                  float(pos_scale), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride), _ptr(behv_pos),
-                                                  _ptr(behv_neg), int(head.bins), _ptr(low), _ptr(rng), int(mode), self.stream),
-              'es_rollout_openloop_binned')
+        check(self.lib.es_rollout_openloop_episodes(*args, _ptr(act_noise), episodes, int(mode), self.stream), 'es_rollout_openloop')
 
     def _head_arrays(self, head):
         """A binned head's (low, high - low) float32 device tensors, uploaded once per head (the last few heads are kept)."""
@@ -347,6 +335,23 @@ class Engine:
             arrs = cache[key] = head.device_arrays(self)
         return arrs
 
+    def _check_closed_env(self, n, layer_sizes, act, ob_mean, ob_std, obs0, env_a, env_b, rew_vec, coin_words, ob_sum, ob_sumsq,
+                          ob_count):
+        """The closed-loop env's arguments for ``n`` pairs (``act``: the env's action dimension).  Returns (steps, band)."""
+        d = self.device
+        _req(ob_mean, torch.float64, 'ob_mean', d); _req(ob_std, torch.float64, 'ob_std', d)
+        _req(obs0, torch.float32, 'obs0', d); _req(env_a, torch.float32, 'env_a', d); _req(env_b, torch.float32, 'env_b', d)
+        _req(rew_vec, torch.float32, 'rew_vec', d)
+        T, obs, band = rew_vec.shape[0], int(layer_sizes[0]), env_a.shape[0]
+        assert env_a.shape == (band, obs) and env_b.shape == (act, obs) and obs0.numel() == obs and rew_vec.shape == (T, act)
+        assert ob_mean.numel() == obs and ob_std.numel() == obs
+        if coin_words is not None:
+            assert coin_words.dtype == torch.int32 and coin_words.numel() == 4 * n and coin_words.is_contiguous()
+        if ob_sum is not None:
+            _req(ob_sum, torch.float64, 'ob_sum', d); _req(ob_sumsq, torch.float64, 'ob_sumsq', d); _req(ob_count, torch.float64, 'ob_count', d)
+            assert ob_sum.numel() == obs and ob_sumsq.numel() == obs and ob_count.numel() == 2
+        return T, band
+
     def rollout_closed(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
                        obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,
                        behv_neg=None, coin_words=None, save_obs_chance: float = 0.0, ob_sum=None, ob_sumsq=None, ob_count=None):
@@ -354,26 +359,9 @@ class Engine:
         ``env_b`` [act, obs] are the transposed transition matrices, ``obs0`` the start observation; the observation
         normalisation (``ob_mean`` / ``ob_std`` float64, ``ob_clip``) happens inside.  ``coin_words`` [n, 4] + the three
         float64 statistics buffers: ObStat increments of the evaluations whose save_obs coin fell."""
-        d = self.device
-        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
-        _req(ob_mean, torch.float64, 'ob_mean', d); _req(ob_std, torch.float64, 'ob_std', d)
-        _req(obs0, torch.float32, 'obs0', d); _req(env_a, torch.float32, 'env_a', d); _req(env_b, torch.float32, 'env_b', d)
-        _req(rew_vec, torch.float32, 'rew_vec', d)
-        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
-        n, T, obs, act = idx.numel(), rew_vec.shape[0], int(layer_sizes[0]), int(layer_sizes[-1])
-        band = env_a.shape[0]
-        assert env_a.shape == (band, obs) and env_b.shape == (act, obs) and obs0.numel() == obs and rew_vec.shape == (T, act)
-        assert ob_mean.numel() == obs and ob_std.numel() == obs
-        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
-        if behv_pos is not None:
-            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
-            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
-        if coin_words is not None:
-            assert coin_words.dtype == torch.int32 and coin_words.numel() == 4 * n and coin_words.is_contiguous()
-        if ob_sum is not None:
-            _req(ob_sum, torch.float64, 'ob_sum', d); _req(ob_sumsq, torch.float64, 'ob_sumsq', d); _req(ob_count, torch.float64, 'ob_count', d)
-            assert ob_sum.numel() == obs and ob_sumsq.numel() == obs and ob_count.numel() == 2
-        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+        n, ls = self._check_rollout(table, idx, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg)
+        T, band = self._check_closed_env(n, layer_sizes, int(layer_sizes[-1]), ob_mean, ob_std, obs0, env_a, env_b, rew_vec,
+                                         coin_words, ob_sum, ob_sumsq, ob_count)
         check(self.lib.es_rollout_closedloop(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
                                              float(sigma), ls, len(layer_sizes) - 1, _ptr(ob_mean), _ptr(ob_std), float(ob_clip),
                                              _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T, float(pos_scale),
@@ -398,53 +386,26 @@ class Engine:
             raise ValueError(f'episodes must be >= 1, got {episodes}')
         if binned and act_noise is not None:
             raise ValueError('a binned head draws no action noise (FFBinned.forward ignores rs): act_noise must be None')
-        d = self.device
-        _req(table, torch.float32, 'table', d); _req(idx, torch.int64, 'idx', d); _req(theta, torch.float32, 'theta', d)
-        _req(ob_mean, torch.float64, 'ob_mean', d); _req(ob_std, torch.float64, 'ob_std', d)
-        _req(obs0, torch.float32, 'obs0', d); _req(env_a, torch.float32, 'env_a', d); _req(env_b, torch.float32, 'env_b', d)
-        _req(rew_vec, torch.float32, 'rew_vec', d)
-        _req(fit_pos, torch.float64, 'fit_pos', d); _req(fit_neg, torch.float64, 'fit_neg', d)
-        n, T, obs = idx.numel(), rew_vec.shape[0], int(layer_sizes[0])
+        n, ls = self._check_rollout(table, idx, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg)
         act = head.adim if binned else int(layer_sizes[-1])
-        band = env_a.shape[0]
-        assert env_a.shape == (band, obs) and env_b.shape == (act, obs) and obs0.numel() == obs and rew_vec.shape == (T, act)
-        assert ob_mean.numel() == obs and ob_std.numel() == obs
-        assert fit_pos.numel() >= n * fit_stride and fit_neg.numel() >= n * fit_stride
-        if behv_pos is not None:
-            _req(behv_pos, torch.float32, 'behv_pos', d); _req(behv_neg, torch.float32, 'behv_neg', d)
-            assert behv_pos.numel() == 3 * n and behv_neg.numel() == 3 * n
-        if coin_words is not None:
-            assert coin_words.dtype == torch.int32 and coin_words.numel() == 4 * n and coin_words.is_contiguous()
-        if ob_sum is not None:
-            _req(ob_sum, torch.float64, 'ob_sum', d); _req(ob_sumsq, torch.float64, 'ob_sumsq', d); _req(ob_count, torch.float64, 'ob_count', d)
-            assert ob_sum.numel() == obs and ob_sumsq.numel() == obs and ob_count.numel() == 2
-        ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
+        T, band = self._check_closed_env(n, layer_sizes, act, ob_mean, ob_std, obs0, env_a, env_b, rew_vec, coin_words, ob_sum,
+                                         ob_sumsq, ob_count)
+        if act_noise is not None:
+            _req(act_noise, torch.float32, 'act_noise', self.device)
+            assert act_noise.numel() == n * 2 * episodes * T * act
+        args = (self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
+                _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T,
+                float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
+                _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count))
         if binned:
             low, rng = self._head_arrays(head)
-            check(self.lib.es_rollout_closedloop_mlp_binned(
-                self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
-                _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T,
-                float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
-                _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), int(head.bins), _ptr(low), _ptr(rng),
-                self.stream), 'es_rollout_closedloop_mlp_binned')
+            check(self.lib.es_rollout_closedloop_mlp_binned(*args, int(head.bins), _ptr(low), _ptr(rng), self.stream),
+                  'es_rollout_closedloop_mlp_binned')
             return
-        if act_noise is not None or episodes != 1:
-            if act_noise is not None:
-                _req(act_noise, torch.float32, 'act_noise', d)
-                assert act_noise.numel() == n * 2 * episodes * T * act
-            check(self.lib.es_rollout_closedloop_mlp_episodes(
-                self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
-                _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T,
-                float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
-                _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), _ptr(act_noise), episodes,
-                self.stream), 'es_rollout_closedloop_mlp_episodes')
-            return
-        check(self.lib.es_rollout_closedloop_mlp(self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(),
-                                                 float(sigma), ls, len(layer_sizes) - 1, _ptr(ob_mean), _ptr(ob_std), float(ob_clip),
-                                                 _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T, float(pos_scale),
-                                                 _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg),
-                                                 int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq),
-                                                 _ptr(ob_count), self.stream), 'es_rollout_closedloop_mlp')
+        # with no noise and one episode this is es_rollout_closedloop_mlp (a forwarder to it): its errors keep that name
+        plain = act_noise is None and episodes == 1
+        check(self.lib.es_rollout_closedloop_mlp_episodes(*args, _ptr(act_noise), episodes, self.stream),
+              'es_rollout_closedloop_mlp' if plain else 'es_rollout_closedloop_mlp_episodes')
 
     def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int, head=None):
         """How ``rollout_closed_mlp`` runs a shape: (CTAs per cluster, clusters resident at once, shared memory bytes per CTA);

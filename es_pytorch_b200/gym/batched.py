@@ -101,15 +101,14 @@ class BatchedRollout:
                 for _ in range(self.coins_per_eval):
                     rs.random()
         noise_rs = streams[0] if (use_ac_noise and streams is not None and len(streams)) else None
-        closed = getattr(self.env, 'is_synthetic_closedloop', False)
         head = model.head() if hasattr(model, 'head') else None
         noisy = noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0
         episodes = self.episodes if noisy else 1
-        if closed and head is not None and self._closed_on_device(model.layer_sizes(), head):
-            # the closed-loop evaluation, all its episodes, as one launch (the observations are not returned: this result never
-            # carries them)
-            from .gym_runner import _device_episode_closed
-            total, pos, _ = _device_episode_closed(model, self.env, self.max_steps, noise_rs if noisy else None, episodes)
+        if head is not None and (getattr(self.env, 'is_synthetic_openloop', False)
+                                 or self._closed_on_device(model.layer_sizes(), head)):
+            # the evaluation, all its episodes, as one launch (the observations are not returned: this result never carries them)
+            from .gym_runner import _device_episode
+            total, pos, _ = _device_episode(model, self.env, self.max_steps, noise_rs if noisy else None, episodes)
             return self.result_from_device(total, pos)
         if episodes > 1:
             rews, behv, steps = self._run_episodes(model, noise_rs, episodes)
@@ -136,14 +135,8 @@ class BatchedRollout:
         return True
 
     def _run_episodes(self, model, rs, episodes: int):
-        """obj.py:57-60 with action noise: ``episodes`` runs of run_model drawing from ``rs``, rewards summed per step in
-        float64 in episode order and divided by the count.  A tanh MLP on the open-loop env runs all episodes as one launch
-        (one forward, the episodes' noise rows back to back) and reports the total of the per-step means.  (The closed-loop
-        env's device path is ``__call__``'s ``_device_episode_closed``.)"""
-        from .gym_runner import _device_episode
-        if getattr(self.env, 'is_synthetic_openloop', False) and hasattr(model, 'is_tanh_mlp') and model.is_tanh_mlp():
-            total, pos, T = _device_episode(model, self.env, self.max_steps, rs, episodes)
-            return [total], [float(pos[0]), float(pos[1]), float(pos[2])] * int(self.max_steps), T - 1
+        """obj.py:57-60 with action noise for a policy ``__call__`` does not run on the device: ``episodes`` runs of run_model
+        drawing from ``rs``, rewards summed per step in float64 in episode order and divided by the count."""
         rews = np.zeros(self.max_steps)
         for _ in range(episodes):
             rew, behv, _, steps = run_model(model, self.env, self.max_steps, rs)

@@ -36,49 +36,15 @@ def hbaselines_pos(env):
 
 
 def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
-    """One evaluation as one launch.  ``episodes`` > 1 with action noise: the per-step mean over that many episodes
-    (obj.py:54-63), their noise drawn back to back from ``rs``; returns the last episode's final position."""
+    """One evaluation on the open- or closed-loop synthetic env as one launch (sigma = 0).  With ``rs`` and a tanh model's
+    ac_std != 0: the action noise of ``episodes`` episodes drawn back to back from ``rs``, the per-step mean over the episodes
+    (obj.py:54-63).  Returns (fitness, the last episode's final position, steps)."""
     from ..engine import get_engine
     from ..core.policy import Policy
     eng = get_engine()
-    sizes = model.layer_sizes()
+    sizes, head = model.layer_sizes(), model.head()
     T = min(int(max_steps), env.T)
     obs_dev, rew_dev = env.device_arrays(eng)
-    theta = eng.to_device(Policy.get_flat(model), torch.float32)
-    P = theta.numel()
-    mean = eng.to_device(np.ascontiguousarray(model._obmean, dtype=np.float64).reshape(-1), torch.float64)
-    std = eng.to_device(np.ascontiguousarray(model._obstd, dtype=np.float64).reshape(-1), torch.float64)
-    obsn = eng.normalise_obs(obs_dev[:T], mean, std, float(model.ob_clip))
-    table = torch.zeros(P + 1, dtype=torch.float32, device=eng.device)      # sigma = 0: the slice is irrelevant
-    idx = torch.zeros(1, dtype=torch.int64, device=eng.device)
-    fit = torch.zeros(2, dtype=torch.float64, device=eng.device)
-    behv = torch.zeros(2, 3, dtype=torch.float32, device=eng.device)
-    noise = None
-    ac_std = float(getattr(model, '_action_std', 0) or 0)
-    if rs is not None and ac_std != 0:
-        # nn.py:47-48: T calls of rs.randn(act) * ac_std; one call of rs.randn(T * act) consumes the stream identically
-        # (legacy gaussians are produced one by one, cached second value included).  [pair 0][+ | -][episodes][T][act]: both
-        # evaluations of the sigma = 0 "pair" see the same noise, only the first is used.
-        nz = (rs.randn(episodes * T * sizes[-1]) * ac_std).astype(np.float32)
-        noise = eng.to_device(np.stack([nz, nz]).reshape(1, 2, -1))
-    else:
-        episodes = 1
-    eng.rollout(table, idx, theta, 0.0, sizes, obsn, rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1,
-                behv[0:1].view(-1), behv[1:2].view(-1), act_noise=noise, episodes=episodes, head=model.head())
-    return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
-
-
-def _device_episode_closed(model, env, max_steps: int, rs=None, episodes: int = 1):
-    """One evaluation on the closed-loop synthetic env as one launch of es_rollout_closedloop_mlp (sigma = 0).  With ``rs`` and
-    a tanh model's ac_std != 0: the action noise of ``episodes`` episodes drawn back to back from ``rs`` (as ``_device_episode``),
-    the per-step mean over the episodes, the last episode's final position."""
-    from ..engine import get_engine
-    from ..core.policy import Policy
-    eng = get_engine()
-    sizes = model.layer_sizes()
-    T = min(int(max_steps), env.T)
-    _, rew_dev = env.device_arrays(eng)
-    obs0, env_a, env_b = env.device_closed(eng)
     theta = eng.to_device(Policy.get_flat(model), torch.float32)
     mean = eng.to_device(np.ascontiguousarray(model._obmean, dtype=np.float64).reshape(-1), torch.float64)
     std = eng.to_device(np.ascontiguousarray(model._obstd, dtype=np.float64).reshape(-1), torch.float64)
@@ -86,19 +52,24 @@ def _device_episode_closed(model, env, max_steps: int, rs=None, episodes: int = 
     idx = torch.zeros(1, dtype=torch.int64, device=eng.device)
     fit = torch.zeros(2, dtype=torch.float64, device=eng.device)
     behv = torch.zeros(2, 3, dtype=torch.float32, device=eng.device)
-    head = model.head()
     noise = None
     ac_std = float(getattr(model, '_action_std', 0) or 0)
     if rs is not None and ac_std != 0 and head == 'tanh':
-        # the closed loop's noise does not depend on the state: one rs.randn(episodes * T * act) call consumes the stream as
-        # the episodes' T calls of rs.randn(act) each (nn.py:47-48); both signs of the sigma = 0 "pair" see it, only + is used
+        # nn.py:47-48: T calls of rs.randn(act) * ac_std per episode; one call of rs.randn(episodes * T * act) consumes the stream
+        # identically (legacy gaussians are produced one by one, cached second value included; neither env's noise depends on
+        # its state).  [pair 0][+ | -][episodes][T][act]: both evaluations of the sigma = 0 "pair" see it, only + is used.
         nz = (rs.randn(episodes * T * sizes[-1]) * ac_std).astype(np.float32)
         noise = eng.to_device(np.stack([nz, nz]).reshape(1, 2, -1))
     else:
         episodes = 1
-    eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), obs0, env_a, env_b,
-                           rew_dev[:T].contiguous(), env.pos_scale, fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1),
-                           head=head, act_noise=noise, episodes=episodes)
+    out = (fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1))
+    if getattr(env, 'is_synthetic_closedloop', False):
+        eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), *env.device_closed(eng),
+                               rew_dev[:T].contiguous(), env.pos_scale, *out, head=head, act_noise=noise, episodes=episodes)
+    else:
+        obsn = eng.normalise_obs(obs_dev[:T], mean, std, float(model.ob_clip))
+        eng.rollout(table, idx, theta, 0.0, sizes, obsn, rew_dev[:T].contiguous(), env.pos_scale, *out, act_noise=noise,
+                    episodes=episodes, head=head)
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 
