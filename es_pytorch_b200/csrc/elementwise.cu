@@ -187,8 +187,23 @@ __global__ void novelty_kernel(const float* __restrict__ behv, int n, const doub
             best[p] = d;
         }
     }
+    // np.mean's sum (numpy's pairwise_sum for n <= 128): sequential below 8 terms, else 8 strided accumulators combined
+    // as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the n % 8 leftover terms in order
     double s = 0.0;
-    for (int i = 0; i < kk; ++i) s = __dadd_rn(s, best[i]);
+    if (kk < 8) {
+        for (int i = 0; i < kk; ++i) s = __dadd_rn(s, best[i]);
+    } else {
+        double r[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] = best[j];
+        int i = 8;
+        for (; i < kk - kk % 8; i += 8)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], best[i + j]);
+        s = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])),
+                      __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
+        for (; i < kk; ++i) s = __dadd_rn(s, best[i]);
+    }
     out[(size_t)e * out_stride] = __ddiv_rn(s, (double)kk);
 }
 

@@ -35,9 +35,10 @@ __device__ __forceinline__ double rk_unkey(unsigned long long k) {
     return __longlong_as_double((long long)b);
 }
 
-// keys of the smallest / largest finite value (per objective); the minimum is stored inverted so that all-zero bytes mean
-// "no finite value yet" for both (one memset initialises the histogram and the statistics)
-struct RkStats { unsigned long long kmin_inv, kmax; };
+// keys of the smallest / largest finite value (per objective) and of the smallest / largest value of all (np.min / np.max,
+// which return NaN if there is one: its key is the largest); the minima are stored inverted so that all-zero bytes mean
+// "no value yet" (one memset initialises the histogram and the statistics)
+struct RkStats { unsigned long long kmin_inv, kmax, kall_min_inv, kall_max; };
 __device__ __forceinline__ unsigned long long rk_kmin(const RkStats& st) { return ~st.kmin_inv; }
 
 __device__ __forceinline__ double rk_value(const double* __restrict__ fpos, const double* __restrict__ fneg, int K,
@@ -49,21 +50,26 @@ __global__ void rank_keys_kernel(const double* __restrict__ fpos, const double* 
                                  unsigned long long* __restrict__ keys, RkStats* __restrict__ stats) {
     const int n = 2 * K;
     const int c = blockIdx.y;
-    unsigned long long lo = 0xFFFFFFFFFFFFFFFFull, hi = 0ull;
+    unsigned long long lo = 0xFFFFFFFFFFFFFFFFull, hi = 0ull, alo = 0xFFFFFFFFFFFFFFFFull, ahi = 0ull;
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
         const double x = rk_value(fpos, fneg, K, n_obj, c, e);
         const unsigned long long k = rk_key(x);
         keys[(size_t)c * n + e] = k;
         if (isfinite(x)) { lo = min(lo, k); hi = max(hi, k); }
+        alo = min(alo, k); ahi = max(ahi, k);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
         hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        alo = min(alo, __shfl_xor_sync(0xffffffffu, alo, o));
+        ahi = max(ahi, __shfl_xor_sync(0xffffffffu, ahi, o));
     }
     if ((threadIdx.x & 31) == 0) {
         if (lo != 0xFFFFFFFFFFFFFFFFull) atomicMax(&stats[c].kmin_inv, ~lo);
         if (hi != 0ull) atomicMax(&stats[c].kmax, hi);
+        if (alo != 0xFFFFFFFFFFFFFFFFull) atomicMax(&stats[c].kall_min_inv, ~alo);
+        if (ahi != 0ull) atomicMax(&stats[c].kall_max, ahi);
     }
 }
 
@@ -150,7 +156,9 @@ __global__ void rank_scatter_kernel(const unsigned long long* __restrict__ keys,
     }
 }
 
-// rank of global element gi of objective c: bucket start + #{(key_j, j) < (key_i, i) inside the bucket}
+// rank of global element gi of objective c: bucket start + #{(key_j, j) < (key_i, i) inside the bucket}.
+// *rev = its rank by descending key with equal keys still by ascending index: the q-th of a tie group of g whose ascending
+// ranks start at s goes to n - s - g + q (equal keys share a bucket)
 struct RkTables {
     const unsigned long long* keys;      // [n_obj][2K]
     const RkStats* stats;
@@ -159,19 +167,22 @@ struct RkTables {
     const unsigned long long* skeys;     // keys grouped by bucket
     const int* sidx;                     // their element indices
 };
-__device__ __forceinline__ int rk_rank_of(const RkTables& tb, int n, int c, int gi) {
+__device__ __forceinline__ int rk_rank_of(const RkTables& tb, int n, int c, int gi, int* rev) {
     double mn, scale;
     rk_range(tb.stats[c], mn, scale);
     const unsigned long long k = tb.keys[(size_t)c * n + gi];
     const int b = rk_bucket(k, mn, scale);
     const unsigned s0 = tb.start[(size_t)c * RK_NB + b], cnt = tb.hist[(size_t)c * RK_NB + b];
-    int r = (int)s0;
+    int lt = 0, q = 0, g = 0;
     for (unsigned j = 0; j < cnt; ++j) {
         const unsigned long long kj = tb.skeys[(size_t)c * n + s0 + j];
         const int ij = tb.sidx[(size_t)c * n + s0 + j];
-        r += (kj < k) || (kj == k && ij < gi);
+        lt += kj < k;
+        q += kj == k && ij < gi;
+        g += kj == k;
     }
-    return r;
+    *rev = n - (int)s0 - lt - g + q;
+    return (int)s0 + lt + q;
 }
 
 // ---- rank -> fitness-shaping value (the _rank of each Ranker subclass, src/utils/rankers.py:53-83) -----------------
@@ -225,18 +236,25 @@ __global__ void rank_finalize_kernel(const RkTables tb, const double* __restrict
     if (k >= k_count) return;
     const int n_local = 2 * k_count;
     double yp = 0.0, yn = 0.0;
-    int rp0 = 0, rn0 = 0;
-    bool reversed = false;
+    int rp0 = 0, rn0 = 0, vp0 = 0, vn0 = 0;
+    bool reversed = false, all_nan = false;
     for (int c = 0; c < n_obj; ++c) {
-        const int rp = rk_rank_of(tb, 2 * K, c, k_begin + k), rn = rk_rank_of(tb, 2 * K, c, K + k_begin + k);
-        if (c == 0) { rp0 = rp; rn0 = rn; }
+        int vp, vn;
+        const int rp = rk_rank_of(tb, 2 * K, c, k_begin + k, &vp), rn = rk_rank_of(tb, 2 * K, c, K + k_begin + k, &vn);
+        if (c == 0) { rp0 = rp; rn0 = rn; vp0 = vp; vn0 = vn; }
         if (ranks_out) { ranks_out[(size_t)c * n_local + k] = rp; ranks_out[(size_t)c * n_local + k_count + k] = rn; }
         double shift = 0.0, ymax = 1.0, xp = 0.0, xn = 0.0;
         if (xf.kind == ES_RANK_MAX_NORMALIZED) {
-            const double mn = rk_unkey(rk_kmin(stats[c])), mx = rk_unkey(stats[c].kmax);
+            // np.min / np.max: NaN if there is one (its key is the largest), else the infinities count
+            const double mx = rk_unkey(stats[c].kall_max);
+            const double mn = (mx != mx) ? mx : rk_unkey(~stats[c].kall_min_inv);
             shift = (mn > 0.0) ? -mn : mn;                      // x + (-mn if mn > 0 else mn), rankers.py:71
-            ymax = __dadd_rn(mx, shift);                        // np.max(y): the add is monotone
-            if (c == 0) reversed = ymax < 0.0;                  // dividing by a negative maximum reverses the order
+            ymax = __dadd_rn(mx, shift);                        // np.max(y): the add is monotone (and propagates NaN)
+            if (c == 0) {
+                reversed = ymax < 0.0;                          // dividing by a negative maximum reverses the order
+                // every y <= ymax is -inf or NaN: every shaped value is NaN, and a stable sort keeps them in index order
+                all_nan = !(ymax > -INFINITY);
+            }
             xp = fpos[(size_t)(k_begin + k) * n_obj + c];
             xn = fneg[(size_t)(k_begin + k) * n_obj + c];
         }
@@ -250,7 +268,8 @@ __global__ void rank_finalize_kernel(const RkTables tb, const double* __restrict
         // EliteRanker (rankers.py:86-103): the elite_n largest shaped values are kept with their own sign-less weight and
         // the noise index of their pair; nothing is subtracted.  Slot = distance from the elite threshold (rank order).
         const int thr = xf.n - xf.elite_n;
-        if (reversed) { rp0 = xf.n - 1 - rp0; rn0 = xf.n - 1 - rn0; }
+        if (all_nan) { rp0 = k_begin + k; rn0 = K + k_begin + k; }
+        else if (reversed) { rp0 = vp0; rn0 = vn0; }           // equal shaped values stay in index order (stable sort)
         const bool ep = rp0 >= thr, en = rn0 >= thr;
         if (ep) {
             if (elite_vals) elite_vals[rp0 - thr] = yp;
