@@ -1,0 +1,612 @@
+"""Stage-by-stage judge of one captured ES generation (DeviceGeneration.run, or es.step on its fused route).
+
+TEST INFRASTRUCTURE ONLY.  Nothing here launches a kernel: a ``Capture`` holds what the generation started from and what it
+produced, and ``judge`` checks every stage against a reference computed from the DEVICE'S OWN INPUTS TO THAT STAGE, so that a
+near-tie that flips one rank cannot cascade into the checks of later stages:
+
+  1 draws       numpy's streams replayed in the reference's order (es_oracle.es_test_params): per pair ``sample_idx``, per
+                evaluation its ``rs.random()`` coin (two raw words), then with action noise ``rs.randn(T act) ac_std``.  Indices,
+                coin words and the end states (key, position, has_gauss) exact, the cached gaussian to 2 ulp, the action noise
+                by test_gpu_noise_table._mismatches (equal, or one float32 ulp away next to a rounding midpoint);
+  2 obstat      sum, sumsq, count and n_saved exactly against ObStatOracle fed, in evaluation order, with the replayed coins and
+                ob_sum_sq_cnt(obs_stream[1:T+1]);
+  3 normalise   the normalised observations bit for bit against orc.normalise_obs with the generation's mean / std;
+  4 fitness     every evaluation against float64 (``fitness_truth``: torch.float64 on the tensors' device, from the device's
+                indices, theta, normalised observations and action noise), judged by test_gpu_rollout_f64._check (EVAL_REL of
+                the reward mass per evaluation, RMS_BOUND of the spread, behaviours within float32 rounding); the float64 truth
+                tied to the plain CPU reference tests/f64_rollout.rollout_f64 on sampled pairs to TIE_REL of the mass;
+  5 novelty     (archive) bit for bit against orc.novelty of the device's behaviours, in column 1 of the [pos|neg][k][2] rows;
+  6 weights     bit for bit against orc.centered_ranker / orc.moo_ranker on the device's fitness, n_ranked equal; and against
+                the ranks of the float64 truth: how many ranks differ, the largest shift and the largest |dw| (bounded by
+                the caller: they depend on the rollout arithmetic and the population);
+  7 gradient    gsum against the float64 sum_k w_k eps_k of the device's weights and indices: rc_f64.truth_device / judge with
+                rc_layout(P, K, sm), unchanged;
+  8 optimizer   theta', m', v' bit for bit against orc.AdamOracle applied in float32 to the device's gsum and theta.
+
+Every check is a ``Check``: a measured value, its bound and whether it passed.  Tolerance checks measure a ratio against a
+positive bound.  Exact checks measure a distance -- float32 / float64 values in units in the last place of the reference
+value, integers in units -- against the bound 0; their margin is the distance itself (1 is the smallest that fails), so a
+margin reported for an exact check is an ulp distance, not a multiple of a tolerance.
+``assert_ok`` raises a ``StageFailure`` that names every failing stage.
+"""
+from __future__ import annotations
+
+import math
+import os
+import sys
+from dataclasses import dataclass, field
+from typing import List, NamedTuple, Optional, Sequence
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from oracle import es_oracle as orc  # noqa: E402
+import f64_rollout as f64  # noqa: E402
+import rc_f64 as rc  # noqa: E402
+import test_gpu_noise_table as noise_criterion  # noqa: E402
+import test_gpu_rollout_f64 as rollout_f64  # noqa: E402
+
+F32 = np.float32
+TIE_REL = 1e-12           # the device float64 truth against the CPU float64 reference, relative to the reward mass
+# |kappa| of e = kappa f + c + r fitted over a population: the part of the fitness error proportional to the fitness.  Largest
+# value measured on an H100 SXM (80 GB): 8.7e-7 (ES_ROLLOUT_TC3, configs 3, 4 and 5, every generation); ES_ROLLOUT_F32 at most 9.4e-9
+KAPPA_BOUND = 2e-6
+STAGES = ('draws', 'obstat', 'normalise', 'fitness', 'novelty', 'weights', 'gradient', 'optimizer')
+
+
+class Check(NamedTuple):
+    stage: str
+    name: str
+    value: float
+    bound: float
+    ok: bool
+    detail: str = ''
+
+    @property
+    def margin(self) -> float:
+        """How far the value is from passing: value / bound, or for an exact check (bound 0) the distance itself."""
+        return self.value / self.bound if self.bound > 0 else self.value
+
+    def __str__(self):
+        return f'[{self.stage}] {self.name}: {self.value:.4g} (bound {self.bound:.4g}){"" if self.ok else "  FAILED"}' + \
+               (f'  {self.detail}' if self.detail else '')
+
+
+class StageFailure(AssertionError):
+    def __init__(self, failed: Sequence[Check]):
+        self.failed = list(failed)
+        self.stages = sorted({c.stage for c in failed}, key=STAGES.index)
+        super().__init__('generation stage(s) ' + ', '.join(self.stages) + ' failed:\n' + '\n'.join(map(str, failed)))
+
+
+@dataclass
+class Capture:
+    """One generation as captured.  Arrays are numpy except ``table`` (a torch tensor: on the device for the benchmarked
+    sizes) and ``act_noise`` (numpy or torch, read one stream's block at a time)."""
+    sizes: List[int]
+    T: int
+    sigma: float
+    l2coeff: float
+    ob_clip: float
+    pos_scale: float
+    save_obs_chance: float
+    ac_std: float
+    lr: float
+    table: torch.Tensor
+    obs_stream: np.ndarray                  # [T + 1, obs] float32
+    rew_vec: np.ndarray                     # [T, act] float32
+    # the state at the start
+    theta0: np.ndarray
+    m0: np.ndarray
+    v0: np.ndarray
+    t0: int
+    streams0: list                          # [(key uint32[624], pos, has_gauss, gauss)] per stream
+    ob_mean: np.ndarray
+    ob_std: np.ndarray
+    # what the generation produced
+    idx: np.ndarray                         # int64 [K]
+    coin_words: np.ndarray                  # uint32 [K, 4]: (+ evaluation's two words, - evaluation's two words)
+    obsn: np.ndarray                        # float32 [T, obs]
+    fit: np.ndarray                         # float64 [2, K, n_obj]
+    stats: np.ndarray                       # float64 [2 obs + 2]: sum, sumsq, count, n_saved
+    weights: np.ndarray                     # float32 [K]
+    n_ranked: int
+    gsum: np.ndarray                        # float32 [P]
+    theta1: np.ndarray
+    m1: np.ndarray
+    v1: np.ndarray
+    t1: int
+    streams1: list                          # the streams after the generation
+    behv: Optional[np.ndarray] = None       # float32 [2, K, 3]
+    act_noise: object = None                # float32 [K, 2, T * act]
+    archive: Optional[np.ndarray] = None    # float64 [A, 2]
+    nov_k: int = 10
+    moo_w: float = 0.5
+    beta1: float = 0.9
+    beta2: float = 0.999
+    epsilon: float = 1e-08
+    extra: dict = field(default_factory=dict)
+
+    @property
+    def P(self) -> int:
+        return f64.n_params(self.sizes)
+
+    @property
+    def K(self) -> int:
+        return len(self.idx)
+
+    @property
+    def n_per_stream(self) -> int:
+        return self.K // len(self.streams0)
+
+    @property
+    def act(self) -> int:
+        return self.sizes[-1]
+
+
+# ---------------------------------------------------------------------------------------------- distances
+def ulps(got, want) -> float:
+    """Largest |got - want| in units in the last place of ``want`` (its own float dtype); integers: in units."""
+    got, want = np.asarray(got), np.asarray(want)
+    if got.shape != want.shape:
+        return math.inf
+    if want.dtype.kind in 'iub':
+        return float(np.abs(got.astype(np.float64) - want.astype(np.float64)).max(initial=0.0))
+    if np.isnan(got).any() or np.isnan(want).any():
+        return 0.0 if np.array_equal(np.isnan(got), np.isnan(want)) and np.array_equal(got[~np.isnan(got)], want[~np.isnan(want)]) \
+            else math.inf
+    d = np.abs(got.astype(np.float64) - want.astype(np.float64))
+    sp = np.spacing(np.abs(want).astype(want.dtype)).astype(np.float64)
+    return float((d / sp).max(initial=0.0))
+
+
+def _exact(stage, name, got, want, detail=''):
+    u = ulps(got, want)
+    return Check(stage, name, u, 0.0, u == 0, detail)
+
+
+def _np(x):
+    return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+
+
+# ---------------------------------------------------------------------------------------------- 1. draws
+def replay_stream(cap: Capture, r: int):
+    """Stream r in the reference's order.  Returns (indices, coin words [n, 4] uint32, end state, generator of the
+    noise block [n, 2, T act] float64 (ac_std * randn) -- drawn lazily so that only one stream's block is held)."""
+    key, pos, has, gauss = cap.streams0[r]
+    rs = np.random.RandomState()
+    rs.set_state(('MT19937', np.asarray(key, dtype=np.uint32), int(pos), int(has), float(gauss)))
+    n, L, P = cap.n_per_stream, cap.table.numel(), cap.P
+    nrm = cap.T * cap.act if cap.ac_std else 0
+    idx = np.empty(n, dtype=np.int64)
+    words = np.empty((n, 4), dtype=np.uint32)
+    noise = np.empty((n, 2, nrm), dtype=np.float64) if nrm else None
+    for k in range(n):
+        idx[k] = orc.sample_idx(L, rs, P)
+        for s in range(2):
+            # fit_fn's rs.random() (simple_example.py:38): two raw 32-bit words
+            words[k, 2 * s] = int.from_bytes(rs.bytes(4), 'little')
+            words[k, 2 * s + 1] = int.from_bytes(rs.bytes(4), 'little')
+            if nrm:
+                noise[k, s] = rs.randn(nrm) * cap.ac_std          # FeedForward.forward's T x rs.randn(act) * ac_std
+    return idx, words, rs.get_state(), noise
+
+
+def saved_flags(words: np.ndarray, chance: float) -> np.ndarray:
+    """[..., 4] coin words -> [..., 2] save_obs flags (rs.random() < chance)."""
+    w = words.astype(np.uint64).reshape(-1, 2, 2)
+    u = ((w[..., 0] >> np.uint64(5)).astype(np.float64) * 67108864.0 + (w[..., 1] >> np.uint64(6)).astype(np.float64)) \
+        / 9007199254740992.0
+    return (u < chance).reshape(words.shape[:-1] + (2,))
+
+
+def stage_draws(cap: Capture) -> List[Check]:
+    """Leaves the replayed coin words of every stream in ``cap.extra['replay_words']`` (stage 2 counts the saves from them)."""
+    out = []
+    n = cap.n_per_stream
+    bad_idx = bad_words = bad_state = 0.0
+    noise_mism = 0
+    noise_fail = ''
+    cap.extra['replay_words'] = []
+    for r in range(len(cap.streams0)):
+        idx, words, st, noise = replay_stream(cap, r)
+        cap.extra['replay_words'].append(words)
+        sl = slice(r * n, (r + 1) * n)
+        bad_idx = max(bad_idx, ulps(cap.idx[sl], idx))
+        bad_words = max(bad_words, ulps(cap.coin_words[sl], words))
+        key1, pos1, has1, gauss1 = cap.streams1[r]
+        bad_state = max(bad_state, ulps(np.asarray(key1, dtype=np.uint32), st[1]), abs(int(pos1) - st[2]), abs(int(has1) - st[3]))
+        g = abs(float(gauss1) - st[4]) / np.spacing(abs(st[4])) if st[4] != 0 else abs(float(gauss1)) * math.inf
+        if g > 2:
+            bad_state = max(bad_state, g)
+        if cap.ac_std:
+            got = _np(cap.act_noise[sl])
+            try:
+                noise_mism += noise_criterion._mismatches(got.reshape(-1), noise.reshape(-1))
+            except AssertionError as ex:
+                noise_fail = f'stream {r}: ' + str(ex)[:200]
+    out.append(Check('draws', 'noise indices (units)', bad_idx, 0.0, bad_idx == 0))
+    out.append(Check('draws', 'coin words (units)', bad_words, 0.0, bad_words == 0))
+    out.append(Check('draws', 'end states: key / pos / has_gauss (units), cached gaussian beyond 2 ulp', bad_state, 0.0,
+                     bad_state == 0))
+    if cap.ac_std:
+        out.append(Check('draws', 'action noise outside the midpoint criterion', 0.0 if not noise_fail else 1.0, 0.0,
+                         not noise_fail, f'{noise_mism} values one ulp away next to a midpoint' + (f'; {noise_fail}' if noise_fail else '')))
+        cap.extra['noise_1ulp'] = noise_mism
+    return out
+
+
+# ---------------------------------------------------------------------------------------------- 2. obstat
+def stage_obstat(cap: Capture) -> List[Check]:
+    obs = cap.obs_stream.shape[1]
+    flags = np.concatenate([saved_flags(replay_words, cap.save_obs_chance) for replay_words in cap.extra['replay_words']])
+    s, q, c = orc.ob_sum_sq_cnt(cap.obs_stream[1:cap.T + 1])
+    st = orc.ObStatOracle((obs,), 0)
+    zeros = np.zeros(obs)
+    for saved in flags.reshape(-1):                          # evaluation order: stream, pair, + then -
+        if saved:
+            st.inc(s, q, c)
+        else:
+            st.inc(zeros, zeros, 0)
+    n_saved = int(flags.sum())
+    cap.extra['n_saved'] = n_saved
+    return [_exact('obstat', 'sum (ulp)', cap.stats[:obs], st.sum),
+            _exact('obstat', 'sumsq (ulp)', cap.stats[obs:2 * obs], st.sumsq),
+            _exact('obstat', 'count (ulp)', cap.stats[2 * obs:2 * obs + 1], np.array([float(st.count)])),
+            _exact('obstat', 'n_saved (units)', cap.stats[2 * obs + 1:], np.array([float(n_saved)]), f'{n_saved} saves')]
+
+
+# ---------------------------------------------------------------------------------------------- 3. normalise
+def stage_normalise(cap: Capture) -> List[Check]:
+    want = orc.normalise_obs(cap.obs_stream[:cap.T], cap.ob_mean, cap.ob_std, cap.ob_clip)
+    return [_exact('normalise', 'obsn (ulp)', cap.obsn, want)]
+
+
+# ---------------------------------------------------------------------------------------------- 4. fitness
+def fitness_truth(cap: Capture, chunk: int = 200):
+    """(fitness [2, K], behaviour [2, K, 3], reward mass [2, K], position magnitude [2, K, 3]) in float64 (f64_rollout's
+    definitions), computed with torch.float64 on the table's device in chunks of pairs: a measurement reference."""
+    dev = cap.table.device
+    d64 = torch.float64
+    sizes, T, act, K, P = cap.sizes, cap.T, cap.act, cap.K, cap.P
+    theta = torch.from_numpy(np.ascontiguousarray(cap.theta0)).to(dev, d64)
+    X = torch.from_numpy(np.ascontiguousarray(cap.obsn)).to(dev, d64)
+    C = torch.from_numpy(np.ascontiguousarray(cap.rew_vec)).to(dev, d64)
+    idx_all = torch.from_numpy(np.ascontiguousarray(cap.idx)).to(dev)
+    ar = torch.arange(P, device=dev)
+    s32 = float(np.float32(cap.sigma))
+    ps = float(cap.pos_scale)
+    lay = f64.layer_slices(sizes)
+    sel = [j % act for j in range(3)]
+    fit, mass = np.zeros((2, K)), np.zeros((2, K))
+    behv, mag = np.zeros((2, K, 3)), np.zeros((2, K, 3))
+    for b0 in range(0, K, chunk):
+        b1 = min(K, b0 + chunk)
+        eps = cap.table[idx_all[b0:b1, None] + ar[None, :]].to(d64)
+        nz_block = None if not cap.ac_std else torch.as_tensor(_np(cap.act_noise[b0:b1])).to(dev, d64)
+        for s, sign in enumerate((1.0, -1.0)):
+            W = theta[None, :] + sign * s32 * eps                                 # [B, P]
+            B = W.shape[0]
+            wo, bo, fi, fo = lay[0]
+            W1 = W[:, wo:wo + fi * fo].reshape(B, fo, fi)
+            a = torch.tanh((X @ W1.reshape(B * fo, fi).T).reshape(T, B, fo).permute(1, 0, 2) + W[:, bo:bo + fo][:, None, :])
+            for wo, bo, fi, fo in lay[1:]:
+                a = torch.tanh(torch.bmm(a, W[:, wo:wo + fi * fo].reshape(B, fo, fi).transpose(1, 2)) + W[:, bo:bo + fo][:, None, :])
+            if nz_block is not None:
+                a = a + nz_block[:, s].reshape(B, T, act)
+            prod = a * C[None]
+            fit[s, b0:b1] = prod.sum(dim=(1, 2)).cpu().numpy()
+            mass[s, b0:b1] = prod.abs().sum(dim=(1, 2)).cpu().numpy()
+            terms = ps * a[:, :, sel]
+            behv[s, b0:b1] = terms.sum(dim=1).cpu().numpy()
+            mag[s, b0:b1] = (torch.cumsum(terms, dim=1).abs().sum(dim=1) + terms.abs().sum(dim=1)).cpu().numpy()
+    return fit, behv, mass, mag
+
+
+def tie_pairs(cap: Capture) -> List[int]:
+    """The first and last pair of every stream (>= 16 evaluations with 4 streams or more)."""
+    n = cap.n_per_stream
+    return sorted({p for r in range(len(cap.streams0)) for p in (r * n, r * n + n - 1)})
+
+
+def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] = None) -> List[Check]:
+    tf, tb, mass, mag = truth
+    f = cap.fit[:, :, 0]
+    b = cap.behv
+    case = type('Case', (), dict(T=cap.T, ps=cap.pos_scale))()
+    err = np.abs(f - tf)
+    spread = max(tf.std(), 1e-3 * math.sqrt(cap.T))
+    rms = math.sqrt((err ** 2).mean())
+    worst = float((err / mass).max())
+    out = [Check('fitness', 'max err/mass', worst, rollout_f64.EVAL_REL[mode], worst <= rollout_f64.EVAL_REL[mode]),
+           Check('fitness', 'rms/spread', rms / spread, rollout_f64.RMS_BOUND[mode], rms <= rollout_f64.RMS_BOUND[mode] * spread)]
+    if b is not None:
+        tol = 2 * rollout_f64.U * mag + rollout_f64.ACT_ERR[mode] * cap.pos_scale * cap.T
+        r = float((np.abs(b - tb) / tol).max())
+        out.append(Check('fitness', 'behaviour err/tol', r, 1.0, r <= 1.0))
+    # the error's part proportional to the fitness, fitted over the population (e = kappa f + c + r), and the rms of what remains:
+    # a positive rescaling and a common offset leave every rank unchanged, so they are reported apart from the residual
+    A = np.stack([tf.reshape(-1), np.ones(tf.size)], 1)
+    coef = np.linalg.lstsq(A, (f - tf).reshape(-1), rcond=None)[0]
+    kappa, resid = coef[0], (f - tf).reshape(-1) - A @ coef
+    cap.extra['fitness'] = dict(rms_over_spread=rms / spread, mean_err=float((f - tf).mean()), mean_fitness=float(tf.mean()),
+                                kappa=float(kappa), resid_rms_over_spread=float(math.sqrt((resid ** 2).mean()) / spread))
+    out.append(Check('fitness', 'rms/spread of the error less its fitted scale and offset',
+                     cap.extra['fitness']['resid_rms_over_spread'], rollout_f64.RMS_BOUND[mode],
+                     cap.extra['fitness']['resid_rms_over_spread'] <= rollout_f64.RMS_BOUND[mode]))
+    out.append(Check('fitness', '|fitted relative scale of the error|', abs(float(kappa)), KAPPA_BOUND,
+                     abs(float(kappa)) <= KAPPA_BOUND))
+    try:                                                   # the one assert helper of the rollout tests decides as well
+        rollout_f64._check('generation', mode, case, f, b, None, truth)
+        helper_ok = True
+    except AssertionError:
+        helper_ok = False
+    if helper_ok != all(c.ok for c in out[:3 if b is not None else 2]):
+        out.append(Check('fitness', 'test_gpu_rollout_f64._check disagrees', 1.0, 0.0, False))
+    # the device float64 truth against the plain CPU reference on sampled pairs
+    tie = tie_pairs(cap) if tie is None else list(tie)
+    P = cap.P
+    table_np = np.concatenate([_np(cap.table[int(cap.idx[k]):int(cap.idx[k]) + P]) for k in tie])
+    noise = None
+    if cap.ac_std:
+        noise = np.stack([_np(cap.act_noise[k]) for k in tie])
+    cf, cb, cm, cmag = f64.rollout_f64(table_np, np.arange(len(tie)) * P, cap.theta0, cap.sigma, cap.sizes, cap.obsn, cap.rew_vec,
+                                       cap.pos_scale, noise, 1)
+    rel = float(max((np.abs(cf - tf[:, tie]) / cm).max(), (np.abs(cb - tb[:, tie]) / np.maximum(cmag, 1e-300)).max()))
+    out.append(Check('fitness', f'float64 truth vs CPU reference ({2 * len(tie)} evaluations), rel', rel, TIE_REL, rel <= TIE_REL))
+    return out
+
+
+# ---------------------------------------------------------------------------------------------- 5. novelty
+def stage_novelty(cap: Capture) -> List[Check]:
+    if cap.archive is None:
+        return []
+    b = cap.behv
+    want = np.array([[orc.novelty(b[s, k, :2], cap.archive, cap.nov_k) for k in range(cap.K)] for s in range(2)])
+    return [_exact('novelty', 'novelty column 1 (ulp)', cap.fit[:, :, 1], want)]
+
+
+# ---------------------------------------------------------------------------------------------- 6. weights
+def reference_weights(cap: Capture, fit: np.ndarray):
+    if cap.archive is None:
+        w, n = orc.centered_ranker(fit[0][:, :1], fit[1][:, :1])
+    else:
+        w, n = orc.moo_ranker(fit[0], fit[1], cap.moo_w)
+    return np.asarray(w, dtype=F32).reshape(-1), n
+
+
+def rank_report(cap: Capture, truth_fit: np.ndarray):
+    """Against the float64 truth's ranks (column 0; with an archive the device's novelty is the truth's second column):
+    (ranks differing, largest rank shift, largest |dw|)."""
+    f = cap.fit[:, :, 0].reshape(-1)
+    t = truth_fit.reshape(-1)
+    dr = np.abs(orc.rank(f) - orc.rank(t))
+    tfit = cap.fit.copy()
+    tfit[:, :, 0] = truth_fit
+    wt, _ = reference_weights(cap, tfit)
+    return int((dr != 0).sum()), int(dr.max()), float(np.abs(cap.weights.astype(np.float64) - wt).max())
+
+
+def stage_weights(cap: Capture, truth_fit=None, shift_bound=None, dw_bound=None) -> List[Check]:
+    w, n = reference_weights(cap, cap.fit)
+    out = [_exact('weights', 'weights (ulp)', cap.weights, w),
+           Check('weights', 'n_ranked (units)', float(abs(cap.n_ranked - n)), 0.0, cap.n_ranked == n)]
+    if truth_fit is not None:
+        nd, shift, dw = rank_report(cap, truth_fit)
+        cap.extra['ranks_vs_truth'] = dict(ranks_differing=nd, max_rank_shift=shift, max_abs_dw=dw)
+        out.append(Check('weights', 'largest rank shift against the float64 truth', shift, shift_bound, shift <= shift_bound,
+                         f'{nd} of {2 * cap.K} ranks differ'))
+        out.append(Check('weights', 'largest |dw| against the float64 truth', dw, dw_bound, dw <= dw_bound))
+    return out
+
+
+# ---------------------------------------------------------------------------------------------- 7. gradient
+def stage_gradient(cap: Capture, sm: int) -> List[Check]:
+    dev = cap.table.device
+    idx = torch.from_numpy(np.ascontiguousarray(cap.idx)).to(dev)
+    w = torch.from_numpy(np.ascontiguousarray(cap.weights)).to(dev)
+    truth, mass = rc.truth_device(cap.table, idx, w, cap.P)
+    worst, rms = rc.judge(cap.gsum, truth.cpu().numpy(), mass.cpu().numpy(), rc.rc_layout(cap.P, cap.K, sm))
+    return [Check('gradient', 'rc worst (of its per-column bound)', worst, 1.0, worst <= 1.0),
+            Check('gradient', 'rc rms (U M_p)', rms, rc.RMS_BOUND, rms <= rc.RMS_BOUND)]
+
+
+# ---------------------------------------------------------------------------------------------- 8. optimizer
+def adam_reference(cap: Capture, n_ranked: int):
+    """es.approx_grad's update in float32 (es.py:100-101, policy.py:73-74) on the device's gsum and theta."""
+    opt = orc.AdamOracle(cap.P, cap.lr, cap.beta1, cap.beta2, cap.epsilon)
+    opt.m, opt.v, opt.t = cap.m0.astype(F32).copy(), cap.v0.astype(F32).copy(), int(cap.t0)
+    flat = cap.theta0.astype(F32).copy()
+    grad = (cap.gsum.astype(F32) / F32(n_ranked)).astype(F32)
+    g = ((F32(cap.l2coeff) * flat).astype(F32) - grad).astype(F32)
+    flat += opt.step(g)
+    return flat, opt.m, opt.v, opt.t
+
+
+def stage_optimizer(cap: Capture) -> List[Check]:
+    _, n = reference_weights(cap, cap.fit)
+    th, m, v, t = adam_reference(cap, n)
+    return [_exact('optimizer', 'theta (ulp)', cap.theta1, th), _exact('optimizer', 'm (ulp)', cap.m1, m),
+            _exact('optimizer', 'v (ulp)', cap.v1, v), Check('optimizer', 't (units)', abs(cap.t1 - t), 0.0, cap.t1 == t)]
+
+
+# ---------------------------------------------------------------------------------------------- all stages
+def judge(cap: Capture, mode: int, sm: int, shift_bound: float, dw_bound: float, truth=None,
+          tie: Optional[Sequence[int]] = None) -> List[Check]:
+    """Every stage of ``cap``, in order; a stage that raises counts as failed.  ``truth``: fitness_truth(cap) when already
+    computed (re-judging mutated copies of a large capture whose mutation leaves the rollout inputs alone)."""
+    if truth is None:
+        truth = fitness_truth(cap)
+    checks = []
+    for stage, fn in (('draws', lambda: stage_draws(cap)), ('obstat', lambda: stage_obstat(cap)),
+                      ('normalise', lambda: stage_normalise(cap)), ('fitness', lambda: stage_fitness(cap, mode, truth, tie)),
+                      ('novelty', lambda: stage_novelty(cap)),
+                      ('weights', lambda: stage_weights(cap, truth[0], shift_bound, dw_bound)),
+                      ('gradient', lambda: stage_gradient(cap, sm)), ('optimizer', lambda: stage_optimizer(cap))):
+        try:
+            checks += fn()
+        except Exception as ex:                                    # noqa: BLE001 -- reported as the stage's failure
+            checks.append(Check(stage, f'raised {type(ex).__name__}', math.inf, 0.0, False, str(ex)[:300]))
+    return checks
+
+
+def failed(checks: Sequence[Check]) -> List[Check]:
+    return [c for c in checks if not c.ok]
+
+
+def assert_ok(checks: Sequence[Check]):
+    bad = failed(checks)
+    if bad:
+        raise StageFailure(bad)
+
+
+def report(title: str, checks: Sequence[Check]) -> str:
+    return '\n'.join([f'== {title}'] + [f'  {c}' for c in checks])
+
+
+# ---------------------------------------------------------------------------------------------- modelled pipeline bugs
+def _copy(cap: Capture, **changes) -> Capture:
+    import copy
+    out = copy.copy(cap)
+    out.extra = {}
+    for k, v in changes.items():
+        setattr(out, k, v)
+    return out
+
+
+def _block(a, r, n):
+    return slice(r * n, (r + 1) * n)
+
+
+def _stats_with(cap: Capture, n_saved: int, obs_stream: np.ndarray) -> np.ndarray:
+    """The generation statistics of ``n_saved`` saves of ``obs_stream``'s post-step rows, summed in order."""
+    obs = cap.obs_stream.shape[1]
+    s, q, c = orc.ob_sum_sq_cnt(obs_stream[1:cap.T + 1])
+    st = orc.ObStatOracle((obs,), 0)
+    for _ in range(n_saved):
+        st.inc(s, q, c)
+    return np.concatenate([st.sum, st.sumsq, [float(st.count), float(n_saved)]])
+
+
+def _n_saved(cap: Capture) -> int:
+    return int(cap.stats[2 * cap.obs_stream.shape[1] + 1])
+
+
+def _optimizer_after(cap: Capture, n_ranked=None, l2coeff=None, t0=None):
+    c = _copy(cap, l2coeff=cap.l2coeff if l2coeff is None else l2coeff, t0=cap.t0 if t0 is None else t0)
+    th, m, v, _ = adam_reference(c, reference_weights(cap, cap.fit)[1] if n_ranked is None else n_ranked)
+    return dict(theta1=th, m1=m, v1=v)
+
+
+def _gsum_of(cap: Capture, idx: np.ndarray, w: np.ndarray) -> np.ndarray:
+    """sum_k w_k eps_idx_k, rounded once to float32 (a correct reconstruction of the given pairing)."""
+    dev = cap.table.device
+    t, _ = rc.truth_device(cap.table, torch.from_numpy(np.ascontiguousarray(idx)).to(dev),
+                           torch.from_numpy(np.ascontiguousarray(w)).to(dev), cap.P)
+    return t.cpu().numpy().astype(F32)
+
+
+def _m_shift_stream(c):
+    n = c.n_per_stream
+    idx = c.idx.copy()
+    idx[_block(idx, 1, n)] = np.roll(idx[_block(idx, 1, n)], -1)       # stream 1 writes pair k + 1's index into slot k
+    return _copy(c, idx=idx)
+
+
+def _m_swap_streams(c):
+    n, R = c.n_per_stream, len(c.streams0)
+    a, b = _block(None, 0, n), _block(None, R - 1, n)
+    ch = {}
+    for name, axis in (('idx', 0), ('coin_words', 0), ('fit', 1), ('behv', 1), ('weights', 0)):
+        x = getattr(c, name)
+        if x is None:
+            continue
+        x = x.copy()
+        if axis == 0:
+            x[a], x[b] = x[b].copy(), x[a].copy()
+        else:
+            x[:, a], x[:, b] = x[:, b].copy(), x[:, a].copy()
+        ch[name] = x
+    return _copy(c, **ch)
+
+
+def _m_coin_to_neg(c):
+    w = c.coin_words.copy()
+    w[:, 2:4] = w[:, 0:2]
+    return _copy(c, coin_words=w)
+
+
+def _m_drop_save(c):
+    return _copy(c, stats=_stats_with(c, _n_saved(c) - 1, c.obs_stream))
+
+
+def _m_sign_swap(c):
+    f = c.fit.copy()
+    k = c.K // 2
+    f[:, k] = f[::-1, k].copy()
+    return _copy(c, fit=f)
+
+
+def _m_novelty_column(c):
+    return _copy(c, fit=c.fit[:, :, ::-1].copy())
+
+
+def _m_novelty_off_by_one(c):
+    f = c.fit.copy()
+    f[:, :, 1] = np.roll(f[:, :, 1].reshape(-1), -1).reshape(2, c.K)
+    return _copy(c, fit=f)
+
+
+def _m_weights_next(c):
+    g = _gsum_of(c, np.roll(c.idx, -1), c.weights)                      # w_k paired with idx[k + 1]
+    c2 = _copy(c, gsum=g)
+    return _copy(c2, **_optimizer_after(c2))
+
+
+def _m_gsum_over_k(c):
+    return _copy(c, **_optimizer_after(c, n_ranked=c.K))
+
+
+def _m_l2_sign(c):
+    return _copy(c, **_optimizer_after(c, l2coeff=-c.l2coeff))
+
+
+def _m_adam_t(c):
+    return _copy(c, t1=c.t0, **_optimizer_after(c, t0=c.t0 - 1))
+
+
+def _m_std_squared(c):
+    return _copy(c, obsn=orc.normalise_obs(c.obs_stream[:c.T], c.ob_mean, np.square(c.ob_std), c.ob_clip))
+
+
+def _m_stale_colsum(c):
+    old = np.random.RandomState(12).randn(*c.obs_stream.shape).astype(F32)    # the stream's content before it was rewritten
+    return _copy(c, stats=_stats_with(c, _n_saved(c), old))
+
+
+# name -> (what it models, mutation); each returns a mutated copy of a correct capture
+MUTATIONS = {
+    'shift_stream_indices': ("one stream's indices shifted by a pair", _m_shift_stream),
+    'swap_stream_blocks': ("two streams' blocks swapped", _m_swap_streams),
+    'plus_coin_on_minus': ('the + coin applied to the - evaluation', _m_coin_to_neg),
+    'drop_save': ('one save dropped from the count', _m_drop_save),
+    'sign_swap': ("one pair's signs swapped", _m_sign_swap),
+    'novelty_column': ('novelty in the wrong column', _m_novelty_column),
+    'novelty_off_by_one': ('novelty of the next evaluation', _m_novelty_off_by_one),
+    'weights_next': ('weights paired with idx[k + 1]', _m_weights_next),
+    'gsum_over_k': ('gsum divided by K instead of 2K', _m_gsum_over_k),
+    'l2_sign': ("the l2 term's sign flipped", _m_l2_sign),
+    'adam_t': ("Adam's t not advanced", _m_adam_t),
+    'std_squared': ('normalisation by std^2', _m_std_squared),
+    'stale_colsum': ('a stale column-sum cache from a previous obs stream', _m_stale_colsum),
+}
+NEEDS_ARCHIVE = ('novelty_column', 'novelty_off_by_one')
+
+
+def rejection(checks: Sequence[Check]):
+    """(stages that failed, the largest margin among the failed checks) -- (None, 0) when everything passed."""
+    bad = failed(checks)
+    if not bad:
+        return None, 0.0
+    return sorted({c.stage for c in bad}, key=STAGES.index), max(c.margin for c in bad)

@@ -1,0 +1,124 @@
+"""CPU: the stage-by-stage generation judge (tests/gen_stages.py) on generations of the oracle (oracle.es_oracle.generation)
+standing in for the device's, and the modelled pipeline bugs it must reject.
+
+The captured generation is the second of two on the same streams and optimizer (3 streams x 7 pairs, 17-64-64-6, T = 48, one
+save_obs coin per evaluation at chance 0.3, Adam), so Adam's state, the streams' state and the observation statistics are
+carried over and the normalisation runs with the first generation's mean / std.  Variants: NSRA (a 16-entry archive, k = 10,
+w = 0.5) and action noise (ac_std = 0.01).  The oracle computes its rollouts in float32 on the CPU, so the fitness is judged
+with the float32 rollout's bounds (ES_ROLLOUT_F32); gsum is the oracle's own numpy reconstruction (es_oracle.scale_noise).
+The oracle does not hand out the raw coin words it drew, so the captured words (and the action noise) are the judge's own replay
+of the streams: on the host the coin-word check compares the replay with itself, and what ties the oracle's coins to the judge
+is the obs statistics (count and n_saved from the oracle's rs.random() calls) and the streams' end states.  The
+'+ coin on the - evaluation' bug is rejected here by that word check alone.
+"""
+import os
+import sys
+
+import numpy as np
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import gen_stages as gs  # noqa: E402
+import rc_f64 as rc  # noqa: E402
+from oracle import es_oracle as orc  # noqa: E402
+
+F32 = np.float32
+MODE_F32 = 0                    # _lib.ES_ROLLOUT_F32
+SIZES, T, SEEDS, N_PER = [17, 64, 64, 6], 48, (1000, 1001, 1002), 7
+CHANCE, LR, SIGMA, L2 = 0.3, 0.01, 0.02, 0.005
+# rank shifts against the float64 truth at 42 evaluations: the oracle's float32 fitness is within ~1e-7 of the spread
+SHIFT_BOUND, DW_BOUND = 1, 1.0 / 41
+
+
+def _state(rs):
+    st = rs.get_state()
+    return (st[1].copy(), int(st[2]), int(st[3]), float(st[4]))
+
+
+def _capture(variant):
+    archive = np.random.RandomState(17).randn(16, 2) if variant == 'nsra' else None
+    ac_std = 0.01 if variant == 'noise' else 0.0
+    dims = orc.layer_dims(SIZES[0], SIZES[1:-1], SIZES[-1])
+    P = orc.n_params(dims)
+    rs0 = np.random.RandomState(5)
+    table = rs0.randn(P + 20_000).astype(F32)
+    theta = (rs0.randn(P) * 0.1).astype(F32)
+    env = orc.SyntheticEnvSpec(SIZES[0], SIZES[-1], T)
+    streams = [np.random.RandomState(s) for s in SEEDS]
+    opt = orc.AdamOracle(P, LR)
+    kw = dict(coins_per_eval=1, rank_states=streams, save_obs_chance=CHANCE, ac_std=ac_std, archive=archive, nov_k=10,
+              moo_w=0.5 if archive is not None else None)
+    obmean, obstd = np.zeros(SIZES[0]), np.ones(SIZES[0])
+    g1 = orc.generation(table, theta, opt, SIGMA, dims, env, [None] * 3, N_PER, obmean, obstd, 5.0, T, 500, L2, **kw)
+    stat = orc.ObStatOracle((SIZES[0],), 1e-2)                   # Policy.update_obstat's running statistics
+    stat.inc(g1['obstat'].sum, g1['obstat'].sumsq, g1['obstat'].count)
+    obmean, obstd = stat.mean, stat.std
+    theta0, m0, v0, t0 = theta.copy(), opt.m.copy(), opt.v.copy(), opt.t
+    streams0 = [_state(rs) for rs in streams]
+    g2 = orc.generation(table, theta, opt, SIGMA, dims, env, [None] * 3, N_PER, obmean, obstd, 5.0, T, 500, L2, **kw)
+    idx = g2['inds'].astype(np.int64)
+    K = len(idx)
+    w = np.asarray(g2['weights'], dtype=F32).reshape(-1)
+    gsum = np.asarray(orc.scale_noise(w, idx, table, P, 500), dtype=F32)
+    ob = g2['obstat']
+    stats = np.concatenate([ob.sum, ob.sumsq, [float(ob.count), float(ob.count) / T]])
+    behv = None
+    if archive is not None:                                     # the final positions the oracle's novelty was computed from
+        behv = np.zeros((2, K, 3), dtype=F32)
+        for k in range(K):
+            for s, sign in enumerate((1.0, -1.0)):
+                layers = orc.unflatten(orc.pheno_params(theta0, SIGMA, sign * table[idx[k]:idx[k] + P]), dims)
+                _, b, _, _ = orc.run_model(env, layers, obmean, obstd, 5.0, T, batched=True)
+                behv[s, k] = b[-3:]
+    cap = gs.Capture(sizes=SIZES, T=T, sigma=SIGMA, l2coeff=L2, ob_clip=5.0, pos_scale=env.pos_scale, save_obs_chance=CHANCE,
+                     ac_std=ac_std, lr=LR, table=torch.from_numpy(table), obs_stream=env.obs_stream, rew_vec=env.rew_vec,
+                     theta0=theta0, m0=m0, v0=v0, t0=t0, streams0=streams0, ob_mean=obmean, ob_std=obstd, idx=idx,
+                     coin_words=np.zeros((K, 4), dtype=np.uint32), obsn=orc.normalise_obs(env.obs_stream[:T], obmean, obstd, 5.0),
+                     fit=np.stack([g2['pos'], g2['neg']]), stats=stats, weights=w, n_ranked=g2['n_ranked'], gsum=gsum,
+                     theta1=theta.copy(), m1=opt.m.copy(), v1=opt.v.copy(), t1=opt.t, streams1=[_state(rs) for rs in streams],
+                     behv=behv, archive=archive)
+    # the coin words and the action noise: the streams' draws between the indices, in the order the oracle consumed them
+    noise = []
+    for r in range(len(SEEDS)):
+        _, words, _, nz = gs.replay_stream(cap, r)
+        cap.coin_words[r * N_PER:(r + 1) * N_PER] = words
+        if ac_std:
+            noise.append(nz.astype(F32))
+    if ac_std:
+        cap.act_noise = np.concatenate(noise)
+    return cap
+
+
+_CAPS = {}
+
+
+def _cap(variant):
+    if variant not in _CAPS:
+        _CAPS[variant] = _capture(variant)
+    return _CAPS[variant]
+
+
+def _judge(cap):
+    return gs.judge(cap, MODE_F32, rc.H100_SMS, SHIFT_BOUND, DW_BOUND, tie=list(range(cap.K)))
+
+
+@pytest.mark.parametrize('variant', ['plain', 'nsra', 'noise'])
+def test_judge_passes_the_oracle_generation(variant):
+    cap = _cap(variant)
+    checks = _judge(cap)
+    print('\n' + gs.report(f'oracle generation, {variant}', checks))
+    gs.assert_ok(checks)
+    assert cap.extra['n_saved'] > 0 and cap.t0 == 1
+    assert not np.array_equal(cap.ob_std, np.ones_like(cap.ob_std))
+
+
+@pytest.mark.parametrize('name', sorted(gs.MUTATIONS))
+def test_judge_rejects_modelled_bugs(name):
+    what, mutate = gs.MUTATIONS[name]
+    cap = _cap('nsra' if name in gs.NEEDS_ARCHIVE else 'plain')
+    checks = _judge(mutate(cap))
+    stages, margin = gs.rejection(checks)
+    print(f'\n{name} ({what}): rejected by {stages}, margin {margin:.3g}x')
+    assert stages is not None, f'{what}: not rejected'
+    assert margin >= 10, (what, stages, margin)
