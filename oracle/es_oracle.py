@@ -33,9 +33,12 @@ Pinning status (SURVEY.md section 8c):
     plus the real ``test_params`` on two thread-emulated MPI ranks (rank-major ``_share_results`` rows, per-rank RNG streams,
     summed steps, ``ObStat.mpi_inc``): what a process carrying two 'virtual ranks' must reproduce.
 
-  * the CLOSED-LOOP synthetic env (``ClosedLoopEnvSpec`` / ``run_model_closed``) has no reference implementation
-    (SURVEY.md section 8d names only the transition ``obs' = tanh(A obs + B a)``): for that variant this module is the
-    definition -- parity unpinned against the reference by construction; frozen by ``tests/golden/closed_loop.npz``.
+  * the CLOSED-LOOP synthetic env (``ClosedLoopEnvSpec``, stepped by ``run_model``) has no reference implementation
+    (SURVEY.md section 8d names only the transition ``obs' = tanh(A obs + B a)``): for that variant, with its action noise
+    and multi-episode evaluations, this module is the definition -- parity unpinned against the reference by construction;
+    the noise-free single episode is frozen by ``tests/golden/closed_loop.npz``.
+  * the binned head of FFBinned (``binned_action``, src/nn/nn.py:99-117) is pinned bit for bit against the package's
+    ``FFBinned.forward`` by ``tests/test_binned_host.py``.
 
 Float semantics are those of the reference's pinned stack (numpy 1.18 value-based
 casting): every array op on float32 data stays float32 and python scalars are
@@ -255,70 +258,90 @@ class ClosedLoopEnvSpec(SyntheticEnvSpec):
         return np.tanh(acc).astype(F32)
 
 
-def run_model_closed(env: ClosedLoopEnvSpec, layers, obmean, obstd, ob_clip: float, max_steps: int):
-    """gym_runner.py:33-67 on the closed-loop env (``ac_std == 0``): the literal per-step loop -- normalise the current
-    observation, forward, step the env with the action."""
-    n = min(int(max_steps), env.T)
-    rews, behv, obs = [], [], []
-    pos = np.zeros(3, dtype=F32)
-    ps = F32(env.pos_scale)
-    ob = env.obs_stream[0].copy()
-    for t in range(n):
-        a = mlp_forward(layers, normalise_obs(ob, obmean, obstd, ob_clip)).astype(F32)
-        acc = F32(0.0)
-        for j in range(env.act_dim):           # float32 dot, index order
-            acc = F32(acc + F32(a[j] * env.rew_vec[t, j]))
-        rews.append(float(acc))
-        for j in range(3):
-            pos[j] = F32(pos[j] + F32(ps * a[j % env.act_dim]))
-        behv.extend([float(pos[0]), float(pos[1]), float(pos[2])])
-        ob = env.step_obs(ob, a)
-        obs.append(ob)
-    step = n - 1
-    behv += behv[-3:] * (max_steps - int(len(behv) / 3))
-    return rews, behv, np.stack(obs), step
+def binned_action(out: np.ndarray, bins: int, low: np.ndarray, high: np.ndarray) -> np.ndarray:
+    """FFBinned's head (nn.py:99-117): [..., adim * bins] network outputs -> [..., adim] float32 actions.  The first maximal
+    bin of each dimension (numpy's argmax, like torch's, returns the first), then, with float32 ``low`` / ``high`` (the env's
+    Box), ``((c * idx) * range) + low`` with ``c = float32(1 / (bins - 1))``, every operation rounded to float32 as torch
+    evaluates it."""
+    out = np.asarray(out, dtype=F32)
+    low = np.asarray(low, dtype=F32)
+    rng = (np.asarray(high, dtype=F32) - low).astype(F32)
+    idx = out.reshape(out.shape[:-1] + (low.shape[0], int(bins))).argmax(-1)
+    c = F32(1.0 / (bins - 1.0))
+    return (((c * idx.astype(F32)).astype(F32) * rng).astype(F32) + low).astype(F32)
 
 
 def run_model(env: SyntheticEnvSpec, layers, obmean, obstd, ob_clip: float, max_steps: int,
-              batched: bool = False, ac_std: float = 0.0, rs: Optional[np.random.RandomState] = None):
-    """gym_runner.py:33-67 on the synthetic env, ``ac_std == 0`` (no RNG consumed in
-    the forward, nn.py:47).  Returns (rews list, behv list (3 per step, padded),
-    obs ndarray [steps, obs_dim] of post-step observations, step = last loop index).
+              batched: bool = False, ac_std: float = 0.0, rs: Optional[np.random.RandomState] = None,
+              episodes: int = 1, binned: Optional[Tuple[int, np.ndarray, np.ndarray]] = None):
+    """gym_runner.py:33-67 on the synthetic envs, inside obj.py:54-63's ``eps_per_policy`` loop.  Returns (rews list,
+    behv list (3 per step, padded), obs ndarray [steps, obs_dim] of post-step observations, step = last loop index).
 
-    ``batched=True`` evaluates all steps in one matrix product (same arithmetic up
-    to BLAS summation order) so large parity cases finish in seconds; the per-step
-    loop is the literal restatement.
+    Every step: forward the normalised observation (nn.py:42-50), add the action noise, reward ``<a_t, c_t>`` as a float32
+    dot in index order, integrate the position from the first three action components, and on the closed loop
+    (``env.closed_loop``) step the env with the action.  The open loop's observations do not depend on the actions, so
+    its forwards run before the steps: ``batched=True`` evaluates them in one matrix product (same arithmetic up to BLAS
+    summation order) so large parity cases finish in seconds; otherwise one forward per step, the literal restatement.
 
     ``ac_std != 0`` with a stream ``rs``: FeedForward.forward adds ``rs.randn(*a.shape) * ac_std`` to the action at every
     step (nn.py:47-48; legacy polar-method gaussians from the SAME RandomState that draws the noise indices and the
     save_obs coins).  ``a += ndarray`` on a float32 tensor yields the float64 sum (numpy's reflected add wraps the
-    result back into a tensor), which the env casts to float32 (``np.asarray(action, dtype=float32)``)."""
-    if getattr(env, 'closed_loop', False):
-        assert ac_std == 0, 'the closed-loop variant is defined without action noise'
-        return run_model_closed(env, layers, obmean, obstd, ob_clip, max_steps)
+    result back into a tensor), which the env casts to float32 (``np.asarray(action, dtype=float32)``).
+
+    ``binned=(bins, low, high)``: FFBinned's head (``binned_action``) in place of the tanh output.  FFBinned.forward ignores
+    ``rs``, so a binned policy draws no noise.
+
+    ``episodes=E``: ``max(1, E)`` episodes from a fresh env, each drawing its own noise; as obj.py:57-60, the rewards are
+    summed per step into a float64 array of ``max_steps`` zeros in episode order and divided by the count.  Behaviour,
+    observations and step are the last episode's.  One episode returns its own reward list, unpadded."""
+    closed = getattr(env, 'closed_loop', False)
     n = min(int(max_steps), env.T)
-    xs = normalise_obs(env.obs_stream[:n], obmean, obstd, ob_clip)
-    if batched:
-        acts = mlp_forward(layers, xs)
-    else:
-        acts = np.stack([mlp_forward(layers, xs[t]) for t in range(n)])
-    rews, behv = [], []
-    pos = np.zeros(3, dtype=F32)
+
+    def forward(x):
+        out = mlp_forward(layers, x)
+        return out if binned is None else binned_action(out, *binned)
+
+    if not closed:
+        xs = normalise_obs(env.obs_stream[:n], obmean, obstd, ob_clip)
+        acts = forward(xs) if batched else np.stack([forward(xs[t]) for t in range(n)])
+    noisy = binned is None and ac_std != 0 and rs is not None
     ps = F32(env.pos_scale)
-    for t in range(n):
-        a = acts[t].astype(F32)
-        if ac_std != 0 and rs is not None:
-            a = (a.astype(np.float64) + rs.randn(env.act_dim) * ac_std).astype(F32)
-        acc = F32(0.0)
-        for j in range(env.act_dim):           # float32 dot, index order
-            acc = F32(acc + F32(a[j] * env.rew_vec[t, j]))
-        rews.append(float(acc))
-        for j in range(3):
-            pos[j] = F32(pos[j] + F32(ps * a[j % env.act_dim]))
-        behv.extend([float(pos[0]), float(pos[1]), float(pos[2])])
-    step = n - 1                                 # gym_runner.py:50,67 returns the loop index
+    n_eps = max(1, int(episodes))
+    total = np.zeros(int(max_steps))
+    for _ in range(n_eps):
+        rews, behv, obs = [], [], []
+        pos = np.zeros(3, dtype=F32)
+        ob = env.obs_stream[0].copy()
+        for t in range(n):
+            a = (forward(normalise_obs(ob, obmean, obstd, ob_clip)) if closed else acts[t]).astype(F32)
+            if noisy:
+                a = (a.astype(np.float64) + rs.randn(env.act_dim) * ac_std).astype(F32)
+            acc = F32(0.0)
+            for j in range(env.act_dim):           # float32 dot, index order
+                acc = F32(acc + F32(a[j] * env.rew_vec[t, j]))
+            rews.append(float(acc))
+            for j in range(3):
+                pos[j] = F32(pos[j] + F32(ps * a[j % env.act_dim]))
+            behv.extend([float(pos[0]), float(pos[1]), float(pos[2])])
+            if closed:
+                ob = env.step_obs(ob, a)
+                obs.append(ob)
+        total[:n] += np.array(rews)
     behv += behv[-3:] * (max_steps - int(len(behv) / 3))
-    return rews, behv, env.obs_stream[1:n + 1].copy(), step
+    obs = np.stack(obs) if closed else env.obs_stream[1:n + 1].copy()
+    if n_eps > 1:
+        rews = (total / n_eps).tolist()
+    return rews, behv, obs, n - 1                # gym_runner.py:50,67 returns the loop index
+
+
+def _rollout_kw(episodes: int, binned) -> dict:
+    """The ``episodes`` / ``binned`` keywords the generation functions pass to ``run_model``, left out at their defaults.
+    A single tanh episode is then ``run_model``'s original nine-argument call, so a caller that substitutes its own
+    rollout with that signature for ``run_model`` keeps working."""
+    kw = {} if episodes == 1 else dict(episodes=episodes)
+    if binned is not None:
+        kw['binned'] = binned
+    return kw
 
 
 def reward_result(rews: List[float]) -> List[float]:
@@ -386,13 +409,15 @@ def es_test_params(table: np.ndarray, flat: np.ndarray, std: float, dims, env: S
                 rank_seeds: Sequence[int], n_per_rank: int, obmean, obstd, ob_clip: float,
                 max_steps: int, coins_per_eval: int = 0, save_obs_chance: float = 0.0,
                 archive: Optional[np.ndarray] = None, nov_k: int = 10, batched: bool = True,
-                rank_states: Optional[List[np.random.RandomState]] = None, ac_std: float = 0.0):
+                rank_states: Optional[List[np.random.RandomState]] = None, ac_std: float = 0.0,
+                episodes: int = 1, binned=None):
     """es.py:54-81 replayed for R virtual MPI ranks (one legacy RandomState per rank,
     utils.py:63-65).  Per pair: ``nt.sample(rs)`` (one ``randint``), evaluate +noise,
     evaluate -noise (es.py:68-72); each evaluation's fit_fn draws ``coins_per_eval``
     ``rs.random()`` values first (1 in simple_example.py:38 / obj.py:54, 0 for the
-    index-only variant).  Returns (pos[K,n_obj], neg[K,n_obj], inds[K], steps,
-    obstat) with K = R*n_per_rank in rank-major order, all float64 like es.py:89."""
+    index-only variant), then runs ``run_model`` with ``episodes`` and ``binned``.
+    Returns (pos[K,n_obj], neg[K,n_obj], inds[K], steps, obstat) with K = R*n_per_rank
+    in rank-major order, all float64 like es.py:89."""
     P = len(flat)
     n_obj = 1 if archive is None else 2
     gen_obstat = ObStatOracle((env.obs_dim,), 0)
@@ -409,7 +434,8 @@ def es_test_params(table: np.ndarray, flat: np.ndarray, std: float, dims, env: S
                 for _c in range(coins_per_eval):
                     save_obs = rs.random() < save_obs_chance
                 layers = unflatten(pheno_params(flat, std, noise if sign > 0 else -noise), dims)
-                rews, behv, obs, step = run_model(env, layers, obmean, obstd, ob_clip, max_steps, batched, ac_std, rs)
+                rews, behv, obs, step = run_model(env, layers, obmean, obstd, ob_clip, max_steps, batched, ac_std, rs,
+                                                  **_rollout_kw(episodes, binned))
                 res.append(reward_result(rews) if archive is None else nsr_result(rews, behv[-3:], archive, nov_k))
                 steps_total += step
                 o = obs if save_obs else np.array([np.zeros((env.obs_dim,))])
@@ -615,13 +641,15 @@ def approx_grad(flat: np.ndarray, optim, ranked_fits: np.ndarray, noise_inds: np
 def generation(table, flat, optim, std, dims, env, rank_seeds, n_per_rank, obmean, obstd, ob_clip, max_steps,
                batch_size, l2coeff, moo_w: Optional[float] = None, archive=None, nov_k=10,
                coins_per_eval=0, rank_states=None, batched=True, shaping: str = 'centered',
-               elite_percent: Optional[float] = None, save_obs_chance: float = 0.0, ac_std: float = 0.0):
+               elite_percent: Optional[float] = None, save_obs_chance: float = 0.0, ac_std: float = 0.0,
+               episodes: int = 1, binned=None):
     """One whole generation (es.py:38-47 without the reporter / noiseless eval).  ``shaping`` / ``elite_percent`` select
     the other rankers of rankers.py:61-103 (obj.py:48-50 picks EliteRanker(CenteredRanker(), elite))."""
     pos, neg, inds, steps, obstat = es_test_params(table, flat, std, dims, env, rank_seeds, n_per_rank, obmean, obstd,
                                                 ob_clip, max_steps, coins_per_eval=coins_per_eval, archive=archive,
                                                 nov_k=nov_k, batched=batched, rank_states=rank_states,
-                                                save_obs_chance=save_obs_chance, ac_std=ac_std)
+                                                save_obs_chance=save_obs_chance, ac_std=ac_std, episodes=episodes,
+                                                binned=binned)
     grad_inds = inds
     if elite_percent is not None:
         w, grad_inds, _, n_ranked = elite_ranker(pos, neg, inds, shaping, elite_percent)
@@ -637,20 +665,22 @@ def generation(table, flat, optim, std, dims, env, rank_seeds, n_per_rank, obmea
 
 
 def es_step(table, flat, optim, std, dims, env, rank_states, n_per_rank, obmean, obstd, ob_clip, max_steps, batch_size,
-            l2coeff, coins_per_eval=1, save_obs_chance=0.0, batched=True, **kw):
+            l2coeff, coins_per_eval=1, save_obs_chance=0.0, batched=True, episodes=1, binned=None, **kw):
     """``es.step`` (es.py:38-51): the generation, then the noiseless evaluation ``fit_fn(policy.pheno(zeros), False)`` of the
     UPDATED parameters that every rank runs for itself.  The scripts' fit_fn draws its save_obs coin(s) in every call
-    (simple_example.py:38, obj.py:54), so each rank's stream advances by ``coins_per_eval`` doubles here too.  Returns the
-    generation's dict plus ``noiseless`` (the result list of rank 0)."""
+    (simple_example.py:38, obj.py:54), so each rank's stream advances by ``coins_per_eval`` doubles here too, and it runs
+    its ``episodes`` whether or not it adds noise (obj.py:57).  Returns the generation's dict plus ``noiseless`` (the result
+    list of rank 0)."""
     out = generation(table, flat, optim, std, dims, env, [None] * len(rank_states), n_per_rank, obmean, obstd, ob_clip,
                      max_steps, batch_size, l2coeff, coins_per_eval=coins_per_eval, rank_states=rank_states, batched=batched,
-                     save_obs_chance=save_obs_chance, **kw)
+                     save_obs_chance=save_obs_chance, episodes=episodes, binned=binned, **kw)
     noiseless = None
     for rs in rank_states:
         for _c in range(coins_per_eval):
             rs.random()
         layers = unflatten(pheno_params(flat, std, None), dims)
-        rews, behv, obs, step = run_model(env, layers, obmean, obstd, ob_clip, max_steps, batched)
+        rews, behv, obs, step = run_model(env, layers, obmean, obstd, ob_clip, max_steps, batched,
+                                          **_rollout_kw(episodes, binned))
         res = reward_result(rews) if kw.get('archive') is None else nsr_result(rews, behv[-3:], kw['archive'], kw.get('nov_k', 10))
         noiseless = res if noiseless is None else noiseless
     out['noiseless'] = noiseless

@@ -1,4 +1,4 @@
-"""Frozen vectors of the CLOSED-LOOP variant (oracle.es_oracle.ClosedLoopEnvSpec / run_model_closed): there is no reference
+"""Frozen vectors of the CLOSED-LOOP variant (oracle.es_oracle.ClosedLoopEnvSpec / run_model): there is no reference
 implementation of this env (SURVEY.md section 8d names it as an optional synthetic variant), so the oracle is its definition
 and these vectors pin the oracle against accidental change.  python tests/golden/make_closed_golden.py -> closed_loop.npz"""
 import os

@@ -5,14 +5,11 @@ import re
 import subprocess
 import tempfile
 
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import binned_oracle as bo  # noqa: E402
+from oracle import es_oracle as orc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -48,7 +45,7 @@ def test_oracle_action_is_ffbinned_forward_bit_for_bit():
                 last.bias.copy_(b.reshape(-1))
                 got = net(ob, rs=None).numpy()
                 raw = net.model(ob).numpy()
-            want = bo.binned_action(raw, bins, low, high)
+            want = orc.binned_action(raw, bins, low, high)
             assert got.dtype == np.float32
             assert np.array_equal(got.view(np.uint32), want.view(np.uint32)), (bins, idx, got, want)
 
@@ -56,11 +53,12 @@ def test_oracle_action_is_ffbinned_forward_bit_for_bit():
 def test_oracle_action_ties_pick_the_first_bin():
     low, high = np.array([-0.3], np.float32), np.array([2.7], np.float32)
     for bins in (2, 5, 11):
-        assert bo.binned_action(np.full(bins, 0.25, np.float32), bins, low, high)[0] == low[0]
+        assert orc.binned_action(np.full(bins, 0.25, np.float32), bins, low, high)[0] == low[0]
         out = np.full(bins, 0.25, np.float32)
         out[bins - 1] = 0.5
         out[1] = 0.5
-        assert bo.binned_action(out, bins, low, high)[0] == bo.binned_action(np.eye(bins, dtype=np.float32)[1], bins, low, high)[0]
+        assert orc.binned_action(out, bins, low, high)[0] == orc.binned_action(np.eye(bins, dtype=np.float32)[1], bins, low,
+                                                                               high)[0]
 
 
 def test_head_descriptor_and_fuse_decision():
@@ -127,7 +125,6 @@ def test_run_model_keeps_uncovered_binned_policies_in_the_python_loop():
     from es_pytorch_b200.gym.gym_runner import run_model
     from es_pytorch_b200.gym.synthetic_env import ClosedLoopEnv, SyntheticEnv
     from es_pytorch_b200.nn.nn import FFBinned
-    from oracle import es_oracle as orc
     T = 12
     for closed in (False, True):
         env = (ClosedLoopEnv if closed else SyntheticEnv)(376, 17, T)
@@ -142,8 +139,8 @@ def test_run_model_keeps_uncovered_binned_policies_in_the_python_loop():
         sizes = net.layer_sizes()
         layers = orc.unflatten(Policy.get_flat(net).astype(np.float32), orc.layer_dims(sizes[0], sizes[1:-1], sizes[-1]))
         spec = (orc.ClosedLoopEnvSpec if closed else orc.SyntheticEnvSpec)(376, 17, T)
-        want, _, _, _ = bo.run_model(spec, layers, np.zeros(376), np.ones(376), 5.0, T, 16, env.action_space.low,
-                                     env.action_space.high)
+        want, _, _, _ = orc.run_model(spec, layers, np.zeros(376), np.ones(376), 5.0, T,
+                                      binned=(16, env.action_space.low, env.action_space.high))
         assert np.array_equal(np.array(rews), np.array(want))
 
 

@@ -3,7 +3,7 @@
 For every problem:
 (a) the loop does not amplify rounding: a 1e-9 move of the start observation grows at most 100-fold over the episode
     (closed_f64.growth); a known-chaotic problem is refused by the same gate;
-(b) the float32 oracle (closed_noise_oracle.run_model_episodes, fed the problem's noise array) is within 1e-6 of the reward
+(b) the float32 oracle (es_oracle.run_model, fed the problem's noise array) is within 1e-6 of the reward
     mass of the truth for every evaluation: a tenth of the GPU bound, so the bound has room for a float32 kernel;
 (c) with sigma = 0 the truth's two signs are identical and match the float32 oracle to float32 grade (the truth itself);
 (d) for each kernel and each shape, every modelled bug (closed_f64.mutations) moves the fitness, a position or an ObStat sum by
@@ -21,7 +21,6 @@ from oracle import es_oracle as orc
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import closed_f64 as cf  # noqa: E402
-import closed_noise_oracle as cno  # noqa: E402
 import test_gpu_closed_f64 as G  # noqa: E402
 
 GROWTH_MAX = 100.0
@@ -48,9 +47,9 @@ def _oracle(p, d, k, s, sigma=G.SIGMA):
     sign = 1.0 if s == 0 else -1.0
     layers = orc.unflatten(orc.pheno_params(d['theta'], sigma, sign * orc.table_get(d['table'], int(d['idx'][k]), d['P'])), dims)
     if d['noise'] is None:
-        return cno.run_model_episodes(d['spec'], layers, d['mean'], d['std'], d['clip'], p.T)
+        return orc.run_model(d['spec'], layers, d['mean'], d['std'], d['clip'], p.T)
     rs = _Stream(d['noise'][k, s].reshape(-1).astype(np.float64) / p.ac_std)
-    return cno.run_model_episodes(d['spec'], layers, d['mean'], d['std'], d['clip'], p.T, p.ac_std, rs, p.E)
+    return orc.run_model(d['spec'], layers, d['mean'], d['std'], d['clip'], p.T, ac_std=p.ac_std, rs=rs, episodes=p.E)
 
 
 _cache = {}

@@ -3,16 +3,12 @@ closed-loop kernels' compilation for sm_90a."""
 import os
 import re
 import subprocess
-import sys
 import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import es_oracle as orc
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import closed_noise_oracle as cno  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OBS, ACT, HID, T = 9, 3, (8, 8), 13          # T * ACT odd: the gaussian cache crosses episodes
@@ -26,51 +22,52 @@ def _problem(seed=3):
 
 
 @pytest.mark.parametrize('E', [1, 2, 5])
-def test_noise_free_oracle_is_run_model_closed(E):
+def test_noise_free_closed_oracle_is_one_episode(E):
+    """Without noise (ac_std = 0, or no stream) E episodes are the single noise-free episode, values and stream state
+    identical."""
     layers, spec = _problem()
     mean, std = np.full(OBS, 0.1), np.full(OBS, 0.9)
-    want = orc.run_model_closed(spec, layers, mean, std, 5.0, T)
+    want = orc.run_model(spec, layers, mean, std, 5.0, T)
     rs = np.random.RandomState(1)
     before = rs.get_state()
     for ac_std, r in ((0.0, rs), (0.05, None)):
-        got = cno.run_model_episodes(spec, layers, mean, std, 5.0, T, ac_std, r, E)
+        got = orc.run_model(spec, layers, mean, std, 5.0, T, ac_std=ac_std, rs=r, episodes=E)
         assert got[0] == want[0] and got[1] == want[1] and np.array_equal(got[2], want[2]) and got[3] == want[3]
     after = rs.get_state()
     assert all(np.array_equal(a, b) for a, b in zip(before, after))          # no noise, no draw
 
 
 @pytest.mark.parametrize('E', [1, 2, 3])
-def test_oracle_consumes_one_randn_call_per_evaluation(E):
+def test_closed_oracle_consumes_one_randn_call_per_evaluation(E):
     layers, spec = _problem()
     rs, ref = np.random.RandomState(7), np.random.RandomState(7)
     rs.randn(1); ref.randn(1)                                               # start with a cached gaussian
-    rews, behv, obs, step = cno.run_model_episodes(spec, layers, np.zeros(OBS), np.ones(OBS), 5.0, T, 0.05, rs, E)
+    rews, behv, obs, step = orc.run_model(spec, layers, np.zeros(OBS), np.ones(OBS), 5.0, T, ac_std=0.05, rs=rs, episodes=E)
     ref.randn(E * T * ACT)
     a, b = rs.get_state(), ref.get_state()
     assert np.array_equal(a[1], b[1]) and a[2:] == b[2:]                    # key, position, has_gauss and the cached value
     # the noise moves the trajectory, and the last episode is the one reported
-    clean = orc.run_model_closed(spec, layers, np.zeros(OBS), np.ones(OBS), 5.0, T)
+    clean = orc.run_model(spec, layers, np.zeros(OBS), np.ones(OBS), 5.0, T)
     assert rews != clean[0] and not np.array_equal(obs, clean[2])
     assert len(rews) == T and step == T - 1 and len(behv) == 3 * T
 
 
-def test_oracle_wrappers_restore_run_model():
-    layers, spec = _problem()
+def test_closed_test_params_runs_the_noisy_episodes():
+    """es_test_params on the closed loop with action noise and two episodes: pair 0's + evaluation by hand."""
+    _, spec = _problem()
     dims = orc.layer_dims(OBS, HID, ACT)
     P = orc.n_params(dims)
     rs = np.random.RandomState(3)
     table = rs.randn(P + 500).astype(np.float32)
     theta = (rs.randn(P) * 0.3).astype(np.float32)
-    kept = orc.run_model
-    pos, neg, inds, _, _ = cno.es_test_params(table, theta, 0.05, dims, spec, [5], 2, np.zeros(OBS), np.ones(OBS), 5.0, T,
+    pos, neg, inds, _, _ = orc.es_test_params(table, theta, 0.05, dims, spec, [5], 2, np.zeros(OBS), np.ones(OBS), 5.0, T,
                                               coins_per_eval=1, ac_std=0.05, episodes=2)
-    assert orc.run_model is kept and pos.shape == (2, 1) and neg.shape == (2, 1)
-    # by hand: pair 0's + evaluation
+    assert pos.shape == (2, 1) and neg.shape == (2, 1)
     r = np.random.RandomState(5)
     idx = orc.sample_idx(len(table), r, P)
     r.random()
     lay = orc.unflatten(orc.pheno_params(theta, 0.05, orc.table_get(table, idx, P)), dims)
-    rews, _, _, _ = cno.run_model_episodes(spec, lay, np.zeros(OBS), np.ones(OBS), 5.0, T, 0.05, r, 2)
+    rews, _, _, _ = orc.run_model(spec, lay, np.zeros(OBS), np.ones(OBS), 5.0, T, ac_std=0.05, rs=r, episodes=2)
     assert inds[0] == idx and pos[0, 0] == sum(rews)
 
 

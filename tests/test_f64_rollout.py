@@ -10,7 +10,6 @@ import pytest
 from oracle import es_oracle as orc
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import episodes_oracle as eo  # noqa: E402
 import f64_rollout as f64  # noqa: E402
 
 
@@ -55,8 +54,8 @@ def test_f64_reference_matches_the_oracle(obs, hidden, act, T, E, noisy):
         for s, nz in ((0, eps), (1, -eps)):
             layers = orc.unflatten(orc.pheno_params(theta, sigma, nz), dims)
             if noisy:
-                rews, bb, _, _ = eo.run_model_episodes(env, layers, mean, std, 5.0, T, False, 1.0,
-                                                       _Replay(noise[k, s].reshape(E * T, act)), E)
+                rews, bb, _, _ = orc.run_model(env, layers, mean, std, 5.0, T, ac_std=1.0,
+                                               rs=_Replay(noise[k, s].reshape(E * T, act)), episodes=E)
             else:
                 rews, bb, _, _ = orc.run_model(env, layers, mean, std, 5.0, T)
             ref = orc.reward_result(rews)[0]

@@ -1,6 +1,6 @@
 """GPU: binned-action policies (FFBinned, src/nn/nn.py:99-117) on the device -- es_rollout_openloop_binned (the general float32
 kernel of rollout_f32.cu, and rollout_tcw.cu under ES_ROLLOUT_TC3) and es_rollout_closedloop_mlp_binned (the cluster kernel of rollout_closedw.cu) against the oracle
-(tests/binned_oracle.py: es_oracle's loops with FFBinned's forward), and es.step with FFBinned against its python loop.
+(oracle.es_oracle.run_model with FFBinned's head), and es.step with FFBinned against its python loop.
 
 An arg-max turns a rounding difference into a different action only when two bins are within that difference of each other.
 So every parity problem is first checked on the float64 truth: the smallest gap between the two largest outputs over every
@@ -16,17 +16,11 @@ the oracle then take the same decisions, and what follows from them is exact whe
   * closed loop: the observations follow the kernel's fast tanh (absolute error ~1e-7), which moves no decision, so fitness and
     positions are compared with test_gpu_closed_wide.py's tolerances and the ObStat sums with 1e-4 of their magnitude.
 Problems are searched over a few seeds for one that meets the margin; the test asserts that one was found."""
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import es_oracle as orc
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import binned_oracle as bo  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -39,6 +33,26 @@ HIGH = np.array([2.7, 1.0, 0.35, -0.5, 3.0, 0.45, 1.0, 0.6], dtype=np.float32)
 def _head(adim, bins):
     from es_pytorch_b200.nn.nn import BinnedHead
     return BinnedHead(bins, LOW[:adim].copy(), HIGH[:adim].copy())
+
+
+def _binned(head):
+    """The oracle's description of a binned head."""
+    return head.bins, head.low, head.high
+
+
+def raw_outputs_f64(layers, x: np.ndarray) -> np.ndarray:
+    """The float64 truth of the tanh stack's outputs ([..., adim * bins]) for float32 inputs ``x``."""
+    h = np.asarray(x, dtype=np.float64)
+    for w, b in layers:
+        h = np.tanh(h @ np.asarray(w, np.float64).T + np.asarray(b, np.float64))
+    return h
+
+
+def top_two_gap(out: np.ndarray, bins: int) -> float:
+    """The smallest gap between the largest and the second largest output of any action dimension's bins in ``out``
+    ([..., adim * bins]): the margin by which every arg-max decision is taken."""
+    o = np.sort(np.asarray(out).reshape(-1, int(bins)), axis=1)
+    return float((o[:, -1] - o[:, -2]).min())
 
 
 def _layers(theta, table, idx, P, dims, sign, sigma=SIGMA):
@@ -56,7 +70,7 @@ def _open_problem(obs, hidden, adim, bins, T, n, mean, std, clip, seeds=range(40
         table = rs.randn(P + 20_000).astype(np.float32)
         theta = (rs.randn(P) * scale).astype(np.float32)
         idx = rs.randint(0, 20_000, size=n).astype(np.int64)
-        margin = min(bo.top_two_gap(bo.raw_outputs_f64(_layers(theta, table, i, P, dims, s), xs), bins)
+        margin = min(top_two_gap(raw_outputs_f64(_layers(theta, table, i, P, dims, s), xs), bins)
                      for i in idx for s in (1.0, -1.0))
         if margin > DELTA:
             return dims, P, table, theta, idx, spec, margin
@@ -67,8 +81,8 @@ def _open_oracle(dims, P, table, theta, idx, spec, head, mean, std, clip, T, sig
     fit, pos = np.zeros((2, len(idx))), np.zeros((2, len(idx), 3), dtype=np.float32)
     for k, i in enumerate(idx):
         for s, sign in enumerate((1.0, -1.0)):
-            rews, behv, _, _ = bo.run_model(spec, _layers(theta, table, i, P, dims, sign, sigma), mean, std, clip, T, head.bins,
-                                            head.low, head.high, batched=True)
+            rews, behv, _, _ = orc.run_model(spec, _layers(theta, table, i, P, dims, sign, sigma), mean, std, clip, T,
+                                             batched=True, binned=_binned(head))
             fit[s, k] = sum(rews)
             pos[s, k] = np.array(behv[-3:], dtype=np.float32)
     return fit, pos
@@ -185,9 +199,9 @@ def test_exact_ties_take_the_first_bin_open_loop(eng, hidden, n_pairs, tc3):
         theta = _tie_theta(rs, dims, P, bins, winners)
         f, b = _open_device(eng, [obs, *hidden, adim * bins], table, idx, theta, spec, head, z, o, 5.0, T, sigma=0.0,
                             mode=_lib.ES_ROLLOUT_TC3 if tc3 else _lib.ES_ROLLOUT_F32)
-        a = head.low if winners is None else bo.binned_action(np.eye(bins, dtype=np.float32)[winners].reshape(-1), bins,
-                                                                   head.low, head.high)
-        rews, behv, _, _ = bo.run_model(spec, orc.unflatten(theta, dims), z, o, 5.0, T, bins, head.low, head.high)
+        a = head.low if winners is None else orc.binned_action(np.eye(bins, dtype=np.float32)[winners].reshape(-1), bins,
+                                                                    head.low, head.high)
+        rews, behv, _, _ = orc.run_model(spec, orc.unflatten(theta, dims), z, o, 5.0, T, binned=_binned(head))
         acc = [np.float32(0)] * T
         for t in range(T):
             for j in range(adim):
@@ -213,8 +227,10 @@ def _closed_problem(obs, hidden, adim, bins, T, n, mean, std, clip, band=8, seed
         for i in idx:
             for s in (1.0, -1.0):
                 layers = _layers(theta, table, i, P, dims, s)
-                xs = bo.closed_inputs(spec, layers, mean, std, clip, T, bins, head.low, head.high)
-                margin = min(margin, bo.top_two_gap(bo.raw_outputs_f64(layers, xs), bins))
+                _, _, obs_after, _ = orc.run_model(spec, layers, mean, std, clip, T, binned=_binned(head))
+                # the normalised observations the network saw: obs_0, then every post-step observation but the last
+                xs = orc.normalise_obs(np.concatenate([spec.obs_stream[:1], obs_after[:-1]]), mean, std, clip)
+                margin = min(margin, top_two_gap(raw_outputs_f64(layers, xs), bins))
         if margin > delta:
             return dims, P, table, theta, idx, spec, margin
     raise AssertionError('no seed gives a closed-loop problem whose decisions all have a float64 margin > delta')
@@ -222,10 +238,10 @@ def _closed_problem(obs, hidden, adim, bins, T, n, mean, std, clip, band=8, seed
 
 def _assert_contractive(spec, layers, mean, std, clip, head, steps=150):
     s = orc.ClosedLoopEnvSpec(spec.obs_dim, spec.act_dim, steps, band=spec.band)
-    _, _, a, _ = bo.run_model(s, layers, mean, std, clip, steps, head.bins, head.low, head.high)
+    _, _, a, _ = orc.run_model(s, layers, mean, std, clip, steps, binned=_binned(head))
     s.obs_stream = s.obs_stream.copy()
     s.obs_stream[0] += np.float32(0.3)
-    _, _, b, _ = bo.run_model(s, layers, mean, std, clip, steps, head.bins, head.low, head.high)
+    _, _, b, _ = orc.run_model(s, layers, mean, std, clip, steps, binned=_binned(head))
     assert np.abs(a[-1] - b[-1]).max() < 1e-6, 'the loop is not contractive at this shape: the comparison would mean nothing'
 
 
@@ -275,8 +291,8 @@ def test_closed_loop_cluster_against_the_oracle(eng, obs, hidden, adim, bins):
     stat = orc.ObStatOracle((obs,), 0)
     for k, i in enumerate(idx):
         for s, sign in enumerate((1.0, -1.0)):
-            rews, behv, obsv, _ = bo.run_model(spec, _layers(theta, table, i, P, dims, sign), mean, std, clip, T, bins,
-                                               head.low, head.high)
+            rews, behv, obsv, _ = orc.run_model(spec, _layers(theta, table, i, P, dims, sign), mean, std, clip, T,
+                                                binned=_binned(head))
             assert abs(f[s, k] - sum(rews)) <= 2e-5 * max(1.0, np.abs(rews).sum()), (margin, k, s)
             assert np.abs(b[s, k] - np.array(behv[-3:], np.float32)).max() <= 1e-5
             if saved[2 * k + s]:
@@ -301,7 +317,7 @@ def test_exact_ties_take_the_first_bin_closed_loop(eng):
         theta = _tie_theta(rs, dims, P, bins, winners)
         f, b, _, _, _ = _closed_device(eng, [obs, *hidden, adim * bins], table, np.zeros(2, np.int64), theta, spec, head, z, o,
                                        5.0, sigma=0.0)
-        rews, behv, _, _ = bo.run_model(spec, orc.unflatten(theta, dims), z, o, 5.0, T, bins, head.low, head.high)
+        rews, behv, _, _ = orc.run_model(spec, orc.unflatten(theta, dims), z, o, 5.0, T, binned=_binned(head))
         assert np.all(f == sum(rews)) and np.all(b == np.array(behv[-3:], np.float32))
 
 

@@ -1,6 +1,6 @@
 """GPU parity of the CLOSED-LOOP synthetic env (SURVEY.md section 8d's optional variant, reported separately from the
 open-loop headline): es_rollout_closedloop, a whole DeviceGeneration and es.step on it, against the oracle's literal
-per-step loop (oracle.es_oracle.run_model_closed).  float32 arithmetic in a different summation order than torch's
+per-step loop (oracle.es_oracle.run_model).  float32 arithmetic in a different summation order than torch's
 matrix-vector products: tolerances are stated per test; indices, coins and rank weights stay exact."""
 import numpy as np
 import pytest

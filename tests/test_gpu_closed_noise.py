@@ -1,21 +1,15 @@
 """GPU: closed-loop rollouts with action noise and multi-episode evaluations (es_rollout_closedloop_mlp_episodes) against the
-literal per-step loop of tests/closed_noise_oracle.py, on the one-CTA kernel (rollout_closed.cu) and the cluster kernel
+oracle's literal per-step loop (oracle.es_oracle.run_model), on the one-CTA kernel (rollout_closed.cu) and the cluster kernel
 (rollout_closedw.cu), plus DeviceGeneration, es.step and the per-call fit_fn on top of them.
 
 The kernels add float32(gaussian * ac_std) to the float32 action in float32; the reference adds the float64 product and rounds
 once, so an action may differ by one float32 ulp.  Every case is first checked to be contractive under its noise, so those
 differences stay at rounding size; the bounds are test_gpu_closed_wide.py's."""
-import os
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import es_oracle as orc
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import closed_noise_oracle as cno  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -59,10 +53,10 @@ def _gauss(k, sgn, E, T, act):
 
 def _assert_contractive(spec, layers, mean, std, clip, ac_std, steps=150):
     s = orc.ClosedLoopEnvSpec(spec.obs_dim, spec.act_dim, steps, band=spec.band)
-    _, _, a, _ = cno.run_model_closed(s, layers, mean, std, clip, steps, ac_std, np.random.RandomState(5))
+    _, _, a, _ = orc.run_model(s, layers, mean, std, clip, steps, ac_std=ac_std, rs=np.random.RandomState(5))
     s.obs_stream = s.obs_stream.copy()
     s.obs_stream[0] += np.float32(0.3)
-    _, _, b, _ = cno.run_model_closed(s, layers, mean, std, clip, steps, ac_std, np.random.RandomState(5))
+    _, _, b, _ = orc.run_model(s, layers, mean, std, clip, steps, ac_std=ac_std, rs=np.random.RandomState(5))
     assert np.abs(a[-1] - b[-1]).max() < 1e-6, 'the loop is not contractive under this noise: the comparison would mean nothing'
 
 
@@ -125,8 +119,8 @@ def test_noisy_closed_rollout_matches_the_oracle(eng, name, obs, hidden, act, T,
     ref_sum, ref_sq = np.zeros(obs), np.zeros(obs)
     for k in range(n):
         for sgn, sign in enumerate((1.0, -1.0)):
-            rews, bh, ob, _ = cno.run_model_episodes(spec, _layers(theta, table, idx[k], P, dims, sign), mean, std, clip, T, ac_std,
-                                                     np.random.RandomState(1000 + 2 * k + sgn), E)
+            rews, bh, ob, _ = orc.run_model(spec, _layers(theta, table, idx[k], P, dims, sign), mean, std, clip, T, ac_std=ac_std,
+                                            rs=np.random.RandomState(1000 + 2 * k + sgn), episodes=E)
             want = sum(rews)
             assert abs(run.f[sgn, k] - want) <= 2e-5 * max(1.0, np.abs(rews).sum()), (k, sgn, run.f[sgn, k], want)
             pos_tol = max(1e-5, T * float(np.spacing(np.float32(np.abs(bh[-3:]).max()))))
@@ -202,7 +196,7 @@ def test_device_generation_with_closed_action_noise_matches_the_oracle(eng, E):
         st0 = [np.random.RandomState() for _ in seeds]
         for a, b in zip(st0, ref):
             a.set_state(b.get_state())
-        res = cno.generation(table, flat, opt, 0.05, dims, spec, [None] * 3, n, np.zeros(obs), np.ones(obs), 5.0, T, 500, 0.005,
+        res = orc.generation(table, flat, opt, 0.05, dims, spec, [None] * 3, n, np.zeros(obs), np.ones(obs), 5.0, T, 500, 0.005,
                              coins_per_eval=1, rank_states=ref, save_obs_chance=0.3, ac_std=ac_std, episodes=E)
         fpos, fneg = gen.evaluate(n)
         assert np.array_equal(gen.idx.cpu().numpy(), res['inds'].astype(np.int64))
@@ -258,7 +252,7 @@ def test_es_step_with_closed_action_noise_matches_the_oracle(eng, width, E):
     ac_std = 0.01
     for g in range(2):
         tr, _ = es.step(cfg, dist.world(), policy, nt, env, fit_fn, streams[0], ranker, Reporter())
-        ref = cno.es_step(table, flat, opt, 0.05, dims, spec, ref_streams, n, np.zeros(obs), np.ones(obs), 5.0, T, 500, 0.005,
+        ref = orc.es_step(table, flat, opt, 0.05, dims, spec, ref_streams, n, np.zeros(obs), np.ones(obs), 5.0, T, 500, 0.005,
                           coins_per_eval=1, save_obs_chance=0.25, batched=False, ac_std=ac_std, episodes=E)
         assert np.array_equal(np.asarray(ranker.noise_inds), ref['inds'])
         err = max(np.abs(ranker.fits_pos - ref['pos']).max(), np.abs(ranker.fits_neg - ref['neg']).max())
@@ -280,8 +274,8 @@ def test_es_step_with_closed_action_noise_matches_the_oracle(eng, width, E):
     assert eng.launches - l0 == 1
     for b in ref_streams:
         b.random()
-    rews, _, _, _ = cno.run_model_episodes(spec, orc.unflatten(flat, dims), np.zeros(obs), np.ones(obs), 5.0, T, ac_std,
-                                           ref_streams[0], E)
+    rews, _, _, _ = orc.run_model(spec, orc.unflatten(flat, dims), np.zeros(obs), np.ones(obs), 5.0, T, ac_std=ac_std,
+                                  rs=ref_streams[0], episodes=E)
     assert abs(direct.result[0] - sum(rews)) <= 1e-4
     for a, b in zip(streams, ref_streams):
         sa, sb = a.get_state(), b.get_state()

@@ -1,17 +1,12 @@
 """GPU: multi-episode evaluations (obj.py:54-63, ``eps_per_policy``): es_rollout_openloop_episodes against the episode
 oracle, E = 1 against es_rollout_openloop_noisy, the tensor-core modes against float32, DeviceGeneration and es.step."""
 import ctypes as C
-import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import es_oracle as orc
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import episodes_oracle as eo  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -71,8 +66,8 @@ def test_f32_episodes_match_the_oracle(eng, shape, E):
         eps = orc.table_get(pb['table'], int(pb['idx'][k]), pb['P'])
         for s, nz in ((0, eps), (1, -eps)):
             layers = orc.unflatten(orc.pheno_params(pb['theta'], 0.02, nz), pb['dims'])
-            rews, bb, _, _ = eo.run_model_episodes(pb['env'], layers, np.zeros(obs), np.ones(obs), 5.0, T, True, 1.0,
-                                                   _Replay(pb['noise'][k, s].reshape(E * T, act)), E)
+            rews, bb, _, _ = orc.run_model(pb['env'], layers, np.zeros(obs), np.ones(obs), 5.0, T, True, ac_std=1.0,
+                                           rs=_Replay(pb['noise'][k, s].reshape(E * T, act)), episodes=E)
             assert abs(f[s, k] - orc.reward_result(rews)[0]) <= 1e-5 * max(1.0, np.abs(rews).sum()), (k, s)
             assert np.allclose(b[s, k], bb[-3:], rtol=1e-4, atol=1e-5), (k, s)          # the last episode's position
 
@@ -158,8 +153,8 @@ def test_device_generation_episodes_match_the_oracle(eng, monkeypatch, jump):
     for g in range(2):
         fpos, fneg = gen.evaluate(n)
         gen.update(fpos, fneg)
-        res = eo.generation(table, flat, opt, 0.02, dims, env, [None] * 3, n, np.zeros(obs), np.ones(obs), 5.0, T, 500, 0.005,
-                            coins_per_eval=1, rank_states=ref, save_obs_chance=0.4, ac_std=ac_std, episodes=E)
+        res = orc.generation(table, flat, opt, 0.02, dims, env, [None] * 3, n, np.zeros(obs), np.ones(obs), 5.0, T, 500, 0.005,
+                             coins_per_eval=1, rank_states=ref, save_obs_chance=0.4, ac_std=ac_std, episodes=E)
         assert np.array_equal(gen.idx.cpu().numpy(), res['inds'].astype(np.int64))
         assert np.abs(fpos.cpu().numpy()[:, 0] - res['pos'][:, 0]).max() <= 1e-4
         assert np.abs(fneg.cpu().numpy()[:, 0] - res['neg'][:, 0]).max() <= 1e-4

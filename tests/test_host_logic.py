@@ -502,7 +502,7 @@ def test_closed_loop_env_is_the_oracles_env():
 
 def test_run_model_python_loop_on_the_closed_loop_env_is_the_oracles_loop():
     """gym_runner.run_model's python loop (module forward + ClosedLoopEnv.step: the route of an opaque fit_fn, and the
-    reference's own loop shape, src/gym/gym_runner.py:50-54) against the oracle's run_model_closed on the same parameters
+    reference's own loop shape, src/gym/gym_runner.py:50-54) against the oracle's closed-loop run_model on the same parameters
     and a non-trivial observation normalisation: rewards, positions, post-step observations, last index."""
     import torch
     from es_pytorch_b200.core.policy import Policy

@@ -1,14 +1,9 @@
-"""CPU: the multi-episode oracle (obj.py:54-63, ``eps_per_policy``) and BatchedRollout's ``episodes`` argument."""
-import os
-import sys
-
+"""CPU: the oracle's multi-episode evaluations (obj.py:54-63, ``eps_per_policy``) and BatchedRollout's ``episodes``
+argument."""
 import numpy as np
 import pytest
 
 from oracle import es_oracle as orc
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import episodes_oracle as eo  # noqa: E402
 
 OBS, ACT, HID, T = 5, 3, (8, 8), 13          # T * ACT odd: the gaussian cache crosses episodes and evaluations
 
@@ -39,19 +34,22 @@ def _same_states(a, b):
         assert np.array_equal(sx[0], sy[0]) and sx[1:] == sy[1:]
 
 
-def _test_params(episodes, ac_std, seeds=(21, 22), n=3, mod=eo, **kw):
+def _test_params(episodes, ac_std, seeds=(21, 22), n=3, **kw):
+    """es_test_params with ``episodes`` episodes per evaluation; None leaves the argument at its default."""
     dims, table, theta, env = _problem()
     streams = _streams(seeds)
     args = (table, theta, 0.05, dims, env, [None] * len(seeds), n, np.zeros(OBS), np.ones(OBS), 5.0, T)
     kw = dict(coins_per_eval=1, save_obs_chance=0.5, rank_states=streams, ac_std=ac_std, **kw)
-    out = mod.es_test_params(*args, episodes=episodes, **kw) if mod is eo else mod.es_test_params(*args, **kw)
-    return out, streams
+    if episodes is not None:
+        kw['episodes'] = episodes
+    return orc.es_test_params(*args, **kw), streams
 
 
 @pytest.mark.parametrize('ac_std', [0.0, 0.01])
 def test_one_episode_is_the_oracle(ac_std):
+    """``episodes=1`` is the single-episode path: values and stream state identical."""
     (pos, neg, inds, steps, ob), sa = _test_params(1, ac_std)
-    (pos0, neg0, inds0, steps0, ob0), sb = _test_params(None, ac_std, mod=orc)
+    (pos0, neg0, inds0, steps0, ob0), sb = _test_params(None, ac_std)
     assert np.array_equal(pos, pos0) and np.array_equal(neg, neg0) and np.array_equal(inds, inds0) and steps == steps0
     assert np.array_equal(ob.sum, ob0.sum) and np.array_equal(ob.sumsq, ob0.sumsq) and ob.count == ob0.count
     _same_states(sa, sb)
@@ -61,11 +59,10 @@ def test_one_episode_generation_and_step_are_the_oracle():
     dims, table, theta, env = _problem()
     P = len(theta)
     res = []
-    for mod in (eo, orc):
+    for episodes in ({'episodes': 1}, {}):
         flat, opt, streams = theta.copy(), orc.AdamOracle(P, 0.01), _streams((5, 6))
         args = (table, flat, opt, 0.05, dims, env, streams, 2, np.zeros(OBS), np.ones(OBS), 5.0, T, 100, 0.005)
-        kw = dict(coins_per_eval=1, save_obs_chance=0.5, ac_std=0.01)
-        out = mod.es_step(*args, episodes=1, **kw) if mod is eo else mod.es_step(*args, **kw)
+        out = orc.es_step(*args, coins_per_eval=1, save_obs_chance=0.5, ac_std=0.01, **episodes)
         res.append((out, flat, streams))
     (a, fa, sa), (b, fb, sb) = res
     assert np.array_equal(fa, fb) and a['noiseless'] == b['noiseless']
