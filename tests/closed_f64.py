@@ -11,8 +11,8 @@ TEST INFRASTRUCTURE ONLY.  It takes the data the kernels get and evaluates them 
 * every episode restarts from ``obs0`` with the position at 0; the fitness is ``sum_t mean_e r_{e,t}``, the reward mass
   ``sum_t mean_e sum_j |a_tj c_tj|`` (the scale of the fitness error of an implementation whose actions carry a relative
   error, as in f64_rollout.py);
-* behaviour, position magnitude (f64_rollout.episode's) and the float64 column sums of the post-step observations and of their
-  squares (the ObStat increments) are the last episode's.
+* behaviour, position magnitude (f64_rollout.episode's), the float64 column sums of the post-step observations and of their
+  squares (the ObStat increments) and the final observation ``olast`` are the last episode's.
 
 The evaluations of a call are stacked, so that a step is one batched matrix product per layer; so are *variants* of every
 evaluation: ``simulate(variants=)`` runs, beside the truth, copies of it computed wrongly on purpose (the bugs a kernel could have, see
@@ -281,7 +281,7 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
             osum += ob * lv
             osq += ob * ob * lv
             oabs += np.abs(ob) * lv
-        out = dict(behv=pos.copy(), mag=mag, osum=osum, osq=osq, oabs=oabs)
+        out = dict(behv=pos.copy(), mag=mag, osum=osum, osq=osq, oabs=oabs, olast=ob.copy())
         if e == 0:
             first = out
         if e == E - 1:

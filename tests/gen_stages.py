@@ -23,6 +23,20 @@ near-tie that flips one rank cannot cascade into the checks of later stages:
                 rc_layout(P, K, sm), unchanged;
   8 optimizer   theta', m', v' bit for bit against orc.AdamOracle applied in float32 to the device's gsum and theta.
 
+Episodes (``Capture.episodes`` = E): every evaluation draws E T act gaussians after its coin, the E episodes back to back;
+its fitness is sum_t (r_1t + ... + r_Et) / E and its behaviour the last episode's.  Objectives (``Capture.objective``):
+'reward' (one column) or 'nsr' (NSRResult: reward in column 0, novelty in column NOVELTY_COLUMN = 1, ranked by the
+MultiObjective blend w r_0 + (1 - w) r_1 with w = ``moo_w``); a capture with an archive and no objective is 'nsr'.
+
+The closed loop (``Capture.obs0`` given: ClosedLoopEnv's obs_0, A^T [band, obs], B^T [act, obs]) has no full-population truth:
+  2 obstat      count and n_saved exact; sum and sumsq against the float64 truth's osum / osq of the saved evaluations within
+                test_gpu_closed_f64's bound (T ulps of their magnitude per saved evaluation plus OBS_ERR per observation);
+  3 normalise   inside the rollout kernel: judged through the fitness;
+  4 fitness     closed_f64.truth on a sample (``closed_sample``: every saved evaluation, the first and last pair of each
+                stream, random pairs up to about 64 evaluations), with test_gpu_closed_f64's bounds, after closed_f64.growth
+                has shown that the sample does not amplify rounding (<= GROWTH_BOUND);
+  6 weights     exact against the oracle on the device's fitness; the ranks against the truth are not compared (reported).
+
 Every check is a ``Check``: a measured value, its bound and whether it passed.  Tolerance checks measure a ratio against a
 positive bound.  Exact checks measure a distance -- float32 / float64 values in units in the last place of the reference
 value, integers in units -- against the bound 0; their margin is the distance itself (1 is the smallest that fails), so a
@@ -42,16 +56,25 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from oracle import es_oracle as orc  # noqa: E402
+import closed_f64 as cf  # noqa: E402
 import f64_rollout as f64  # noqa: E402
 import rc_f64 as rc  # noqa: E402
+import test_gpu_closed_f64 as closed_bounds  # noqa: E402
 import test_gpu_noise_table as noise_criterion  # noqa: E402
 import test_gpu_rollout_f64 as rollout_f64  # noqa: E402
 
 F32 = np.float32
 TIE_REL = 1e-12           # the device float64 truth against the CPU float64 reference, relative to the reward mass
 # |kappa| of e = kappa f + c + r fitted over a population: the part of the fitness error proportional to the fitness.  Largest
-# value measured on an H100 SXM (80 GB): 8.7e-7 (ES_ROLLOUT_TC3, configs 3, 4 and 5, every generation); ES_ROLLOUT_F32 at most 9.4e-9
-KAPPA_BOUND = 2e-6
+# values measured on an H100 SXM (80 GB, 700 W): ES_ROLLOUT_TC3 8.7e-7 at 376-64-64-17 (rollout_tc2.cu, configs 3, 4 and 5,
+# every generation) and 1.33e-6 at the shipped configs' wide policies (rollout_tcw.cu: 1.04e-6 .. 1.33e-6 over simple_conf,
+# nsra, ns and flagrun); ES_ROLLOUT_F32 at most 2.7e-8; ES_ROLLOUT_TC (single float16 products, rollout_tcw.cu) 4.1e-5 at
+# simple_conf
+KAPPA_BOUND = 2.7e-6
+KAPPA_BOUND_TC = 8e-5
+NOVELTY_COLUMN = 1        # NSRResult's row: [reward, novelty]
+GROWTH_BOUND = 100.0      # closed loop: the largest growth of a 1e-9 move of obs_0 over an episode (test_gpu_closed_f64.py)
+CLOSED_SAMPLE = 64        # closed loop: evaluations in the fitness truth's sample, at least
 STAGES = ('draws', 'obstat', 'normalise', 'fitness', 'novelty', 'weights', 'gradient', 'optimizer')
 
 
@@ -119,14 +142,34 @@ class Capture:
     t1: int
     streams1: list                          # the streams after the generation
     behv: Optional[np.ndarray] = None       # float32 [2, K, 3]
-    act_noise: object = None                # float32 [K, 2, T * act]
+    act_noise: object = None                # float32 [K, 2, E * T * act], the episodes back to back
     archive: Optional[np.ndarray] = None    # float64 [A, 2]
     nov_k: int = 10
-    moo_w: float = 0.5
+    moo_w: float = 0.5                      # 'nsr': the weight of the reward column's ranks (the novelty's: 1 - moo_w)
     beta1: float = 0.9
     beta2: float = 0.999
     epsilon: float = 1e-08
+    episodes: int = 1
+    objective: Optional[str] = None         # 'reward' or 'nsr' (novelty in column NOVELTY_COLUMN); None: 'nsr' with an archive
+    # the closed loop (ClosedLoopEnv.device_closed): obs_0 [obs], A^T [band, obs], B^T [act, obs]; obs_stream and obsn unused
+    obs0: Optional[np.ndarray] = None
+    env_a: Optional[np.ndarray] = None
+    env_b: Optional[np.ndarray] = None
+    band: Optional[int] = None
     extra: dict = field(default_factory=dict)
+
+    def __post_init__(self):
+        if self.objective is None:
+            self.objective = 'reward' if self.archive is None else 'nsr'
+        assert self.objective in ('reward', 'nsr') and (self.objective == 'nsr') == (self.archive is not None)
+
+    @property
+    def closed(self) -> bool:
+        return self.obs0 is not None
+
+    @property
+    def obs_dim(self) -> int:
+        return self.sizes[0]
 
     @property
     def P(self) -> int:
@@ -172,13 +215,13 @@ def _np(x):
 
 # ---------------------------------------------------------------------------------------------- 1. draws
 def replay_stream(cap: Capture, r: int):
-    """Stream r in the reference's order.  Returns (indices, coin words [n, 4] uint32, end state, generator of the
-    noise block [n, 2, T act] float64 (ac_std * randn) -- drawn lazily so that only one stream's block is held)."""
+    """Stream r in the reference's order.  Returns (indices, coin words [n, 4] uint32, end state, the noise block
+    [n, 2, E T act] float64 (ac_std * randn, the E episodes of an evaluation back to back) or None)."""
     key, pos, has, gauss = cap.streams0[r]
     rs = np.random.RandomState()
     rs.set_state(('MT19937', np.asarray(key, dtype=np.uint32), int(pos), int(has), float(gauss)))
     n, L, P = cap.n_per_stream, cap.table.numel(), cap.P
-    nrm = cap.T * cap.act if cap.ac_std else 0
+    nrm = cap.episodes * cap.T * cap.act if cap.ac_std else 0
     idx = np.empty(n, dtype=np.int64)
     words = np.empty((n, 4), dtype=np.uint32)
     noise = np.empty((n, 2, nrm), dtype=np.float64) if nrm else None
@@ -189,7 +232,7 @@ def replay_stream(cap: Capture, r: int):
             words[k, 2 * s] = int.from_bytes(rs.bytes(4), 'little')
             words[k, 2 * s + 1] = int.from_bytes(rs.bytes(4), 'little')
             if nrm:
-                noise[k, s] = rs.randn(nrm) * cap.ac_std          # FeedForward.forward's T x rs.randn(act) * ac_std
+                noise[k, s] = rs.randn(nrm) * cap.ac_std          # per episode FeedForward.forward's T x rs.randn(act) * ac_std
     return idx, words, rs.get_state(), noise
 
 
@@ -238,7 +281,20 @@ def stage_draws(cap: Capture) -> List[Check]:
 
 
 # ---------------------------------------------------------------------------------------------- 2. obstat
-def stage_obstat(cap: Capture) -> List[Check]:
+def _replay_words(cap: Capture) -> list:
+    if 'replay_words' not in cap.extra:
+        cap.extra['replay_words'] = [replay_stream(cap, r)[1] for r in range(len(cap.streams0))]
+    return cap.extra['replay_words']
+
+
+def replayed_saves(cap: Capture) -> np.ndarray:
+    """[2, K] bool: the evaluations whose replayed save_obs coin fell."""
+    return np.concatenate([saved_flags(w, cap.save_obs_chance) for w in _replay_words(cap)]).T.copy()
+
+
+def stage_obstat(cap: Capture, truth=None) -> List[Check]:
+    if cap.closed:
+        return _stage_obstat_closed(cap, truth)
     obs = cap.obs_stream.shape[1]
     flags = np.concatenate([saved_flags(replay_words, cap.save_obs_chance) for replay_words in cap.extra['replay_words']])
     s, q, c = orc.ob_sum_sq_cnt(cap.obs_stream[1:cap.T + 1])
@@ -257,19 +313,62 @@ def stage_obstat(cap: Capture) -> List[Check]:
             _exact('obstat', 'n_saved (units)', cap.stats[2 * obs + 1:], np.array([float(n_saved)]), f'{n_saved} saves')]
 
 
+def _truth_columns(truth, saved: np.ndarray):
+    """The sampled truth's [2, n] positions of the saved evaluations ([2, K] mask); raises when the sample misses one."""
+    col = {p: j for j, p in enumerate(truth['pairs'])}
+    s_idx, k_idx = np.nonzero(saved)
+    missing = sorted({int(k) for k in k_idx if int(k) not in col})
+    if missing:
+        raise ValueError(f'saved evaluations of pairs {missing[:8]} are not in the truth sample')
+    return s_idx, np.array([col[int(k)] for k in k_idx], dtype=np.int64)
+
+
+def _stage_obstat_closed(cap: Capture, truth) -> List[Check]:
+    """Every evaluation's ObStat increment is its own post-step observations (obs_1 .. obs_T of the last episode): count and
+    n_saved exact, the sums within test_gpu_closed_f64's bound of the truth's (the device adds them with float64 atomics,
+    in no fixed order)."""
+    obs, T = cap.obs_dim, cap.T
+    saved = replayed_saves(cap)
+    n_saved = int(saved.sum())
+    cap.extra['n_saved'] = n_saved
+    s_idx, j_idx = _truth_columns(truth, saved)
+    U, ns = 2.0 ** -24, max(1, n_saved)
+    want_s = truth['osum'][s_idx, j_idx].sum(axis=0)
+    want_q = truth['osq'][s_idx, j_idx].sum(axis=0)
+    bound_s = 2 * T * U * truth['oabs'][s_idx, j_idx].sum(axis=0) + closed_bounds.OBS_ERR * T * ns
+    bound_q = 2 * T * U * want_q + 2 * closed_bounds.OBS_ERR * T * ns
+    rs = float((np.abs(cap.stats[:obs] - want_s) / bound_s).max())
+    rq = float((np.abs(cap.stats[obs:2 * obs] - want_q) / bound_q).max())
+    return [Check('obstat', 'sum err/bound against the float64 truth', rs, 1.0, rs <= 1.0),
+            Check('obstat', 'sumsq err/bound against the float64 truth', rq, 1.0, rq <= 1.0),
+            _exact('obstat', 'count (ulp)', cap.stats[2 * obs:2 * obs + 1], np.array([float(T * n_saved)])),
+            _exact('obstat', 'n_saved (units)', cap.stats[2 * obs + 1:], np.array([float(n_saved)]), f'{n_saved} saves')]
+
+
 # ---------------------------------------------------------------------------------------------- 3. normalise
 def stage_normalise(cap: Capture) -> List[Check]:
+    if cap.closed:
+        return []                                         # the closed-loop kernel normalises every step itself
     want = orc.normalise_obs(cap.obs_stream[:cap.T], cap.ob_mean, cap.ob_std, cap.ob_clip)
     return [_exact('normalise', 'obsn (ulp)', cap.obsn, want)]
 
 
 # ---------------------------------------------------------------------------------------------- 4. fitness
-def fitness_truth(cap: Capture, chunk: int = 200):
+ACT_BYTES = 2 ** 29       # fitness_truth: the float64 activations of one layer held per chunk of pairs, at most
+
+
+def fitness_truth(cap: Capture, chunk: Optional[int] = None, behaviour_episode: int = -1, noise=None):
     """(fitness [2, K], behaviour [2, K, 3], reward mass [2, K], position magnitude [2, K, 3]) in float64 (f64_rollout's
-    definitions), computed with torch.float64 on the table's device in chunks of pairs: a measurement reference."""
+    definitions), computed with torch.float64 on the table's device in chunks of pairs: a measurement reference.  The
+    forward pass is shared by the E episodes (only the noise differs); fitness and mass are the per-step means over them,
+    behaviour and magnitude the episode ``behaviour_episode``'s.  ``chunk`` (default: up to 200 pairs, fewer where one
+    layer's activations over T steps would pass ACT_BYTES); ``noise``: in place of ``cap.act_noise``."""
     dev = cap.table.device
     d64 = torch.float64
-    sizes, T, act, K, P = cap.sizes, cap.T, cap.act, cap.K, cap.P
+    sizes, T, act, K, P, E = cap.sizes, cap.T, cap.act, cap.K, cap.P, cap.episodes
+    if chunk is None:
+        chunk = max(1, min(200, ACT_BYTES // (8 * T * max(sizes[1:]))))
+    noise = cap.act_noise if noise is None else noise
     theta = torch.from_numpy(np.ascontiguousarray(cap.theta0)).to(dev, d64)
     X = torch.from_numpy(np.ascontiguousarray(cap.obsn)).to(dev, d64)
     C = torch.from_numpy(np.ascontiguousarray(cap.rew_vec)).to(dev, d64)
@@ -284,7 +383,7 @@ def fitness_truth(cap: Capture, chunk: int = 200):
     for b0 in range(0, K, chunk):
         b1 = min(K, b0 + chunk)
         eps = cap.table[idx_all[b0:b1, None] + ar[None, :]].to(d64)
-        nz_block = None if not cap.ac_std else torch.as_tensor(_np(cap.act_noise[b0:b1])).to(dev, d64)
+        nz_block = None if not cap.ac_std else torch.as_tensor(_np(noise[b0:b1])).to(dev, d64)
         for s, sign in enumerate((1.0, -1.0)):
             W = theta[None, :] + sign * s32 * eps                                 # [B, P]
             B = W.shape[0]
@@ -293,12 +392,23 @@ def fitness_truth(cap: Capture, chunk: int = 200):
             a = torch.tanh((X @ W1.reshape(B * fo, fi).T).reshape(T, B, fo).permute(1, 0, 2) + W[:, bo:bo + fo][:, None, :])
             for wo, bo, fi, fo in lay[1:]:
                 a = torch.tanh(torch.bmm(a, W[:, wo:wo + fi * fo].reshape(B, fo, fi).transpose(1, 2)) + W[:, bo:bo + fo][:, None, :])
-            if nz_block is not None:
-                a = a + nz_block[:, s].reshape(B, T, act)
-            prod = a * C[None]
-            fit[s, b0:b1] = prod.sum(dim=(1, 2)).cpu().numpy()
-            mass[s, b0:b1] = prod.abs().sum(dim=(1, 2)).cpu().numpy()
-            terms = ps * a[:, :, sel]
+            if nz_block is None:
+                prod = a * C[None]
+                fit[s, b0:b1] = prod.sum(dim=(1, 2)).cpu().numpy()
+                mass[s, b0:b1] = prod.abs().sum(dim=(1, 2)).cpu().numpy()
+                ab = a
+            else:
+                nz_e = nz_block[:, s].reshape(B, E, T, act)
+                f_acc = torch.zeros(B, dtype=d64, device=dev)
+                m_acc = torch.zeros(B, dtype=d64, device=dev)
+                for e in range(E):
+                    prod = (a + nz_e[:, e]) * C[None]
+                    f_acc += prod.sum(dim=(1, 2))
+                    m_acc += prod.abs().sum(dim=(1, 2))
+                fit[s, b0:b1] = (f_acc / E).cpu().numpy()
+                mass[s, b0:b1] = (m_acc / E).cpu().numpy()
+                ab = a + nz_e[:, behaviour_episode]
+            terms = ps * ab[:, :, sel]
             behv[s, b0:b1] = terms.sum(dim=1).cpu().numpy()
             mag[s, b0:b1] = (torch.cumsum(terms, dim=1).abs().sum(dim=1) + terms.abs().sum(dim=1)).cpu().numpy()
     return fit, behv, mass, mag
@@ -310,7 +420,64 @@ def tie_pairs(cap: Capture) -> List[int]:
     return sorted({p for r in range(len(cap.streams0)) for p in (r * n, r * n + n - 1)})
 
 
+def closed_sample(cap: Capture, seed: int = 0) -> List[int]:
+    """The pairs the closed-loop truth covers: every pair with a saved evaluation (the replayed coins), the first and last
+    pair of every stream, then random pairs until the sample holds CLOSED_SAMPLE evaluations."""
+    saved = replayed_saves(cap)
+    pairs = set(np.nonzero(saved.any(axis=0))[0].tolist()) | set(tie_pairs(cap))
+    for p in np.random.RandomState(seed).permutation(cap.K):
+        if 2 * len(pairs) >= CLOSED_SAMPLE:
+            break
+        pairs.add(int(p))
+    return sorted(pairs)
+
+
+def closed_truth(cap: Capture, pairs: Optional[Sequence[int]] = None, growth: bool = True):
+    """closed_f64.truth of the pairs ``pairs`` (default closed_sample) from the device's indices, theta, observation
+    statistics and action noise, plus 'pairs' and 'growth' (closed_f64.growth of the same evaluations; nan when not
+    ``growth``)."""
+    pairs = closed_sample(cap) if pairs is None else list(pairs)
+    P = cap.P
+    table_np = np.concatenate([_np(cap.table[int(cap.idx[k]):int(cap.idx[k]) + P]) for k in pairs])
+    noise = None
+    if cap.ac_std:
+        noise = np.stack([_np(cap.act_noise[k]) for k in pairs])
+    args = (table_np, np.arange(len(pairs)) * P, cap.theta0, cap.sigma, cap.sizes, cap.ob_mean, cap.ob_std, cap.ob_clip,
+            cap.obs0, cap.env_a, cap.env_b, cap.rew_vec, cap.pos_scale)
+    kw = dict(act_noise=noise, episodes=cap.episodes if cap.ac_std else 1)
+    out = cf.truth(*args, **kw)
+    out['growth'] = cf.growth(*args, **kw) if growth else math.nan
+    out['pairs'] = pairs
+    return out
+
+
+def _stage_fitness_closed(cap: Capture, truth) -> List[Check]:
+    """The sampled evaluations against the float64 truth, with test_gpu_closed_f64._check's bounds."""
+    pairs = truth['pairs']
+    U = 2.0 ** -24
+    f = cap.fit[:, pairs, 0]
+    tf, mass = truth['fit'], truth['mass']
+    err = np.abs(f - tf)
+    spread = max(tf.std(), 1e-3 * math.sqrt(cap.T))
+    rms = math.sqrt((err ** 2).mean())
+    worst = float((err / mass).max())
+    g = truth['growth']
+    out = [Check('fitness', 'closed loop: growth of a 1e-9 move of obs_0 (the sample is not chaotic)', g, GROWTH_BOUND,
+                 g <= GROWTH_BOUND, f'{2 * len(pairs)} evaluations sampled'),
+           Check('fitness', 'max err/mass', worst, closed_bounds.EVAL_REL, worst <= closed_bounds.EVAL_REL),
+           Check('fitness', 'rms/spread', rms / spread, closed_bounds.RMS_BOUND, rms <= closed_bounds.RMS_BOUND * spread)]
+    if cap.behv is not None:
+        tol = 2 * U * truth['mag'] + closed_bounds.ACT_ERR * float(np.float32(cap.pos_scale)) * cap.T
+        r = float((np.abs(cap.behv[:, pairs] - truth['behv']) / tol).max())
+        out.append(Check('fitness', 'behaviour err/tol', r, 1.0, r <= 1.0))
+    cap.extra['fitness'] = dict(sampled_evaluations=2 * len(pairs), rms_over_spread=rms / spread, max_err_over_mass=worst,
+                                growth=g)
+    return out
+
+
 def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] = None) -> List[Check]:
+    if cap.closed:
+        return _stage_fitness_closed(cap, truth)
     tf, tb, mass, mag = truth
     f = cap.fit[:, :, 0]
     b = cap.behv
@@ -335,8 +502,8 @@ def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] =
     out.append(Check('fitness', 'rms/spread of the error less its fitted scale and offset',
                      cap.extra['fitness']['resid_rms_over_spread'], rollout_f64.RMS_BOUND[mode],
                      cap.extra['fitness']['resid_rms_over_spread'] <= rollout_f64.RMS_BOUND[mode]))
-    out.append(Check('fitness', '|fitted relative scale of the error|', abs(float(kappa)), KAPPA_BOUND,
-                     abs(float(kappa)) <= KAPPA_BOUND))
+    kb = KAPPA_BOUND_TC if mode == rollout_f64.TC else KAPPA_BOUND
+    out.append(Check('fitness', '|fitted relative scale of the error|', abs(float(kappa)), kb, abs(float(kappa)) <= kb))
     try:                                                   # the one assert helper of the rollout tests decides as well
         rollout_f64._check('generation', mode, case, f, b, None, truth)
         helper_ok = True
@@ -352,7 +519,7 @@ def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] =
     if cap.ac_std:
         noise = np.stack([_np(cap.act_noise[k]) for k in tie])
     cf, cb, cm, cmag = f64.rollout_f64(table_np, np.arange(len(tie)) * P, cap.theta0, cap.sigma, cap.sizes, cap.obsn, cap.rew_vec,
-                                       cap.pos_scale, noise, 1)
+                                       cap.pos_scale, noise, cap.episodes)
     rel = float(max((np.abs(cf - tf[:, tie]) / cm).max(), (np.abs(cb - tb[:, tie]) / np.maximum(cmag, 1e-300)).max()))
     out.append(Check('fitness', f'float64 truth vs CPU reference ({2 * len(tie)} evaluations), rel', rel, TIE_REL, rel <= TIE_REL))
     return out
@@ -364,15 +531,19 @@ def stage_novelty(cap: Capture) -> List[Check]:
         return []
     b = cap.behv
     want = np.array([[orc.novelty(b[s, k, :2], cap.archive, cap.nov_k) for k in range(cap.K)] for s in range(2)])
-    return [_exact('novelty', 'novelty column 1 (ulp)', cap.fit[:, :, 1], want)]
+    return [_exact('novelty', f'novelty column {NOVELTY_COLUMN} (ulp)', cap.fit[:, :, NOVELTY_COLUMN], want,
+                   f'archive of {len(cap.archive)}, k = {cap.nov_k}')]
 
 
 # ---------------------------------------------------------------------------------------------- 6. weights
-def reference_weights(cap: Capture, fit: np.ndarray):
-    if cap.archive is None:
+def reference_weights(cap: Capture, fit: np.ndarray, moo_w: Optional[float] = None):
+    """Centered ranks of the reward, or for 'nsr' the MultiObjective blend of the reward's (weight ``moo_w``, default the
+    capture's) and the novelty's ranks."""
+    if cap.objective == 'reward':
         w, n = orc.centered_ranker(fit[0][:, :1], fit[1][:, :1])
     else:
-        w, n = orc.moo_ranker(fit[0], fit[1], cap.moo_w)
+        cols = [0, NOVELTY_COLUMN]
+        w, n = orc.moo_ranker(fit[0][:, cols], fit[1][:, cols], cap.moo_w if moo_w is None else moo_w)
     return np.asarray(w, dtype=F32).reshape(-1), n
 
 
@@ -392,7 +563,11 @@ def stage_weights(cap: Capture, truth_fit=None, shift_bound=None, dw_bound=None)
     w, n = reference_weights(cap, cap.fit)
     out = [_exact('weights', 'weights (ulp)', cap.weights, w),
            Check('weights', 'n_ranked (units)', float(abs(cap.n_ranked - n)), 0.0, cap.n_ranked == n)]
-    if truth_fit is not None:
+    if cap.closed:
+        cap.extra['ranks_vs_truth'] = 'not compared: the closed loop has a float64 truth of a sample only'
+        out.append(Check('weights', 'ranks against the float64 truth: not compared (closed loop, sampled truth)', 0.0, 0.0,
+                         True))
+    elif truth_fit is not None:
         nd, shift, dw = rank_report(cap, truth_fit)
         cap.extra['ranks_vs_truth'] = dict(ranks_differing=nd, max_rank_shift=shift, max_abs_dw=dw)
         out.append(Check('weights', 'largest rank shift against the float64 truth', shift, shift_bound, shift <= shift_bound,
@@ -434,15 +609,22 @@ def stage_optimizer(cap: Capture) -> List[Check]:
 # ---------------------------------------------------------------------------------------------- all stages
 def judge(cap: Capture, mode: int, sm: int, shift_bound: float, dw_bound: float, truth=None,
           tie: Optional[Sequence[int]] = None) -> List[Check]:
-    """Every stage of ``cap``, in order; a stage that raises counts as failed.  ``truth``: fitness_truth(cap) when already
-    computed (re-judging mutated copies of a large capture whose mutation leaves the rollout inputs alone)."""
-    if truth is None:
+    """Every stage of ``cap``, in order; a stage that raises counts as failed.  ``truth``: fitness_truth(cap) (closed loop:
+    closed_truth(cap)) when already computed (re-judging mutated copies of a large capture whose mutation leaves the rollout
+    inputs alone)."""
+    if truth is None and not cap.closed:
         truth = fitness_truth(cap)
+    held = [truth]
+
+    def tr():                   # the closed loop's sample holds the saved evaluations: computed after the draws' replay
+        if held[0] is None:
+            held[0] = cap.extra['closed_truth'] = closed_truth(cap)
+        return held[0]
     checks = []
-    for stage, fn in (('draws', lambda: stage_draws(cap)), ('obstat', lambda: stage_obstat(cap)),
-                      ('normalise', lambda: stage_normalise(cap)), ('fitness', lambda: stage_fitness(cap, mode, truth, tie)),
+    for stage, fn in (('draws', lambda: stage_draws(cap)), ('obstat', lambda: stage_obstat(cap, tr() if cap.closed else None)),
+                      ('normalise', lambda: stage_normalise(cap)), ('fitness', lambda: stage_fitness(cap, mode, tr(), tie)),
                       ('novelty', lambda: stage_novelty(cap)),
-                      ('weights', lambda: stage_weights(cap, truth[0], shift_bound, dw_bound)),
+                      ('weights', lambda: stage_weights(cap, None if cap.closed else tr()[0], shift_bound, dw_bound)),
                       ('gradient', lambda: stage_gradient(cap, sm)), ('optimizer', lambda: stage_optimizer(cap))):
         try:
             checks += fn()
@@ -585,6 +767,77 @@ def _m_stale_colsum(c):
     return _copy(c, stats=_stats_with(c, _n_saved(c), old))
 
 
+def _rescored(c: Capture, moo_w: Optional[float] = None) -> Capture:
+    """``c`` with everything after the fitness recomputed correctly from its (mutated) fitness rows: weights, n_ranked,
+    gsum and the Adam step -- so that a modelled bug upstream is rejected by the stage it sits in, not by a mismatch it
+    leaves downstream."""
+    w, n = reference_weights(c, c.fit, moo_w)
+    c2 = _copy(c, weights=w, n_ranked=n, gsum=_gsum_of(c, c.idx, w))
+    return _copy(c2, **_optimizer_after(c2, n_ranked=n))
+
+
+def _m_ep0_noise(c):
+    nz = _np(c.act_noise).reshape(c.K, 2, c.episodes, -1).copy()
+    nz[:, :, 1:] = nz[:, :, :1]
+    tf, tb, _, _ = fitness_truth(c, noise=nz.reshape(c.K, 2, -1))
+    f = c.fit.copy()
+    f[:, :, 0] = tf
+    return _rescored(_copy(c, fit=f, behv=None if c.behv is None else tb.astype(F32)))
+
+
+def _m_episodes_not_divided(c):
+    f = c.fit.copy()
+    f[:, :, 0] *= c.episodes
+    return _rescored(_copy(c, fit=f))
+
+
+def _m_first_episode_behaviour(c):
+    _, tb, _, _ = fitness_truth(c, behaviour_episode=0)
+    return _copy(c, behv=tb.astype(F32))
+
+
+def _m_novelty_over_reward(c):
+    f = np.zeros_like(c.fit)                                            # column 1 never written (the buffer's zeros)
+    f[:, :, 0] = c.fit[:, :, NOVELTY_COLUMN]
+    return _rescored(_copy(c, fit=f))
+
+
+def _m_moo_w_swapped(c):
+    return _rescored(c, moo_w=1 - c.moo_w)                              # w r_novelty + (1 - w) r_reward
+
+
+def _m_archive_clipped(c):
+    """sum of the min(k, A) smallest distances over k."""
+    f = c.fit.copy()
+    a = np.asarray(c.archive, np.float64)
+    for s in range(2):
+        for k in range(c.K):
+            d = np.sqrt(((a - c.behv[s, k, :2].astype(np.float64)[None, :]) ** 2).sum(axis=1))
+            f[s, k, NOVELTY_COLUMN] = float(np.sort(d)[:c.nov_k].sum() / c.nov_k)
+    return _rescored(_copy(c, fit=f))
+
+
+def _closed_saved_sums(c, shift: str = None, drop: int = 0):
+    """Closed loop: the statistics of the saved evaluations from the float64 truth, computed wrongly on purpose:
+    ``shift`` 'pre' sums obs_0 .. obs_{T-1}, 'short' obs_1 .. obs_{T-1} with T - 1 rows each; ``drop`` leaves out that many
+    saved evaluations (the last ones)."""
+    truth = c.extra.get('closed_truth') or closed_truth(c, growth=False)
+    saved = replayed_saves(c)
+    s_idx, j_idx = _truth_columns(truth, saved)
+    if drop:
+        s_idx, j_idx = s_idx[:-drop], j_idx[:-drop]
+    osum, osq = truth['osum'][s_idx, j_idx], truth['osq'][s_idx, j_idx]
+    last = truth['olast'][s_idx, j_idx]
+    rows = c.T
+    o0 = np.asarray(c.obs0, np.float64)[None, :]
+    if shift == 'pre':
+        osum, osq = osum - last + o0, osq - last ** 2 + o0 ** 2
+    elif shift == 'short':
+        osum, osq, rows = osum - last, osq - last ** 2, c.T - 1
+    n = len(s_idx)
+    return _copy(c, stats=np.concatenate([osum.sum(axis=0), osq.sum(axis=0), [float(rows * n), float(n)]]))
+
+
 # name -> (what it models, mutation); each returns a mutated copy of a correct capture
 MUTATIONS = {
     'shift_stream_indices': ("one stream's indices shifted by a pair", _m_shift_stream),
@@ -600,8 +853,22 @@ MUTATIONS = {
     'adam_t': ("Adam's t not advanced", _m_adam_t),
     'std_squared': ('normalisation by std^2', _m_std_squared),
     'stale_colsum': ('a stale column-sum cache from a previous obs stream', _m_stale_colsum),
+    'episode0_noise': ("episode 0's noise reused for every episode", _m_ep0_noise),
+    'episodes_not_divided': ('the episode sum not divided by E', _m_episodes_not_divided),
+    'first_episode_behaviour': ('behaviour taken from the first episode', _m_first_episode_behaviour),
+    'novelty_over_reward': ('novelty written to the reward column', _m_novelty_over_reward),
+    'moo_w_swapped': ('the MultiObjective blend with w and 1 - w swapped', _m_moo_w_swapped),
+    'archive_clipped_to_k': ('novelty averaged over k instead of min(k, A) archive entries', _m_archive_clipped),
+    'closed_obstat_pre_step': ('closed-loop ObStat summed over obs_0 .. obs_{T-1}', lambda c: _closed_saved_sums(c, 'pre')),
+    'closed_count_t_minus_1': ('closed-loop ObStat of T - 1 rows per saved evaluation', lambda c: _closed_saved_sums(c, 'short')),
+    'closed_drop_saved': ('one saved evaluation dropped from the closed-loop ObStat', lambda c: _closed_saved_sums(c, drop=1)),
 }
 NEEDS_ARCHIVE = ('novelty_column', 'novelty_off_by_one')
+# what capture a mutation models a bug of, beyond a plain open-loop one: 'episodes' (E > 1 with action noise), 'nsr'
+# (an archive; 'moo_w_swapped' needs w != 0.5, 'archive_clipped_to_k' fewer entries than k) and 'closed' (the closed loop)
+NEEDS = {'episode0_noise': 'episodes', 'episodes_not_divided': 'episodes', 'first_episode_behaviour': 'episodes',
+         'novelty_over_reward': 'nsr', 'moo_w_swapped': 'nsr', 'archive_clipped_to_k': 'nsr',
+         'closed_obstat_pre_step': 'closed', 'closed_count_t_minus_1': 'closed', 'closed_drop_saved': 'closed'}
 
 
 def rejection(checks: Sequence[Check]):

@@ -37,18 +37,28 @@ def _state(rs):
 
 
 def _capture(variant):
-    archive = np.random.RandomState(17).randn(16, 2) if variant == 'nsra' else None
-    ac_std = 0.01 if variant == 'noise' else 0.0
+    """Variants: 'plain', 'nsra' (16-entry archive, w = 0.5), 'noise' (ac_std 0.01), 'episodes' (E = 3, ac_std 0.01),
+    'nsr' (a 5-entry archive with k = 10, w = 0.25) and 'closed' (the closed-loop env, theta of scale 1 / sqrt(fan_in) as
+    test_gpu_closed_f64's init regime)."""
+    archive = {'nsra': np.random.RandomState(17).randn(16, 2), 'nsr': np.random.RandomState(18).randn(5, 2)}.get(variant)
+    moo_w = {'nsra': 0.5, 'nsr': 0.25}.get(variant)
+    ac_std = 0.01 if variant in ('noise', 'episodes') else 0.0
+    episodes = 3 if variant == 'episodes' else 1
+    closed = variant == 'closed'
     dims = orc.layer_dims(SIZES[0], SIZES[1:-1], SIZES[-1])
     P = orc.n_params(dims)
     rs0 = np.random.RandomState(5)
     table = rs0.randn(P + 20_000).astype(F32)
     theta = (rs0.randn(P) * 0.1).astype(F32)
-    env = orc.SyntheticEnvSpec(SIZES[0], SIZES[-1], T)
+    if closed:
+        theta = np.concatenate([rs0.randn(fi * fo + fo) / np.sqrt(fi) for fi, fo in zip(SIZES[:-1], SIZES[1:])]).astype(F32)
+    # closed loop: the first generation's statistics give std ~0.1, which amplifies the normalised observations ten-fold; at
+    # b_gain 0.1 a 1e-9 move of obs_0 grows 0.6-fold over the episode (at the default 0.5: 1.2e3-fold, chaotic)
+    env = orc.ClosedLoopEnvSpec(SIZES[0], SIZES[-1], T, b_gain=0.1) if closed else orc.SyntheticEnvSpec(SIZES[0], SIZES[-1], T)
     streams = [np.random.RandomState(s) for s in SEEDS]
     opt = orc.AdamOracle(P, LR)
     kw = dict(coins_per_eval=1, rank_states=streams, save_obs_chance=CHANCE, ac_std=ac_std, archive=archive, nov_k=10,
-              moo_w=0.5 if archive is not None else None)
+              moo_w=moo_w, episodes=episodes)
     obmean, obstd = np.zeros(SIZES[0]), np.ones(SIZES[0])
     g1 = orc.generation(table, theta, opt, SIGMA, dims, env, [None] * 3, N_PER, obmean, obstd, 5.0, T, 500, L2, **kw)
     stat = orc.ObStatOracle((SIZES[0],), 1e-2)                   # Policy.update_obstat's running statistics
@@ -74,10 +84,14 @@ def _capture(variant):
     cap = gs.Capture(sizes=SIZES, T=T, sigma=SIGMA, l2coeff=L2, ob_clip=5.0, pos_scale=env.pos_scale, save_obs_chance=CHANCE,
                      ac_std=ac_std, lr=LR, table=torch.from_numpy(table), obs_stream=env.obs_stream, rew_vec=env.rew_vec,
                      theta0=theta0, m0=m0, v0=v0, t0=t0, streams0=streams0, ob_mean=obmean, ob_std=obstd, idx=idx,
-                     coin_words=np.zeros((K, 4), dtype=np.uint32), obsn=orc.normalise_obs(env.obs_stream[:T], obmean, obstd, 5.0),
+                     coin_words=np.zeros((K, 4), dtype=np.uint32),
+                     obsn=None if closed else orc.normalise_obs(env.obs_stream[:T], obmean, obstd, 5.0),
                      fit=np.stack([g2['pos'], g2['neg']]), stats=stats, weights=w, n_ranked=g2['n_ranked'], gsum=gsum,
                      theta1=theta.copy(), m1=opt.m.copy(), v1=opt.v.copy(), t1=opt.t, streams1=[_state(rs) for rs in streams],
-                     behv=behv, archive=archive)
+                     behv=behv, archive=archive, episodes=episodes, **({'moo_w': moo_w} if archive is not None else {}))
+    if closed:
+        cap.obs0, cap.band = env.obs_stream[0].copy(), env.band
+        cap.env_a, cap.env_b = np.ascontiguousarray(env.env_a.T), np.ascontiguousarray(env.env_b.T)
     # the coin words and the action noise: the streams' draws between the indices, in the order the oracle consumed them
     noise = []
     for r in range(len(SEEDS)):
@@ -103,7 +117,7 @@ def _judge(cap):
     return gs.judge(cap, MODE_F32, rc.H100_SMS, SHIFT_BOUND, DW_BOUND, tie=list(range(cap.K)))
 
 
-@pytest.mark.parametrize('variant', ['plain', 'nsra', 'noise'])
+@pytest.mark.parametrize('variant', ['plain', 'nsra', 'noise', 'episodes', 'nsr', 'closed'])
 def test_judge_passes_the_oracle_generation(variant):
     cap = _cap(variant)
     checks = _judge(cap)
@@ -111,12 +125,19 @@ def test_judge_passes_the_oracle_generation(variant):
     gs.assert_ok(checks)
     assert cap.extra['n_saved'] > 0 and cap.t0 == 1
     assert not np.array_equal(cap.ob_std, np.ones_like(cap.ob_std))
+    if variant == 'closed':                       # every saved evaluation in the truth's sample, the whole population here
+        assert len(cap.extra['closed_truth']['pairs']) == cap.K and cap.extra['ranks_vs_truth'].startswith('not compared')
+
+
+def _variant(name):
+    """The capture a modelled bug is judged on: the 'nsr' capture has w = 0.25 and 5 archive entries for k = 10."""
+    return gs.NEEDS.get(name, 'nsra' if name in gs.NEEDS_ARCHIVE else 'plain')
 
 
 @pytest.mark.parametrize('name', sorted(gs.MUTATIONS))
 def test_judge_rejects_modelled_bugs(name):
     what, mutate = gs.MUTATIONS[name]
-    cap = _cap('nsra' if name in gs.NEEDS_ARCHIVE else 'plain')
+    cap = _cap(_variant(name))
     checks = _judge(mutate(cap))
     stages, margin = gs.rejection(checks)
     print(f'\n{name} ({what}): rejected by {stages}, margin {margin:.3g}x')
