@@ -217,19 +217,31 @@ int es_obstat_accumulate_coins(es_ctx* ctx, double* sum, double* sumsq, double* 
                                            n_coins, chance, (cudaStream_t)stream);
 }
 
-// the checks the open- and closed-loop rollouts share; `ptrs`: the entry point's own pointers are set
-static int es_rollout_check(const char* fn, bool ptrs, const EsRollout& r) {
-    ES_REQUIRE(ptrs && r.table && r.idx && r.theta && r.layer_sizes && r.rew_vec && r.fit_pos && r.fit_neg, "%s: NULL pointer", fn);
+// the checks the open- and closed-loop rollouts share (`ptrs`: the entry point's own pointers are set), then the call's shape
+// from the caller's layer sizes into r
+static int es_rollout_check(const char* fn, bool ptrs, const int* layer_sizes, EsRollout& r) {
+    ES_REQUIRE(ptrs && r.table && r.idx && r.theta && layer_sizes && r.rew_vec && r.fit_pos && r.fit_neg, "%s: NULL pointer", fn);
     ES_REQUIRE(r.n_layers >= 1 && r.n_layers <= ES_MAX_LAYERS, "%s: n_layers must be in [1,%d]", fn, ES_MAX_LAYERS);
     ES_REQUIRE(r.n_pairs >= 0 && r.T >= 1 && r.fit_stride >= 1, "%s: bad sizes", fn);
     ES_REQUIRE((r.behv_pos == nullptr) == (r.behv_neg == nullptr), "%s: behv_pos/behv_neg must both be set or NULL", fn);
     int64_t count = 0;
     for (int l = 0; l < r.n_layers; ++l) {
-        ES_REQUIRE(r.layer_sizes[l] > 0 && r.layer_sizes[l + 1] > 0, "%s: layer size <= 0", fn);
-        count += (int64_t)r.layer_sizes[l] * r.layer_sizes[l + 1] + r.layer_sizes[l + 1];
+        ES_REQUIRE(layer_sizes[l] > 0 && layer_sizes[l + 1] > 0, "%s: layer size <= 0", fn);
+        count += (int64_t)layer_sizes[l] * layer_sizes[l + 1] + layer_sizes[l + 1];
     }
     ES_REQUIRE(count == r.P, "%s: layer sizes give %lld params, P=%d", fn, (long long)count, r.P);
     ES_REQUIRE(r.table_len > r.P, "%s: table smaller than the network", fn);
+    r.dims[0] = layer_sizes[0];
+    int at = 0;
+    for (int l = 0; l < r.n_layers; ++l) {             // state-dict order (src/core/policy.py:33-35)
+        r.dims[l + 1] = layer_sizes[l + 1];
+        r.w_off[l] = at; at += r.dims[l] * r.dims[l + 1];
+        r.b_off[l] = at; at += r.dims[l + 1];
+    }
+    // (a binned head with bins < 2 is refused by es_binned_check before any kernel runs)
+    const int out = r.dims[r.n_layers];
+    r.act = r.bins ? out / r.bins : out;
+    r.head_scale = r.bins ? (float)(1.0 / (r.bins - 1.0)) : 0.f;
     return ES_OK;
 }
 
@@ -238,7 +250,7 @@ static int es_rollout_check(const char* fn, bool ptrs, const EsRollout& r) {
 static int es_binned_check(const char* fn, const EsRollout& r) {
     ES_REQUIRE(r.bins >= 2, "%s: bins must be >= 2 (the action is idx / (bins - 1)), got %d", fn, r.bins);
     ES_REQUIRE(r.head_low && r.head_range, "%s: NULL low / range", fn);
-    const int out = r.layer_sizes[r.n_layers];
+    const int out = r.dims[r.n_layers];
     ES_REQUIRE(out % r.bins == 0, "%s: the last layer's %d outputs are not adim * bins for bins %d", fn, out, r.bins);
     if (out > 256) {
         es_set_error("%s: binned heads up to adim * bins = 256 outputs supported, got %d * %d", fn, out / r.bins, r.bins);
@@ -252,8 +264,8 @@ static int es_binned_check(const char* fn, const EsRollout& r) {
 enum EsHead { ES_HEAD_TANH, ES_HEAD_BINNED, ES_HEAD_TANH_ONE_CTA };
 
 // an open-loop entry point after ES_ENTER: its checks in order, then the mode's kernel; `fn` names it in every message
-static int es_openloop(es_ctx* ctx, const char* fn, const EsRollout& r, EsHead head, int mode, cudaStream_t stream) {
-    int rc = es_rollout_check(fn, r.obsn != nullptr, r);
+static int es_openloop(es_ctx* ctx, const char* fn, EsRollout r, const int* layer_sizes, EsHead head, int mode, cudaStream_t stream) {
+    int rc = es_rollout_check(fn, r.obsn != nullptr, layer_sizes, r);
     if (rc) return rc;
     if (head == ES_HEAD_BINNED) {
         rc = es_binned_check(fn, r);
@@ -264,7 +276,7 @@ static int es_openloop(es_ctx* ctx, const char* fn, const EsRollout& r, EsHead h
             return ES_ERR_UNSUPPORTED;
         }
         if (mode == ES_ROLLOUT_TC3 && !es_tcw_covers_binned(r)) {
-            const int* dims = r.layer_sizes;
+            const int* dims = r.dims;
             char why[96];                               // the part of the shape outside the coverage
             if (r.n_layers < 3 || r.n_layers > 5) {
                 snprintf(why, sizeof why, "%d hidden layers", r.n_layers - 1);
@@ -305,9 +317,9 @@ int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_
     ES_REQUIRE(n_episodes >= 1, "es_rollout_openloop: n_episodes must be >= 1, got %d", n_episodes);
     // without action noise the episodes are identical and their mean is exactly the one episode (E copies of a float32 value
     // sum exactly in float64, and (E r) / E == r)
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, obsn, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
-    return es_openloop(ctx, "es_rollout_openloop", r, ES_HEAD_TANH, mode, (cudaStream_t)stream);
+    return es_openloop(ctx, "es_rollout_openloop", r, layer_sizes, ES_HEAD_TANH, mode, (cudaStream_t)stream);
 }
 
 int es_rollout_openloop_noisy(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
@@ -332,9 +344,9 @@ int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_le
                                float* behv_pos, float* behv_neg, int bins, const float* low, const float* range, int mode,
                                void* stream) {
     ES_ENTER(ctx);
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec, T, pos_scale,
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, obsn, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
-    return es_openloop(ctx, "es_rollout_openloop_binned", r, ES_HEAD_BINNED, mode, (cudaStream_t)stream);
+    return es_openloop(ctx, "es_rollout_openloop_binned", r, layer_sizes, ES_HEAD_BINNED, mode, (cudaStream_t)stream);
 }
 
 // the shapes es_rollout_closedloop's one-CTA kernel (rollout_closed.cu) covers: two hidden layers <= 64, act <= 64, obs <= 384
@@ -345,23 +357,24 @@ static bool es_closed_one_cta_covers(const int* dims, int n_layers) {
 // a closed-loop entry point after ES_ENTER: its checks in order (the cluster plan refuses a shape whatever n_pairs is;
 // rollout_closed.cu checks its own coverage when it runs), the scratch rows of E > 1 episodes, then the kernel; `fn` names it in
 // every message
-static int es_closedloop(es_ctx* ctx, const char* fn, const EsRollout& r, EsClosedEnv env, EsHead head, cudaStream_t stream) {
-    int rc = es_rollout_check(fn, env.ob_mean && env.ob_std && env.obs0 && env.env_a && env.env_b, r);
+static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* layer_sizes, EsClosedEnv env, EsHead head,
+                         cudaStream_t stream) {
+    int rc = es_rollout_check(fn, env.ob_mean && env.ob_std && env.obs0 && env.env_a && env.env_b, layer_sizes, r);
     if (rc) return rc;
     if (head == ES_HEAD_TANH_ONE_CTA && r.n_layers != 3) {
         es_set_error("%s: two hidden layers (n_layers == 3) supported, got %d", fn, r.n_layers);
         return ES_ERR_UNSUPPORTED;
     }
-    ES_REQUIRE(env.band >= 1 && env.band <= r.layer_sizes[0], "%s: band must be in [1, obs_dim]", fn);
+    ES_REQUIRE(env.band >= 1 && env.band <= r.dims[0], "%s: band must be in [1, obs_dim]", fn);
     ES_REQUIRE((env.ob_sum == nullptr) == (env.ob_sumsq == nullptr) && (env.ob_sum == nullptr) == (env.ob_count == nullptr),
                "%s: ob_sum/ob_sumsq/ob_count must all be set or NULL", fn);
     int C = 0;
     size_t smem = 0;
     if (head == ES_HEAD_BINNED) {
         rc = es_binned_check(fn, r);
-        if (!rc) rc = es_closedw_binned_plan(r.layer_sizes, r.n_layers, env.band, r.bins, &C, &smem);
+        if (!rc) rc = es_closedw_binned_plan(r.dims, r.n_layers, env.band, r.bins, &C, &smem);
     } else if (head == ES_HEAD_TANH) {
-        rc = es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
+        rc = es_closedw_plan(r.dims, r.n_layers, env.band, &C, &smem);
     }
     if (rc) return rc;
     if (r.n_pairs == 0) return ES_OK;
@@ -371,7 +384,7 @@ static int es_closedloop(es_ctx* ctx, const char* fn, const EsRollout& r, EsClos
         if (rc) return rc;
         env.ep_rows = (double*)rows;
     }
-    if (head == ES_HEAD_TANH_ONE_CTA || (head == ES_HEAD_TANH && es_closed_one_cta_covers(r.layer_sizes, r.n_layers)))
+    if (head == ES_HEAD_TANH_ONE_CTA || (head == ES_HEAD_TANH && es_closed_one_cta_covers(r.dims, r.n_layers)))
         return es_impl_rollout_closed(ctx, r, env, stream);
     return es_impl_rollout_closedw(ctx, r, env, stream);
 }
@@ -383,10 +396,10 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
                           double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
                           double* ob_count, void* stream) {
     ES_ENTER(ctx);
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, nullptr, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    return es_closedloop(ctx, "es_rollout_closedloop", r, env, ES_HEAD_TANH_ONE_CTA, (cudaStream_t)stream);
+    return es_closedloop(ctx, "es_rollout_closedloop", r, layer_sizes, env, ES_HEAD_TANH_ONE_CTA, (cudaStream_t)stream);
 }
 
 // both plan entry points after ES_ENTER (`bins`: a binned head's, 0 for a tanh head)
@@ -428,10 +441,10 @@ int es_rollout_closedloop_mlp_episodes(es_ctx* ctx, const float* table, int64_t 
     ES_ENTER(ctx);
     ES_REQUIRE(n_episodes >= 1, "es_rollout_closedloop_mlp: n_episodes must be >= 1, got %d", n_episodes);
     // without action noise the episodes are identical: the noise-free kernels run one (as es_rollout_openloop_episodes)
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, nullptr, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    return es_closedloop(ctx, "es_rollout_closedloop_mlp", r, env, ES_HEAD_TANH, (cudaStream_t)stream);
+    return es_closedloop(ctx, "es_rollout_closedloop_mlp", r, layer_sizes, env, ES_HEAD_TANH, (cudaStream_t)stream);
 }
 
 int es_rollout_closedloop_mlp(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
@@ -461,10 +474,10 @@ int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t ta
                                      float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins, const float* low,
                                      const float* range, void* stream) {
     ES_ENTER(ctx);
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, nullptr, rew_vec, T, pos_scale,
+    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, nullptr, rew_vec, T, pos_scale,
                          fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    return es_closedloop(ctx, "es_rollout_closedloop_mlp_binned", r, env, ES_HEAD_BINNED, (cudaStream_t)stream);
+    return es_closedloop(ctx, "es_rollout_closedloop_mlp_binned", r, layer_sizes, env, ES_HEAD_BINNED, (cudaStream_t)stream);
 }
 
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,

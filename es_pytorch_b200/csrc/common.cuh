@@ -82,7 +82,7 @@ __host__ __device__ inline EsMlpOffsets es_mlp_offsets(int obs, int h1, int h2, 
     return o;
 }
 
-// one rollout call of the antithetic pairs idx[0 .. n_pairs), validated by api.cu
+// one rollout call of the antithetic pairs idx[0 .. n_pairs), validated and completed by api.cu; the kernels take it by value
 struct EsRollout {
     const float* table;
     int64_t table_len;
@@ -91,7 +91,6 @@ struct EsRollout {
     const float* theta;
     int P;
     float sigma;
-    const int* layer_sizes;     // [n_layers + 1]
     int n_layers;
     const float* obsn;          // open loop: normalised observations [T][obs]
     const float* rew_vec;       // [T][act]
@@ -110,7 +109,25 @@ struct EsRollout {
     int bins;
     const float* head_low;      // dev float [adim]
     const float* head_range;    // dev float [adim]
+    // filled by api.cu from the caller's layer sizes once they are checked
+    int dims[ES_MAX_LAYERS + 1];                        // obs, hidden..., the last layer's outputs
+    int w_off[ES_MAX_LAYERS], b_off[ES_MAX_LAYERS];     // flat offsets of W_l [dims[l+1]][dims[l]] and b_l, state-dict order
+    int act;                    // the env's action dimension: dims[n_layers], or adim = dims[n_layers] / bins
+    float head_scale;           // a binned head's float32(1 / (bins - 1))
 };
+
+// the call restricted to the pairs [p0, p0 + np)
+static inline EsRollout es_rollout_rows(const EsRollout& r, int p0, int np) {
+    EsRollout c = r;
+    c.idx += p0;
+    c.n_pairs = np;
+    c.fit_pos += (size_t)p0 * r.fit_stride;
+    c.fit_neg += (size_t)p0 * r.fit_stride;
+    if (r.behv_pos) { c.behv_pos += (size_t)p0 * 3; c.behv_neg += (size_t)p0 * 3; }
+    if (r.act_noise) c.act_noise += (size_t)p0 * 2 * r.n_episodes * r.T * r.act;
+    return c;
+}
+
 // the closed-loop env, the observation normalisation and the ObStat increments of es_rollout_closedloop
 struct EsClosedEnv {
     const double* ob_mean;
@@ -165,8 +182,7 @@ int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaS
 // binned heads (EsRollout::bins >= 2): every shape es_closedw_plan covers with act = adim; the cluster kernel at every C
 int es_closedw_binned_plan(const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes);
 // U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
-int es_launch_ubase(es_ctx*, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
-                    float* ubase, cudaStream_t);
+int es_launch_ubase(es_ctx*, const EsRollout&, int n_tiles, float* ubase, cudaStream_t);
 int es_impl_novelty(es_ctx*, const float*, int, const double*, int, int, double*, int, cudaStream_t);
 int es_impl_fitness_objective(es_ctx*, int, double*, int, const float*, int, int, cudaStream_t);
 int es_impl_rank_transform(es_ctx*, const double*, const double*, int, int, int, double, double, int, int, int,
@@ -233,5 +249,33 @@ __device__ __forceinline__ float es_hsum2(es_f32x2 v) {
     float a, b;
     es_unpack2(v, a, b);
     return a + b;
+}
+// the action of dimension j of a binned-action policy (FFBinned, src/nn/nn.py:99-117) from its bins outputs out(0 .. bins - 1):
+// the first maximal bin, as torch.argmax (a NaN counts as the maximum), mapped to (scale * idx) * range[j] + low[j] with every
+// operation rounded to float32 as the reference's torch expression does
+template <typename Out>
+__device__ __forceinline__ float es_binned_action(int bins, float scale, const float* low, const float* range, int j, Out out) {
+    int best = 0;
+    float bv = out(0);
+    for (int b = 1; b < bins && bv == bv; ++b) {
+        const float v = out(b);
+        if (v > bv || v != v) { bv = v; best = b; }
+    }
+    return __fadd_rn(__fmul_rn(__fmul_rn(scale, (float)best), __ldg(range + j)), __ldg(low + j));
+}
+// tanh(x) = 1 - 2 / (1 + e^2x) with the fast exponential and division: absolute error ~1e-7 (tanhf is ~40 dependent
+// instructions per call); the closed-loop kernels end every phase of a step in one
+__device__ __forceinline__ float es_tanh_exp(float x) {
+    const float e = __expf(2.f * x);
+    return 1.f - __fdividef(2.f, 1.f + e);
+}
+// raw observation i of the closed-loop env into a buffer with a wrap-around halo of the band (band <= obs): slot q = k + band / 2
+// holds observation k mod obs for k in [-band / 2, obs + band - band / 2), so the band around any i is a linear read
+template <typename V>
+__device__ __forceinline__ void es_put_obs(V* __restrict__ buf, int i, V v, int obs, int band) {
+    const int half = band >> 1;
+    buf[i + half] = v;
+    if (i >= obs - half) buf[i - obs + half] = v;
+    if (i < band - half) buf[i + obs + half] = v;
 }
 #endif

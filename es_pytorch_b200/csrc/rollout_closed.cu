@@ -90,12 +90,6 @@ __device__ __forceinline__ float cl_normalise(float o, double mean, double rstd,
     x = fmin(fmax(x, -clip), clip);
     return (float)x;
 }
-// tanh(x) = 1 - 2 / (1 + e^2x) with the fast exponential and division: absolute error ~1e-7 (tanhf is ~40 dependent
-// instructions per call, and every phase of a step ends in one)
-__device__ __forceinline__ float cl_tanh(float x) {
-    const float e = __expf(2.f * x);
-    return 1.f - __fdividef(2.f, 1.f + e);
-}
 // the float32 pairs (es_f32x2) of this kernel hold (+, -) of a weight times (x+, x-) of an input
 // the four rows of a warp: z[r] (+, -) -> tanh(z + bias) of row 4 w + r, written by the lane that ends up with that sum
 // (lanes 4 q: row 4 w + q / 2, sign q & 1); NZ: plus that lane's action noise nz
@@ -108,8 +102,8 @@ __device__ __forceinline__ void cl_finish_rows(const es_f32x2 (&z)[4], int warp,
     const float c = es_warp_sum8(v, lane);
     if ((lane & 3) == 0) {
         const int q = lane >> 2, o = 4 * warp + (q >> 1), sg = q & 1;
-        out2[2 * o + sg] = (o < rows) ? (NZ ? __fadd_rn(cl_tanh(c + (sg ? bias_m : bias_p)[o]), nz)
-                                            : cl_tanh(c + (sg ? bias_m : bias_p)[o])) : 0.f;
+        out2[2 * o + sg] = (o < rows) ? (NZ ? __fadd_rn(es_tanh_exp(c + (sg ? bias_m : bias_p)[o]), nz)
+                                            : es_tanh_exp(c + (sg ? bias_m : bias_p)[o])) : 0.f;
     }
 }
 
@@ -135,7 +129,7 @@ __device__ __forceinline__ void cl_rollout(const ClParams& p) {
     float4* __restrict__ stat = reinterpret_cast<float4*>(cl_smem + L.stat);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int obs = p.obs, h1 = p.h1, h2 = p.h2, act = p.act, T = p.T, band = p.band, half = p.band >> 1;
+    const int obs = p.obs, h1 = p.h1, h2 = p.h2, act = p.act, T = p.T, band = p.band;
     const int act_pad = L.act_pad, o2s = L.o2_stride;
     const EsMlpOffsets off = es_mlp_offsets(obs, h1, h2, act);
     const bool l3_warp = 4 * warp < act;                        // warps that hold rows of layer 3
@@ -148,13 +142,6 @@ __device__ __forceinline__ void cl_rollout(const ClParams& p) {
     for (int i = tid; i < CL_A; i += CL_THREADS) a2[i] = make_float2(0.f, 0.f);
     for (int i = tid; i < obs; i += CL_THREADS) { nmean[i] = p.ob_mean[i]; nrstd[i] = 1.0 / p.ob_std[i]; }
     __syncthreads();
-
-    // a raw observation and its halo copies: slot q = k + half for k in [-half, obs + band - half)
-    auto put_obs = [&](float2* __restrict__ buf, int i, float2 v) {
-        buf[i + half] = v;
-        if (i >= obs - half) buf[i - obs + half] = v;
-        if (i < band - half) buf[i + obs + half] = v;
-    };
 
     for (int pair = blockIdx.x; pair < p.n_pairs; pair += gridDim.x) {
         const long long base = es_checked_slice(p.idx[pair], p.n_params, p.table_len, p.err);
@@ -197,7 +184,7 @@ __device__ __forceinline__ void cl_rollout(const ClParams& p) {
         auto start_episode = [&]() {                                // a fresh env: obs_0, position 0
             for (int i = tid; i < obs; i += CL_THREADS) {
                 const float v = p.obs0[i];
-                put_obs(o2, i, make_float2(v, v));
+                es_put_obs(o2, i, make_float2(v, v), obs, band);
                 const float xn = cl_normalise(v, nmean[i], nrstd[i], p.ob_clip);
                 x2[i] = make_float2(xn, xn);
                 stat[i] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -308,8 +295,8 @@ __device__ __forceinline__ void cl_rollout(const ClParams& p) {
                         ap = fmaf(w0, av.x, ap); am = fmaf(w0, av.y, am);
                         ap1 = fmaf(w1_, av.z, ap1); am1 = fmaf(w1_, av.w, am1);
                     }
-                    const float np_ = cl_tanh(ap + ap1), nm = cl_tanh(am + am1);
-                    put_obs(o2 + (cur ^ 1) * o2s, i, make_float2(np_, nm));
+                    const float np_ = es_tanh_exp(ap + ap1), nm = es_tanh_exp(am + am1);
+                    es_put_obs(o2 + (cur ^ 1) * o2s, i, make_float2(np_, nm), obs, band);
                     const double mu = nmean[i], rs_ = nrstd[i];
                     x2[i] = make_float2(cl_normalise(np_, mu, rs_, p.ob_clip), cl_normalise(nm, mu, rs_, p.ob_clip));
                     if (add_stat) {                                     // float32 column sums in step order (numpy's axis-0 reduction)
@@ -402,7 +389,7 @@ int cl_launch(es_ctx* ctx, const ClParams& p, cudaStream_t stream) {
 }  // namespace
 
 int es_impl_rollout_closed(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {
-    const int* dims = r.layer_sizes;
+    const int* dims = r.dims;
     ClParams p;
     p.table = r.table; p.table_len = r.table_len; p.idx = r.idx; p.n_pairs = r.n_pairs; p.theta = r.theta; p.sigma = r.sigma;
     p.obs = dims[0]; p.h1 = dims[1]; p.h2 = dims[2]; p.act = dims[3]; p.T = r.T; p.n_params = r.P;
@@ -412,7 +399,7 @@ int es_impl_rollout_closed(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& e
     p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.fit_stride = r.fit_stride; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
     p.ob_sum = env.ob_sum; p.ob_sumsq = env.ob_sumsq; p.ob_count = env.ob_count;
     p.err = r.err;
-    p.act_noise = r.act_noise; p.n_eps = r.act_noise ? r.n_episodes : 1; p.ep_row = env.ep_rows;
+    p.act_noise = r.act_noise; p.n_eps = r.n_episodes; p.ep_row = env.ep_rows;
     if (p.h1 > CL_H || p.h2 > CL_H || p.act > CL_A || p.obs > 384 || p.band > CL_HALO || p.obs < p.band || (p.band & 1)) {
         es_set_error("es_rollout_closedloop: supports even band <= obs <= 384, hidden <= %d, act <= %d, band <= %d (got %d-%d-%d-%d, band %d)",
                      CL_H, CL_A, CL_HALO, p.obs, p.h1, p.h2, p.act, p.band);

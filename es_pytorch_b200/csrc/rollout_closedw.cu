@@ -4,7 +4,7 @@
 //
 // Semantics are rollout_closed.cu's: theta +- sigma eps through es_pheno_pm (slices checked by es_checked_slice and the ctx's
 // error word), clip((o - mean) / std) in float64 (here an exact float64 division, as the reference), Linear + tanh after every
-// layer including the output (the same fast tanh as rollout_closed.cu, cw_tanh: absolute error ~1e-7), the reward as a
+// layer including the output (the same fast tanh as rollout_closed.cu, es_tanh_exp: absolute error ~1e-7), the reward as a
 // float32 dot in index order summed in float64 in step order, the position integrator, behaviour outputs with fit_stride, and
 // the ObStat increments (float32 column sums in step order, added in float64) of evaluations whose save_obs coin fell.  The env
 // step is the oracle's arithmetic exactly: one float32 accumulator, A's diagonals then B's columns in index order, every product
@@ -74,22 +74,8 @@ constexpr int CW_HALO = 16;                // band <= 16
 constexpr int CW_SMEM_MAX = 227 * 1024 - 1024;    // dynamic shared memory per CTA: 227 KiB less 1 KiB for the static cw_layers
 
 struct CwParams {
-    const float* table; long long table_len; const int64_t* idx; int n_pairs;
-    const float* theta; float sigma;
-    int n_layers, T, n_params;
-    int dims[CW_MAX_LAYERS + 1];
-    int woff[CW_MAX_LAYERS], boff[CW_MAX_LAYERS];     // flat offsets of W_l [d_{l+1}][d_l] and b_l
-    const double* ob_mean; const double* ob_std; double ob_clip;
-    const float* obs0; const float* env_a; const float* env_b; int band;
-    const float* crew; float pos_scale;
-    const uint32_t* coins; double chance;
-    double* fit_pos; double* fit_neg; int fit_stride;
-    float* behv_pos; float* behv_neg;
-    double* ob_sum; double* ob_sumsq; double* ob_count;
-    int* err;
-    int adim, bins; float scale; const float* low; const float* range;      // binned head (rollout_closedw_binned_kernel only)
-    const float* act_noise; int n_eps;      // [n_pairs][2][n_eps][T][act] (rollout_closedw_noisy_kernel only)
-    double* ep_row;                         // [clusters][T] per-step episode sums (n_eps > 1)
+    EsRollout r;
+    EsClosedEnv env;                        // ep_rows: [clusters][T] per-step episode sums (n_episodes > 1)
 };
 
 __host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
@@ -132,11 +118,6 @@ __device__ __forceinline__ float cw_normalise(float o, double mean, double std, 
     double x = ((double)o - mean) / std;
     x = fmin(fmax(x, -clip), clip);
     return (float)x;
-}
-// rollout_closed.cu's cl_tanh: tanh(x) = 1 - 2 / (1 + e^2x) with the fast exponential and division, absolute error ~1e-7
-__device__ __forceinline__ float cw_tanh(float x) {
-    const float e = __expf(2.f * x);
-    return 1.f - __fdividef(2.f, 1.f + e);
 }
 // the warp-wide sums of v[0..3] in 7 shuffles (transposing butterfly, the xor-16, 8, 4, 2, 1 tree for every row): lane L
 // returns the sum over the lanes of v[L / 8]
@@ -182,8 +163,8 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
     __shared__ CwLayer cw_layers[NL];
     const unsigned C = cw_cluster_nctas(), rank = cw_cluster_rank();
     const int n_clusters = gridDim.x / C, cluster = blockIdx.x / C;
-    const int obs = p.dims[0], act = BINNED ? p.adim : p.dims[NL], T = p.T, band = p.band, half = p.band >> 1;
-    const CwLayout L = BINNED ? cw_layout(NL, p.dims, (int)C, band, act, true) : cw_layout(NL, p.dims, (int)C, band);
+    const int obs = p.r.dims[0], act = p.r.act, T = p.r.T, band = p.env.band;
+    const CwLayout L = BINNED ? cw_layout(NL, p.r.dims, (int)C, band, act, true) : cw_layout(NL, p.r.dims, (int)C, band);
     double* __restrict__ nmean = reinterpret_cast<double*>(cw_smem + L.norm);
     double* __restrict__ nstd = nmean + obs;
     double* __restrict__ rfit = reinterpret_cast<double*>(cw_smem + L.racc);
@@ -199,32 +180,26 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const bool rew_warp = rank == 0 && warp == CW_WARPS - 1;
 
-    for (int i = tid; i < band * obs; i += CW_THREADS) cw_smem[L.env_a + i] = p.env_a[i];
-    for (int i = tid; i < act * obs; i += CW_THREADS) cw_smem[L.env_b + i] = p.env_b[i];
-    for (int i = tid; i < obs; i += CW_THREADS) { nmean[i] = p.ob_mean[i]; nstd[i] = p.ob_std[i]; }
+    for (int i = tid; i < band * obs; i += CW_THREADS) cw_smem[L.env_a + i] = p.env.env_a[i];
+    for (int i = tid; i < act * obs; i += CW_THREADS) cw_smem[L.env_b + i] = p.env.env_b[i];
+    for (int i = tid; i < obs; i += CW_THREADS) { nmean[i] = p.env.ob_mean[i]; nstd[i] = p.env.ob_std[i]; }
     for (int i = tid; i < L.w[0] - L.x; i += CW_THREADS) cw_smem[L.x + i] = 0.f;     // x and every a_l, padding included
     if (tid == 0) {
 #pragma unroll
         for (int l = 0; l < NL; ++l) {                      // this CTA owns rows [r0, r0 + nr) of layer l (nr may be <= 0)
             const int r0 = (int)rank * L.rows[l];
-            cw_layers[l] = {p.dims[l], min(L.rows[l], p.dims[l + 1] - r0), L.stride[l], r0, L.w[l], L.bias[l],
-                            l ? L.act[l - 1] : L.x, L.act[l], p.woff[l], p.boff[l]};
+            cw_layers[l] = {p.r.dims[l], min(L.rows[l], p.r.dims[l + 1] - r0), L.stride[l], r0, L.w[l], L.bias[l],
+                            l ? L.act[l - 1] : L.x, L.act[l], p.r.w_off[l], p.r.b_off[l]};
         }
     }
     cw_cluster_sync();                                      // START: every CTA of the cluster runs and has zeroed its buffers
 
-    auto put_obs = [&](float* __restrict__ buf, int i, float v) {   // slot q = k + half for k in [-half, obs + band - half)
-        buf[i + half] = v;
-        if (i >= obs - half) buf[i - obs + half] = v;
-        if (i < band - half) buf[i + obs + half] = v;
-    };
-
-    for (int ev = cluster; ev < 2 * p.n_pairs; ev += n_clusters) {
+    for (int ev = cluster; ev < 2 * p.r.n_pairs; ev += n_clusters) {
         const int pair = ev >> 1, neg = ev & 1;
-        const long long base = es_checked_slice(p.idx[pair], p.n_params, p.table_len, p.err);
-        const float* __restrict__ eps = p.table + base;
-        const float* __restrict__ th = p.theta;
-        const float sg = p.sigma;
+        const long long base = es_checked_slice(p.r.idx[pair], p.r.P, p.r.table_len, p.r.err);
+        const float* __restrict__ eps = p.r.table + base;
+        const float* __restrict__ th = p.r.theta;
+        const float sg = p.r.sigma;
         auto w_at = [&](int at) {                           // theta + sigma eps or theta - sigma eps
             float wp, wm;
             es_pheno_pm(sg, eps[at], th[at], wp, wm);
@@ -242,23 +217,23 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
         }
         auto start_episode = [&]() {                        // a fresh env: obs_0, position 0
             for (int i = tid; i < obs; i += CW_THREADS) {
-                const float v = p.obs0[i];
-                put_obs(o2, i, v);
-                x[i] = cw_normalise(v, nmean[i], nstd[i], p.ob_clip);
+                const float v = p.env.obs0[i];
+                es_put_obs(o2, i, v, obs, band);
+                x[i] = cw_normalise(v, nmean[i], nstd[i], p.env.ob_clip);
                 stat[i] = make_float2(0.f, 0.f);
             }
         };
         start_episode();
         if (tid == 0) { rfit[0] = 0.0; rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
         bool save = false;                                  // the evaluation's save_obs coin (legacy random_sample < chance)
-        if (p.coins) {
-            const uint32_t* c = p.coins + (size_t)pair * 4 + 2 * neg;
-            save = mt19937_random_sample(c[0], c[1]) < p.chance;
+        if (p.env.coins) {
+            const uint32_t* c = p.env.coins + (size_t)pair * 4 + 2 * neg;
+            save = mt19937_random_sample(c[0], c[1]) < p.env.save_obs_chance;
         }
-        const bool keep_stat = rank == 0 && p.ob_sum && save;
+        const bool keep_stat = rank == 0 && p.env.ob_sum && save;
         __syncthreads();
 
-        const int n_eps = NOISY ? p.n_eps : 1;
+        const int n_eps = NOISY ? p.r.n_episodes : 1;
         for (int ep = 0; ep < n_eps; ++ep) {
             const bool last_ep = ep == n_eps - 1;
             const bool add_stat = keep_stat && last_ep;     // behaviour and ObStat: the last episode's
@@ -270,12 +245,12 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
 
             // this cluster's episode sums, and the noise of the output row this lane owns (row 4 warp + lane / 8 of the last
             // layer's pass, lanes 8 i)
-            double* __restrict__ erow = NOISY ? p.ep_row + (size_t)cluster * T : nullptr;
+            double* __restrict__ erow = NOISY ? p.env.ep_rows + (size_t)cluster * T : nullptr;
             const float* __restrict__ nzp = nullptr;
             if (NOISY && (lane & 7) == 0) {
                 const CwLayer& lo = cw_layers[NL - 1];
                 const int r = 4 * warp + (lane >> 3);
-                if (r < lo.nr) nzp = p.act_noise + (((size_t)pair * 2 + neg) * n_eps + ep) * T * act + lo.r0 + r;
+                if (r < lo.nr) nzp = p.r.act_noise + (((size_t)pair * 2 + neg) * n_eps + ep) * T * act + lo.r0 + r;
             }
 
             for (int t = 0; t < T; ++t) {
@@ -283,7 +258,7 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                 float crow0 = 0.f, crow1 = 0.f;
                 double esum = 0.0;                              // the earlier episodes' rewards of this step
                 if (rew_warp) {                                 // this step's reward coefficients: in flight under the layers
-                    const float* __restrict__ c = p.crew + (size_t)t * act;
+                    const float* __restrict__ c = p.r.rew_vec + (size_t)t * act;
                     if (lane < act) crow0 = __ldg(c + lane);
                     if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
                     if (NOISY && lane == 0 && ep > 0) esum = erow[t];
@@ -311,7 +286,7 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                         const float s = cw_warp_sum4(z, lane);
                         const int r = g + (lane >> 3);
                         if ((lane & 7) == 0 && r < nr) {
-                            const float y = (NOISY && l == NL - 1) ? __fadd_rn(cw_tanh(s + bias[r]), nz) : cw_tanh(s + bias[r]);
+                            const float y = (NOISY && l == NL - 1) ? __fadd_rn(es_tanh_exp(s + bias[r]), nz) : es_tanh_exp(s + bias[r]);
                             for (unsigned q = 0; q < C; ++q) cw_store_remote(out + r0 + r, q, y);
                         }
                     }
@@ -319,15 +294,9 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                 }
                 if (BINNED) {                                   // the actions from this CTA's copy of the last layer's outputs
                     if (tid < act) {
-                        const float* __restrict__ o = cw_smem + L.act[NL - 1] + tid * p.bins;
-                        int best = 0;
-                        float bv = o[0];
-                        for (int b = 1; b < p.bins && bv == bv; ++b) {      // first maximal bin; a NaN counts as the maximum
-                            const float v = o[b];
-                            if (v > bv || v != v) { bv = v; best = b; }
-                        }
-                        cw_smem[L.abin + tid] = __fadd_rn(__fmul_rn(__fmul_rn(p.scale, (float)best), __ldg(p.range + tid)),
-                                                          __ldg(p.low + tid));
+                        const float* __restrict__ o = cw_smem + L.act[NL - 1] + tid * p.r.bins;
+                        cw_smem[L.abin + tid] = es_binned_action(p.r.bins, p.r.head_scale, p.r.head_low, p.r.head_range, tid,
+                                                                 [&](int b) { return o[b]; });
                     }
                     __syncthreads();
                 }
@@ -338,9 +307,9 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                     float acc = 0.f;
                     for (int d = 0; d < band; ++d) acc = __fadd_rn(acc, __fmul_rn(envA[d * obs + i], oc[i + d]));
                     for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, __fmul_rn(envB[j * obs + i], action[j]));
-                    const float nv = cw_tanh(acc);
-                    put_obs(o2 + (cur ^ 1) * L.o2_stride, i, nv);
-                    x[i] = cw_normalise(nv, nmean[i], nstd[i], p.ob_clip);
+                    const float nv = es_tanh_exp(acc);
+                    es_put_obs(o2 + (cur ^ 1) * L.o2_stride, i, nv, obs, band);
+                    x[i] = cw_normalise(nv, nmean[i], nstd[i], p.env.ob_clip);
                     if (add_stat) {                             // float32 column sums in step order (numpy's axis-0 reduction)
                         float2 st = stat[i];
                         st.x = __fadd_rn(st.x, nv); st.y = __fadd_rn(st.y, __fmul_rn(nv, nv));
@@ -362,7 +331,7 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                         } else {                                // ... and its mean (obj.py:57-61)
                             rfit[0] += (esum + (double)acc) / n_eps;
                         }
-                        const float ps = p.pos_scale;
+                        const float ps = p.r.pos_scale;
                         rpos[0] = __fadd_rn(rpos[0], __fmul_rn(ps, action[0]));
                         rpos[1] = __fadd_rn(rpos[1], __fmul_rn(ps, action[1 % act]));
                         rpos[2] = __fadd_rn(rpos[2], __fmul_rn(ps, action[2 % act]));
@@ -373,18 +342,18 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
             }
         }
         if (rew_warp && lane == 0) {
-            (neg ? p.fit_neg : p.fit_pos)[(size_t)pair * p.fit_stride] = rfit[0];
-            float* bv = neg ? p.behv_neg : p.behv_pos;
+            (neg ? p.r.fit_neg : p.r.fit_pos)[(size_t)pair * p.r.fit_stride] = rfit[0];
+            float* bv = neg ? p.r.behv_neg : p.r.behv_pos;
             if (bv) { bv[(size_t)pair * 3 + 0] = rpos[0]; bv[(size_t)pair * 3 + 1] = rpos[1]; bv[(size_t)pair * 3 + 2] = rpos[2]; }
         }
         if (keep_stat) {
             // ObStat.inc of a saved rollout: float32 column sums added in float64 (the order over rollouts is the atomics')
             for (int i = tid; i < obs; i += CW_THREADS) {
                 const float2 st = stat[i];
-                atomicAdd(p.ob_sum + i, (double)st.x);
-                atomicAdd(p.ob_sumsq + i, (double)st.y);
+                atomicAdd(p.env.ob_sum + i, (double)st.x);
+                atomicAdd(p.env.ob_sumsq + i, (double)st.y);
             }
-            if (tid == 0) { atomicAdd(p.ob_count, (double)T); atomicAdd(p.ob_count + 1, 1.0); }
+            if (tid == 0) { atomicAdd(p.env.ob_count, (double)T); atomicAdd(p.env.ob_count + 1, 1.0); }
         }
         cw_cluster_sync();                                  // REUSE (the last one: EXIT)
     }
@@ -486,8 +455,8 @@ int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& 
     int C = 0, max_clusters = 0;
     size_t smem = 0;
     const bool binned = r.bins != 0, noisy = r.act_noise != nullptr;       // (never both: the binned entry passes no noise)
-    int rc = binned ? es_closedw_binned_plan(r.layer_sizes, r.n_layers, env.band, r.bins, &C, &smem)
-                    : es_closedw_plan(r.layer_sizes, r.n_layers, env.band, &C, &smem);
+    int rc = binned ? es_closedw_binned_plan(r.dims, r.n_layers, env.band, r.bins, &C, &smem)
+                    : es_closedw_plan(r.dims, r.n_layers, env.band, &C, &smem);
     if (rc) return rc;
     const CwKernel kernel = cw_kernel(r.n_layers, binned, noisy);
     rc = cw_max_clusters(kernel, C, smem, &max_clusters);
@@ -496,26 +465,9 @@ int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& 
         es_set_error("es_rollout_closedloop_mlp: no cluster of %d CTAs with %zu bytes of shared memory each fits on this device", C, smem);
         return ES_ERR_UNSUPPORTED;
     }
-    CwParams p;
-    p.table = r.table; p.table_len = r.table_len; p.idx = r.idx; p.n_pairs = r.n_pairs; p.theta = r.theta; p.sigma = r.sigma;
-    p.n_layers = r.n_layers; p.T = r.T; p.n_params = r.P;
-    int at = 0;
-    for (int l = 0; l <= r.n_layers; ++l) p.dims[l] = r.layer_sizes[l];
-    for (int l = 0; l < r.n_layers; ++l) {                 // state-dict order: W_l [out][in], then b_l
-        p.woff[l] = at; at += p.dims[l] * p.dims[l + 1];
-        p.boff[l] = at; at += p.dims[l + 1];
-    }
-    p.ob_mean = env.ob_mean; p.ob_std = env.ob_std; p.ob_clip = env.ob_clip;
-    p.obs0 = env.obs0; p.env_a = env.env_a; p.env_b = env.env_b; p.band = env.band; p.crew = r.rew_vec; p.pos_scale = r.pos_scale;
-    p.coins = env.coins; p.chance = env.save_obs_chance;
-    p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.fit_stride = r.fit_stride; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
-    p.ob_sum = env.ob_sum; p.ob_sumsq = env.ob_sumsq; p.ob_count = env.ob_count;
-    p.err = r.err;
-    p.bins = r.bins; p.adim = binned ? r.layer_sizes[r.n_layers] / r.bins : 0; p.scale = binned ? (float)(1.0 / (r.bins - 1.0)) : 0.f;
-    p.low = r.head_low; p.range = r.head_range;
+    const CwParams p = {r, env};
     const long long evals = 2ll * r.n_pairs;
     const int clusters = evals < max_clusters ? (int)evals : max_clusters;
-    p.act_noise = r.act_noise; p.n_eps = noisy ? r.n_episodes : 1; p.ep_row = env.ep_rows;
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cw_config(C, smem, clusters, stream, &attr);
     ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));

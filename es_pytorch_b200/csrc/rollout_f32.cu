@@ -103,9 +103,8 @@ rollout_f32_stage_kernel(const float* __restrict__ table, const int64_t* __restr
     rf_stage_weights(W, table + es_checked_slice(idx[blockIdx.x >> 1], d.P, d.table_len, d.err), theta, sigma, blockIdx.x & 1, d);
 }
 
-// the policy head of a binned-action policy (FFBinned, src/nn/nn.py:99-117): the last layer has adim * bins outputs; the
-// action of dimension j is the first maximal of its bins outputs, idx, mapped to (scale * idx) * range[j] + low[j] with
-// scale = float32(1 / (bins - 1)), every operation rounded to float32 as the reference's torch expression does
+// the policy head of a binned-action policy (FFBinned, src/nn/nn.py:99-117; es_binned_action): the last layer has adim * bins
+// outputs
 struct RfHead {
     int adim, bins;
     float scale;
@@ -174,18 +173,11 @@ rf_rollout(const float* __restrict__ table, const int64_t* __restrict__ idx, con
             float* tmp = xin; xin = xout; xout = tmp;
         }
         if (BINNED) {
-            // xin holds the [RF_TM][adim * bins] outputs: the actions go to xout (free), which then becomes xin.  The first
-            // maximal bin wins, as torch.argmax; a NaN output counts as the maximum, as in torch
+            // xin holds the [RF_TM][adim * bins] outputs: the actions go to xout (free), which then becomes xin
             for (int i = threadIdx.x; i < rows * act_dim; i += RF_THREADS) {
                 const int r = i / act_dim, j = i - r * act_dim;
                 const float* o = xin + r * d.xpitch + j * h.bins;
-                int best = 0;
-                float bv = o[0];
-                for (int b = 1; b < h.bins && bv == bv; ++b) {
-                    const float v = o[b];
-                    if (v > bv || v != v) { bv = v; best = b; }
-                }
-                xout[r * d.xpitch + j] = __fadd_rn(__fmul_rn(__fmul_rn(h.scale, (float)best), __ldg(h.range + j)), __ldg(h.low + j));
+                xout[r * d.xpitch + j] = es_binned_action(h.bins, h.scale, h.low, h.range, j, [&](int b) { return o[b]; });
             }
             __syncthreads();
             float* tmp = xin; xin = xout; xout = tmp;
@@ -279,6 +271,17 @@ __global__ void __launch_bounds__(RF_THREADS, 1) rollout_f32_binned_kernel(RF_KE
 
 static int rf_round4(int x) { return (x + 3) & ~3; }
 
+// one launch of a rollout kernel over the pairs of c (`head`: the binned kernels' RfHead; none for the tanh kernels)
+template <typename K, typename... Head>
+static int rf_launch(es_ctx* ctx, K k, dim3 grid, size_t smem, cudaStream_t stream, const EsRollout& c, const RfDesc& d, double* part,
+                     unsigned* tickets, const float* wglobal, Head... head) {
+    ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<grid, RF_THREADS, smem, stream>>>(c.table, c.idx, c.theta, c.sigma, d, c.obsn, c.rew_vec, c.T, c.pos_scale, c.fit_pos, c.fit_neg,
+                                          c.fit_stride, c.behv_pos, c.behv_neg, part, tickets, wglobal, c.act_noise, c.n_episodes, head...);
+    ES_LAUNCHED(ctx);
+    return ES_OK;
+}
+
 int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     // obs-64-64-act networks with enough pairs to fill the GPU: the packed-FMA kernel of rollout_f32x.cu (one CTA per pair);
     // fewer pairs than half the SMs (single evaluations, es.step's noiseless evaluation) stay here, where the episode's time
@@ -295,14 +298,14 @@ int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     d.P = r.P;
     d.table_len = r.table_len;
     d.err = r.err;
-    int off = 0, soff = 0, xmax = 0;
+    int soff = 0, xmax = 0;
     for (int l = 0; l < n_layers; ++l) {
-        d.in[l] = r.layer_sizes[l];
-        d.out[l] = r.layer_sizes[l + 1];
+        d.in[l] = r.dims[l];
+        d.out[l] = r.dims[l + 1];
         d.in4[l] = rf_round4(d.in[l]);
         d.pitch[l] = ((d.in4[l] >> 2) & 1) ? d.in4[l] : d.in4[l] + 4;   // (pitch/4) odd -> conflict-free float4 rows
-        d.w_off[l] = off; off += d.in[l] * d.out[l];
-        d.b_off[l] = off; off += d.out[l];
+        d.w_off[l] = r.w_off[l];
+        d.b_off[l] = r.b_off[l];
         d.sw_off[l] = soff; soff += d.out[l] * d.pitch[l];
         if (d.in4[l] > xmax) xmax = d.in4[l];
         if (rf_round4(d.out[l]) > xmax) xmax = rf_round4(d.out[l]);
@@ -354,38 +357,19 @@ int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
                 if (rc) return rc;
             }
         }
-        double* fp = r.fit_pos + (size_t)p0 * r.fit_stride;
-        double* fn = r.fit_neg + (size_t)p0 * r.fit_stride;
-        float* bp = r.behv_pos ? r.behv_pos + (size_t)p0 * 3 : nullptr;
-        float* bn = r.behv_neg ? r.behv_neg + (size_t)p0 * 3 : nullptr;
-        const int n_eps = r.act_noise ? r.n_episodes : 1;
-        const float* an = r.act_noise ? r.act_noise + (size_t)p0 * 2 * n_eps * T * r.layer_sizes[n_layers] : nullptr;
-        if (r.bins) {
-            const RfHead h = {r.layer_sizes[n_layers] / r.bins, r.bins, (float)(1.0 / (r.bins - 1.0)), r.head_low, r.head_range};
-            if (gw) {
-                rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, d, wglobal);
-                ES_LAUNCHED(ctx);
-            }
-            const size_t smem = gw ? act_smem : smem_w;
-            auto k = gw ? rollout_f32_binned_kernel<true> : rollout_f32_binned_kernel<false>;
-            ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            k<<<dim3(2 * np, n_splits), RF_THREADS, smem, stream>>>(
-                r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
-                wglobal, an, n_eps, h);
-        } else if (gw) {
-            rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, d, wglobal);
+        const EsRollout c = es_rollout_rows(r, p0, np);
+        if (gw) {
+            rollout_f32_stage_kernel<<<2 * np, RF_THREADS, 0, stream>>>(c.table, c.idx, c.theta, c.sigma, d, wglobal);
             ES_LAUNCHED(ctx);
-            ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)act_smem));
-            rollout_f32_kernel<true><<<dim3(2 * np, n_splits), RF_THREADS, act_smem, stream>>>(
-                r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
-                wglobal, an, n_eps);
-        } else {
-            ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_f32_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_w));
-            rollout_f32_kernel<false><<<dim3(2 * np, n_splits), RF_THREADS, smem_w, stream>>>(
-                r.table, r.idx + p0, r.theta, r.sigma, d, r.obsn, r.rew_vec, T, r.pos_scale, fp, fn, r.fit_stride, bp, bn, part, tickets,
-                nullptr, an, n_eps);
         }
-        ES_LAUNCHED(ctx);
+        const size_t smem = gw ? act_smem : smem_w;
+        const dim3 grid(2 * np, n_splits);
+        const RfHead h = {r.act, r.bins, r.head_scale, r.head_low, r.head_range};
+        const int rc = r.bins ? rf_launch(ctx, gw ? rollout_f32_binned_kernel<true> : rollout_f32_binned_kernel<false>, grid, smem, stream,
+                                          c, d, part, tickets, wglobal, h)
+                              : rf_launch(ctx, gw ? rollout_f32_kernel<true> : rollout_f32_kernel<false>, grid, smem, stream, c, d, part,
+                                          tickets, wglobal);
+        if (rc) return rc;
     }
     return ES_OK;
 }

@@ -379,7 +379,7 @@ __global__ void rollout_f32x_prep_kernel(const float* __restrict__ obsn, int T, 
 // Returns ES_OK after launching, or ES_ERR_UNSUPPORTED (no error text) when the shape is not covered: the caller falls
 // back to the general kernel of rollout_f32.cu.
 int es_impl_rollout_f32x(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
-    const int* ls = r.layer_sizes;
+    const int* ls = r.dims;
     if (r.n_layers != 3 || ls[1] != FX_H || ls[2] != FX_H || ls[3] > 32 || ls[0] < 1) return ES_ERR_UNSUPPORTED;
     const FxSmem L = fx_layout(ls[0], ls[3]);
     if (L.total > 227 * 1024) return ES_ERR_UNSUPPORTED;
@@ -391,9 +391,9 @@ int es_impl_rollout_f32x(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     p.nkc = es_div_up(p.obs, FX_KC);
     p.n_tiles = es_div_up(r.T, FX_MT);
     p.sigma = r.sigma; p.pos_scale = r.pos_scale;
-    p.off = es_mlp_offsets(p.obs, FX_H, FX_H, p.act);
+    p.off = {r.w_off[0], r.b_off[0], r.w_off[1], r.b_off[1], r.w_off[2], r.b_off[2]};
     p.table_len = r.table_len; p.P = r.P; p.err = r.err;
-    p.n_eps = r.act_noise ? r.n_episodes : 1;
+    p.n_eps = r.n_episodes;
 
     const size_t xst_bytes = (size_t)p.n_tiles * p.nkc * FX_STAGE_FLOATS * sizeof(float);
     const size_t ub_bytes = (size_t)p.n_tiles * FX_MT * FX_H * sizeof(float);
@@ -409,7 +409,7 @@ int es_impl_rollout_f32x(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
         if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
         rollout_f32x_prep_kernel<<<blocks, 256, 0, stream>>>(r.obsn, r.T, p.obs, p.nkc, p.n_tiles, xst);
         ES_LAUNCHED(ctx);
-        rc = es_launch_ubase(ctx, r.obsn, r.theta, p.off, r.T, p.obs, p.n_tiles, ubase, stream);
+        rc = es_launch_ubase(ctx, r, p.n_tiles, ubase, stream);
         if (rc) return rc;
     }
     const int grid = r.n_pairs < ctx->sm_count ? r.n_pairs : ctx->sm_count;

@@ -82,27 +82,13 @@ struct T2Maps {
 };
 
 struct T2Params {
-    const float* table;
-    const int64_t* idx;
-    const float* theta;
+    EsRollout r;
     const uint8_t* xnt;           // [n_mtiles][nkc][pieces][16 KB stage image]
     const float* ubase;           // [n_mtiles * 128][64] row-major
-    const float* rew_vec;         // [T][act]
-    const float* act_noise;       // [n_pairs][2][n_eps][T][act] scaled action noise (mt_gauss.cu) or NULL
     uint8_t* images;              // [gridDim.x][2][image bytes]
-    double* fit_pos;
-    double* fit_neg;
-    float* behv_pos;
-    float* behv_neg;
     size_t shadow_stride;         // elements per shifted copy
     int use_tma;                  // eps1 by TMA from the shadows; 0: the builders convert the float32 slice
-    int n_pairs, obs, act, T, nkc, n_mtiles, fit_stride;
-    float sigma, pos_scale;
-    EsMlpOffsets off;
-    long long table_len;
-    int P;
-    int* err;
-    int n_eps;                    // episodes per evaluation (NOISE instantiations; 1 otherwise)
+    int nkc, n_mtiles;
 };
 
 template <bool SPLIT> struct T2Cfg {
@@ -170,7 +156,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int NMT = p.n_mtiles, NKC = p.nkc;
-    const int my_pairs = (p.n_pairs - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    const int my_pairs = (p.r.n_pairs - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
     // ---- one-time setup -----------------------------------------------------------------------------------------------
     if (tid == 0) {
@@ -215,13 +201,13 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 const uint32_t b = i & 1, u = i >> 1;
                 const uint8_t* img = my_images + (size_t)b * I.total;
                 const int pair = blockIdx.x + i * gridDim.x;
-                const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, p.err);
+                const long long slice = es_checked_slice(p.r.idx[pair], p.r.P, p.r.table_len, p.r.err);
                 mbar_wait(&bars[B2_IMG_READY + b], u & 1);                             // builders have finished image i
                 if (i > 0) mbar_wait(&bars[B2_EPS_FREE], (i - 1) & 1);                 // previous pair's last L1 has retired
                 if (lane == 0) {
                     mbar_expect_tx(&bars[B2_EPS_TX], (uint32_t)(NP * NKC * T2_B1_CHUNK));
                     if (p.use_tma) {
-                        const int unit0 = t2_shadow_unit(slice + p.off.w1, p.shadow_stride);
+                        const int unit0 = t2_shadow_unit(slice + p.r.w_off[0], p.shadow_stride);
 #pragma unroll
                         for (int pc = 0; pc < NP; ++pc)
                             for (int kc = 0; kc < NKC; ++kc)
@@ -236,11 +222,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 if (p.use_tma) {
                     // the unit holding column `obs` received the first elements of the next row: it carries the bias element
                     // eps_b1[n] (the observation tile has a constant 1 there) and zeros (obs % 8 == 0 on this path)
-                    const int kcb = p.obs >> 6, ub = (p.obs & 63) >> 3;
+                    const int kcb = p.r.dims[0] >> 6, ub = (p.r.dims[0] & 63) >> 3;
 #pragma unroll
                     for (int rr = 0; rr < 2; ++rr) {
                         const int n = 2 * lane + rr;
-                        const float eb = ldg_stream(p.table + slice + p.off.b1 + n);
+                        const float eb = ldg_stream(p.r.table + slice + p.r.b_off[0] + n);
                         __half hi, lo;
                         split_h1(eb, hi, lo);
                         const uint32_t off = (uint32_t)(kcb * NP) * T2_B1_CHUNK + n * 128 + ((ub ^ (n & 7)) << 4);      // [kc][piece] blocks
@@ -253,8 +239,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 if (lane == 0) mbar_arrive(&bars[B2_EPS_READY]);
                 if (p.use_tma && lane == 0 && i + 1 < my_pairs) {
                     // the next pair's eps1 rows into L2 now, so that its TMA at the pair boundary does not wait on HBM
-                    const long long nslice = es_checked_slice(p.idx[pair + gridDim.x], p.P, p.table_len, nullptr);
-                    const int nunit0 = t2_shadow_unit(nslice + p.off.w1, p.shadow_stride);
+                    const long long nslice = es_checked_slice(p.r.idx[pair + gridDim.x], p.r.P, p.r.table_len, nullptr);
+                    const int nunit0 = t2_shadow_unit(nslice + p.r.w_off[0], p.shadow_stride);
 #pragma unroll
                     for (int pc = 0; pc < NP; ++pc)
                         for (int kc = 0; kc < NKC; ++kc) tma_prefetch_3d(pc ? &maps.lo : &maps.hi, 0, nunit0 + 8 * kc, 0);
@@ -275,12 +261,12 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
             constexpr int BT = T2_BLD_WARPS * 32;
             const T2Image I = t2_image<SPLIT>(NKC, !p.use_tma);
             uint8_t* my_images = p.images + (size_t)blockIdx.x * 2 * I.total;
-            const float sg = p.sigma;
+            const float sg = p.r.sigma;
             for (int j = 0; j < my_pairs; ++j) {
                 const int pair = blockIdx.x + j * gridDim.x;
                 mbar_wait(&bars[B2_IMG_FREE + (j & 1)], (((uint32_t)j >> 1) & 1) ^ 1);
-                const long long slice = es_checked_slice(p.idx[pair], p.P, p.table_len, nullptr);
-                const float* __restrict__ eps = p.table + slice;
+                const long long slice = es_checked_slice(p.r.idx[pair], p.r.P, p.r.table_len, nullptr);
+                const float* __restrict__ eps = p.r.table + slice;
                 uint8_t* img = my_images + (size_t)(j & 1) * I.total;
                 // W2+- / W3+-: element pairs (n, k), (n, k+1)
                 const int n2 = T2_H * T2_H / 2, n3 = T2_ACT_PAD * T2_H / 2;
@@ -288,12 +274,12 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     const bool l3 = e2 >= n2;
                     const int k2 = 2 * (l3 ? e2 - n2 : e2);
                     const int n = k2 >> 6, kk = k2 & 63;
-                    const int at = (l3 ? p.off.w3 : p.off.w2) + k2;
-                    const bool live = !l3 || n < p.act;
+                    const int at = (l3 ? p.r.w_off[2] : p.r.w_off[1]) + k2;
+                    const bool live = !l3 || n < p.r.act;
                     float wp0 = 0.f, wp1 = 0.f, wn0 = 0.f, wn1 = 0.f;
                     if (live) {
-                        es_pheno_pm(sg, ldg_stream(eps + at), __ldg(p.theta + at), wp0, wn0);
-                        es_pheno_pm(sg, ldg_stream(eps + at + 1), __ldg(p.theta + at + 1), wp1, wn1);
+                        es_pheno_pm(sg, ldg_stream(eps + at), __ldg(p.r.theta + at), wp0, wn0);
+                        es_pheno_pm(sg, ldg_stream(eps + at + 1), __ldg(p.r.theta + at + 1), wp1, wn1);
                     }
                     const uint32_t blk = l3 ? T2_W3_BLOCK : T2_B1_CHUNK;
                     uint8_t* base = img + (l3 ? I.w3 : I.w2) + sw128_off(n, kk);
@@ -314,11 +300,11 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     float* bias = (float*)(img + I.bias);
                     for (int e = btid; e < T2_H + T2_ACT_PAD; e += BT) {
                         if (e < T2_H) {
-                            es_pheno_pm(sg, ldg_stream(eps + p.off.b2 + e), __ldg(p.theta + p.off.b2 + e), bias[e], bias[T2_H + e]);
+                            es_pheno_pm(sg, ldg_stream(eps + p.r.b_off[1] + e), __ldg(p.r.theta + p.r.b_off[1] + e), bias[e], bias[T2_H + e]);
                         } else {
                             const int j2 = e - T2_H;
                             float vp = 0.f, vn = 0.f;
-                            if (j2 < p.act) es_pheno_pm(sg, ldg_stream(eps + p.off.b3 + j2), __ldg(p.theta + p.off.b3 + j2), vp, vn);
+                            if (j2 < p.r.act) es_pheno_pm(sg, ldg_stream(eps + p.r.b_off[2] + j2), __ldg(p.r.theta + p.r.b_off[2] + j2), vp, vn);
                             bias[2 * T2_H + j2] = vp; bias[2 * T2_H + T2_ACT_PAD + j2] = vn;
                         }
                     }
@@ -329,8 +315,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     for (int e2 = btid; e2 < T2_H * Kp / 2; e2 += BT) {
                         const int n = (2 * e2) / Kp, k = (2 * e2) - n * Kp;
                         float x0 = 0.f, x1 = 0.f;
-                        if (k < p.obs) x0 = ldg_stream(eps + p.off.w1 + (size_t)n * p.obs + k); else if (k == p.obs) x0 = ldg_stream(eps + p.off.b1 + n);
-                        if (k + 1 < p.obs) x1 = ldg_stream(eps + p.off.w1 + (size_t)n * p.obs + k + 1); else if (k + 1 == p.obs) x1 = ldg_stream(eps + p.off.b1 + n);
+                        if (k < p.r.dims[0]) x0 = ldg_stream(eps + p.r.w_off[0] + (size_t)n * p.r.dims[0] + k); else if (k == p.r.dims[0]) x0 = ldg_stream(eps + p.r.b_off[0] + n);
+                        if (k + 1 < p.r.dims[0]) x1 = ldg_stream(eps + p.r.w_off[0] + (size_t)n * p.r.dims[0] + k + 1); else if (k + 1 == p.r.dims[0]) x1 = ldg_stream(eps + p.r.b_off[0] + n);
                         uint8_t* dst = img + I.b1 + (size_t)((k >> 6) * NP) * T2_B1_CHUNK + sw128_off(n, k & 63);     // [kc][piece] blocks
                         if (SPLIT) {
                             __half h0, l0, h1, l1;
@@ -347,10 +333,10 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&bars[B2_IMG_READY + (j & 1)]);
                 if (j + 1 < my_pairs) {                                      // L2 prefetch of the next pair's operands
-                    const long long nidx = es_checked_slice(p.idx[blockIdx.x + (j + 1) * gridDim.x], p.P, p.table_len, nullptr);
-                    const char* nxt = (const char*)(p.table + nidx);
-                    const int lines = (p.off.b3 + p.act) * 4 / 128 + 2;
-                    const int skip = p.use_tma ? p.off.b1 * 4 / 128 : 0;         // with the shadows eps1 comes by TMA
+                    const long long nidx = es_checked_slice(p.r.idx[blockIdx.x + (j + 1) * gridDim.x], p.r.P, p.r.table_len, nullptr);
+                    const char* nxt = (const char*)(p.r.table + nidx);
+                    const int lines = (p.r.b_off[2] + p.r.act) * 4 / 128 + 2;
+                    const int skip = p.use_tma ? p.r.b_off[0] * 4 / 128 : 0;         // with the shadows eps1 comes by TMA
                     for (int l = skip + btid; l < lines; l += BT) prefetch_l2(nxt + (size_t)l * 128);
                 }
             }
@@ -362,8 +348,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
         const int half = cw >> 2;                             // rows 64*half .. 64*half + 63 of the tile
         const int q = lane & 3;
         const int r0 = half * 64 + (cw & 3) * 16 + (lane >> 2);   // this thread's rows: r0 and r0 + 8
-        const float sg = p.sigma;
-        const bool want_pos = p.behv_pos != nullptr;
+        const float sg = p.r.sigma;
+        const bool want_pos = p.r.behv_pos != nullptr;
         const uint64_t a_desc0 = wg_desc_sw128(smem_u32(smem + L.xst));
         const uint64_t b1_desc0 = wg_desc_sw128(smem_u32(smem + L.b1));
         const uint64_t w2d = wg_desc_sw128(smem_u32(smem + L.w2)), w3d = wg_desc_sw128(smem_u32(smem + L.w3));
@@ -500,10 +486,10 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                             const int t = (e & 2) ? tb : ta;
                             const float z = __fadd_rn(d3[4 * c + e], b3[col]);
                             float a = SPLIT ? tanh_acc(z) : tanh_fast(z);
-                            if (col < p.act && t < p.T) {
+                            if (col < p.r.act && t < p.r.T) {
                                 if (NOISE && nz)                // a += rs.randn(act) * ac_std (src/nn/nn.py:47-48), drawn by mt_gauss.cu
-                                    a += __ldg(nz + (size_t)t * p.act + col);
-                                const float r = a * __ldg(p.rew_vec + (size_t)t * p.act + col);
+                                    a += __ldg(nz + (size_t)t * p.r.act + col);
+                                const float r = a * __ldg(p.r.rew_vec + (size_t)t * p.r.act + col);
                                 if (e & 2) rb += r; else ra += r;
                                 // position integrator: action components 0, 1, 2
                                 q0 += (col == 0) ? a : 0.f; q1 += (col == 1) ? a : 0.f; q2 += (col == 2) ? a : 0.f;
@@ -525,7 +511,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                                 const int t = (e & 2) ? tb : ta;
                                 const float z = __fadd_rn(d3[4 * c + e], b3[col]);
                                 const float a = SPLIT ? tanh_acc(z) : tanh_fast(z);
-                                if (col < p.act && t < p.T) {
+                                if (col < p.r.act && t < p.r.T) {
                                     const float r = a * rw[4 * c + e];
                                     if (e & 2) rb += r; else ra += r;
                                     q0 += (col == 0) ? a : 0.f; q1 += (col == 1) ? a : 0.f; q2 += (col == 2) ? a : 0.f;
@@ -539,8 +525,8 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                         else     { fit_p += r2; pp0 += q0; pp1 += q1; pp2 += q2; }
                         return;
                     }
-                    const int n_ep = p.n_eps;
-                    const float* __restrict__ nz = p.act_noise ? p.act_noise + ((size_t)pair * 2 + sgn) * n_ep * p.T * p.act : nullptr;
+                    const int n_ep = p.r.n_episodes;
+                    const float* __restrict__ nz = p.r.act_noise ? p.r.act_noise + ((size_t)pair * 2 + sgn) * n_ep * p.r.T * p.r.act : nullptr;
                     float ra, rb, q0, q1, q2;
                     epi3_episode(sgn, d3, nz, ra, rb, q0, q1, q2);
                     double r2 = (q == 0) ? (double)ra + (double)rb : 0.0;   // rows beyond T contribute 0
@@ -548,7 +534,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                         double sa = (double)ra, sb = (double)rb;
 #pragma unroll 1
                         for (int ep = 1; ep < n_ep; ++ep) {
-                            epi3_episode(sgn, d3, nz + (size_t)ep * p.T * p.act, ra, rb, q0, q1, q2);
+                            epi3_episode(sgn, d3, nz + (size_t)ep * p.r.T * p.r.act, ra, rb, q0, q1, q2);
                             sa += (double)ra; sb += (double)rb;
                         }
                         if (q == 0) r2 = sa / n_ep + sb / n_ep;
@@ -582,7 +568,7 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                         for (int e = 0; e < 4; ++e) {
                             const int col = 8 * c + 2 * q + (e & 1);
                             const int t = (e & 2) ? tb : ta;
-                            rw[4 * c + e] = (col < p.act && t < p.T) ? __ldg(p.rew_vec + (size_t)t * p.act + col) : 0.f;
+                            rw[4 * c + e] = (col < p.r.act && t < p.r.T) ? __ldg(p.r.rew_vec + (size_t)t * p.r.act + col) : 0.f;
                         }
                     }
                 }
@@ -613,16 +599,16 @@ __global__ void __launch_bounds__(T2_THREADS, 1) rollout_tc2_kernel(const __grid
                     for (int w = 0; w < T2_CONS_WARPS; ++w)
 #pragma unroll
                         for (int k = 0; k < 8; ++k) tot[k] += all[w * 8 + k];
-                    p.fit_pos[(size_t)pair * p.fit_stride] = tot[0];
-                    p.fit_neg[(size_t)pair * p.fit_stride] = tot[1];
+                    p.r.fit_pos[(size_t)pair * p.r.fit_stride] = tot[0];
+                    p.r.fit_neg[(size_t)pair * p.r.fit_stride] = tot[1];
                     if (want_pos) {
                         // components 1 and 2 of an action narrower than 3 repeat component 0 (index % act)
                         for (int s2 = 0; s2 < 2; ++s2) {
                             const double* ts = tot + 2 + 3 * s2;
-                            float* out = (s2 ? p.behv_neg : p.behv_pos) + pair * 3;
-                            out[0] = p.pos_scale * (float)ts[0];
-                            out[1] = p.pos_scale * (float)(p.act > 1 ? ts[1] : ts[0]);
-                            out[2] = p.pos_scale * (float)(p.act > 2 ? ts[2] : ts[0]);
+                            float* out = (s2 ? p.r.behv_neg : p.r.behv_pos) + pair * 3;
+                            out[0] = p.r.pos_scale * (float)ts[0];
+                            out[1] = p.r.pos_scale * (float)(p.r.act > 1 ? ts[1] : ts[0]);
+                            out[2] = p.r.pos_scale * (float)(p.r.act > 2 ? ts[2] : ts[0]);
                         }
                     }
                 }
@@ -731,17 +717,17 @@ int t2_encode_map(CUtensorMap* map, void* base, size_t stride, int obs) {
 }
 
 template <bool SPLIT>
-int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, cudaStream_t stream) {
+int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, cudaStream_t stream) {
     const T2Smem L = t2_layout<SPLIT>(p.nkc);
     const size_t smem = (size_t)L.total + 1024;       // + alignment slack
     if (smem > 227 * 1024) {
-        es_set_error("es_rollout_openloop(TC%s): obs_dim %d needs %zu bytes of shared memory (> 227 KB)", SPLIT ? "3" : "", p.obs, smem);
+        es_set_error("es_rollout_openloop(TC%s): obs_dim %d needs %zu bytes of shared memory (> 227 KB)", SPLIT ? "3" : "", p.r.dims[0], smem);
         return ES_ERR_UNSUPPORTED;
     }
     constexpr int NP = SPLIT ? 2 : 1;
     const size_t xnt_bytes = (size_t)p.n_mtiles * p.nkc * NP * T2_STAGE;
     const size_t ub_bytes = (size_t)p.n_mtiles * T2_MT * T2_H * sizeof(float);
-    const int grid = p.n_pairs < ctx->sm_count ? p.n_pairs : ctx->sm_count;
+    const int grid = p.r.n_pairs < ctx->sm_count ? p.r.n_pairs : ctx->sm_count;
     const size_t img_bytes = (((size_t)grid * 2 * t2_image<SPLIT>(p.nkc, !p.use_tma).total) + 255) & ~(size_t)255;
     void* scratch = nullptr;
     int rc = es_ctx_scratch(ctx, xnt_bytes + ub_bytes + img_bytes, &scratch);
@@ -755,12 +741,12 @@ int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, c
         const size_t total = (size_t)p.n_mtiles * p.nkc * T2_MT * T2_KC;
         int blocks = es_div_up((int64_t)total, 256);
         if (blocks > ctx->sm_count * 8) blocks = ctx->sm_count * 8;
-        rollout_tc2_prep_kernel<SPLIT><<<blocks, 256, 0, stream>>>(obsn, p.T, p.obs, p.nkc, p.n_mtiles, xnt);
+        rollout_tc2_prep_kernel<SPLIT><<<blocks, 256, 0, stream>>>(p.r.obsn, p.r.T, p.r.dims[0], p.nkc, p.n_mtiles, xnt);
         ES_LAUNCHED(ctx);
-        rc = es_launch_ubase(ctx, obsn, p.theta, p.off, p.T, p.obs, p.n_mtiles, ubase, stream);
+        rc = es_launch_ubase(ctx, p.r, p.n_mtiles, ubase, stream);
         if (rc) return rc;
     }
-    if (p.act_noise) {
+    if (p.r.act_noise) {
         ES_CHECK_CUDA(cudaFuncSetAttribute(rollout_tc2_kernel<SPLIT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         rollout_tc2_kernel<SPLIT, true><<<grid, T2_THREADS, smem, stream>>>(p, maps);
     } else {
@@ -773,9 +759,8 @@ int t2_launch(es_ctx* ctx, T2Params& p, const T2Maps& maps, const float* obsn, c
 
 }  // namespace
 
-int es_launch_ubase(es_ctx* ctx, const float* obsn, const float* theta, const EsMlpOffsets& off, int T, int obs, int n_tiles,
-                    float* ubase, cudaStream_t stream) {
-    rollout_ubase_kernel<<<n_tiles * T2_MT / T2_UB_ROWS, 256, 0, stream>>>(obsn, theta, off.w1, off.b1, T, obs, ubase);
+int es_launch_ubase(es_ctx* ctx, const EsRollout& r, int n_tiles, float* ubase, cudaStream_t stream) {
+    rollout_ubase_kernel<<<n_tiles * T2_MT / T2_UB_ROWS, 256, 0, stream>>>(r.obsn, r.theta, r.w_off[0], r.b_off[0], r.T, r.dims[0], ubase);
     ES_LAUNCHED(ctx);
     return ES_OK;
 }
@@ -797,7 +782,7 @@ template <bool SPLIT> static int t2_max_obs() {
 }
 
 int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t stream) {
-    const int* ls = r.layer_sizes;
+    const int* ls = r.dims;
     const int max_obs = split ? t2_max_obs<true>() : t2_max_obs<false>();
     if (r.n_layers != 3 || ls[1] != T2_H || ls[2] != T2_H || ls[3] > T2_ACT_PAD) {
         es_set_error("es_rollout_openloop(TC%s): the tensor-core path covers obs(<=%d)-64-64-act(<=32) tanh MLPs; "
@@ -810,17 +795,12 @@ int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t
                      "obs_dim <= %d)", split ? "3" : "", ls[0], max_obs);
         return ES_ERR_UNSUPPORTED;
     }
+    const int obs = ls[0];
     T2Params p;
     memset(&p, 0, sizeof(p));
-    p.table = r.table; p.idx = r.idx; p.theta = r.theta; p.act_noise = r.act_noise; p.rew_vec = r.rew_vec;
-    p.fit_pos = r.fit_pos; p.fit_neg = r.fit_neg; p.behv_pos = r.behv_pos; p.behv_neg = r.behv_neg;
-    p.n_pairs = r.n_pairs; p.obs = ls[0]; p.act = ls[3]; p.T = r.T; p.fit_stride = r.fit_stride;
-    p.sigma = r.sigma; p.pos_scale = r.pos_scale;
-    p.nkc = es_div_up(p.obs + 1, T2_KC);                 // + the constant-1 column that carries the L1 bias
+    p.r = r;
+    p.nkc = es_div_up(obs + 1, T2_KC);                   // + the constant-1 column that carries the L1 bias
     p.n_mtiles = es_div_up(r.T, T2_MT);
-    p.off = es_mlp_offsets(p.obs, T2_H, T2_H, p.act);
-    p.table_len = r.table_len; p.P = r.P; p.err = r.err;
-    p.n_eps = r.act_noise ? r.n_episodes : 1;
 
     // float16 shadows of the table (hi always, lo when a split rollout asks for it): 8 shifted copies each, built once per
     // (table pointer, length) and addressed through two TMA tensor maps.  Needs 16-byte aligned rows in every slice (obs % 8
@@ -828,9 +808,9 @@ int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t
     T2Maps maps;
     memset(&maps, 0, sizeof(maps));
     p.use_tma = 0;
-    if (p.obs % 8 == 0 && !ctx->sh16_failed) {
-        const size_t stride = ((size_t)r.table_len + 64 * (size_t)p.obs + 79) & ~(size_t)7;       // room for the last slice's rows
-        const bool fresh = ctx->sh16_src != r.table || ctx->sh16_len != r.table_len || ctx->sh16_stride != stride || ctx->sh16_obs != p.obs;
+    if (obs % 8 == 0 && !ctx->sh16_failed) {
+        const size_t stride = ((size_t)r.table_len + 64 * (size_t)obs + 79) & ~(size_t)7;       // room for the last slice's rows
+        const bool fresh = ctx->sh16_src != r.table || ctx->sh16_len != r.table_len || ctx->sh16_stride != stride || ctx->sh16_obs != obs;
         if (fresh) es_tc2_free_shadows(ctx);
         bool ok = true;
         if (!ctx->sh16_hi) {
@@ -853,10 +833,10 @@ int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t
             void* m = nullptr;
             ok = posix_memalign(&m, 64, sizeof(T2Maps)) == 0;
             if (ok) { memset(m, 0, sizeof(T2Maps)); ctx->sh16_maps = m; ctx->sh16_maps_lo = 0; }
-            if (ok) ok = t2_encode_map(&((T2Maps*)ctx->sh16_maps)->hi, ctx->sh16_hi, stride, p.obs) == 0;
+            if (ok) ok = t2_encode_map(&((T2Maps*)ctx->sh16_maps)->hi, ctx->sh16_hi, stride, obs) == 0;
         }
         if (ok && split && !ctx->sh16_maps_lo) {
-            ok = t2_encode_map(&((T2Maps*)ctx->sh16_maps)->lo, ctx->sh16_lo, stride, p.obs) == 0;
+            ok = t2_encode_map(&((T2Maps*)ctx->sh16_maps)->lo, ctx->sh16_lo, stride, obs) == 0;
             if (ok) ctx->sh16_maps_lo = 1;
         }
         if (!ok) {
@@ -864,11 +844,11 @@ int es_impl_rollout_tc2(es_ctx* ctx, const EsRollout& r, int split, cudaStream_t
             es_tc2_free_shadows(ctx);
             ctx->sh16_failed = 1;
         } else {
-            ctx->sh16_src = r.table; ctx->sh16_len = r.table_len; ctx->sh16_stride = stride; ctx->sh16_obs = p.obs;
+            ctx->sh16_src = r.table; ctx->sh16_len = r.table_len; ctx->sh16_stride = stride; ctx->sh16_obs = obs;
             maps = *(T2Maps*)ctx->sh16_maps;
             p.use_tma = 1;
             p.shadow_stride = stride;
         }
     }
-    return split ? t2_launch<true>(ctx, p, maps, r.obsn, stream) : t2_launch<false>(ctx, p, maps, r.obsn, stream);
+    return split ? t2_launch<true>(ctx, p, maps, stream) : t2_launch<false>(ctx, p, maps, stream);
 }

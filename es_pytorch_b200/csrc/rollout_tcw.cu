@@ -446,20 +446,18 @@ int tw_run(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     TwLayers& L = p.L;
     L.n_layers = r.n_layers;
     uint32_t o = 0;
-    int po = 0;
     for (int l = 0; l < r.n_layers; ++l) {
-        L.in[l] = r.layer_sizes[l];
-        L.out[l] = r.layer_sizes[l + 1];
+        L.in[l] = r.dims[l];
+        L.out[l] = r.dims[l + 1];
         L.kc[l] = es_div_up(L.in[l], 64);
         L.nb[l] = es_div_up(L.out[l], 64);
-        L.pw[l] = po; po += L.in[l] * L.out[l];
-        L.pb[l] = po; po += L.out[l];
+        L.pw[l] = r.w_off[l];
+        L.pb[l] = r.b_off[l];
         L.w_off[l] = o; o += (uint32_t)(L.kc[l] * L.nb[l] * NP) * TW_BLOCK;
     }
     for (int l = 0; l < r.n_layers; ++l) { L.b_off[l] = o; o += (uint32_t)L.nb[l] * 64 * sizeof(float); }
     L.img_bytes = (o + 1023) & ~1023u;
     const int T = r.T, n_mtiles = es_div_up(T, TW_MT);
-    const int n_eps = r.act_noise ? r.n_episodes : 1;
     // pairs per launch: <= 256 MiB of images
     int chunk = (int)((256u << 20) / (2 * (size_t)L.img_bytes));
     if (chunk < 1) chunk = 1;
@@ -471,17 +469,17 @@ int tw_run(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     if (rc) return rc;
     uint8_t* images = (uint8_t*)scratch;
     double* part = (double*)((uint8_t*)scratch + img_total);
-    const int act = r.bins ? L.out[r.n_layers - 1] / r.bins : L.out[r.n_layers - 1];
-    if (r.bins) { p.bins = r.bins; p.scale = (float)(1.0 / (r.bins - 1.0)); p.low = r.head_low; p.range = r.head_range; }
+    if (r.bins) { p.bins = r.bins; p.scale = r.head_scale; p.low = r.head_low; p.range = r.head_range; }
     for (int p0 = 0; p0 < r.n_pairs; p0 += chunk) {
         const int np = (r.n_pairs - p0 < chunk) ? r.n_pairs - p0 : chunk;
-        rollout_tcw_build_kernel<SPLIT><<<np, 256, 0, stream>>>(r.table, r.idx + p0, r.theta, r.sigma, r.table_len, r.P, r.err, L, images);
+        const EsRollout c = es_rollout_rows(r, p0, np);
+        rollout_tcw_build_kernel<SPLIT><<<np, 256, 0, stream>>>(c.table, c.idx, c.theta, c.sigma, c.table_len, c.P, c.err, L, images);
         ES_LAUNCHED(ctx);
         p.images = images;
         p.obsn = r.obsn; p.rew_vec = r.rew_vec;
-        p.act_noise = r.act_noise ? r.act_noise + (size_t)p0 * 2 * n_eps * T * act : nullptr;
+        p.act_noise = c.act_noise;
         p.part = part;
-        p.n_evals = 2 * np; p.n_mtiles = n_mtiles; p.obs = L.in[0]; p.act = act; p.T = T; p.n_eps = n_eps;
+        p.n_evals = 2 * np; p.n_mtiles = n_mtiles; p.obs = L.in[0]; p.act = r.act; p.T = T; p.n_eps = r.n_episodes;
         const int n_items = p.n_evals * n_mtiles;
         const int grid = n_items < ctx->sm_count ? n_items : ctx->sm_count;
         if constexpr (SPLIT) {
@@ -496,9 +494,8 @@ int tw_run(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
             rc = p.act_noise ? tw_launch_main<SPLIT, true>(ctx, p, grid, stream) : tw_launch_main<SPLIT, false>(ctx, p, grid, stream);
             if (rc) return rc;
         }
-        rollout_tcw_finish_kernel<<<es_div_up(2 * np, 128), 128, 0, stream>>>(
-            part, 2 * np, n_mtiles, act, r.pos_scale, r.fit_pos + (size_t)p0 * r.fit_stride, r.fit_neg + (size_t)p0 * r.fit_stride,
-            r.fit_stride, r.behv_pos ? r.behv_pos + (size_t)p0 * 3 : nullptr, r.behv_neg ? r.behv_neg + (size_t)p0 * 3 : nullptr);
+        rollout_tcw_finish_kernel<<<es_div_up(2 * np, 128), 128, 0, stream>>>(part, 2 * np, n_mtiles, c.act, c.pos_scale, c.fit_pos,
+                                                                            c.fit_neg, c.fit_stride, c.behv_pos, c.behv_neg);
         ES_LAUNCHED(ctx);
     }
     return ES_OK;
@@ -507,7 +504,7 @@ int tw_run(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
 }  // namespace
 
 bool es_tcw_covers(const EsRollout& r) {
-    const int* ls = r.layer_sizes;
+    const int* ls = r.dims;
     if (r.n_layers < 3 || r.n_layers > TW_MAX_LAYERS) return false;      // 2 to 4 hidden layers
     if (r.n_layers == 3 && ls[1] == 64 && ls[2] == 64) return false;    // obs-64-64-act: rollout_tc2.cu
     if (ls[0] < 1 || ls[0] > 256 || ls[r.n_layers] < 1 || ls[r.n_layers] > 32) return false;
@@ -519,7 +516,7 @@ bool es_tcw_covers(const EsRollout& r) {
 // binned heads (ES_ROLLOUT_TC3): 2 to 4 hidden layers of multiples of 64 in [64, 256] (obs-64-64-X included), obs <= 256 and
 // adim * bins <= 256 (up to four N blocks in the last layer)
 bool es_tcw_covers_binned(const EsRollout& r) {
-    const int* ls = r.layer_sizes;
+    const int* ls = r.dims;
     if (r.n_layers < 3 || r.n_layers > TW_MAX_LAYERS) return false;
     if (ls[0] < 1 || ls[0] > 256 || ls[r.n_layers] < 1 || ls[r.n_layers] > 256) return false;
     for (int l = 1; l < r.n_layers; ++l)
