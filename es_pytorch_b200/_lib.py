@@ -18,6 +18,7 @@ ES_ROLLOUT_TC = 1
 ES_ROLLOUT_TC3 = 2
 ES_MT_N = 624
 ES_OBJ_MEAN_REWARD, ES_OBJ_DIST, ES_OBJ_XDIST = 1, 2, 3
+ES_ACT_TANH, ES_ACT_RELU, ES_ACT_LEAKY_RELU, ES_ACT_ELU, ES_ACT_SIGMOID = 0, 1, 2, 3, 4
 
 _vp, _i32, _i64, _u64, _f32, _f64 = C.c_void_p, C.c_int, C.c_int64, C.c_uint64, C.c_float, C.c_double
 
@@ -56,6 +57,13 @@ SIGNATURES = {
                                                 _i32, _vp, _vp, _vp]),
     'es_rollout_closedloop_mlp_binned_plan': (_i32, [_vp, C.POINTER(_i32), _i32, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32),
                                                      C.POINTER(_i64)]),
+    'es_rollout_openloop_activation': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _i32,
+                                              _f32, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _f32, _i32, _vp]),
+    'es_rollout_closedloop_mlp_activation': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64,
+                                                    _vp, _vp, _i32, _vp, _vp, _i32, _f32, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _vp,
+                                                    _vp, _vp, _vp, _i32, _i32, _f32, _vp]),
+    'es_rollout_closedloop_mlp_activation_plan': (_i32, [_vp, C.POINTER(_i32), _i32, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32),
+                                                         C.POINTER(_i64)]),
     'es_draw_noisy': (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _u64, _i32, _i32, _f64, _vp, _vp, _vp, _vp]),
     'es_randn': (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
     'es_randn_plan': (_i32, [_vp, _i64, C.POINTER(C.c_size_t), C.POINTER(_i32)]),

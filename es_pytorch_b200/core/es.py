@@ -97,11 +97,12 @@ def _obstat_from(h_stats, obs_dim):
 
 def _can_fuse_step(comm, policy: Policy, fit_fn, ranker: Ranker) -> bool:
     """``step`` can keep the whole generation on the device (one synchronisation) when the evaluation is a
-    ``BatchedRollout`` of a network the fused rollouts evaluate (a tanh MLP or a binned-action one: ``BaseNet.head``) and
+    ``BatchedRollout`` of a network the fused rollouts evaluate (a tanh MLP or a binned-action one: ``BaseNet.head``; with
+    ``fuse_activations``, a FeedForward with another activation: ``BaseNet.activation``) and
     the ranker is a float32 shaping without elite selection (the others return host arrays of a different dtype / length:
     they take the call-by-call route)."""
     from .._lib import ES_RANK_MAX_NORMALIZED
-    if not getattr(fit_fn, 'is_batched_rollout', False) or _head(policy._module) is None:
+    if not getattr(fit_fn, 'is_batched_rollout', False) or _fused_policy(policy._module, fit_fn) is None:
         return False
     if comm.size != dist.world().size:                       # a communicator this package does not drive
         return False
@@ -115,6 +116,17 @@ def _can_fuse_step(comm, policy: Policy, fit_fn, ranker: Ranker) -> bool:
 def _head(module):
     """``module.head()`` for the package's networks, None for a module without one."""
     return module.head() if hasattr(module, 'head') else None
+
+
+def _fused_policy(module, fit_fn):
+    """(head, activation) of a network the fused rollouts evaluate for ``fit_fn``: (``module.head()``, None) for the tanh and
+    binned networks, ('tanh', its ``nn.Activation``) for a FeedForward with another activation when the BatchedRollout opts in
+    (``fuse_activations``); None for anything else."""
+    head = _head(module)
+    if head is not None:
+        return head, None
+    act = fit_fn.fused_activation(module) if hasattr(fit_fn, 'fused_activation') else None
+    return None if act is None else ('tanh', act)
 
 
 def _step_fused(cfg, comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: ObStat, fit_fn, rs, ranker: Ranker,
@@ -183,12 +195,13 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
     eng = get_engine()
     gen = fit_fn._gen
     theta = policy.theta_dev(eng)
-    head = _head(policy._module)
+    head, activation = _fused_policy(policy._module, fit_fn)
     head_key = None if head in (None, 'tanh') else head.key()
+    act_key = None if activation is None else activation.key()
     if (gen is None or gen.theta is not theta or gen.n_streams != len(streams) or gen.table is not nt.device_table(eng)
             or gen.coins_per_eval != int(fit_fn.coins_per_eval) or gen.rollout_mode != fit_fn.rollout_mode
             or (gen.archive is None) != (fit_fn.archive is None) or gen.episodes != fit_fn.episodes
-            or gen.head_key != head_key or gen.objective != objective):
+            or gen.head_key != head_key or gen.act_key != act_key or gen.objective != objective):
         env = fit_fn.env
         obs_dev, rew_dev = env.device_arrays(eng)
         T = fit_fn.max_steps
@@ -200,7 +213,8 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
                                archive=archive, nov_k=fit_fn.nov_k, rollout_mode=fit_fn.rollout_mode, engine=eng,
                                ac_std=float(getattr(policy._module, '_action_std', 0.0) or 0.0),
                                closed=env.device_closed(eng) if getattr(env, 'is_synthetic_closedloop', False) else None,
-                               episodes=fit_fn.episodes, head=head, closed_act_noise=True, objective=objective)
+                               episodes=fit_fn.episodes, head=head, closed_act_noise=True, objective=objective,
+                               activation=activation)
         fit_fn._gen = gen
     else:
         gen.load_states(streams)
@@ -230,8 +244,9 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
 
 
 def _test_params_batched(comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: ObStat, fit_fn, rs):
-    if _head(policy._module) is None:
-        raise NotImplementedError('the fused rollout evaluates tanh MLPs (FeedForward or FFBinned with torch.nn.Tanh)')
+    if _fused_policy(policy._module, fit_fn) is None:
+        raise NotImplementedError('the fused rollout evaluates tanh MLPs (FeedForward or FFBinned with torch.nn.Tanh), and with '
+                                  'BatchedRollout(fuse_activations=True) FeedForward with ReLU, LeakyReLU, ELU or Sigmoid')
     streams = fit_fn.rank_streams if fit_fn.rank_streams is not None else [rs]
     gen = _device_generation(fit_fn, policy, nt, streams)
     fpos, fneg = gen.evaluate(n)

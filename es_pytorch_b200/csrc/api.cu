@@ -1,5 +1,6 @@
 // api.cu -- extern "C" surface of libes_b200.so (declared in include/es_b200.h):
 // argument validation, context/scratch management, dispatch to the kernels.
+#include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
 #include "common.cuh"
@@ -117,6 +118,10 @@ static int es_async_error(es_ctx* ctx, const char* where) {
             es_set_error("%s: es_draw_noisy consumed more MT19937 words than its jump-ahead pass had generated (a > 12 sigma "
                          "event of the polar method's acceptance count, or a bug): the draws of that call are invalid; set "
                          "ES_MT_JUMP=0 to use the sequential kernel", where);
+        else if (code == ES_ASYNC_F16_RANGE)
+            es_set_error("%s: a previous ES_ROLLOUT_TC3 rollout met a hidden activation beyond float16 range (|h| > 65504), which its "
+                         "split float16 operands cannot hold: the results of that call are invalid; use ES_ROLLOUT_F32 for such "
+                         "policies", where);
         else if (code == ES_ASYNC_RANDN_OVERFLOW)
             es_set_error("%s: es_randn needed more MT19937 words than its windows had generated (a > 12 sigma event of the "
                          "polar method's acceptance count, or a bug): the values of that call are invalid", where);
@@ -259,9 +264,38 @@ static int es_binned_check(const char* fn, const EsRollout& r) {
     return ES_OK;
 }
 
-// the policies an entry point takes: tanh MLPs, binned heads (EsRollout::bins, which es_binned_check refuses below 2), or
-// es_rollout_closedloop's tanh MLPs (two hidden layers, rollout_closed.cu only)
-enum EsHead { ES_HEAD_TANH, ES_HEAD_BINNED, ES_HEAD_TANH_ONE_CTA };
+// the activation arguments of the *_activation entry points
+static int es_activation_check(const char* fn, int activation, float act_param) {
+    ES_REQUIRE(activation >= ES_ACT_TANH && activation <= ES_ACT_SIGMOID,
+               "%s: unknown activation %d (ES_ACT_TANH, ES_ACT_RELU, ES_ACT_LEAKY_RELU, ES_ACT_ELU or ES_ACT_SIGMOID)", fn, activation);
+    ES_REQUIRE(isfinite(act_param), "%s: the activation parameter must be finite, got %g", fn, (double)act_param);
+    return ES_OK;
+}
+
+// the policies an entry point takes: tanh MLPs, binned heads (EsRollout::bins, which es_binned_check refuses below 2),
+// es_rollout_closedloop's tanh MLPs (two hidden layers, rollout_closed.cu only), or MLPs with another activation
+// (EsRollout::activation)
+enum EsHead { ES_HEAD_TANH, ES_HEAD_BINNED, ES_HEAD_TANH_ONE_CTA, ES_HEAD_ACT };
+
+// the part of a shape outside the wide tensor-core kernel's coverage (`max_out`: the widest last layer it takes), into why
+static void es_tcw_why(const EsRollout& r, int max_out, char* why, size_t n) {
+    const int* dims = r.dims;
+    if (r.n_layers < 3 || r.n_layers > 5) {
+        snprintf(why, n, "%d hidden layers", r.n_layers - 1);
+        return;
+    }
+    if (dims[0] > 256) {
+        snprintf(why, n, "obs %d", dims[0]);
+        return;
+    }
+    for (int l = 1; l < r.n_layers; ++l)
+        if (dims[l] % 64 || dims[l] > 256) {
+            snprintf(why, n, "hidden layer %d of width %d", l, dims[l]);
+            return;
+        }
+    if (dims[r.n_layers] > max_out) snprintf(why, n, "%d outputs", dims[r.n_layers]);
+    else snprintf(why, n, "the shape");
+}
 
 // an open-loop entry point after ES_ENTER: its checks in order, then the mode's kernel; `fn` names it in every message
 static int es_openloop(es_ctx* ctx, const char* fn, EsRollout r, const int* layer_sizes, EsHead head, int mode, cudaStream_t stream) {
@@ -276,26 +310,27 @@ static int es_openloop(es_ctx* ctx, const char* fn, EsRollout r, const int* laye
             return ES_ERR_UNSUPPORTED;
         }
         if (mode == ES_ROLLOUT_TC3 && !es_tcw_covers_binned(r)) {
-            const int* dims = r.dims;
-            char why[96];                               // the part of the shape outside the coverage
-            if (r.n_layers < 3 || r.n_layers > 5) {
-                snprintf(why, sizeof why, "%d hidden layers", r.n_layers - 1);
-            } else if (dims[0] > 256) {
-                snprintf(why, sizeof why, "obs %d", dims[0]);
-            } else {
-                snprintf(why, sizeof why, "the shape");
-                for (int l = 1; l < r.n_layers; ++l)
-                    if (dims[l] % 64 || dims[l] > 256) {
-                        snprintf(why, sizeof why, "hidden layer %d of width %d", l, dims[l]);
-                        break;
-                    }
-            }
+            char why[96];
+            es_tcw_why(r, 256, why, sizeof why);
             es_set_error("%s: ES_ROLLOUT_TC3 covers binned heads with 2 to 4 hidden layers of widths in {64, 128, 192, 256} and obs "
                          "<= 256, got %s; use ES_ROLLOUT_F32", fn, why);
             return ES_ERR_UNSUPPORTED;
         }
+    } else if (head == ES_HEAD_ACT) {
+        if (mode == ES_ROLLOUT_TC) {
+            es_set_error("%s: ES_ROLLOUT_TC refuses activations other than tanh (its single float16 products are bounded for "
+                         "tanh's outputs only); use ES_ROLLOUT_TC3 or ES_ROLLOUT_F32", fn);
+            return ES_ERR_UNSUPPORTED;
+        }
+        if (mode == ES_ROLLOUT_TC3 && !es_tcw_covers_act(r)) {
+            char why[96];
+            es_tcw_why(r, 32, why, sizeof why);
+            es_set_error("%s: ES_ROLLOUT_TC3 covers activations other than tanh for 2 to 4 hidden layers of widths in {64, 128, 192, "
+                         "256}, obs <= 256 and act <= 32, got %s; use ES_ROLLOUT_F32", fn, why);
+            return ES_ERR_UNSUPPORTED;
+        }
     } else if (r.n_pairs == 0) {
-        return ES_OK;                               // a tanh head returns before it looks at the mode, a binned head after
+        return ES_OK;                               // a tanh head returns before it looks at the mode, the others after
     }
     if (mode != ES_ROLLOUT_F32 && mode != ES_ROLLOUT_TC && mode != ES_ROLLOUT_TC3) {
         es_set_error("%s: unknown mode %d", fn, mode);
@@ -303,6 +338,7 @@ static int es_openloop(es_ctx* ctx, const char* fn, EsRollout r, const int* laye
     }
     if (r.n_pairs == 0) return ES_OK;
     if (mode == ES_ROLLOUT_F32) return es_impl_rollout_f32(ctx, r, stream);
+    if (head == ES_HEAD_ACT) return es_impl_rollout_tcw_act(ctx, r, stream);
     // tensor cores: binned heads and the shipped configs' wide policies on rollout_tcw.cu; obs-64-64-act and everything else on
     // rollout_tc2.cu
     if (head == ES_HEAD_BINNED || es_tcw_covers(r)) return es_impl_rollout_tcw(ctx, r, mode == ES_ROLLOUT_TC3, stream);
@@ -317,8 +353,11 @@ int es_rollout_openloop_episodes(es_ctx* ctx, const float* table, int64_t table_
     ES_REQUIRE(n_episodes >= 1, "es_rollout_openloop: n_episodes must be >= 1, got %d", n_episodes);
     // without action noise the episodes are identical and their mean is exactly the one episode (E copies of a float32 value
     // sum exactly in float64, and (E r) / E == r)
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, obsn, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .obsn = obsn, .rew_vec = rew_vec, .T = T, .pos_scale = pos_scale,
+                         .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride, .behv_pos = behv_pos,
+                         .behv_neg = behv_neg, .act_noise = act_noise, .err = ctx->err_dev,
+                         .n_episodes = act_noise ? n_episodes : 1};
     return es_openloop(ctx, "es_rollout_openloop", r, layer_sizes, ES_HEAD_TANH, mode, (cudaStream_t)stream);
 }
 
@@ -344,9 +383,34 @@ int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_le
                                float* behv_pos, float* behv_neg, int bins, const float* low, const float* range, int mode,
                                void* stream) {
     ES_ENTER(ctx);
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, obsn, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .obsn = obsn, .rew_vec = rew_vec, .T = T, .pos_scale = pos_scale,
+                         .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride, .behv_pos = behv_pos,
+                         .behv_neg = behv_neg, .act_noise = nullptr, .err = ctx->err_dev, .n_episodes = 1, .bins = bins,
+                         .head_low = low, .head_range = range};
     return es_openloop(ctx, "es_rollout_openloop_binned", r, layer_sizes, ES_HEAD_BINNED, mode, (cudaStream_t)stream);
+}
+
+int es_rollout_openloop_activation(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                   const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const float* obsn,
+                                   const float* rew_vec, int T, float pos_scale, double* fit_pos, double* fit_neg, int fit_stride,
+                                   float* behv_pos, float* behv_neg, const float* act_noise, int n_episodes, int activation,
+                                   float act_param, int mode, void* stream) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_openloop_activation";
+    const int rc = es_activation_check(fn, activation, act_param);
+    if (rc) return rc;
+    if (activation == ES_ACT_TANH)
+        return es_rollout_openloop_episodes(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, obsn, rew_vec,
+                                            T, pos_scale, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, n_episodes,
+                                            mode, stream);
+    ES_REQUIRE(n_episodes >= 1, "%s: n_episodes must be >= 1, got %d", fn, n_episodes);
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .activation = activation, .obsn = obsn, .rew_vec = rew_vec, .T = T,
+                         .pos_scale = pos_scale, .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride,
+                         .behv_pos = behv_pos, .behv_neg = behv_neg, .act_noise = act_noise, .err = ctx->err_dev,
+                         .n_episodes = act_noise ? n_episodes : 1, .act_param = act_param};
+    return es_openloop(ctx, fn, r, layer_sizes, ES_HEAD_ACT, mode, (cudaStream_t)stream);
 }
 
 // the shapes es_rollout_closedloop's one-CTA kernel (rollout_closed.cu) covers: two hidden layers <= 64, act <= 64, obs <= 384
@@ -373,7 +437,7 @@ static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* la
     if (head == ES_HEAD_BINNED) {
         rc = es_binned_check(fn, r);
         if (!rc) rc = es_closedw_binned_plan(r.dims, r.n_layers, env.band, r.bins, &C, &smem);
-    } else if (head == ES_HEAD_TANH) {
+    } else if (head == ES_HEAD_TANH || head == ES_HEAD_ACT) {
         rc = es_closedw_plan(r.dims, r.n_layers, env.band, &C, &smem);
     }
     if (rc) return rc;
@@ -384,6 +448,7 @@ static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* la
         if (rc) return rc;
         env.ep_rows = (double*)rows;
     }
+    if (head == ES_HEAD_ACT) return es_impl_rollout_closedw_act(ctx, r, env, stream);
     if (head == ES_HEAD_TANH_ONE_CTA || (head == ES_HEAD_TANH && es_closed_one_cta_covers(r.dims, r.n_layers)))
         return es_impl_rollout_closed(ctx, r, env, stream);
     return es_impl_rollout_closedw(ctx, r, env, stream);
@@ -396,13 +461,15 @@ int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, co
                           double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
                           double* ob_count, void* stream) {
     ES_ENTER(ctx);
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, nullptr, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1};
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .obsn = nullptr, .rew_vec = rew_vec, .T = T, .pos_scale = pos_scale,
+                         .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride, .behv_pos = behv_pos,
+                         .behv_neg = behv_neg, .act_noise = nullptr, .err = ctx->err_dev, .n_episodes = 1};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
     return es_closedloop(ctx, "es_rollout_closedloop", r, layer_sizes, env, ES_HEAD_TANH_ONE_CTA, (cudaStream_t)stream);
 }
 
-// both plan entry points after ES_ENTER (`bins`: a binned head's, 0 for a tanh head)
+// the plan entry points after ES_ENTER (`bins`: a binned head's, 0 for the others)
 static int es_closedloop_plan(es_ctx* ctx, const char* fn, const int* layer_sizes, int n_layers, int band, EsHead head, int bins,
                               int* cluster_size, int* clusters, int64_t* smem_bytes) {
     ES_REQUIRE(layer_sizes && cluster_size && clusters && smem_bytes, "%s: NULL pointer", fn);
@@ -416,12 +483,13 @@ static int es_closedloop_plan(es_ctx* ctx, const char* fn, const int* layer_size
     const int rc = binned ? es_closedw_binned_plan(layer_sizes, n_layers, band, bins, &C, &smem)
                           : es_closedw_plan(layer_sizes, n_layers, band, &C, &smem);
     if (rc) return rc;
-    if (!binned && es_closed_one_cta_covers(layer_sizes, n_layers)) {
+    if (head == ES_HEAD_TANH && es_closed_one_cta_covers(layer_sizes, n_layers)) {
         *cluster_size = 0; *clusters = ctx->sm_count; *smem_bytes = 0;
         return ES_OK;
     }
     *cluster_size = C; *smem_bytes = (int64_t)smem;
-    return es_closedw_max_clusters(n_layers, bins, C, smem, clusters);
+    return head == ES_HEAD_ACT ? es_closedw_act_max_clusters(n_layers, C, smem, clusters)
+                               : es_closedw_max_clusters(n_layers, bins, C, smem, clusters);
 }
 
 int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int* cluster_size, int* clusters,
@@ -441,8 +509,11 @@ int es_rollout_closedloop_mlp_episodes(es_ctx* ctx, const float* table, int64_t 
     ES_ENTER(ctx);
     ES_REQUIRE(n_episodes >= 1, "es_rollout_closedloop_mlp: n_episodes must be >= 1, got %d", n_episodes);
     // without action noise the episodes are identical: the noise-free kernels run one (as es_rollout_openloop_episodes)
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, nullptr, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, act_noise, ctx->err_dev, act_noise ? n_episodes : 1};
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .obsn = nullptr, .rew_vec = rew_vec, .T = T, .pos_scale = pos_scale,
+                         .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride, .behv_pos = behv_pos,
+                         .behv_neg = behv_neg, .act_noise = act_noise, .err = ctx->err_dev,
+                         .n_episodes = act_noise ? n_episodes : 1};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
     return es_closedloop(ctx, "es_rollout_closedloop_mlp", r, layer_sizes, env, ES_HEAD_TANH, (cudaStream_t)stream);
 }
@@ -474,10 +545,50 @@ int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t ta
                                      float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins, const float* low,
                                      const float* range, void* stream) {
     ES_ENTER(ctx);
-    const EsRollout r = {table, table_len, idx, n_pairs, theta, P, sigma, n_layers, nullptr, rew_vec, T, pos_scale,
-                         fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, nullptr, ctx->err_dev, 1, bins, low, range};
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .obsn = nullptr, .rew_vec = rew_vec, .T = T, .pos_scale = pos_scale,
+                         .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride, .behv_pos = behv_pos,
+                         .behv_neg = behv_neg, .act_noise = nullptr, .err = ctx->err_dev, .n_episodes = 1, .bins = bins,
+                         .head_low = low, .head_range = range};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
     return es_closedloop(ctx, "es_rollout_closedloop_mlp_binned", r, layer_sizes, env, ES_HEAD_BINNED, (cudaStream_t)stream);
+}
+
+int es_rollout_closedloop_mlp_activation(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                         const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                         const double* ob_mean, const double* ob_std, double ob_clip, const float* obs0,
+                                         const float* env_a, int band, const float* env_b, const float* rew_vec, int T,
+                                         float pos_scale, const uint32_t* coin_words, double save_obs_chance, double* fit_pos,
+                                         double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum,
+                                         double* ob_sumsq, double* ob_count, const float* act_noise, int n_episodes, int activation,
+                                         float act_param, void* stream) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_closedloop_mlp_activation";
+    const int rc = es_activation_check(fn, activation, act_param);
+    if (rc) return rc;
+    if (activation == ES_ACT_TANH)
+        return es_rollout_closedloop_mlp_episodes(ctx, table, table_len, idx, n_pairs, theta, P, sigma, layer_sizes, n_layers, ob_mean,
+                                                  ob_std, ob_clip, obs0, env_a, band, env_b, rew_vec, T, pos_scale, coin_words,
+                                                  save_obs_chance, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg, ob_sum, ob_sumsq,
+                                                  ob_count, act_noise, n_episodes, stream);
+    ES_REQUIRE(n_episodes >= 1, "%s: n_episodes must be >= 1, got %d", fn, n_episodes);
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .activation = activation, .obsn = nullptr, .rew_vec = rew_vec,
+                         .T = T, .pos_scale = pos_scale, .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride,
+                         .behv_pos = behv_pos, .behv_neg = behv_neg, .act_noise = act_noise, .err = ctx->err_dev,
+                         .n_episodes = act_noise ? n_episodes : 1, .act_param = act_param};
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    return es_closedloop(ctx, fn, r, layer_sizes, env, ES_HEAD_ACT, (cudaStream_t)stream);
+}
+
+int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int activation,
+                                              int* cluster_size, int* clusters, int64_t* smem_bytes) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_closedloop_mlp_activation_plan";
+    const int rc = es_activation_check(fn, activation, 0.f);
+    if (rc) return rc;
+    return es_closedloop_plan(ctx, fn, layer_sizes, n_layers, band, activation == ES_ACT_TANH ? ES_HEAD_TANH : ES_HEAD_ACT, 0,
+                              cluster_size, clusters, smem_bytes);
 }
 
 int es_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,

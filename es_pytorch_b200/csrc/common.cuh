@@ -40,6 +40,7 @@ struct es_ctx {
 #define ES_ASYNC_BAD_INDEX 1
 #define ES_ASYNC_RNG_OVERFLOW 2      // es_draw_noisy (jump-ahead path): the stream consumed more words than were generated ahead
 #define ES_ASYNC_RANDN_OVERFLOW 3    // es_randn: the n values needed more words than its windows generated
+#define ES_ASYNC_F16_RANGE 4         // es_rollout_openloop_activation (TC3): a hidden activation beyond float16 range
 
 void es_set_error(const char* fmt, ...);
 
@@ -92,6 +93,10 @@ struct EsRollout {
     int P;
     float sigma;
     int n_layers;
+    // the policy's activation after every layer (ES_ACT_*; 0 = tanh) and its float32 parameter (leaky ReLU's slope, ELU's
+    // alpha).  Both sit in alignment holes of the struct, so its size and every other member's offset are those of a call
+    // without them, and the kernels that take the struct by value are unchanged
+    int activation;
     const float* obsn;          // open loop: normalised observations [T][obs]
     const float* rew_vec;       // [T][act]
     int T;
@@ -114,7 +119,9 @@ struct EsRollout {
     int w_off[ES_MAX_LAYERS], b_off[ES_MAX_LAYERS];     // flat offsets of W_l [dims[l+1]][dims[l]] and b_l, state-dict order
     int act;                    // the env's action dimension: dims[n_layers], or adim = dims[n_layers] / bins
     float head_scale;           // a binned head's float32(1 / (bins - 1))
+    float act_param;
 };
+static_assert(sizeof(void*) != 8 || sizeof(EsRollout) == 272, "EsRollout's members must keep their offsets");
 
 // the call restricted to the pairs [p0, p0 + np)
 static inline EsRollout es_rollout_rows(const EsRollout& r, int p0, int np) {
@@ -181,6 +188,13 @@ int es_closedw_max_clusters(int n_layers, int bins, int cluster_size, size_t sme
 int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // binned heads (EsRollout::bins >= 2): every shape es_closedw_plan covers with act = adim; the cluster kernel at every C
 int es_closedw_binned_plan(const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes);
+// policies with an activation other than tanh (EsRollout::activation != ES_ACT_TANH): on ES_ROLLOUT_TC3 the shapes of
+// es_tcw_covers_act, rollout_tcw.cu's code (rollout_tcw_act.cu); in the closed loop every shape es_closedw_plan covers, on the
+// cluster kernel's code at every C (rollout_closedw_act.cu), and its resident clusters
+bool es_tcw_covers_act(const EsRollout&);
+int es_impl_rollout_tcw_act(es_ctx*, const EsRollout&, cudaStream_t);
+int es_closedw_act_max_clusters(int n_layers, int cluster_size, size_t smem_bytes, int* clusters);
+int es_impl_rollout_closedw_act(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
 int es_launch_ubase(es_ctx*, const EsRollout&, int n_tiles, float* ubase, cudaStream_t);
 int es_impl_novelty(es_ctx*, const float*, int, const double*, int, int, double*, int, cudaStream_t);
@@ -262,6 +276,27 @@ __device__ __forceinline__ float es_binned_action(int bins, float scale, const f
         if (v > bv || v != v) { bv = v; best = b; }
     }
     return __fadd_rn(__fmul_rn(__fmul_rn(scale, (float)best), __ldg(range + j)), __ldg(low + j));
+}
+// a policy activation (ES_ACT_*, include/es_b200.h) other than tanh, in float32 as torch's CPU kernels evaluate it: ReLU is
+// clamp_min(x, 0) (a NaN passes), leaky ReLU and ELU round their float32 parameter's product once, ELU takes expm1 (exp(x) - 1
+// loses every digit near 0), sigmoid is 1 / (1 + e^-x) with the fast exponential and division (absolute error ~1e-7: e^-x
+// carries (2 + 1.2 |x|) ulp, scaled by sigmoid(x) (1 - sigmoid(x)) <= 0.25, which falls as e^-|x|; the division 2 ulp; the IEEE
+// forms made the wide tensor-core kernel with action noise spill)
+template <int ACT>
+__device__ __forceinline__ float es_act(float x, float param) {
+    if constexpr (ACT == ES_ACT_RELU) return x < 0.f ? 0.f : x;
+    else if constexpr (ACT == ES_ACT_LEAKY_RELU) return x > 0.f ? x : __fmul_rn(x, param);
+    else if constexpr (ACT == ES_ACT_ELU) return x > 0.f ? x : __fmul_rn(param, expm1f(x));
+    else return __fdividef(1.f, 1.f + __expf(-x));
+}
+// the same for a kind known at run time (uniform over the launch)
+__device__ __forceinline__ float es_act(int kind, float param, float x) {
+    switch (kind) {
+        case ES_ACT_RELU: return es_act<ES_ACT_RELU>(x, param);
+        case ES_ACT_LEAKY_RELU: return es_act<ES_ACT_LEAKY_RELU>(x, param);
+        case ES_ACT_ELU: return es_act<ES_ACT_ELU>(x, param);
+        default: return es_act<ES_ACT_SIGMOID>(x, param);
+    }
 }
 // tanh(x) = 1 - 2 / (1 + e^2x) with the fast exponential and division: absolute error ~1e-7 (tanhf is ~40 dependent
 // instructions per call); the closed-loop kernels end every phase of a step in one

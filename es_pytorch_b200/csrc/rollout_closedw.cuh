@@ -1,0 +1,329 @@
+// rollout_closedw.cuh -- the closed-loop cluster rollout's code (see rollout_closedw.cu for the design and the barrier argument):
+// the shared-memory layout, the body every CTA of a cluster runs and the launch configuration.  rollout_closedw.cu instantiates
+// it for tanh policies and binned heads, rollout_closedw_act.cu for the other activations.
+#pragma once
+#include <math.h>
+#include "common.cuh"
+#include "mt19937.cuh"
+
+namespace {
+
+constexpr int CW_THREADS = 512;
+constexpr int CW_WARPS = CW_THREADS / 32;
+constexpr int CW_MAX_LAYERS = 5;           // 2 to 4 hidden layers
+constexpr int CW_MAX_WIDTH = 256;
+constexpr int CW_MAX_OBS = 384;
+constexpr int CW_MAX_ACT = 64;
+constexpr int CW_HALO = 16;                // band <= 16
+constexpr int CW_SMEM_MAX = 227 * 1024 - 1024;    // dynamic shared memory per CTA: 227 KiB less 1 KiB for the static cw_layers
+
+struct CwParams {
+    EsRollout r;
+    EsClosedEnv env;                        // ep_rows: [clusters][T] per-step episode sums (n_episodes > 1)
+};
+
+__host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
+__host__ __device__ inline int cw_pad4(int n) { return (n + 3) & ~3; }
+
+struct CwLayout {                          // offsets in floats into dynamic shared memory (all multiples of 4)
+    int norm, racc, x, prod, abin, stat, o2, o2_stride, env_a, env_b, total;
+    int act[CW_MAX_LAYERS], w[CW_MAX_LAYERS], bias[CW_MAX_LAYERS], rows[CW_MAX_LAYERS], stride[CW_MAX_LAYERS];
+};
+// act: the actions the env sees (dims[n_layers], or adim for a binned head, whose actions get their own buffer `abin`)
+__host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int C, int band, int act, bool binned) {
+    CwLayout L;
+    const int obs = dims[0];
+    int at = 0;
+    L.norm = at; at += 4 * obs;                            // double mean[obs], double std[obs]  (first: 8-byte aligned)
+    L.racc = at; at += 8;                                  // double fitness, float position[3]
+    L.x = at; at += cw_pad32(obs);                         // the normalised observation, zero padded
+    for (int l = 0; l < n_layers; ++l) { L.act[l] = at; at += cw_pad32(dims[l + 1]); }    // a_l, zero padded
+    for (int l = 0; l < n_layers; ++l) {
+        L.rows[l] = (dims[l + 1] + C - 1) / C;
+        L.stride[l] = cw_pad32(dims[l]);
+        L.w[l] = at; at += cw_pad4(L.rows[l]) * L.stride[l];
+        L.bias[l] = at; at += cw_pad4(L.rows[l]);
+    }
+    L.prod = at; at += cw_pad4(act);
+    L.abin = at; if (binned) at += cw_pad4(act);
+    L.stat = at; at += 2 * obs;                            // float2 (sum, sumsq) of the post-step observations
+    L.o2_stride = cw_pad4(obs + CW_HALO);
+    L.o2 = at; at += 2 * L.o2_stride;                      // [2 buffers] raw observations with halo
+    L.env_a = at; at += cw_pad4(band * obs);
+    L.env_b = at; at += cw_pad4(act * obs);
+    L.total = at;
+    return L;
+}
+__host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int C, int band) {
+    return cw_layout(n_layers, dims, C, band, dims[n_layers], false);
+}
+
+__device__ __forceinline__ float cw_normalise(float o, double mean, double std, double clip) {
+    double x = ((double)o - mean) / std;
+    x = fmin(fmax(x, -clip), clip);
+    return (float)x;
+}
+// the warp-wide sums of v[0..3] in 7 shuffles (transposing butterfly, the xor-16, 8, 4, 2, 1 tree for every row): lane L
+// returns the sum over the lanes of v[L / 8]
+__device__ __forceinline__ float cw_warp_sum4(const float (&v)[4], int lane) {
+    const bool h16 = lane & 16, h8 = lane & 8;
+    float a[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) a[i] = (h16 ? v[i + 2] : v[i]) + __shfl_xor_sync(0xffffffffu, h16 ? v[i] : v[i + 2], 16);
+    float c = (h8 ? a[1] : a[0]) + __shfl_xor_sync(0xffffffffu, h8 ? a[0] : a[1], 8);
+    c += __shfl_xor_sync(0xffffffffu, c, 4);
+    c += __shfl_xor_sync(0xffffffffu, c, 2);
+    c += __shfl_xor_sync(0xffffffffu, c, 1);
+    return c;
+}
+// all threads of all CTAs of the cluster; orders every earlier shared-memory access (local and remote) before every later one
+__device__ __forceinline__ void cw_cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ unsigned cw_cluster_rank() {
+    unsigned r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ unsigned cw_cluster_nctas() {
+    unsigned r;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+    return r;
+}
+// v into the same shared-memory word of CTA `rank` of the cluster
+__device__ __forceinline__ void cw_store_remote(float* local, unsigned rank, float v) {
+    const unsigned a = (unsigned)__cvta_generic_to_shared(local);
+    unsigned r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(r), "f"(v) : "memory");
+}
+
+// one layer of this CTA in the step loop (read from shared memory: a per-layer index into registers would go to local memory)
+struct CwLayer { int in, nr, S, r0, w, bias, xin, out, woff, boff; };
+
+// ACT: every layer of the policy applies the call's activation (p.r.activation, es_act) instead of tanh; the env's own
+// tanh(A obs + B a) stays tanh
+template <int NL, bool BINNED, bool NOISY, bool ACT = false>
+__device__ __forceinline__ void cw_rollout(const CwParams& p) {
+    extern __shared__ __align__(16) float cw_smem[];
+    __shared__ CwLayer cw_layers[NL];
+    const unsigned C = cw_cluster_nctas(), rank = cw_cluster_rank();
+    const int n_clusters = gridDim.x / C, cluster = blockIdx.x / C;
+    const int obs = p.r.dims[0], act = p.r.act, T = p.r.T, band = p.env.band;
+    const CwLayout L = BINNED ? cw_layout(NL, p.r.dims, (int)C, band, act, true) : cw_layout(NL, p.r.dims, (int)C, band);
+    double* __restrict__ nmean = reinterpret_cast<double*>(cw_smem + L.norm);
+    double* __restrict__ nstd = nmean + obs;
+    double* __restrict__ rfit = reinterpret_cast<double*>(cw_smem + L.racc);
+    float* __restrict__ rpos = cw_smem + L.racc + 2;
+    float* __restrict__ x = cw_smem + L.x;
+    float* __restrict__ prod = cw_smem + L.prod;
+    float2* __restrict__ stat = reinterpret_cast<float2*>(cw_smem + L.stat);
+    float* __restrict__ o2 = cw_smem + L.o2;
+    const float* __restrict__ envA = cw_smem + L.env_a;
+    const float* __restrict__ envB = cw_smem + L.env_b;
+    const float* __restrict__ action = cw_smem + (BINNED ? L.abin : L.act[NL - 1]);
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const bool rew_warp = rank == 0 && warp == CW_WARPS - 1;
+
+    for (int i = tid; i < band * obs; i += CW_THREADS) cw_smem[L.env_a + i] = p.env.env_a[i];
+    for (int i = tid; i < act * obs; i += CW_THREADS) cw_smem[L.env_b + i] = p.env.env_b[i];
+    for (int i = tid; i < obs; i += CW_THREADS) { nmean[i] = p.env.ob_mean[i]; nstd[i] = p.env.ob_std[i]; }
+    for (int i = tid; i < L.w[0] - L.x; i += CW_THREADS) cw_smem[L.x + i] = 0.f;     // x and every a_l, padding included
+    if (tid == 0) {
+#pragma unroll
+        for (int l = 0; l < NL; ++l) {                      // this CTA owns rows [r0, r0 + nr) of layer l (nr may be <= 0)
+            const int r0 = (int)rank * L.rows[l];
+            cw_layers[l] = {p.r.dims[l], min(L.rows[l], p.r.dims[l + 1] - r0), L.stride[l], r0, L.w[l], L.bias[l],
+                            l ? L.act[l - 1] : L.x, L.act[l], p.r.w_off[l], p.r.b_off[l]};
+        }
+    }
+    cw_cluster_sync();                                      // START: every CTA of the cluster runs and has zeroed its buffers
+
+    for (int ev = cluster; ev < 2 * p.r.n_pairs; ev += n_clusters) {
+        const int pair = ev >> 1, neg = ev & 1;
+        const long long base = es_checked_slice(p.r.idx[pair], p.r.P, p.r.table_len, p.r.err);
+        const float* __restrict__ eps = p.r.table + base;
+        const float* __restrict__ th = p.r.theta;
+        const float sg = p.r.sigma;
+        auto w_at = [&](int at) {                           // theta + sigma eps or theta - sigma eps
+            float wp, wm;
+            es_pheno_pm(sg, eps[at], th[at], wp, wm);
+            return neg ? wm : wp;
+        };
+#pragma unroll 1
+        for (int l = 0; l < NL; ++l) {                      // this CTA's rows of every layer, zero padded to a multiple of 4
+            const CwLayer ly = cw_layers[l];
+            const int R4 = cw_pad4(max(ly.nr, 0)), in = ly.in, S = ly.S;
+            float* __restrict__ W = cw_smem + ly.w;
+            for (int r = warp; r < R4; r += CW_WARPS)
+                for (int k = lane; k < S; k += 32)
+                    W[r * S + k] = (r < ly.nr && k < in) ? w_at(ly.woff + (ly.r0 + r) * in + k) : 0.f;
+            for (int r = tid; r < R4; r += CW_THREADS) cw_smem[ly.bias + r] = r < ly.nr ? w_at(ly.boff + ly.r0 + r) : 0.f;
+        }
+        auto start_episode = [&]() {                        // a fresh env: obs_0, position 0
+            for (int i = tid; i < obs; i += CW_THREADS) {
+                const float v = p.env.obs0[i];
+                es_put_obs(o2, i, v, obs, band);
+                x[i] = cw_normalise(v, nmean[i], nstd[i], p.env.ob_clip);
+                stat[i] = make_float2(0.f, 0.f);
+            }
+        };
+        start_episode();
+        if (tid == 0) { rfit[0] = 0.0; rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
+        bool save = false;                                  // the evaluation's save_obs coin (legacy random_sample < chance)
+        if (p.env.coins) {
+            const uint32_t* c = p.env.coins + (size_t)pair * 4 + 2 * neg;
+            save = mt19937_random_sample(c[0], c[1]) < p.env.save_obs_chance;
+        }
+        const bool keep_stat = rank == 0 && p.env.ob_sum && save;
+        __syncthreads();
+
+        const int n_eps = NOISY ? p.r.n_episodes : 1;
+        for (int ep = 0; ep < n_eps; ++ep) {
+            const bool last_ep = ep == n_eps - 1;
+            const bool add_stat = keep_stat && last_ep;     // behaviour and ObStat: the last episode's
+            if (NOISY && ep > 0) {
+                start_episode();
+                if (tid == 0) { rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
+                __syncthreads();
+            }
+
+            // this cluster's episode sums, and the noise of the output row this lane owns (row 4 warp + lane / 8 of the last
+            // layer's pass, lanes 8 i)
+            double* __restrict__ erow = NOISY ? p.env.ep_rows + (size_t)cluster * T : nullptr;
+            const float* __restrict__ nzp = nullptr;
+            if (NOISY && (lane & 7) == 0) {
+                const CwLayer& lo = cw_layers[NL - 1];
+                const int r = 4 * warp + (lane >> 3);
+                if (r < lo.nr) nzp = p.r.act_noise + (((size_t)pair * 2 + neg) * n_eps + ep) * T * act + lo.r0 + r;
+            }
+
+            for (int t = 0; t < T; ++t) {
+                const int cur = t & 1;
+                float crow0 = 0.f, crow1 = 0.f;
+                double esum = 0.0;                              // the earlier episodes' rewards of this step
+                if (rew_warp) {                                 // this step's reward coefficients: in flight under the layers
+                    const float* __restrict__ c = p.r.rew_vec + (size_t)t * act;
+                    if (lane < act) crow0 = __ldg(c + lane);
+                    if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
+                    if (NOISY && lane == 0 && ep > 0) esum = erow[t];
+                }
+                float nz = 0.f;                                 // this lane's action noise: in flight under the layers
+                if (NOISY && nzp) nz = __ldg(nzp + (size_t)t * act);
+                // ---- the layers: 4 rows per warp and pass, each row's tanh stored into every CTA's a_l, then B_l ----
+#pragma unroll 1
+                for (int l = 0; l < NL; ++l) {
+                    const CwLayer ly = cw_layers[l];
+                    const int S = ly.S, r0 = ly.r0, nr = ly.nr, nj = S >> 5;
+                    const float* __restrict__ xin = cw_smem + ly.xin + lane;
+                    const float* __restrict__ W = cw_smem + ly.w + lane;
+                    const float* __restrict__ bias = cw_smem + ly.bias;
+                    float* __restrict__ out = cw_smem + ly.out;
+                    for (int g = 4 * warp; g < nr; g += 4 * CW_WARPS) {
+                        float z[4] = {0.f, 0.f, 0.f, 0.f};
+                        const float* __restrict__ wr = W + g * S;
+#pragma unroll 4
+                        for (int j = 0; j < nj; ++j) {
+                            const float xv = xin[32 * j];
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) z[r] = fmaf(wr[r * S + 32 * j], xv, z[r]);
+                        }
+                        const float s = cw_warp_sum4(z, lane);
+                        const int r = g + (lane >> 3);
+                        if ((lane & 7) == 0 && r < nr) {
+                            const float h = ACT ? es_act(p.r.activation, p.r.act_param, s + bias[r]) : es_tanh_exp(s + bias[r]);
+                            const float y = (NOISY && l == NL - 1) ? __fadd_rn(h, nz) : h;
+                            for (unsigned q = 0; q < C; ++q) cw_store_remote(out + r0 + r, q, y);
+                        }
+                    }
+                    cw_cluster_sync();                          // B_l
+                }
+                if (BINNED) {                                   // the actions from this CTA's copy of the last layer's outputs
+                    if (tid < act) {
+                        const float* __restrict__ o = cw_smem + L.act[NL - 1] + tid * p.r.bins;
+                        cw_smem[L.abin + tid] = es_binned_action(p.r.bins, p.r.head_scale, p.r.head_low, p.r.head_range, tid,
+                                                                 [&](int b) { return o[b]; });
+                    }
+                    __syncthreads();
+                }
+                // ---- env step, redundantly in every CTA: thread i owns observation i ----
+                if (tid < obs) {
+                    const float* __restrict__ oc = o2 + cur * L.o2_stride;
+                    const int i = tid;
+                    float acc = 0.f;
+                    for (int d = 0; d < band; ++d) acc = __fadd_rn(acc, __fmul_rn(envA[d * obs + i], oc[i + d]));
+                    for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, __fmul_rn(envB[j * obs + i], action[j]));
+                    const float nv = es_tanh_exp(acc);
+                    es_put_obs(o2 + (cur ^ 1) * L.o2_stride, i, nv, obs, band);
+                    x[i] = cw_normalise(nv, nmean[i], nstd[i], p.env.ob_clip);
+                    if (add_stat) {                             // float32 column sums in step order (numpy's axis-0 reduction)
+                        float2 st = stat[i];
+                        st.x = __fadd_rn(st.x, nv); st.y = __fadd_rn(st.y, __fmul_rn(nv, nv));
+                        stat[i] = st;
+                    }
+                }
+                // ---- reward (float32 dot in index order, summed in float64) and position: rank 0's last warp ----
+                if (rew_warp) {
+                    if (lane < act) prod[lane] = __fmul_rn(action[lane], crow0);
+                    if (lane + 32 < act) prod[lane + 32] = __fmul_rn(action[lane + 32], crow1);
+                    __syncwarp();
+                    if (lane == 0) {
+                        float acc = 0.f;
+                        for (int j = 0; j < act; ++j) acc = __fadd_rn(acc, prod[j]);
+                        if (!NOISY) {
+                            rfit[0] += (double)acc;
+                        } else if (!last_ep) {                  // the float64 per-step sum over the episodes, in their order
+                            erow[t] = esum + (double)acc;
+                        } else {                                // ... and its mean (obj.py:57-61)
+                            rfit[0] += (esum + (double)acc) / n_eps;
+                        }
+                        const float ps = p.r.pos_scale;
+                        rpos[0] = __fadd_rn(rpos[0], __fmul_rn(ps, action[0]));
+                        rpos[1] = __fadd_rn(rpos[1], __fmul_rn(ps, action[1 % act]));
+                        rpos[2] = __fadd_rn(rpos[2], __fmul_rn(ps, action[2 % act]));
+                    }
+                    __syncwarp();
+                }
+                __syncthreads();                                // x and the raw observation before the next step's layer 0
+            }
+        }
+        if (rew_warp && lane == 0) {
+            (neg ? p.r.fit_neg : p.r.fit_pos)[(size_t)pair * p.r.fit_stride] = rfit[0];
+            float* bv = neg ? p.r.behv_neg : p.r.behv_pos;
+            if (bv) { bv[(size_t)pair * 3 + 0] = rpos[0]; bv[(size_t)pair * 3 + 1] = rpos[1]; bv[(size_t)pair * 3 + 2] = rpos[2]; }
+        }
+        if (keep_stat) {
+            // ObStat.inc of a saved rollout: float32 column sums added in float64 (the order over rollouts is the atomics')
+            for (int i = tid; i < obs; i += CW_THREADS) {
+                const float2 st = stat[i];
+                atomicAdd(p.env.ob_sum + i, (double)st.x);
+                atomicAdd(p.env.ob_sumsq + i, (double)st.y);
+            }
+            if (tid == 0) { atomicAdd(p.env.ob_count, (double)T); atomicAdd(p.env.ob_count + 1, 1.0); }
+        }
+        cw_cluster_sync();                                  // REUSE (the last one: EXIT)
+    }
+}
+
+typedef void (*CwKernel)(const CwParams);
+
+// a launch of `clusters` clusters of C CTAs (attr: the cluster-dimension attribute the config points to)
+static cudaLaunchConfig_t cw_config(int C, size_t smem, int clusters, cudaStream_t stream, cudaLaunchAttribute* attr) {
+    attr->id = cudaLaunchAttributeClusterDimension;
+    attr->val.clusterDim.x = C; attr->val.clusterDim.y = 1; attr->val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(clusters * C); cfg.blockDim = dim3(CW_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    return cfg;
+}
+
+// the number of clusters of the shape that can be resident at once (the persistent grid), 0 when none fits
+static int cw_max_clusters(CwKernel k, int C, size_t smem, int* clusters) {
+    ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = cw_config(C, smem, 1, nullptr, &attr);
+    ES_CHECK_CUDA(cudaOccupancyMaxActiveClusters(clusters, k, &cfg));
+    return ES_OK;
+}
+}  // namespace

@@ -38,8 +38,11 @@ struct RfDesc {
     int* err;                    // ctx error word (es_checked_slice)
 };
 
+// ACT: the call's activation `act` (es_act, parameter act_param) after the layer; else tanh
+template <bool ACT>
 __device__ __forceinline__ void rf_dense(const float* __restrict__ Wsm, const float* __restrict__ bsm, int in4, int pitch,
-                                         int out, const float* __restrict__ Xin, float* __restrict__ Xout, int xpitch) {
+                                         int out, const float* __restrict__ Xin, float* __restrict__ Xout, int xpitch, int act,
+                                         float act_param) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_blocks = (out + 31) >> 5;
     const int tasks = n_blocks * (RF_TM / RF_RT);
@@ -68,7 +71,8 @@ __device__ __forceinline__ void rf_dense(const float* __restrict__ Wsm, const fl
         }
         if (valid) {
 #pragma unroll
-            for (int r = 0; r < RF_RT; ++r) Xout[(size_t)(tg * RF_RT + r) * xpitch + n] = tanhf(acc[r]);
+            for (int r = 0; r < RF_RT; ++r)
+                Xout[(size_t)(tg * RF_RT + r) * xpitch + n] = ACT ? es_act(act, act_param, acc[r]) : tanhf(acc[r]);
         }
     }
 }
@@ -113,15 +117,16 @@ struct RfHead {
 };
 
 // GW: weights in the global scratch filled by rollout_f32_stage_kernel instead of shared memory.  BINNED: the head above;
-// else the tanh outputs are the actions (`h` unused)
-template <bool GW, bool BINNED>
+// else the outputs are the actions (`h` unused).  ACT: every layer applies the activation `act` (es_act) instead of tanh
+template <bool GW, bool BINNED, bool ACT = false>
 __device__ __forceinline__ void
 rf_rollout(const float* __restrict__ table, const int64_t* __restrict__ idx, const float* __restrict__ theta,
            float sigma, const RfDesc& d, const float* __restrict__ obsn,
            const float* __restrict__ rew_vec, int T, float pos_scale, double* __restrict__ fit_pos,
            double* __restrict__ fit_neg, int fit_stride, float* __restrict__ behv_pos,
            float* __restrict__ behv_neg, double* __restrict__ part, unsigned* __restrict__ tickets,
-           const float* __restrict__ wglobal, const float* __restrict__ act_noise, int n_eps, const RfHead& h) {
+           const float* __restrict__ wglobal, const float* __restrict__ act_noise, int n_eps, const RfHead& h, int act = 0,
+           float act_param = 0.f) {
     extern __shared__ __align__(16) float smem[];
     float* Wsm = GW ? const_cast<float*>(wglobal) + (size_t)blockIdx.x * d.w_floats : smem;    // [w_floats]
     float* Xa = GW ? smem : smem + d.w_floats;          // [RF_TM][xpitch]
@@ -168,7 +173,7 @@ rf_rollout(const float* __restrict__ table, const int64_t* __restrict__ idx, con
                 for (int i = threadIdx.x; i < RF_TM * padw; i += RF_THREADS)
                     xout[(i / padw) * d.xpitch + d.out[l] + (i % padw)] = 0.f;
             }
-            rf_dense(Wsm + d.sw_off[l], Wsm + d.sb_off[l], d.in4[l], d.pitch[l], d.out[l], xin, xout, d.xpitch);
+            rf_dense<ACT>(Wsm + d.sw_off[l], Wsm + d.sb_off[l], d.in4[l], d.pitch[l], d.out[l], xin, xout, d.xpitch, act, act_param);
             __syncthreads();
             float* tmp = xin; xin = xout; xout = tmp;
         }
@@ -268,10 +273,17 @@ template <bool GW>
 __global__ void __launch_bounds__(RF_THREADS, 1) rollout_f32_binned_kernel(RF_KERNEL_PARAMS, const RfHead h) {
     rf_rollout<GW, true>(RF_KERNEL_ARGS, h);
 }
+// policies with another activation (es_rollout_openloop_activation): the kind is uniform over the launch, so one kernel serves
+// them all; its branch sits in the store of each layer's outputs, outside the dense loop
+template <bool GW>
+__global__ void __launch_bounds__(RF_THREADS, 1) rollout_f32_act_kernel(RF_KERNEL_PARAMS, int act, float act_param) {
+    rf_rollout<GW, false, true>(RF_KERNEL_ARGS, RfHead{}, act, act_param);
+}
 
 static int rf_round4(int x) { return (x + 3) & ~3; }
 
-// one launch of a rollout kernel over the pairs of c (`head`: the binned kernels' RfHead; none for the tanh kernels)
+// one launch of a rollout kernel over the pairs of c (`head`: the binned kernels' RfHead, the activation kernels' kind and
+// parameter; none for the tanh kernels)
 template <typename K, typename... Head>
 static int rf_launch(es_ctx* ctx, K k, dim3 grid, size_t smem, cudaStream_t stream, const EsRollout& c, const RfDesc& d, double* part,
                      unsigned* tickets, const float* wglobal, Head... head) {
@@ -285,9 +297,9 @@ static int rf_launch(es_ctx* ctx, K k, dim3 grid, size_t smem, cudaStream_t stre
 int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
     // obs-64-64-act networks with enough pairs to fill the GPU: the packed-FMA kernel of rollout_f32x.cu (one CTA per pair);
     // fewer pairs than half the SMs (single evaluations, es.step's noiseless evaluation) stay here, where the episode's time
-    // tiles are split over the idle SMs.  ES_F32_GENERAL=1 forces this kernel (tests compare the two).  Binned heads always
-    // run here.
-    if (!r.bins && 2 * r.n_pairs >= ctx->sm_count && !getenv("ES_F32_GENERAL")) {
+    // tiles are split over the idle SMs.  ES_F32_GENERAL=1 forces this kernel (tests compare the two).  Binned heads and other
+    // activations always run here.
+    if (!r.bins && r.activation == ES_ACT_TANH && 2 * r.n_pairs >= ctx->sm_count && !getenv("ES_F32_GENERAL")) {
         const int rc = es_impl_rollout_f32x(ctx, r, stream);
         if (rc != ES_ERR_UNSUPPORTED) return rc;
     }
@@ -367,6 +379,9 @@ int es_impl_rollout_f32(es_ctx* ctx, const EsRollout& r, cudaStream_t stream) {
         const RfHead h = {r.act, r.bins, r.head_scale, r.head_low, r.head_range};
         const int rc = r.bins ? rf_launch(ctx, gw ? rollout_f32_binned_kernel<true> : rollout_f32_binned_kernel<false>, grid, smem, stream,
                                           c, d, part, tickets, wglobal, h)
+                     : r.activation != ES_ACT_TANH
+                              ? rf_launch(ctx, gw ? rollout_f32_act_kernel<true> : rollout_f32_act_kernel<false>, grid, smem, stream,
+                                          c, d, part, tickets, wglobal, r.activation, r.act_param)
                               : rf_launch(ctx, gw ? rollout_f32_kernel<true> : rollout_f32_kernel<false>, grid, smem, stream, c, d, part,
                                           tickets, wglobal);
         if (rc) return rc;

@@ -285,17 +285,21 @@ class Engine:
 
     def rollout(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], obsn, rew_vec, pos_scale: float,
                 fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None, behv_neg=None, mode: int = ES_ROLLOUT_F32,
-                act_noise=None, episodes: int = 1, head=None):
+                act_noise=None, episodes: int = 1, head=None, activation=None):
         """``act_noise``: float32 [n_pairs, 2, episodes, T, act] scaled action noise (``draw_noisy``), added to every action.
         ``episodes`` > 1 (obj.py:54-63's eps_per_policy): every evaluation is the per-step mean of that many episodes, each
         with its own noise rows; behaviour is the last episode's.  Without ``act_noise`` the episodes are identical and the
         result is the single episode's.
         ``head``: None or ``'tanh'`` (the outputs are the actions), or an ``nn.BinnedHead`` (FFBinned:
         es_rollout_openloop_binned; ``layer_sizes[-1]`` is adim * bins, ``rew_vec`` [T, adim]; no action noise; modes F32 and
-        TC3)."""
+        TC3).
+        ``activation``: None (tanh), or an ``nn.Activation`` every layer applies (es_rollout_openloop_activation: modes F32 and
+        TC3; with TC3 a hidden value beyond float16 range makes the next ``sync`` raise)."""
         binned = head is not None and head != 'tanh'
         if binned and (act_noise is not None or int(episodes) != 1):
             raise ValueError('a binned head draws no action noise: act_noise must be None and episodes 1')
+        if binned and activation is not None:
+            raise ValueError('a binned head is a tanh stack: activation must be None')
         n, ls = self._check_rollout(table, idx, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg)
         d = self.device
         _req(obsn, torch.float32, 'obsn', d); _req(rew_vec, torch.float32, 'rew_vec', d)
@@ -322,6 +326,10 @@ class Engine:
             if ref is None or ref() is not table or ver != table._version:
                 check(self.lib.es_noise_table_changed(self._ctx), 'es_noise_table_changed')
                 self._tc_table = (weakref.ref(table), table._version)
+        if activation is not None:
+            check(self.lib.es_rollout_openloop_activation(*args, _ptr(act_noise), episodes, int(activation.kind), float(activation.param),
+                                                          int(mode), self.stream), 'es_rollout_openloop_activation')
+            return
         check(self.lib.es_rollout_openloop_episodes(*args, _ptr(act_noise), episodes, int(mode), self.stream), 'es_rollout_openloop')
 
     def _head_arrays(self, head):
@@ -372,15 +380,18 @@ class Engine:
     def rollout_closed_mlp(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std, ob_clip: float,
                            obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg, fit_stride: int = 1, behv_pos=None,
                            behv_neg=None, coin_words=None, save_obs_chance: float = 0.0, ob_sum=None, ob_sumsq=None, ob_count=None,
-                           head=None, act_noise=None, episodes: int = 1):
+                           head=None, act_noise=None, episodes: int = 1, activation=None):
         """``rollout_closed`` (same arguments and checks) for every tanh MLP the closed loop covers: 2 to 4 hidden layers of
         at most 256 units, obs <= 384, act <= 64.  The shapes ``rollout_closed`` takes run its kernel; the others one
         thread-block cluster per evaluation (``closed_mlp_plan``).  ``head``: as ``rollout``; a binned head
         (es_rollout_closedloop_mlp_binned) always runs the cluster kernel, ``env_b`` [adim, obs] and ``rew_vec`` [T, adim].
         ``act_noise`` / ``episodes``: as ``rollout`` (es_rollout_closedloop_mlp_episodes): every episode restarts the env and
         steps it with the noisy actions; behaviour and ObStat are the last episode's.  Without ``act_noise`` the episodes are
-        identical and the library runs one on the noise-free kernels."""
+        identical and the library runs one on the noise-free kernels.  ``activation``: as ``rollout``
+        (es_rollout_closedloop_mlp_activation: kinds other than tanh run the cluster kernel at every covered shape)."""
         binned = head is not None and head != 'tanh'
+        if binned and activation is not None:
+            raise ValueError('a binned head is a tanh stack: activation must be None')
         episodes = int(episodes)
         if episodes < 1:
             raise ValueError(f'episodes must be >= 1, got {episodes}')
@@ -402,21 +413,32 @@ class Engine:
             check(self.lib.es_rollout_closedloop_mlp_binned(*args, int(head.bins), _ptr(low), _ptr(rng), self.stream),
                   'es_rollout_closedloop_mlp_binned')
             return
+        if activation is not None:
+            check(self.lib.es_rollout_closedloop_mlp_activation(*args, _ptr(act_noise), episodes, int(activation.kind),
+                                                                float(activation.param), self.stream),
+                  'es_rollout_closedloop_mlp_activation')
+            return
         # with no noise and one episode this is es_rollout_closedloop_mlp (a forwarder to it): its errors keep that name
         plain = act_noise is None and episodes == 1
         check(self.lib.es_rollout_closedloop_mlp_episodes(*args, _ptr(act_noise), episodes, self.stream),
               'es_rollout_closedloop_mlp' if plain else 'es_rollout_closedloop_mlp_episodes')
 
-    def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int, head=None):
+    def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int, head=None, activation=None):
         """How ``rollout_closed_mlp`` runs a shape: (CTAs per cluster, clusters resident at once, shared memory bytes per CTA);
         (0, SM count, 0) for ``rollout_closed``'s one-CTA kernel.  Raises EsLibraryError for a shape it does not cover.
-        ``head``: as ``rollout_closed_mlp`` (a binned head's plan is always a cluster of >= 1 CTA)."""
+        ``head``, ``activation``: as ``rollout_closed_mlp`` (a binned head's plan, and that of an activation other than tanh, is
+        always a cluster of >= 1 CTA)."""
         ls = (C.c_int * len(layer_sizes))(*[int(x) for x in layer_sizes])
         cs, nc, sm = C.c_int(0), C.c_int(0), C.c_int64(0)
         if head is not None and head != 'tanh':
             check(self.lib.es_rollout_closedloop_mlp_binned_plan(self._ctx, ls, len(layer_sizes) - 1, int(band), int(head.bins),
                                                                  C.byref(cs), C.byref(nc), C.byref(sm)),
                   'es_rollout_closedloop_mlp_binned_plan')
+            return cs.value, nc.value, sm.value
+        if activation is not None:
+            check(self.lib.es_rollout_closedloop_mlp_activation_plan(self._ctx, ls, len(layer_sizes) - 1, int(band),
+                                                                     int(activation.kind), C.byref(cs), C.byref(nc), C.byref(sm)),
+                  'es_rollout_closedloop_mlp_activation_plan')
             return cs.value, nc.value, sm.value
         check(self.lib.es_rollout_closedloop_mlp_plan(self._ctx, ls, len(layer_sizes) - 1, int(band), C.byref(cs), C.byref(nc),
                                                       C.byref(sm)), 'es_rollout_closedloop_mlp_plan')

@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from . import dist
-from ._lib import ES_MT_N, ES_OBJ_DIST, ES_OBJ_MEAN_REWARD, ES_OBJ_XDIST, ES_ROLLOUT_F32
+from ._lib import ES_ACT_TANH, ES_MT_N, ES_OBJ_DIST, ES_OBJ_MEAN_REWARD, ES_OBJ_XDIST, ES_ROLLOUT_F32
 from .engine import Engine, get_engine
 from .nn.optimizers import Optimizer
 
@@ -80,7 +80,7 @@ class DeviceGeneration:
                  save_obs_chance: float = 0.0, archive: Optional[torch.Tensor] = None, nov_k: int = 10,
                  moo_w: float = 1.0, rollout_mode: int = ES_ROLLOUT_F32, comm: Optional[dist.Comm] = None,
                  engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1, head=None,
-                 closed_act_noise: bool = False, objective: str = 'reward'):
+                 closed_act_noise: bool = False, objective: str = 'reward', activation=None):
         self.eng = engine or get_engine()
         if objective not in OBJECTIVES:
             raise ValueError(f'objective must be one of {OBJECTIVES}, got {objective!r}')
@@ -108,6 +108,12 @@ class DeviceGeneration:
         # layer's adim * bins outputs become the env's adim actions
         self.head = None if head == 'tanh' else head
         self.head_key = None if self.head is None else self.head.key()       # what a cached generation is valid for
+        # the activation of every layer (nn.BaseNet.activation): None for tanh, else an nn.Activation the rollouts apply
+        # (es_rollout_*_activation); act_key is its part of the cache key
+        self.activation = None if activation is None or activation.kind == ES_ACT_TANH else activation
+        self.act_key = None if self.activation is None else self.activation.key()
+        if self.head is not None and self.activation is not None:
+            raise ValueError('a binned head is a tanh stack: activation must be None or tanh')
         self.obs_dim = self.layer_sizes[0]
         self.act_dim = self.head.adim if self.head is not None else self.layer_sizes[-1]
         self.obs_stream = obs_stream                    # [T+1, obs_dim]
@@ -250,7 +256,8 @@ class DeviceGeneration:
                                      ob_sum=self.gen_sum if self.extra_words else None,
                                      ob_sumsq=self.gen_sumsq if self.extra_words else None,
                                      ob_count=self.gen_count if self.extra_words else None, head=self.head,
-                                     act_noise=self.act_noise if noisy else None, episodes=self.episodes if noisy else 1)
+                                     act_noise=self.act_noise if noisy else None, episodes=self.episodes if noisy else 1,
+                                     activation=self.activation)
             self._score()
         else:
             self._evaluate_openloop(fp, fn)
@@ -276,7 +283,7 @@ class DeviceGeneration:
                       self.pos_scale, fp, fn, self.n_obj, None if self.behv is None else self.behv[0],
                       None if self.behv is None else self.behv[1], self.rollout_mode,
                       act_noise=self.act_noise if self.ac_std != 0.0 else None,
-                      episodes=self.episodes if self.ac_std != 0.0 else 1, head=self.head)
+                      episodes=self.episodes if self.ac_std != 0.0 else 1, head=self.head, activation=self.activation)
         self._score()
         self._gen_stats.zero_()
         if self.extra_words:
@@ -353,10 +360,11 @@ class DeviceGeneration:
             obs0, env_a, env_b = self.closed
             e.rollout_closed_mlp(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,
                                  obs0, env_a, env_b, self.rew_vec, self.pos_scale, fit0[0:1], fit0[1:2], 1, behv0[0].view(-1),
-                                 behv0[1].view(-1), head=self.head)
+                                 behv0[1].view(-1), head=self.head, activation=self.activation)
             return fit0, behv0
         e.rollout(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.obsn, self.rew_vec, self.pos_scale,
-                  fit0[0:1], fit0[1:2], 1, behv0[0].view(-1), behv0[1].view(-1), ES_ROLLOUT_F32, head=self.head)
+                  fit0[0:1], fit0[1:2], 1, behv0[0].view(-1), behv0[1].view(-1), ES_ROLLOUT_F32, head=self.head,
+                  activation=self.activation)
         return fit0, behv0
 
     def skip_eval_coins(self, n_evals: int = 1):

@@ -14,6 +14,10 @@ in order), with the last episode's behaviour.  With action noise every episode d
 T x act gaussians from the stream; without it the episodes are identical and the mean is
 exactly the single episode (E copies of a float32 sum exactly in float64, and (E r) / E == r).
 
+``fuse_activations``: FeedForward policies whose activation is not tanh (ReLU, LeakyReLU, ELU, Sigmoid: ``BaseNet.activation``)
+run the fused device rollouts too (es_rollout_*_activation) -- in ``es.step``, ``es.test_params`` and this object's own
+call.  Off by default: such a policy then runs run_model's python loop with the module's own forward, as the reference does.
+
 ``result`` is the TrainingResult adaptor the script's fit_fn builds (training_result.py:62-97): RewardResult (the default
 without an archive), MeanRewardResult, DistResult, XDistResult, NSResult (novelty alone) or NSRResult (reward and novelty,
 the default with an archive).  The fused generation computes the same column(s) on the device.
@@ -39,7 +43,8 @@ class BatchedRollout:
     def __init__(self, env, max_steps: int, coins_per_eval: int = 1, save_obs_chance: float = 0.0,
                  archive: Optional[np.ndarray] = None, nov_k: int = 10,
                  rank_streams: Optional[Sequence[np.random.RandomState]] = None,
-                 rollout_mode: int = _lib.ES_ROLLOUT_F32, episodes: int = 1, result: Optional[type] = None):
+                 rollout_mode: int = _lib.ES_ROLLOUT_F32, episodes: int = 1, result: Optional[type] = None,
+                 fuse_activations: bool = False):
         if not (getattr(env, 'is_synthetic_openloop', False) or getattr(env, 'is_synthetic_closedloop', False)):
             raise TypeError('BatchedRollout needs a synthetic env (es_pytorch_b200.gym.synthetic_env: open- or closed-loop)')
         self.env = env
@@ -50,6 +55,7 @@ class BatchedRollout:
         self.nov_k = int(nov_k)
         self.rank_streams = list(rank_streams) if rank_streams is not None else None
         self.rollout_mode = rollout_mode
+        self.fuse_activations = bool(fuse_activations)
         if isinstance(episodes, bool) or not isinstance(episodes, (int, np.integer)):
             raise TypeError(f'episodes must be an integer, got {episodes!r}')
         if episodes < 0:
@@ -102,13 +108,16 @@ class BatchedRollout:
                     rs.random()
         noise_rs = streams[0] if (use_ac_noise and streams is not None and len(streams)) else None
         head = model.head() if hasattr(model, 'head') else None
+        activation = self.fused_activation(model) if head is None else None
+        if activation is not None:
+            head = 'tanh'                                   # the outputs are the actions
         noisy = noise_rs is not None and float(getattr(model, '_action_std', 0) or 0) != 0
         episodes = self.episodes if noisy else 1
         if head is not None and (getattr(self.env, 'is_synthetic_openloop', False)
-                                 or self._closed_on_device(model.layer_sizes(), head)):
+                                 or self._closed_on_device(model.layer_sizes(), head, activation)):
             # the evaluation, all its episodes, as one launch (the observations are not returned: this result never carries them)
             from .gym_runner import _device_episode
-            total, pos, _ = _device_episode(model, self.env, self.max_steps, noise_rs if noisy else None, episodes)
+            total, pos, _ = _device_episode(model, self.env, self.max_steps, noise_rs if noisy else None, episodes, activation)
             return self.result_from_device(total, pos)
         if episodes > 1:
             rews, behv, steps = self._run_episodes(model, noise_rs, episodes)
@@ -117,19 +126,27 @@ class BatchedRollout:
         no_obs = np.array([np.zeros(self.env.observation_space.shape)])
         return self._result(rews, behv, no_obs, steps)
 
-    def _closed_on_device(self, sizes, head='tanh') -> bool:
+    def fused_activation(self, model):
+        """The ``nn.Activation`` (not tanh) this object rolls ``model`` out with on the device, or None: only with
+        ``fuse_activations`` and a network whose ``BaseNet.activation`` is one."""
+        if not self.fuse_activations or not hasattr(model, 'activation'):
+            return None
+        act = model.activation()
+        return None if act is None or act.kind == _lib.ES_ACT_TANH else act
+
+    def _closed_on_device(self, sizes, head='tanh', activation=None) -> bool:
         """Whether a closed-loop episode of a tanh MLP runs as one launch (es_rollout_closedloop_mlp): two hidden layers always
         do (a shape outside the kernels' coverage raises there); three or four when the kernels cover the shape; anything else
         runs run_model's python loop.  A binned head (es_rollout_closedloop_mlp_binned) runs as one launch when the cluster
-        kernel covers the shape."""
+        kernel covers the shape, and so does a policy with another activation (es_rollout_closedloop_mlp_activation)."""
         n_hidden = len(sizes) - 2
-        if n_hidden == 2 and head == 'tanh':
+        if n_hidden == 2 and head == 'tanh' and activation is None:
             return True
         if n_hidden not in (2, 3, 4):
             return False
         from ..engine import get_engine
         try:
-            get_engine().closed_mlp_plan(sizes, self.env.band, head)
+            get_engine().closed_mlp_plan(sizes, self.env.band, head, activation)
         except _lib.EsLibraryError:
             return False
         return True

@@ -35,14 +35,15 @@ def hbaselines_pos(env):
     return tuple(env.wrapped_env.get_body_com('torso')[:3])
 
 
-def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
+def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1, activation=None):
     """One evaluation on the open- or closed-loop synthetic env as one launch (sigma = 0).  With ``rs`` and a tanh model's
     ac_std != 0: the action noise of ``episodes`` episodes drawn back to back from ``rs``, the per-step mean over the episodes
-    (obj.py:54-63).  Returns (fitness, the last episode's final position, steps)."""
+    (obj.py:54-63).  ``activation``: the model's ``nn.Activation`` when it is not a tanh one (its outputs are the actions, as
+    a tanh model's).  Returns (fitness, the last episode's final position, steps)."""
     from ..engine import get_engine
     from ..core.policy import Policy
     eng = get_engine()
-    sizes, head = model.layer_sizes(), model.head()
+    sizes, head = model.layer_sizes(), ('tanh' if activation is not None else model.head())
     T = min(int(max_steps), env.T)
     obs_dev, rew_dev = env.device_arrays(eng)
     theta = eng.to_device(Policy.get_flat(model), torch.float32)
@@ -65,11 +66,12 @@ def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1):
     out = (fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1))
     if getattr(env, 'is_synthetic_closedloop', False):
         eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), *env.device_closed(eng),
-                               rew_dev[:T].contiguous(), env.pos_scale, *out, head=head, act_noise=noise, episodes=episodes)
+                               rew_dev[:T].contiguous(), env.pos_scale, *out, head=head, act_noise=noise, episodes=episodes,
+                               activation=activation)
     else:
         obsn = eng.normalise_obs(obs_dev[:T], mean, std, float(model.ob_clip))
         eng.rollout(table, idx, theta, 0.0, sizes, obsn, rew_dev[:T].contiguous(), env.pos_scale, *out, act_noise=noise,
-                    episodes=episodes, head=head)
+                    episodes=episodes, head=head, activation=activation)
     return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), T
 
 

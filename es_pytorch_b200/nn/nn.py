@@ -42,6 +42,36 @@ class BinnedHead(NamedTuple):
         return engine.to_device(low), engine.to_device(rng)
 
 
+class Activation(NamedTuple):
+    """The activation a FeedForward applies after every layer, as the fused rollouts take it (es_rollout_*_activation):
+    ``kind`` one of the ``_lib.ES_ACT_*`` constants, ``param`` LeakyReLU's negative slope or ELU's alpha rounded to float32
+    (torch's CPU kernels compute with the float32 value; 0 for the other kinds)."""
+    kind: int
+    param: float
+
+    def key(self) -> tuple:
+        """What identifies the activation's arithmetic (a cache key)."""
+        return ('activation', int(self.kind), float(self.param))
+
+
+def _activation_of(m: nn.Module) -> Optional[Activation]:
+    """The Activation of one torch module, None for a module the kernels do not evaluate (subclasses included: they may
+    override forward)."""
+    from .._lib import ES_ACT_ELU, ES_ACT_LEAKY_RELU, ES_ACT_RELU, ES_ACT_SIGMOID, ES_ACT_TANH
+    kind = {nn.Tanh: ES_ACT_TANH, nn.ReLU: ES_ACT_RELU, nn.LeakyReLU: ES_ACT_LEAKY_RELU, nn.ELU: ES_ACT_ELU,
+            nn.Sigmoid: ES_ACT_SIGMOID}.get(type(m))
+    if kind is None:
+        return None
+    param = 0.0
+    if kind == ES_ACT_LEAKY_RELU:
+        param = float(np.float32(m.negative_slope))
+    elif kind == ES_ACT_ELU:
+        param = float(np.float32(m.alpha))
+    if not np.isfinite(param):
+        return None
+    return Activation(kind, param)
+
+
 class BaseNet(nn.Module, ABC):
     def __init__(self, layers: List[nn.Module], ob_shape: tuple, ob_clip: float = 5):
         super().__init__()
@@ -71,6 +101,22 @@ class BaseNet(nn.Module, ABC):
         mods = list(self.model)
         return (len(mods) % 2 == 0 and all(isinstance(m, nn.Linear) for m in mods[0::2])
                 and all(isinstance(m, nn.Tanh) for m in mods[1::2]))
+
+    def activation(self) -> Optional[Activation]:
+        """The activation the fused rollouts evaluate for this network (es_rollout_*_activation): a plain-forward FeedForward
+        whose stack is Linear layers each followed by the same kind of supported module (Tanh, ReLU, LeakyReLU, ELU, Sigmoid)
+        with the same float32 parameter.  None for anything else: mixed activations, other modules, FFBinned,
+        FFIntegGausAction* and subclasses with their own forward.  Tanh networks give ``Activation(ES_ACT_TANH, 0.0)``; they
+        are fused by default (``head``), the other kinds only where a ``BatchedRollout(fuse_activations=True)`` asks for it."""
+        if type(self).forward is not FeedForward.forward:
+            return None
+        mods = list(self.model)
+        if len(mods) == 0 or len(mods) % 2 or not all(type(m) is nn.Linear for m in mods[0::2]):
+            return None
+        acts = {_activation_of(m) for m in mods[1::2]}
+        if len(acts) != 1 or None in acts:
+            return None
+        return acts.pop()
 
     def head(self) -> Optional[Union[str, BinnedHead]]:
         """How the fused rollout kernels turn this network's outputs into actions: ``'tanh'`` for the tanh MLPs of

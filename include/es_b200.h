@@ -158,6 +158,39 @@ int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_le
                                double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
                                int bins, const float* low, const float* range, int mode, void* stream);
 
+/* ---- policies with other activations -------------------------------------------------------------------------------
+ * FeedForward takes its activation as an argument (src/nn/nn.py:25-36) and applies it after every layer, the output included.
+ * activation: the kind the policy applies after every layer; act_param: LeakyReLU's negative slope or ELU's alpha as float32
+ * (torch's CPU kernels round both to the tensor's float32), ignored by the other kinds.  Every kind is evaluated in float32
+ * as torch's CPU kernels evaluate it:
+ *   ES_ACT_TANH        tanh(x)
+ *   ES_ACT_RELU        x < 0 ? 0 : x                   (a NaN passes, as clamp_min)
+ *   ES_ACT_LEAKY_RELU  x > 0 ? x : x * act_param       (one rounding)
+ *   ES_ACT_ELU         x > 0 ? x : act_param * expm1(x)
+ *   ES_ACT_SIGMOID     1 / (1 + exp(-x))
+ * An unknown kind, or a NaN or infinite act_param, is refused with ES_ERR_INVALID.                                      */
+#define ES_ACT_TANH        0
+#define ES_ACT_RELU        1
+#define ES_ACT_LEAKY_RELU  2
+#define ES_ACT_ELU         3
+#define ES_ACT_SIGMOID     4
+
+/* es_rollout_openloop_episodes for a policy with any of the activations above.  ES_ACT_TANH is es_rollout_openloop_episodes
+ * itself, bit for bit, in every mode.  The other kinds:
+ *   ES_ROLLOUT_F32 = the general float32 kernel (rollout_f32.cu, never the packed-FMA kernel), every shape it takes;
+ *   ES_ROLLOUT_TC3 = the wide tensor-core kernel's code (rollout_tcw_act.cu) for 2 to 4 hidden layers of widths in {64, 128,
+ *                    192, 256} (obs-64-64-act included), obs <= 256 and act <= 32, ES_ERR_UNSUPPORTED otherwise.  Its split
+ *                    operands need every hidden activation within float16 range: a hidden value beyond 65504 in magnitude
+ *                    (ReLU, leaky ReLU and ELU are unbounded) flags ES_ASYNC_F16_RANGE through the ctx's error word, the
+ *                    results of the call are invalid and es_check_async (or the next entry point) returns ES_ERR_INVALID;
+ *   ES_ROLLOUT_TC  = ES_ERR_UNSUPPORTED.                                                                                */
+int es_rollout_openloop_activation(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                   const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                   const float* obsn, const float* rew_vec, int T, float pos_scale,
+                                   double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                                   const float* act_noise, int n_episodes, int activation, float act_param, int mode,
+                                   void* stream);
+
 /* ---- a3 + a4 + a5 on the CLOSED-LOOP synthetic env (SURVEY.md section 8d's optional variant; never part of the headline) --
  * obs_{t+1} = tanh(A obs_t + B a_t): the observation depends on the policy's own actions, so the episode runs step by step
  * with one pair's perturbed weights resident on chip (rollout_closed.cu).  Replaces the same reference loop as
@@ -238,6 +271,23 @@ int es_rollout_closedloop_mlp_binned(es_ctx* ctx, const float* table, int64_t ta
  * dynamic shared memory per CTA of a binned shape, or its refusal.                                                   */
 int es_rollout_closedloop_mlp_binned_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int bins,
                                           int* cluster_size, int* clusters, int64_t* smem_bytes);
+
+/* es_rollout_closedloop_mlp_episodes for a policy with any activation of es_rollout_openloop_activation.  ES_ACT_TANH is
+ * es_rollout_closedloop_mlp_episodes itself, bit for bit.  The other kinds run rollout_closedw_act.cu, the cluster kernel's
+ * code, at every shape es_rollout_closedloop_mlp covers, a cluster of one CTA included; the env's own tanh(A obs + B a) stays
+ * tanh.  One kernel launch per call.                                                                                   */
+int es_rollout_closedloop_mlp_activation(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                         const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                         const double* ob_mean, const double* ob_std, double ob_clip,
+                                         const float* obs0, const float* env_a, int band, const float* env_b, const float* rew_vec,
+                                         int T, float pos_scale, const uint32_t* coin_words, double save_obs_chance,
+                                         double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos, float* behv_neg,
+                                         double* ob_sum, double* ob_sumsq, double* ob_count, const float* act_noise,
+                                         int n_episodes, int activation, float act_param, void* stream);
+/* es_rollout_closedloop_mlp_plan for es_rollout_closedloop_mlp_activation: ES_ACT_TANH is es_rollout_closedloop_mlp_plan; any
+ * other kind has a cluster size >= 1.                                                                                  */
+int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int activation,
+                                              int* cluster_size, int* clusters, int64_t* smem_bytes);
 
 /* ---- a2 + a4 with action noise: all draws of a generation in stream order ---------------------------------------------
  * When FeedForward._action_std != 0 every step of every rollout draws rs.randn(act_dim) from the SAME RandomState that
