@@ -105,7 +105,8 @@ __device__ __forceinline__ void st_shared_u32(void* p, uint32_t v) {
 __device__ __forceinline__ void wg_bar(int half) { asm volatile("bar.sync %0, 128;" ::"r"(1 + half) : "memory"); }
 
 // ACT: the activation of every layer (ES_ACT_*, es_act with act_param; SPLIT only for kinds other than tanh).  A hidden value
-// the float16 hi part cannot hold (|y| > 65504: ReLU, leaky ReLU and ELU are unbounded) flags ES_ASYNC_F16_RANGE in *err
+// the float16 hi part cannot hold (|y| > 65504: ReLU, leaky ReLU and ELU are unbounded) on a row of the episode (t < T) flags
+// ES_ASYNC_F16_RANGE in *err
 template <bool SPLIT, bool NOISE, bool BINNED, int ACT = ES_ACT_TANH>
 __device__ __forceinline__ void tw_rollout(const TwParams& p, float act_param = 0.f, int* err = nullptr) {
     static_assert(ACT == ES_ACT_TANH || (SPLIT && !BINNED), "other activations: ES_ROLLOUT_TC3, tanh-free heads only");
@@ -249,7 +250,10 @@ __device__ __forceinline__ void tw_rollout(const TwParams& p, float act_param = 
                                 const uint32_t o = sw128_off(rw + 8 * h, 8 * c + 2 * q);
                                 if constexpr (ACT != ES_ACT_TANH) {
                                     const float y0 = es_act<ACT>(z0, act_param), y1 = es_act<ACT>(z1, act_param);
-                                    if (ACT != ES_ACT_SIGMOID && err && (fabsf(y0) > 65504.f || fabsf(y1) > 65504.f))
+                                    // rows at t >= T (the zero observations of a partial tile) are no part of the episode:
+                                    // whatever they reach is never read
+                                    if (ACT != ES_ACT_SIGMOID && err && t0 + rw + 8 * h < p.T &&
+                                        (fabsf(y0) > 65504.f || fabsf(y1) > 65504.f))
                                         *(volatile int*)err = ES_ASYNC_F16_RANGE;
                                     uint32_t hi, lo;
                                     split_h2(y0, y1, hi, lo);

@@ -161,13 +161,14 @@ int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_le
 /* ---- policies with other activations -------------------------------------------------------------------------------
  * FeedForward takes its activation as an argument (src/nn/nn.py:25-36) and applies it after every layer, the output included.
  * activation: the kind the policy applies after every layer; act_param: LeakyReLU's negative slope or ELU's alpha as float32
- * (torch's CPU kernels round both to the tensor's float32), ignored by the other kinds.  Every kind is evaluated in float32
- * as torch's CPU kernels evaluate it:
+ * (torch's CPU kernels round both to the tensor's float32), ignored by the other kinds.  Every kind is evaluated in float32,
+ * ReLU, leaky ReLU and ELU in the forms of torch's CPU kernels, sigmoid with the fast exponential and division:
  *   ES_ACT_TANH        tanh(x)
  *   ES_ACT_RELU        x < 0 ? 0 : x                   (a NaN passes, as clamp_min)
  *   ES_ACT_LEAKY_RELU  x > 0 ? x : x * act_param       (one rounding)
  *   ES_ACT_ELU         x > 0 ? x : act_param * expm1(x)
- *   ES_ACT_SIGMOID     1 / (1 + exp(-x))
+ *   ES_ACT_SIGMOID     __fdividef(1, 1 + __expf(-x))   (absolute error ~1e-7; 0 once 1 + e^-x >= 2^126, x below about -87,
+ *                                                       where the exact value is below 1e-38)
  * An unknown kind, or a NaN or infinite act_param, is refused with ES_ERR_INVALID.                                      */
 #define ES_ACT_TANH        0
 #define ES_ACT_RELU        1
@@ -181,7 +182,7 @@ int es_rollout_openloop_binned(es_ctx* ctx, const float* table, int64_t table_le
  *   ES_ROLLOUT_TC3 = the wide tensor-core kernel's code (rollout_tcw_act.cu) for 2 to 4 hidden layers of widths in {64, 128,
  *                    192, 256} (obs-64-64-act included), obs <= 256 and act <= 32, ES_ERR_UNSUPPORTED otherwise.  Its split
  *                    operands need every hidden activation within float16 range: a hidden value beyond 65504 in magnitude
- *                    (ReLU, leaky ReLU and ELU are unbounded) flags ES_ASYNC_F16_RANGE through the ctx's error word, the
+ *                    at a step t < T (ReLU, leaky ReLU and ELU are unbounded) flags ES_ASYNC_F16_RANGE through the ctx's error word, the
  *                    results of the call are invalid and es_check_async (or the next entry point) returns ES_ERR_INVALID;
  *   ES_ROLLOUT_TC  = ES_ERR_UNSUPPORTED.                                                                                */
 int es_rollout_openloop_activation(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,

@@ -34,11 +34,34 @@ def sigmoid(z):
     return 1.0 / (1.0 + np.exp(-z))
 
 
+def form(activation, xp=np):
+    """The float64 form of an ``nn.Activation`` (None: tanh) -- the functions above -- for numpy arrays, or with
+    ``xp=torch`` the same forms for torch.float64 tensors."""
+    from es_pytorch_b200 import _lib
+    kind = _lib.ES_ACT_TANH if activation is None else int(activation.kind)
+    p = 0.0 if activation is None else float(np.float32(activation.param))
+    if xp is np:
+        return {_lib.ES_ACT_TANH: np.tanh, _lib.ES_ACT_RELU: relu, _lib.ES_ACT_LEAKY_RELU: leaky_relu(p),
+                _lib.ES_ACT_ELU: elu(p), _lib.ES_ACT_SIGMOID: sigmoid}[kind]
+    return {_lib.ES_ACT_TANH: xp.tanh, _lib.ES_ACT_RELU: lambda z: xp.clamp_min(z, 0.0),
+            _lib.ES_ACT_LEAKY_RELU: lambda z: xp.where(z > 0, z, z * p),
+            _lib.ES_ACT_ELU: lambda z: xp.where(z > 0, z, p * xp.expm1(z)),
+            _lib.ES_ACT_SIGMOID: lambda z: 1.0 / (1.0 + xp.exp(-z))}[kind]
+
+
+def per_layer(activation, n_layers: int) -> list:
+    """``activation`` for each of ``n_layers`` layers: a sequence of one function per layer as it is, one function repeated."""
+    acts = list(activation) if isinstance(activation, (list, tuple)) else [activation] * n_layers
+    assert len(acts) == n_layers, (len(acts), n_layers)
+    return acts
+
+
 def episode(w, layer_sizes, obsn, rew_vec, pos_scale, activation, noise: Optional[np.ndarray] = None):
-    """f64_rollout.episode with ``activation`` after every layer."""
+    """f64_rollout.episode with ``activation`` after every layer (or a list of one function per layer)."""
     a = obsn.astype(np.float64)
-    for wo, bo, fi, fo in f64.layer_slices(layer_sizes):
-        a = activation(a @ w[wo:wo + fi * fo].reshape(fo, fi).T + w[bo:bo + fo])
+    lay = f64.layer_slices(layer_sizes)
+    for (wo, bo, fi, fo), act_fn in zip(lay, per_layer(activation, len(lay))):
+        a = act_fn(a @ w[wo:wo + fi * fo].reshape(fo, fi).T + w[bo:bo + fo])
     c = rew_vec.astype(np.float64)
     act = a.shape[1]
     if noise is None:
@@ -76,7 +99,7 @@ def rollout_f64(table, idx, theta, sigma, layer_sizes, obsn, rew_vec, pos_scale,
 
 def closed_truth(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a, env_b, rew_vec, pos_scale,
                  act_noise=None, episodes: int = 1, activation=np.tanh):
-    """closed_f64.truth (no mutation) with the policy's ``activation``: a dict of float64 arrays indexed [2][n] ([2][n][...]
+    """closed_f64.truth (no mutation) with the policy's ``activation`` (or a list of one per layer): a dict of float64 arrays indexed [2][n] ([2][n][...]
     for vectors): 'fit', 'mass', 'behv', 'mag', 'osum', 'osq', 'oabs' (the last episode's, as the kernels keep them)."""
     idx = np.asarray(idx)
     n = len(idx)
@@ -99,8 +122,8 @@ def closed_truth(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, e
         osum, osq, oabs = (np.zeros((N, obs)) for _ in range(3))
         for t in range(T):
             h = np.clip((ob - mean) / std, -float(clip), float(clip))
-            for WT, b, _ in layers:
-                h = activation(np.matmul(h[:, None, :], WT)[:, 0, :] + b)
+            for (WT, b, _), act_fn in zip(layers, per_layer(activation, len(layers))):
+                h = act_fn(np.matmul(h[:, None, :], WT)[:, 0, :] + b)
             a = h if nz_all is None else h + nz_all[:, e, t]
             prod = a * c[t]
             fit += prod.sum(axis=1) / E

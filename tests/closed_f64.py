@@ -155,9 +155,12 @@ def _weights(table, idx, theta, sigma, sizes, pairs):
 
 
 def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a, env_b, rew_vec, pos_scale,
-             act_noise=None, episodes: int = 1, pairs: Optional[Sequence[int]] = None, variants=(None,), obs0_shift=None):
+             act_noise=None, episodes: int = 1, pairs: Optional[Sequence[int]] = None, variants=(None,), obs0_shift=None,
+             activation=np.tanh):
     """The truth (variant None) and its variants for the pairs ``pairs`` (default: all).  ``variants``: mutations (tuples of
-    ``mutations``) or None.  ``obs0_shift``: [V][obs] added to obs0 per variant (``growth``).
+    ``mutations``) or None.  ``obs0_shift``: [V][obs] added to obs0 per variant (``growth``).  ``activation``: the policy's
+    float64 activation after every layer in place of tanh (tests/act_f64.py's forms), or a list of one per layer; the env's
+    own tanh stays.
 
     Returns a dict of float64 arrays indexed [V][2][n] ([V][2][n][...] for vectors): 'fit', 'mass', 'behv' (3), 'mag' (3),
     'osum', 'osq', 'oabs' (obs: the column sums of ob, ob^2 and |ob|) and, with ``obs0_shift``, 'dev' [V][2][n]: the largest
@@ -170,6 +173,8 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
     V = len(variants)
     N = 2 * len(pairs)
     layers = _weights(table, idx, theta, sigma, sizes, pairs)
+    acts = list(activation) if isinstance(activation, (list, tuple)) else [activation] * L
+    assert len(acts) == L
     c = np.asarray(rew_vec, np.float64)
     B = np.asarray(env_b, np.float64)                      # [act][obs]: pre += a @ B
     A = _env_matrix(env_a, obs).T.copy()                   # pre += ob @ A
@@ -240,7 +245,7 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
                 if any_masks[1][l]:
                     h = h * in_mask[l][None]
                 z = np.matmul(h, WT) + biases[l]
-                y = np.tanh(z) * tfac
+                y = acts[l](z) * tfac
                 if any_masks[0][l]:
                     y = y * act_mask[l][None]
                 if l + 1 < L and stale[l + 1].any():

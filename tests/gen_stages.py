@@ -12,9 +12,11 @@ near-tie that flips one rank cannot cascade into the checks of later stages:
                 ob_sum_sq_cnt(obs_stream[1:T+1]);
   3 normalise   the normalised observations bit for bit against orc.normalise_obs with the generation's mean / std;
   4 fitness     every evaluation against float64 (``fitness_truth``: torch.float64 on the tensors' device, from the device's
-                indices, theta, normalised observations and action noise), judged by test_gpu_rollout_f64._check (EVAL_REL of
-                the reward mass per evaluation, RMS_BOUND of the spread, behaviours within float32 rounding); the float64 truth
-                tied to the plain CPU reference tests/f64_rollout.rollout_f64 on sampled pairs to TIE_REL of the mass;
+                indices, theta, normalised observations and action noise, with the policy's activation
+                ``Capture.activation`` in tests/act_f64.py's forms), judged by test_gpu_rollout_f64._check (EVAL_REL of
+                the reward mass per evaluation, RMS_BOUND of the spread -- test_gpu_activations.RMS with an activation --,
+                behaviours within float32 rounding); the float64 truth tied to the plain CPU reference
+                tests/f64_rollout.rollout_f64 (act_f64.rollout_f64 with an activation) on sampled pairs to TIE_REL of the mass;
   5 novelty     (archive) bit for bit against orc.novelty of the device's behaviours, in column 1 of the [pos|neg][k][2] rows;
   6 weights     bit for bit against orc.centered_ranker / orc.moo_ranker on the device's fitness, n_ranked equal; and against
                 the ranks of the float64 truth: how many ranks differ, the largest shift and the largest |dw| (bounded by
@@ -32,7 +34,7 @@ The closed loop (``Capture.obs0`` given: ClosedLoopEnv's obs_0, A^T [band, obs],
   2 obstat      count and n_saved exact; sum and sumsq against the float64 truth's osum / osq of the saved evaluations within
                 test_gpu_closed_f64's bound (T ulps of their magnitude per saved evaluation plus OBS_ERR per observation);
   3 normalise   inside the rollout kernel: judged through the fitness;
-  4 fitness     closed_f64.truth on a sample (``closed_sample``: every saved evaluation, the first and last pair of each
+  4 fitness     closed_f64.truth (with the policy's activation) on a sample (``closed_sample``: every saved evaluation, the first and last pair of each
                 stream, random pairs up to about 64 evaluations), with test_gpu_closed_f64's bounds, after closed_f64.growth
                 has shown that the sample does not amplify rounding (<= GROWTH_BOUND);
   6 weights     exact against the oracle on the device's fitness; the ranks against the truth are not compared (reported).
@@ -56,9 +58,11 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from oracle import es_oracle as orc  # noqa: E402
+import act_f64  # noqa: E402
 import closed_f64 as cf  # noqa: E402
 import f64_rollout as f64  # noqa: E402
 import rc_f64 as rc  # noqa: E402
+import test_gpu_activations as act_bounds  # noqa: E402
 import test_gpu_closed_f64 as closed_bounds  # noqa: E402
 import test_gpu_noise_table as noise_criterion  # noqa: E402
 import test_gpu_rollout_f64 as rollout_f64  # noqa: E402
@@ -72,6 +76,10 @@ TIE_REL = 1e-12           # the device float64 truth against the CPU float64 ref
 # simple_conf
 KAPPA_BOUND = 2.7e-6
 KAPPA_BOUND_TC = 8e-5
+# the same for the other activations (tests/test_gpu_generation_activations.py), measured there: TC3 3.23e-6 (leaky ReLU at
+# obj), 2.51e-6 (ELU at flagrun), 1.99e-6 (ReLU at simple_conf), 1.02e-6 (sigmoid at nsra); F32 at most 7.7e-9 (ReLU at
+# 376-64-64-17).  About twice that
+KAPPA_BOUND_ACT = 6.5e-6
 NOVELTY_COLUMN = 1        # NSRResult's row: [reward, novelty]
 GROWTH_BOUND = 100.0      # closed loop: the largest growth of a 1e-9 move of obs_0 over an episode (test_gpu_closed_f64.py)
 CLOSED_SAMPLE = 64        # closed loop: evaluations in the fitness truth's sample, at least
@@ -156,6 +164,8 @@ class Capture:
     env_a: Optional[np.ndarray] = None
     env_b: Optional[np.ndarray] = None
     band: Optional[int] = None
+    # the policy's activation after every layer (an nn.Activation; None: tanh), applied by every float64 truth
+    activation: object = None
     extra: dict = field(default_factory=dict)
 
     def __post_init__(self):
@@ -357,12 +367,19 @@ def stage_normalise(cap: Capture) -> List[Check]:
 ACT_BYTES = 2 ** 29       # fitness_truth: the float64 activations of one layer held per chunk of pairs, at most
 
 
-def fitness_truth(cap: Capture, chunk: Optional[int] = None, behaviour_episode: int = -1, noise=None):
+def layer_forms(cap: Capture, xp=np) -> list:
+    """The float64 activation of every layer of ``cap``'s policy (act_f64.form of ``cap.activation``; tanh for None), for
+    numpy arrays or (``xp=torch``) torch tensors."""
+    return [act_f64.form(cap.activation, xp)] * (len(cap.sizes) - 1)
+
+
+def fitness_truth(cap: Capture, chunk: Optional[int] = None, behaviour_episode: int = -1, noise=None, acts=None):
     """(fitness [2, K], behaviour [2, K, 3], reward mass [2, K], position magnitude [2, K, 3]) in float64 (f64_rollout's
-    definitions), computed with torch.float64 on the table's device in chunks of pairs: a measurement reference.  The
-    forward pass is shared by the E episodes (only the noise differs); fitness and mass are the per-step means over them,
-    behaviour and magnitude the episode ``behaviour_episode``'s.  ``chunk`` (default: up to 200 pairs, fewer where one
-    layer's activations over T steps would pass ACT_BYTES); ``noise``: in place of ``cap.act_noise``."""
+    definitions, with the policy's activation in act_f64's forms), computed with torch.float64 on the table's device in
+    chunks of pairs: a measurement reference.  The forward pass is shared by the E episodes (only the noise differs); fitness
+    and mass are the per-step means over them, behaviour and magnitude the episode ``behaviour_episode``'s.  ``chunk``
+    (default: up to 200 pairs, fewer where one layer's activations over T steps would pass ACT_BYTES); ``noise``: in place of
+    ``cap.act_noise``; ``acts``: torch functions, one per layer, in place of ``layer_forms(cap, torch)``."""
     dev = cap.table.device
     d64 = torch.float64
     sizes, T, act, K, P, E = cap.sizes, cap.T, cap.act, cap.K, cap.P, cap.episodes
@@ -377,6 +394,7 @@ def fitness_truth(cap: Capture, chunk: Optional[int] = None, behaviour_episode: 
     s32 = float(np.float32(cap.sigma))
     ps = float(cap.pos_scale)
     lay = f64.layer_slices(sizes)
+    acts = layer_forms(cap, torch) if acts is None else list(acts)
     sel = [j % act for j in range(3)]
     fit, mass = np.zeros((2, K)), np.zeros((2, K))
     behv, mag = np.zeros((2, K, 3)), np.zeros((2, K, 3))
@@ -389,9 +407,9 @@ def fitness_truth(cap: Capture, chunk: Optional[int] = None, behaviour_episode: 
             B = W.shape[0]
             wo, bo, fi, fo = lay[0]
             W1 = W[:, wo:wo + fi * fo].reshape(B, fo, fi)
-            a = torch.tanh((X @ W1.reshape(B * fo, fi).T).reshape(T, B, fo).permute(1, 0, 2) + W[:, bo:bo + fo][:, None, :])
-            for wo, bo, fi, fo in lay[1:]:
-                a = torch.tanh(torch.bmm(a, W[:, wo:wo + fi * fo].reshape(B, fo, fi).transpose(1, 2)) + W[:, bo:bo + fo][:, None, :])
+            a = acts[0]((X @ W1.reshape(B * fo, fi).T).reshape(T, B, fo).permute(1, 0, 2) + W[:, bo:bo + fo][:, None, :])
+            for (wo, bo, fi, fo), act_fn in zip(lay[1:], acts[1:]):
+                a = act_fn(torch.bmm(a, W[:, wo:wo + fi * fo].reshape(B, fo, fi).transpose(1, 2)) + W[:, bo:bo + fo][:, None, :])
             if nz_block is None:
                 prod = a * C[None]
                 fit[s, b0:b1] = prod.sum(dim=(1, 2)).cpu().numpy()
@@ -432,10 +450,10 @@ def closed_sample(cap: Capture, seed: int = 0) -> List[int]:
     return sorted(pairs)
 
 
-def closed_truth(cap: Capture, pairs: Optional[Sequence[int]] = None, growth: bool = True):
+def closed_truth(cap: Capture, pairs: Optional[Sequence[int]] = None, growth: bool = True, acts=None):
     """closed_f64.truth of the pairs ``pairs`` (default closed_sample) from the device's indices, theta, observation
-    statistics and action noise, plus 'pairs' and 'growth' (closed_f64.growth of the same evaluations; nan when not
-    ``growth``)."""
+    statistics and action noise, with the policy's activation (``layer_forms(cap)``, or ``acts``: numpy functions, one per
+    layer), plus 'pairs' and 'growth' (closed_f64.growth of the same evaluations; nan when not ``growth``)."""
     pairs = closed_sample(cap) if pairs is None else list(pairs)
     P = cap.P
     table_np = np.concatenate([_np(cap.table[int(cap.idx[k]):int(cap.idx[k]) + P]) for k in pairs])
@@ -444,7 +462,8 @@ def closed_truth(cap: Capture, pairs: Optional[Sequence[int]] = None, growth: bo
         noise = np.stack([_np(cap.act_noise[k]) for k in pairs])
     args = (table_np, np.arange(len(pairs)) * P, cap.theta0, cap.sigma, cap.sizes, cap.ob_mean, cap.ob_std, cap.ob_clip,
             cap.obs0, cap.env_a, cap.env_b, cap.rew_vec, cap.pos_scale)
-    kw = dict(act_noise=noise, episodes=cap.episodes if cap.ac_std else 1)
+    kw = dict(act_noise=noise, episodes=cap.episodes if cap.ac_std else 1,
+              activation=layer_forms(cap) if acts is None else list(acts))
     out = cf.truth(*args, **kw)
     out['growth'] = cf.growth(*args, **kw) if growth else math.nan
     out['pairs'] = pairs
@@ -486,8 +505,10 @@ def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] =
     spread = max(tf.std(), 1e-3 * math.sqrt(cap.T))
     rms = math.sqrt((err ** 2).mean())
     worst = float((err / mass).max())
+    # the rms bound of the policy's activation: test_gpu_rollout_f64's for tanh, test_gpu_activations' for the others
+    rms_bound = rollout_f64.RMS_BOUND[mode] if cap.activation is None else act_bounds.rms_bound(mode, cap.activation)
     out = [Check('fitness', 'max err/mass', worst, rollout_f64.EVAL_REL[mode], worst <= rollout_f64.EVAL_REL[mode]),
-           Check('fitness', 'rms/spread', rms / spread, rollout_f64.RMS_BOUND[mode], rms <= rollout_f64.RMS_BOUND[mode] * spread)]
+           Check('fitness', 'rms/spread', rms / spread, rms_bound, rms <= rms_bound * spread)]
     if b is not None:
         tol = 2 * rollout_f64.U * mag + rollout_f64.ACT_ERR[mode] * cap.pos_scale * cap.T
         r = float((np.abs(b - tb) / tol).max())
@@ -500,17 +521,18 @@ def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] =
     cap.extra['fitness'] = dict(rms_over_spread=rms / spread, mean_err=float((f - tf).mean()), mean_fitness=float(tf.mean()),
                                 kappa=float(kappa), resid_rms_over_spread=float(math.sqrt((resid ** 2).mean()) / spread))
     out.append(Check('fitness', 'rms/spread of the error less its fitted scale and offset',
-                     cap.extra['fitness']['resid_rms_over_spread'], rollout_f64.RMS_BOUND[mode],
-                     cap.extra['fitness']['resid_rms_over_spread'] <= rollout_f64.RMS_BOUND[mode]))
-    kb = KAPPA_BOUND_TC if mode == rollout_f64.TC else KAPPA_BOUND
+                     cap.extra['fitness']['resid_rms_over_spread'], rms_bound,
+                     cap.extra['fitness']['resid_rms_over_spread'] <= rms_bound))
+    kb = KAPPA_BOUND_TC if mode == rollout_f64.TC else KAPPA_BOUND if cap.activation is None else KAPPA_BOUND_ACT
     out.append(Check('fitness', '|fitted relative scale of the error|', abs(float(kappa)), kb, abs(float(kappa)) <= kb))
-    try:                                                   # the one assert helper of the rollout tests decides as well
-        rollout_f64._check('generation', mode, case, f, b, None, truth)
-        helper_ok = True
-    except AssertionError:
-        helper_ok = False
-    if helper_ok != all(c.ok for c in out[:3 if b is not None else 2]):
-        out.append(Check('fitness', 'test_gpu_rollout_f64._check disagrees', 1.0, 0.0, False))
+    if cap.activation is None:                             # the one assert helper of the tanh rollout tests decides as well
+        try:
+            rollout_f64._check('generation', mode, case, f, b, None, truth)
+            helper_ok = True
+        except AssertionError:
+            helper_ok = False
+        if helper_ok != all(c.ok for c in out[:3 if b is not None else 2]):
+            out.append(Check('fitness', 'test_gpu_rollout_f64._check disagrees', 1.0, 0.0, False))
     # the device float64 truth against the plain CPU reference on sampled pairs
     tie = tie_pairs(cap) if tie is None else list(tie)
     P = cap.P
@@ -518,8 +540,11 @@ def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] =
     noise = None
     if cap.ac_std:
         noise = np.stack([_np(cap.act_noise[k]) for k in tie])
-    cf, cb, cm, cmag = f64.rollout_f64(table_np, np.arange(len(tie)) * P, cap.theta0, cap.sigma, cap.sizes, cap.obsn, cap.rew_vec,
-                                       cap.pos_scale, noise, cap.episodes)
+    tie_args = (table_np, np.arange(len(tie)) * P, cap.theta0, cap.sigma, cap.sizes, cap.obsn, cap.rew_vec, cap.pos_scale)
+    if cap.activation is None:
+        cf, cb, cm, cmag = f64.rollout_f64(*tie_args, noise, cap.episodes)
+    else:
+        cf, cb, cm, cmag = act_f64.rollout_f64(*tie_args, act_f64.form(cap.activation), noise, cap.episodes)
     rel = float(max((np.abs(cf - tf[:, tie]) / cm).max(), (np.abs(cb - tb[:, tie]) / np.maximum(cmag, 1e-300)).max()))
     out.append(Check('fitness', f'float64 truth vs CPU reference ({2 * len(tie)} evaluations), rel', rel, TIE_REL, rel <= TIE_REL))
     return out
@@ -838,6 +863,41 @@ def _closed_saved_sums(c, shift: str = None, drop: int = 0):
     return _copy(c, stats=np.concatenate([osum.sum(axis=0), osq.sum(axis=0), [float(rows * n), float(n)]]))
 
 
+def _act_forms_bug(c: Capture, which: str, xp) -> list:
+    """The layer activations of ``c``'s policy evaluated wrongly on purpose: 'tanh_layer' tanh in the first hidden layer,
+    'default_param' torch's default slope (0.01) or alpha (1.0) in place of the policy's, 'no_output' no activation after
+    the output layer."""
+    from es_pytorch_b200 import _lib
+    from es_pytorch_b200.nn.nn import Activation
+    acts = layer_forms(c, xp)
+    if which == 'tanh_layer':
+        acts[0] = xp.tanh
+    elif which == 'default_param':
+        default = {_lib.ES_ACT_LEAKY_RELU: 0.01, _lib.ES_ACT_ELU: 1.0}[int(c.activation.kind)]
+        acts = [act_f64.form(Activation(c.activation.kind, default), xp)] * len(acts)
+    else:
+        acts[-1] = lambda z: z
+    return acts
+
+
+def _m_activation(c: Capture, which: str) -> Capture:
+    """The fitness (and behaviour) of a rollout with ``_act_forms_bug(which)``, everything after it rescored: in the closed
+    loop on the truth's sample, the pairs the fitness stage compares."""
+    f = c.fit.copy()
+    behv = None if c.behv is None else c.behv.copy()
+    if c.closed:
+        tr = closed_truth(c, growth=False, acts=_act_forms_bug(c, which, np))
+        f[:, tr['pairs'], 0] = tr['fit']
+        if behv is not None:
+            behv[:, tr['pairs']] = tr['behv'].astype(F32)
+    else:
+        tf, tb, _, _ = fitness_truth(c, acts=_act_forms_bug(c, which, torch))
+        f[:, :, 0] = tf
+        if behv is not None:
+            behv = tb.astype(F32)
+    return _rescored(_copy(c, fit=f, behv=behv))
+
+
 # name -> (what it models, mutation); each returns a mutated copy of a correct capture
 MUTATIONS = {
     'shift_stream_indices': ("one stream's indices shifted by a pair", _m_shift_stream),
@@ -862,13 +922,21 @@ MUTATIONS = {
     'closed_obstat_pre_step': ('closed-loop ObStat summed over obs_0 .. obs_{T-1}', lambda c: _closed_saved_sums(c, 'pre')),
     'closed_count_t_minus_1': ('closed-loop ObStat of T - 1 rows per saved evaluation', lambda c: _closed_saved_sums(c, 'short')),
     'closed_drop_saved': ('one saved evaluation dropped from the closed-loop ObStat', lambda c: _closed_saved_sums(c, drop=1)),
+    'act_tanh_layer': ('tanh in place of the policy\'s activation in the first hidden layer',
+                       lambda c: _m_activation(c, 'tanh_layer')),
+    'act_default_param': ("torch's default slope (0.01) or alpha (1.0) in place of the policy's",
+                          lambda c: _m_activation(c, 'default_param')),
+    'act_no_output': ('no activation after the output layer', lambda c: _m_activation(c, 'no_output')),
 }
 NEEDS_ARCHIVE = ('novelty_column', 'novelty_off_by_one')
 # what capture a mutation models a bug of, beyond a plain open-loop one: 'episodes' (E > 1 with action noise), 'nsr'
-# (an archive; 'moo_w_swapped' needs w != 0.5, 'archive_clipped_to_k' fewer entries than k) and 'closed' (the closed loop)
+# (an archive; 'moo_w_swapped' needs w != 0.5, 'archive_clipped_to_k' fewer entries than k), 'closed' (the closed loop),
+# 'activation' (a policy activation other than tanh, open or closed loop) and 'param' (leaky ReLU or ELU)
 NEEDS = {'episode0_noise': 'episodes', 'episodes_not_divided': 'episodes', 'first_episode_behaviour': 'episodes',
          'novelty_over_reward': 'nsr', 'moo_w_swapped': 'nsr', 'archive_clipped_to_k': 'nsr',
-         'closed_obstat_pre_step': 'closed', 'closed_count_t_minus_1': 'closed', 'closed_drop_saved': 'closed'}
+         'closed_obstat_pre_step': 'closed', 'closed_count_t_minus_1': 'closed', 'closed_drop_saved': 'closed',
+         'act_tanh_layer': 'activation', 'act_default_param': 'param', 'act_no_output': 'activation'}
+ACT_MUTATIONS = ('act_tanh_layer', 'act_default_param', 'act_no_output')
 
 
 def rejection(checks: Sequence[Check]):

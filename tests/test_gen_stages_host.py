@@ -6,6 +6,9 @@ save_obs coin per evaluation at chance 0.3, Adam), so Adam's state, the streams'
 carried over and the normalisation runs with the first generation's mean / std.  Variants: NSRA (a 16-entry archive, k = 10,
 w = 0.5) and action noise (ac_std = 0.01).  The oracle computes its rollouts in float32 on the CPU, so the fitness is judged
 with the float32 rollout's bounds (ES_ROLLOUT_F32); gsum is the oracle's own numpy reconstruction (es_oracle.scale_noise).
+The oracle's policies are tanh stacks: the activation variants ('activation': leaky ReLU of slope 0.1 on the plain capture;
+'closed_activation': ELU of alpha 0.7 on the closed-loop one) take the oracle's generation with its fitness replaced by the
+float64 truth of the activation (and, in the closed loop, the ObStat sums by the truth's), everything after it rescored.
 The oracle does not hand out the raw coin words it drew, so the captured words (and the action noise) are the judge's own replay
 of the streams: on the host the coin-word check compares the replay with itself, and what ties the oracle's coins to the judge
 is the obs statistics (count and n_saved from the oracle's rs.random() calls) and the streams' end states.  The
@@ -104,12 +107,36 @@ def _capture(variant):
     return cap
 
 
+def _activation_capture(base, act):
+    """``base``'s capture for a policy with activation ``act``: the fitness that policy earns (the float64 truth), the
+    closed loop's ObStat sums of its saved evaluations, and everything after the fitness rescored."""
+    cap = gs._copy(_cap(base), activation=act)
+    f = cap.fit.copy()
+    if cap.closed:
+        cap = gs._closed_saved_sums(cap)
+        f[:, :, 0] = gs.closed_truth(cap, pairs=range(cap.K), growth=False)['fit']
+    else:
+        f[:, :, 0] = gs.fitness_truth(cap)[0]
+    return gs._rescored(gs._copy(cap, fit=f))
+
+
+def _act(kind, param):
+    from es_pytorch_b200 import _lib
+    from es_pytorch_b200.nn.nn import Activation
+    return Activation(getattr(_lib, kind), float(np.float32(param)))
+
+
 _CAPS = {}
 
 
 def _cap(variant):
     if variant not in _CAPS:
-        _CAPS[variant] = _capture(variant)
+        if variant == 'activation':
+            _CAPS[variant] = _activation_capture('plain', _act('ES_ACT_LEAKY_RELU', 0.1))
+        elif variant == 'closed_activation':
+            _CAPS[variant] = _activation_capture('closed', _act('ES_ACT_ELU', 0.7))
+        else:
+            _CAPS[variant] = _capture(variant)
     return _CAPS[variant]
 
 
@@ -117,7 +144,7 @@ def _judge(cap):
     return gs.judge(cap, MODE_F32, rc.H100_SMS, SHIFT_BOUND, DW_BOUND, tie=list(range(cap.K)))
 
 
-@pytest.mark.parametrize('variant', ['plain', 'nsra', 'noise', 'episodes', 'nsr', 'closed'])
+@pytest.mark.parametrize('variant', ['plain', 'nsra', 'noise', 'episodes', 'nsr', 'closed', 'activation', 'closed_activation'])
 def test_judge_passes_the_oracle_generation(variant):
     cap = _cap(variant)
     checks = _judge(cap)
@@ -125,13 +152,14 @@ def test_judge_passes_the_oracle_generation(variant):
     gs.assert_ok(checks)
     assert cap.extra['n_saved'] > 0 and cap.t0 == 1
     assert not np.array_equal(cap.ob_std, np.ones_like(cap.ob_std))
-    if variant == 'closed':                       # every saved evaluation in the truth's sample, the whole population here
+    if variant.startswith('closed'):              # every saved evaluation in the truth's sample, the whole population here
         assert len(cap.extra['closed_truth']['pairs']) == cap.K and cap.extra['ranks_vs_truth'].startswith('not compared')
 
 
 def _variant(name):
     """The capture a modelled bug is judged on: the 'nsr' capture has w = 0.25 and 5 archive entries for k = 10."""
-    return gs.NEEDS.get(name, 'nsra' if name in gs.NEEDS_ARCHIVE else 'plain')
+    need = gs.NEEDS.get(name, 'nsra' if name in gs.NEEDS_ARCHIVE else 'plain')
+    return 'activation' if need == 'param' else need
 
 
 @pytest.mark.parametrize('name', sorted(gs.MUTATIONS))
@@ -143,3 +171,40 @@ def test_judge_rejects_modelled_bugs(name):
     print(f'\n{name} ({what}): rejected by {stages}, margin {margin:.3g}x')
     assert stages is not None, f'{what}: not rejected'
     assert margin >= 10, (what, stages, margin)
+
+
+@pytest.mark.parametrize('name', gs.ACT_MUTATIONS)
+def test_judge_rejects_activation_bugs_in_the_closed_loop(name):
+    what, mutate = gs.MUTATIONS[name]
+    cap = _cap('closed_activation')
+    _judge(cap)                                   # leaves the truth's sample in cap.extra, as the GPU files judge first
+    stages, margin = gs.rejection(_judge(mutate(cap)))
+    print(f'\n{name} ({what}), closed loop: rejected by {stages}, margin {margin:.3g}x')
+    assert stages is not None and margin >= 10, (what, stages, margin)
+
+
+def test_activation_of_tanh_is_the_tanh_truth():
+    """A capture whose activation is tanh gets the truths of one without (no activation): open loop with episodes and
+    action noise, closed loop with its growth, to 1e-13 relative; and the closed loop's truth with another activation is
+    tests/act_f64.closed_truth's."""
+    import act_f64
+    tanh = _act('ES_ACT_TANH', 0.0)
+    cap = _cap('episodes')
+    for want, got in zip(gs.fitness_truth(cap), gs.fitness_truth(gs._copy(cap, activation=tanh))):
+        np.testing.assert_allclose(got, want, rtol=1e-13, atol=1e-300)
+    cap = _cap('closed')
+    want, got = gs.closed_truth(cap), gs.closed_truth(gs._copy(cap, activation=tanh))
+    for k in ('fit', 'mass', 'behv', 'mag', 'osum', 'osq', 'oabs'):
+        np.testing.assert_allclose(got[k], want[k], rtol=1e-13, atol=1e-300, err_msg=k)
+    assert abs(got['growth'] - want['growth']) <= 1e-13 * want['growth']
+    elu = _act('ES_ACT_ELU', 0.7)
+    c = gs._copy(cap, activation=elu)
+    got = gs.closed_truth(c, growth=False)
+    pairs = got['pairs']
+    P = c.P
+    table = np.concatenate([c.table[int(c.idx[k]):int(c.idx[k]) + P].numpy() for k in pairs])
+    want = act_f64.closed_truth(table, np.arange(len(pairs)) * P, c.theta0, c.sigma, c.sizes, c.ob_mean, c.ob_std, c.ob_clip,
+                                c.obs0, c.env_a, c.env_b, c.rew_vec, c.pos_scale, activation=act_f64.elu(0.7))
+    for k in ('fit', 'mass', 'behv', 'mag', 'osum', 'osq', 'oabs'):     # sums in another order: relative to their largest
+        np.testing.assert_allclose(got[k], want[k], rtol=1e-13, atol=1e-13 * np.abs(want[k]).max(), err_msg=k)
+    assert not np.allclose(got['fit'], gs.closed_truth(cap, pairs=pairs, growth=False)['fit'])

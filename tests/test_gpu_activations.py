@@ -6,7 +6,14 @@
   around the SM count and multi-launch float32 chunks;
 * closed loop at clusters of 1, 2 and 4 CTAs against act_f64.closed_truth (closed_f64's, with the activation; test_gpu_closed_f64's
   bounds), ObStat sums included;
-* refusals (ES_ROLLOUT_TC, unknown kinds, a non-finite parameter, obs beyond TC3's coverage) and the float16 guard of TC3;
+* launch edges: TC3 around its launch chunk, F32 with 8 ragged layers and around the switch to staged weights (H = 196 ..
+  198), the wide kernel's layer shapes (widths 192 and mixed, act 32, obs 1 and 256, four hidden layers), the closed loop in
+  clusters of 2 and 8; results independent of the pair order (a reversed run, bit for bit) in F32, TC3 and the closed loop;
+* the bounds shown to reject truths with the activation evaluated wrongly (tanh in one layer, no output activation, torch's
+  default slope / alpha), and the activations' own regimes in F32 and the closed loop (sigmoid's saturated tails, ELU near 0,
+  leaky slopes 0, -0.5 and 3, ELU with alpha 0);
+* refusals (ES_ROLLOUT_TC, unknown kinds, a non-finite parameter, obs beyond TC3's coverage) and the float16 guard of TC3,
+  which looks at the episode's rows only (not the zero observations that pad the last tile);
 * ES_ACT_TANH through the new entry points is the old entry points bit for bit;
 * es.test_params / es.step with BatchedRollout(fuse_activations=True): the DeviceGeneration's results bit for bit, and the
   python loop's within the float bound, with indices and stream states exact;
@@ -27,7 +34,10 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import act_f64  # noqa: E402
 import f64_rollout as f64  # noqa: E402
 from test_gpu_rollout_f64 import ACT_ERR, EVAL_REL, RMS_BOUND, U, Case, _sample  # noqa: E402
+import closed_f64  # noqa: E402
 import test_gpu_closed_f64 as cf  # noqa: E402
+import test_gpu_rollout_f64 as rf  # noqa: E402
+import test_gpu_rollout_wide as rw  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -45,46 +55,71 @@ TANH = Activation(_lib.ES_ACT_TANH, 0.0)
 # passes that relative error on at full size where tanh saturates).  Per evaluation the tanh files' EVAL_REL holds as it is
 # (largest measured err / mass: F32 9.7e-7, TC3 1.8e-6)
 RMS = {F32: 8e-6, TC3: 2.5e-5}
+# sigmoid: its fast exponential's absolute error (~1e-7 per action, common to both modes) over the small fitness spread of a
+# single bounded action: measured up to 2.69e-5 (F32) and 2.18e-5 (TC3) at 7-192-64-128-1 (with another draw of the inputs
+# than test_open_loop_against_float64's, where it is 2.5e-6 / 3.0e-6); about twice that
+RMS_SIGMOID = {F32: 6e-5, TC3: 5e-5}
+
+
+def rms_bound(mode, act):
+    """The rms/spread bound of a rollout in ``mode`` of a policy with activation ``act`` (an nn.Activation)."""
+    return RMS_SIGMOID[mode] if act is not None and act.kind == _lib.ES_ACT_SIGMOID else RMS[mode]
 SHAPES = {'humanoid': [376, 64, 64, 17], 'simple_conf': [15, 256, 256, 3], 'obj': [17, 256, 256, 256, 6],
-          'flagrun': [28, 128, 256, 256, 128, 8]}
+          'flagrun': [28, 128, 256, 256, 128, 8],
+          # test_gpu_rollout_wide.test_wide_layer_shapes': widths of 192 and mixed, act 32, obs 1 and 256, four hidden of 64
+          'mixed': [7, 192, 64, 128, 1], 'act32': [9, 128, 128, 32], 'obs1': [1, 64, 128, 4], 'obs256': [256, 256, 64, 5],
+          'four-hidden-64': [20, 64, 64, 64, 64, 2]}
 
 
 class ActCase(Case):
-    """test_gpu_rollout_f64's Case for a policy with activation ``name``."""
+    """test_gpu_rollout_f64's Case for a policy with activation ``name`` (or ``act``: an (Activation, float64 form) pair)."""
 
-    def __init__(self, eng, name, sizes, T, n, seed, **kw):
+    def __init__(self, eng, name, sizes, T, n, seed, act=None, **kw):
         super().__init__(eng, sizes, T, n, seed, **kw)
-        self.act, self.f64act = ACTS[name] if name != 'tanh' else (TANH, np.tanh)
+        self.act, self.f64act = act or (ACTS[name] if name != 'tanh' else (TANH, np.tanh))
+        self.launches = None
 
-    def run(self, mode, act=None, sigma=None):
+    def upload(self):
+        """After the host arrays were changed in place."""
+        d = lambda a: self.eng.to_device(np.ascontiguousarray(a))
+        self.d_table, self.d_theta, self.d_obsn, self.d_rew = d(self.table), d(self.theta), d(self.obsn), d(self.rew)
+
+    def run(self, mode, act=None, sigma=None, reverse=False):
+        """(fitness [2, n], behaviour [2, n, 3]); ``reverse``: the pairs in reverse order (indices and noise), results
+        returned in the original order.  The call's launches in ``self.launches``."""
         eng, n = self.eng, self.n
+        sl = slice(None, None, -1) if reverse else slice(None)
         fit = torch.full((2, n), float('nan'), dtype=torch.float64, device=eng.device)
         bh = torch.full((2, n, 3), float('nan'), dtype=torch.float32, device=eng.device)
-        nz = None if self.noise is None else eng.to_device(self.noise)
-        eng.rollout(self.d_table, eng.to_device(self.idx), self.d_theta, self.sigma if sigma is None else sigma, self.sizes,
-                    self.d_obsn, self.d_rew, self.ps, fit[0], fit[1], 1, bh[0], bh[1], mode, act_noise=nz, episodes=self.E,
-                    activation=self.act if act is None else act)
+        nz = None if self.noise is None else eng.to_device(np.ascontiguousarray(self.noise[sl]))
+        l0 = eng.launches
+        eng.rollout(self.d_table, eng.to_device(np.ascontiguousarray(self.idx[sl])), self.d_theta,
+                    self.sigma if sigma is None else sigma, self.sizes, self.d_obsn, self.d_rew, self.ps, fit[0], fit[1], 1, bh[0],
+                    bh[1], mode, act_noise=nz, episodes=self.E, activation=self.act if act is None else act)
         eng.sync()
-        f, b = fit.cpu().numpy(), bh.cpu().numpy()
+        self.launches = eng.launches - l0
+        f, b = fit.cpu().numpy()[:, sl], bh.cpu().numpy()[:, sl]
         assert not np.isnan(f).any() and not np.isnan(b).any(), 'an evaluation was not written'
         return f, b
 
-    def truth(self, pairs):
+    def truth(self, pairs, f64act=None):
+        """``f64act``: in place of the policy's float64 activation (one function, or a list of one per layer)."""
         return act_f64.rollout_f64(self.table, self.idx, self.theta, self.sigma, self.sizes, self.obsn, self.rew, self.ps,
-                                   self.f64act, self.noise, self.E, pairs)
+                                   self.f64act if f64act is None else f64act, self.noise, self.E, pairs)
 
 
-def _check(tag, mode, case, f, b, pairs, rms_check=True):
-    tf, tb, mass, mag = case.truth(pairs)
+def _check(tag, mode, case, f, b, pairs, rms_check=True, truth=None):
+    tf, tb, mass, mag = case.truth(pairs) if truth is None else truth
     f, b = f[:, pairs], b[:, pairs]
     err = np.abs(f - tf)
     spread = max(tf.std(), 1e-3 * math.sqrt(case.T))
     rms = math.sqrt((err ** 2).mean())
     worst = (err / mass).max()
-    print(f'\n[act f64] {tag} mode={mode}: rms/spread {rms / spread:.3g} (bound {RMS[mode]:.3g}), max err/mass {worst:.3g} '
+    bound = rms_bound(mode, case.act)
+    print(f'\n[act f64] {tag} mode={mode}: rms/spread {rms / spread:.3g} (bound {bound:.3g}), max err/mass {worst:.3g} '
           f'(bound {EVAL_REL[mode]:.3g})')
     assert np.all(err <= EVAL_REL[mode] * mass), (tag, worst)
-    assert not rms_check or rms <= RMS[mode] * spread, (tag, rms / spread)
+    assert not rms_check or rms <= bound * spread, (tag, rms / spread)
     tol = 2 * U * mag + ACT_ERR[mode] * case.ps * case.T
     assert np.all(np.abs(b - tb) <= tol), (tag, np.abs(b - tb).max())
 
@@ -104,7 +139,9 @@ def _run_check(tag, case, mode, pairs=None, repeat=True):
 @pytest.mark.parametrize('name', list(ACTS))
 def test_open_loop_against_float64(eng, name, shape, mode):
     sizes = SHAPES[shape]
-    case = ActCase(eng, name, sizes, 300, 12, seed=10 * list(ACTS).index(name) + list(SHAPES).index(shape))
+    a, k = list(ACTS).index(name), list(SHAPES).index(shape)
+    # the wide test's shapes (k >= 4) seeded apart: at seed 8 one deep ReLU evaluation has no action above 0 at any step
+    case = ActCase(eng, name, sizes, 300, 12, seed=10 * a + k + (700 if k >= 4 else 0))
     if mode == TC3 and sizes[0] > 256:
         # the wide kernel's activation buffer holds 256 input columns: obs 376 is refused, ES_ROLLOUT_F32 takes it
         with pytest.raises(_lib.EsLibraryError, match=r'obs 376.*ES_ROLLOUT_F32'):
@@ -149,6 +186,151 @@ def test_pair_counts_around_the_sm_count_and_float32_chunks(eng):
     assert eng.launches - l0 == 4                        # two chunks, each a staging and a rollout launch
 
 
+def test_tc3_chunk_edges_and_pair_order(eng):
+    """15-256-256-3 in launch chunks of c pairs (test_gpu_rollout_wide._tcw_chunk): c - 1, c and c + 1 pairs, with pairs c - 1, c
+    and c + 1 against the truth; every run bit-identical to one with the pairs reversed (no result depends on the grid, the
+    chunking or the order of the pairs)."""
+    sizes = [15, 256, 256, 3]
+    c = rw._tcw_chunk(sizes, TC3)
+    for n, name in ((c - 1, 'sigmoid'), (c, 'elu'), (c + 1, 'relu')):
+        case = ActCase(eng, name, sizes, 64, n, seed=n, E=2, ac_std=0.05)
+        f, b = _run_check(f'{name} n={n} (chunk {c})', case, TC3, pairs=_sample(n, must=(c - 1, c, c + 1), k=10), repeat=False)
+        assert case.launches == rw._tcw_launches(sizes, TC3, n)
+        fr, br = case.run(TC3, reverse=True)
+        assert np.array_equal(f, fr) and np.array_equal(b, br), f'{name} n={n}: the reversed run differs'
+
+
+def _f32_launches(sizes, n):
+    """ES_ROLLOUT_F32 with an activation: the general kernel only (never the packed-FMA one), one launch per chunk, two
+    with staged weights."""
+    gw, chunk = rf._f32_layout(sizes)
+    return 2 * -(-n // chunk) if gw else 1
+
+
+@pytest.mark.parametrize('sizes', [[15, 256, 256, 3], [17, 64, 64, 6]], ids=['staged', 'shared'])
+def test_f32_pair_order(eng, sizes):
+    """ES_ROLLOUT_F32 with the weights staged in global memory and in shared memory: the pairs reversed, bit for bit (at
+    least SM count / 2 pairs, so that no episode is split over the SMs)."""
+    gw = rf._f32_layout(sizes)[0]
+    assert gw == (sizes[1] == 256)
+    n = eng.sm_count // 2 + 7
+    case = ActCase(eng, 'leaky', sizes, 90, n, seed=n, E=2, ac_std=0.05)
+    f, b = _run_check(f'leaky F32 n={n}', case, F32, pairs=_sample(n, k=10), repeat=False)
+    assert case.launches == _f32_launches(sizes, n) == (2 if gw else 1)
+    fr, br = case.run(F32, reverse=True)
+    assert np.array_equal(f, fr) and np.array_equal(b, br)
+
+
+# ES_MAX_LAYERS = 8 ragged layers in shared memory, and 15-H-H-3 around the switch to staged weights (H = 197 / 198)
+_F32_SHAPES = [('ragged8', [5, 7, 33, 3, 130, 1, 64, 9, 2], False), ('H196', [15, 196, 196, 3], False),
+               ('H197', [15, 197, 197, 3], False), ('H198', [15, 198, 198, 3], True)]
+
+
+@pytest.mark.parametrize('name', list(ACTS))
+@pytest.mark.parametrize('shape,sizes,gw', _F32_SHAPES, ids=[s[0] for s in _F32_SHAPES])
+def test_f32_ragged_layers_and_the_staged_weights_switch(eng, shape, sizes, gw, name):
+    assert rf._f32_layout(sizes)[0] == gw
+    for n in (5, eng.sm_count // 2 + 3):                        # split over the SMs (few pairs) and not
+        case = ActCase(eng, name, sizes, 77, n, seed=n + len(sizes), E=2, ac_std=0.05)
+        _run_check(f'{name} {shape} n={n}', case, F32, pairs=_sample(n, k=12), repeat=False)
+        assert case.launches == _f32_launches(sizes, n)
+
+
+# ------------------------------------------------------------------------------------------------ the bounds are sensitive
+def _mutated_forms(name, which):
+    """The policy's float64 activation per layer, evaluated wrongly on purpose (tests/gen_stages.py's modelled bugs)."""
+    act, f = ACTS[name]
+    if which == 'default_param':
+        return {'leaky': act_f64.leaky_relu(0.01), 'elu': act_f64.elu(1.0)}[name]
+    return lambda n_layers: ([np.tanh] + [f] * (n_layers - 1) if which == 'tanh_layer' else [f] * (n_layers - 1) + [lambda z: z])
+
+
+@pytest.mark.parametrize('mode,shape', [(F32, 'simple_conf'), (TC3, 'simple_conf'), (F32, 'humanoid')],
+                         ids=['F32-simple_conf', 'TC3-simple_conf', 'F32-humanoid'])
+@pytest.mark.parametrize('name', list(ACTS))
+def test_bounds_reject_mutated_truths(eng, name, mode, shape):
+    """_check accepts the device's fitness against the truth and rejects it against each truth with the activation
+    evaluated wrongly: tanh in the first hidden layer, no activation after the output layer, and (leaky ReLU, ELU) torch's
+    default slope 0.01 / alpha 1.0 in place of the policy's."""
+    sizes = SHAPES[shape]
+    case = ActCase(eng, name, sizes, 300, 40, seed=3, ac_std=0.01)
+    pairs = _sample(40, k=16)
+    f, b = case.run(mode)
+    truth = case.truth(pairs)
+    _check(f'{name} unmutated', mode, case, f, b, pairs, truth=truth)
+    whats = ('tanh_layer', 'no_output') + (('default_param',) if name in ('leaky', 'elu') else ())
+    for what in whats:
+        forms = _mutated_forms(name, what)
+        bad = case.truth(pairs, f64act=forms if what == 'default_param' else forms(len(sizes) - 1))
+        tf, mass = bad[0], bad[2]
+        spread = max(tf.std(), 1e-3 * math.sqrt(case.T))
+        fp = f[:, pairs]
+        print(f'  mutated {what}: rms/spread {math.sqrt(((fp - tf) ** 2).mean()) / spread:.3g}, '
+              f'max err/mass {(np.abs(fp - tf) / mass).max():.3g}')
+        with pytest.raises(AssertionError):
+            _check(f'{name} mutated {what}', mode, case, f, b, pairs, truth=bad)
+
+
+# ------------------------------------------------------------------------------------------------ the activations' own regimes
+def _place_in_sigmoid_tails(theta, sizes, rs):
+    """Every layer's biases moved by +-|z| spread over [0, 100]: pre-activations in sigmoid's saturated tails (where
+    __fdividef(1, 1 + __expf(-z)) returns 0 from z below about -87) and through its transition, without scaling any weight
+    (a scaled weight would scale the rounding of the products with it)."""
+    th = theta.astype(np.float64)
+    for _, bo, _, fo in f64.layer_slices(sizes):
+        th[bo:bo + fo] += rs.permutation(np.linspace(0.0, 100.0, fo)) * rs.choice([-1.0, 1.0], fo)
+    return th.astype(np.float32)
+
+
+# name -> (Activation, float64 form, how theta and the table are changed: 'tails' (_place_in_sigmoid_tails), 'small' (theta,
+# the noise table and the action noise times SMALL: ELU's pre-activations within |z| < 1e-3, where exp(z) - 1 would lose every
+# digit) or None)
+SMALL = np.float32(3e-4)
+REGIMES = {
+    'sigmoid_tails': (Activation(_lib.ES_ACT_SIGMOID, 0.0), act_f64.sigmoid, 'tails'),
+    'elu_near_zero': (ACTS['elu'][0], ACTS['elu'][1], 'small'),
+    'leaky_slope_0': (Activation(_lib.ES_ACT_LEAKY_RELU, 0.0), act_f64.leaky_relu(0.0), None),
+    'leaky_slope_-0.5': (Activation(_lib.ES_ACT_LEAKY_RELU, -0.5), act_f64.leaky_relu(-0.5), None),
+    'leaky_slope_3': (Activation(_lib.ES_ACT_LEAKY_RELU, 3.0), act_f64.leaky_relu(3.0), None),
+    'elu_alpha_0': (Activation(_lib.ES_ACT_ELU, 0.0), act_f64.elu(0.0), None),
+}
+
+
+def _regime_premise(regime, z):
+    """The pre-activations ``z`` (float64, every layer) reach the regime."""
+    if regime == 'sigmoid_tails':
+        assert z.max() > 80 and z.min() < -88 and (np.abs(z) < 2).any()
+    elif regime == 'elu_near_zero':
+        assert np.abs(z).max() < 1e-3 and (z < 0).mean() > 0.2
+    else:
+        assert (z < 0).mean() > 0.2 and (z > 0).mean() > 0.2
+
+
+@pytest.mark.parametrize('regime', list(REGIMES))
+def test_f32_activation_regimes(eng, regime):
+    act, form, how = REGIMES[regime]
+    sizes = [17, 64, 64, 6]
+    case = ActCase(eng, None, sizes, 200, 24, seed=31, act=(act, form), E=2, ac_std=0.05)
+    rs = np.random.RandomState(32)
+    if how == 'tails':
+        case.theta = _place_in_sigmoid_tails(case.theta, sizes, rs)
+    elif how == 'small':
+        case.theta = (case.theta * SMALL).astype(np.float32)
+        case.table = (case.table * SMALL).astype(np.float32)
+        case.noise = (case.noise * SMALL).astype(np.float32)
+    case.upload()
+    zs, h = [], case.obsn.astype(np.float64)
+    for k in (0, case.n - 1):
+        w = f64.perturbed(case.table, case.idx[k], case.theta, case.sigma, 1.0)
+        h = case.obsn.astype(np.float64)
+        for wo, bo, fi, fo in f64.layer_slices(sizes):
+            z = h @ w[wo:wo + fi * fo].reshape(fo, fi).T + w[bo:bo + fo]
+            zs.append(z.ravel())
+            h = form(z)
+    _regime_premise(regime, np.concatenate(zs))
+    _run_check(f'F32 {regime}', case, F32)
+
+
 # ------------------------------------------------------------------------------------------------ refusals and the float16 guard
 def test_refusals(eng):
     case = ActCase(eng, 'relu', [15, 256, 256, 3], 16, 2, seed=1)
@@ -163,6 +345,44 @@ def test_refusals(eng):
         ActCase(eng, 'relu', [15, 100, 64, 3], 16, 2, seed=1).run(TC3)
     # the engine is usable afterwards
     _run_check('after refusals', case, F32, repeat=False)
+
+
+def test_tc3_guard_looks_at_the_episode_rows_only(eng):
+    """A ReLU policy whose forward of a zero observation leaves float16 range while every step of the episode stays inside:
+    observation column 0 held at 5; layer 1's first 128 units with bias +B, cancelled exactly on every live row by weights
+    -B / 5 on that column (their other weights 0), the other 128 units as drawn; layer 2's weights 1 + theta's; sigma 0.  The
+    rows of the last tile beyond T (zero observations) reach ~128 B in layer 2; TC3 must not flag them, and agrees with F32
+    and the float64 truth."""
+    B, sizes, T = 1000.0, [15, 256, 256, 3], 100                  # T = 100: rows 100 .. 127 of the tile are padding
+    case = ActCase(eng, 'relu', sizes, T, 4, seed=12)
+    case.sigma = 0.0
+    case.obsn[:, 0] = 5.0
+    th = case.theta.copy()
+    (w1, b1, fi1, fo1), (w2, b2, fi2, fo2), _ = f64.layer_slices(sizes)
+    W1 = th[w1:w1 + fi1 * fo1].reshape(fo1, fi1)
+    W1[:128] = 0.0
+    W1[:128, 0] = -B / 5
+    th[b1:b1 + 128] = B
+    th[w2:w2 + fi2 * fo2] += 1.0
+    case.theta = th
+    case.upload()
+    # the premise, in float64: padded rows beyond float16 range in layer 2, every live row within it
+    for x in (case.obsn.astype(np.float64), np.zeros((1, sizes[0]))):
+        h = x
+        for wo, bo, fi, fo in f64.layer_slices(sizes)[:2]:
+            h = np.maximum(h @ th[wo:wo + fi * fo].reshape(fo, fi).T.astype(np.float64) + th[bo:bo + fo], 0.0)
+        if x.shape[0] == 1:
+            assert np.abs(h).max() > 65504
+        else:
+            assert np.abs(h).max() < 65504 / 4
+    f3, b3 = case.run(TC3)
+    assert eng.lib.es_check_async(eng._ctx) == 0
+    # (per evaluation only: sigma = 0 leaves every evaluation the same policy, no spread to measure the rms against)
+    _check('relu padded rows TC3', TC3, case, f3, b3, list(range(case.n)), rms_check=False)
+    f, b = case.run(F32)
+    _check('relu padded rows F32', F32, case, f, b, list(range(case.n)), rms_check=False)
+    tf, _, mass, _ = case.truth(list(range(case.n)))
+    assert np.all(np.abs(f3 - f) <= 2 * EVAL_REL[TC3] * mass)
 
 
 def test_tc3_flags_hidden_values_beyond_float16_and_f32_takes_them(eng):
@@ -245,6 +465,57 @@ def test_closed_tanh_through_the_new_entry_point_is_the_old_one(eng, shape):
     for x, y in zip(a[:2], b[:2]):
         assert np.array_equal(x, y)
     assert eng.closed_mlp_plan(list(shape), p.band, activation=TANH) == eng.closed_mlp_plan(list(shape), p.band)
+
+
+def _reversed(p, d):
+    """Problem ``p``'s inputs with the pairs in reverse order (indices, noise and the saved evaluations)."""
+    n = p.n_pairs
+    return dict(d, idx=d['idx'][::-1].copy(), noise=None if d['noise'] is None else d['noise'][::-1].copy(),
+                saved=[(n - 1 - k, s) for k, s in d['saved']])
+
+
+# (shape, band, cluster size, T): simple_conf, and test_gpu_closed_f64's eight-CTA shape (band 16)
+_CLOSED_ORDER = [((15, 256, 256, 3), 8, 2, 60), ((384, 256, 256, cf.largest_eight_cta_width(), 64), 16, 8, 12)]
+
+
+@pytest.mark.parametrize('name', list(ACTS))
+@pytest.mark.parametrize('shape,band,C,T', _CLOSED_ORDER, ids=[f'C{c}' for _, _, c, _ in _CLOSED_ORDER])
+def test_closed_loop_clusters_and_pair_order(eng, name, shape, band, C, T):
+    """Against the float64 truth at clusters of 2 and 8 CTAs, with action noise and 2 episodes; the pairs reversed give
+    every fitness and behaviour bit for bit (the ObStat sums: within the truth's bound, their atomics have no fixed order)."""
+    act, f64act = ACTS[name]
+    p = cf.Problem(name, shape, T, 1.0, 0.5, seed=7 + C, band=band, n_pairs=3, E=2, ac_std=0.05)
+    assert closed_f64.cluster_size(list(shape), band) == C and eng.closed_mlp_plan(list(shape), band, activation=act)[0] == C
+    d = cf.build(p)
+    got = _closed_run(eng, p, d, act)
+    assert got[5] == 1
+    args, kw = cf.truth_args(p, d)
+    tr = act_f64.closed_truth(*args, activation=f64act, **kw)
+    cf._check(f'{name} {shape}', p, got[:5], tr, d['saved'], d['spec'].pos_scale)
+    rev = _closed_run(eng, p, _reversed(p, d), act)
+    assert np.array_equal(got[0], rev[0][:, ::-1]) and np.array_equal(got[1], rev[1][:, ::-1]), 'the reversed run differs'
+    cf._check(f'{name} {shape} reversed', p, (rev[0][:, ::-1], rev[1][:, ::-1]) + rev[2:5], tr, d['saved'], d['spec'].pos_scale)
+
+
+@pytest.mark.parametrize('regime', list(REGIMES))
+def test_closed_loop_activation_regimes(eng, regime):
+    """REGIMES in the closed loop (a cluster of one CTA), with action noise; the loop shown not to amplify rounding first
+    (closed_f64.growth <= 100, as test_gpu_closed_f64's problems)."""
+    act, form, how = REGIMES[regime]
+    p = cf.Problem(regime, (8, 32, 32, 4), 60, 1.0, 0.2, seed=41, n_pairs=4, E=2, ac_std=0.05)
+    d = cf.build(p)
+    if how == 'tails':
+        d['theta'] = _place_in_sigmoid_tails(d['theta'], list(p.sizes), np.random.RandomState(42))
+    elif how == 'small':
+        d['theta'] = (d['theta'] * SMALL).astype(np.float32)
+        d['table'] = (d['table'] * SMALL).astype(np.float32)
+        d['noise'] = (d['noise'] * SMALL).astype(np.float32)
+    args, kw = cf.truth_args(p, d)
+    growth = closed_f64.growth(*args, activation=form, **kw)
+    assert growth <= 100, growth
+    got = _closed_run(eng, p, d, act)
+    tr = act_f64.closed_truth(*args, activation=form, **kw)
+    cf._check(f'closed {regime} (growth {growth:.3g})', p, got[:5], tr, d['saved'], d['spec'].pos_scale)
 
 
 # ------------------------------------------------------------------------------------------------ generations

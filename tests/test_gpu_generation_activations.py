@@ -1,0 +1,121 @@
+"""GPU: whole generations of policies with ReLU, leaky-ReLU, ELU and sigmoid activations (DeviceGeneration(activation=...),
+es.step with BatchedRollout(fuse_activations=True)) at the shipped configs' shapes, judged stage by stage (tests/gen_stages.py)
+against exact and float64 references, the float64 truth applying the policy's activation (tests/act_f64.py's forms).
+
+Built as test_gpu_generation_shipped_configs.py (its Setup, runs, judge, rerun and modelled bugs; the same table, streams,
+theta0, sigma, Adam and save_obs coins), with one activation per config:
+  simple_conf 15-256-256-3 (K = 2400, T = 1000, ac_std 0.01)   ReLU: ES_ROLLOUT_TC3 (two generations) and ES_ROLLOUT_F32 (staged
+                                                                weights, several launches);
+  obj 17-256-256-256-6                                          leaky ReLU (slope 0.1), TC3;
+  flagrun 28-128-256-256-128-8 (10 episodes)                    ELU (alpha 0.7), TC3;
+  nsra (the NSR blend, a 5- then 6-entry archive)                sigmoid, TC3, two generations;
+  376-64-64-17 (configs 3 to 5: K = 10 000, T = 1000)           ReLU, F32 only (TC3 refuses obs 376), two generations;
+  the closed loop                                               ReLU in clusters of 2 (simple_conf), ELU in clusters of 4 (flagrun);
+and one es.step end to end (flagrun, ELU, action noise, 10 episodes) against a DeviceGeneration from the same state.  Each
+family's capture (open loop, NSR, F32, closed loop) is re-judged with the activation bugs gen_stages models: tanh in one
+hidden layer, torch's default slope / alpha in place of the policy's, no activation after the output layer.
+
+Rank shifts against the float64 truth (``RANK_BOUNDS``): about twice the largest values measured on an H100 SXM (80 GB HBM3,
+700 W power limit), where the whole file took 175 s (the closed-loop flagrun truth on the CPU: 96 s of it).
+"""
+import os
+import sys
+import time
+
+import numpy as np
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import gen_stages as gs  # noqa: E402
+import test_gpu_generation_shipped_configs as sc  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+
+# (largest rank shift, largest |dw|) against the float64 truth's ranks, per mode and population.  Measured: a shift of 1 at
+# K = 2400 (TC3 and F32, |dw| 2.1e-4 = 1 / 4799) and K = 4800 (|dw| 1.0e-4), none at K = 320 and 600; F32 at K = 10 000 a
+# shift of 2, |dw| 1.0e-4 = 2 / 19 999
+RANK_BOUNDS = {('tc3', 2400): (2, 2.5 / 4799), ('tc3', 4800): (2, 2.5 / 9599), ('tc3', 320): (2, 2.5 / 639),
+               ('tc3', 600): (2, 2.5 / 1199), ('f32', 2400): (2, 2.5 / 4799), ('f32', 10000): (4, 4.5 / 19999)}
+HUMANOID = dict(sizes=[376, 64, 64, 17], K=10_000, T=1000, E=1, ac_std=0.0)
+T0 = time.perf_counter()
+
+
+def _act(name):
+    from es_pytorch_b200 import _lib
+    from es_pytorch_b200.nn.nn import Activation
+    kind, param, module = {'relu': ('ES_ACT_RELU', 0.0, torch.nn.ReLU()),
+                           'leaky': ('ES_ACT_LEAKY_RELU', 0.1, torch.nn.LeakyReLU(0.1)),
+                           'elu': ('ES_ACT_ELU', 0.7, torch.nn.ELU(0.7)),
+                           'sigmoid': ('ES_ACT_SIGMOID', 0.0, torch.nn.Sigmoid())}[name]
+    return Activation(getattr(_lib, kind), float(np.float32(param))), module
+
+
+@pytest.fixture(scope='module')
+def table(eng):
+    g = torch.Generator(device=eng.device).manual_seed(123)
+    t = torch.randn(sc.TABLE, generator=g, device=eng.device, dtype=torch.float32)
+    yield t
+    del t
+    torch.cuda.empty_cache()
+
+
+def _case(eng, table, name, mode, act, **kw):
+    return sc._case(eng, table, name, mode, activation=_act(act)[0], rank_bounds=RANK_BOUNDS, **kw)
+
+
+_ACT_BUGS = ('act_tanh_layer', 'act_no_output')
+_ALL_ACT_BUGS = gs.ACT_MUTATIONS                                   # + the default slope / alpha: leaky ReLU and ELU
+
+
+def test_simple_conf_relu_tc3_two_generations(eng, table):
+    sc._assert_ok(_case(eng, table, 'simple_conf', 'tc3', 'relu', generations=2, mutations=_ACT_BUGS, mutate_gen=0))
+
+
+def test_simple_conf_relu_f32_staged_weights(eng, table):
+    gw, chunk = sc.rf._f32_layout(sc.SHIPPED['simple_conf']['sizes'])
+    assert gw and sc.SHIPPED['simple_conf']['K'] > chunk           # staged weights, several launches
+    sc._assert_ok(_case(eng, table, 'simple_conf', 'f32', 'relu'))
+
+
+def test_obj_leaky_tc3(eng, table):
+    sc._assert_ok(_case(eng, table, 'obj', 'tc3', 'leaky', mutations=_ALL_ACT_BUGS))
+
+
+def test_flagrun_elu_tc3_ten_episodes(eng, table):
+    sc._assert_ok(_case(eng, table, 'flagrun', 'tc3', 'elu',
+                        mutations=('episode0_noise', 'episodes_not_divided', 'first_episode_behaviour') + _ALL_ACT_BUGS))
+
+
+def test_nsra_sigmoid_tc3_two_generations(eng, table):
+    """w = 1 with a 5-entry archive, then w = 0.5 with 6 entries (as the tanh file's nsra); the NSR and activation bugs on
+    generation 1."""
+    a5, a6 = sc._archive(5), sc._archive(6)
+    sc._assert_ok(_case(eng, table, 'nsra', 'tc3', 'sigmoid', generations=2, archive=a5, archives=[a5, a6], moo_ws=(1.0, 0.5),
+                        mutations=('novelty_over_reward', 'moo_w_swapped') + _ACT_BUGS, mutate_gen=0))
+
+
+def test_humanoid_relu_f32_two_generations(eng, table):
+    """configs 3 to 5's policy: ES_ROLLOUT_TC3 covers obs <= 256, so an activation at obs 376 runs in F32 only."""
+    sc._assert_ok(_case(eng, table, 'humanoid', 'f32', 'relu', generations=2, cfg=HUMANOID, mutations=_ACT_BUGS,
+                        mutate_gen=0))
+
+
+@pytest.mark.parametrize('name,cluster,act', [('simple_conf', 2, 'relu'), ('flagrun', 4, 'elu')])
+def test_closed_loop(eng, table, name, cluster, act):
+    from es_pytorch_b200.gym.synthetic_env import ClosedLoopEnv
+    cfg = sc.SHIPPED[name]
+    band = ClosedLoopEnv(cfg['sizes'][0], cfg['sizes'][-1], 2).band
+    assert sc.cf.plan(cfg['sizes'], band) == cluster
+    assert eng.closed_mlp_plan(cfg['sizes'], band, activation=_act(act)[0])[0] == cluster
+    muts = _ACT_BUGS if name == 'simple_conf' else ()
+    sc._assert_ok(_case(eng, table, name, 'tc3', act, closed=True, mutations=muts))
+
+
+def test_e2e_step_flagrun_elu_ten_episodes(eng, table):
+    act, module = _act('elu')
+    sc._e2e(eng, table, 'flagrun', module=module, activation=act)
+
+
+def test_file_wall_time():
+    print(f'\nactivation generations: file wall time {time.perf_counter() - T0:.0f} s')

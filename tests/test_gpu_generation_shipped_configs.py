@@ -87,9 +87,11 @@ def _archive(n):
 class Setup:
     """The env and the device generation of one case, and how to rebuild it from a captured start state."""
 
-    def __init__(self, eng, table, cfg, mode_name, archive=None, moo_w=0.5, closed=False):
+    def __init__(self, eng, table, cfg, mode_name, archive=None, moo_w=0.5, closed=False, activation=None, rank_bounds=None):
         from es_pytorch_b200.gym.synthetic_env import ClosedLoopEnv, SyntheticEnv
         self.eng, self.table, self.cfg, self.mode_name = eng, table, cfg, mode_name
+        # the policy's activation (an nn.Activation; None: tanh) and the rank-shift bounds it is judged by
+        self.activation, self.rank_bounds = activation, RANK_BOUNDS if rank_bounds is None else rank_bounds
         self.sizes, self.T, self.E, self.ac_std = cfg['sizes'], cfg['T'], cfg['E'], cfg['ac_std']
         self.P = sum(i * o + o for i, o in zip(self.sizes[:-1], self.sizes[1:]))
         self.archive, self.moo_w, self.closed = archive, moo_w, closed
@@ -111,7 +113,8 @@ class Setup:
                                coins_per_eval=1, save_obs_chance=CHANCE, rollout_mode=_mode(self.mode_name), engine=eng,
                                archive=None if self.archive is None else eng.to_device(self.archive, torch.float64),
                                nov_k=NOV_K, moo_w=self.moo_w, ac_std=self.ac_std, episodes=self.E,
-                               closed=self.env.device_closed(eng) if self.closed else None, closed_act_noise=self.closed)
+                               closed=self.env.device_closed(eng) if self.closed else None, closed_act_noise=self.closed,
+                               activation=self.activation)
         if ob is not None:
             gen.set_obstat(*ob)
         return gen
@@ -146,17 +149,21 @@ def _rollout_launches(s: Setup, n):
         return 1
     mode = _mode(s.mode_name)
     if mode == _lib.ES_ROLLOUT_F32:
+        if s.activation is not None:                     # the general kernel only, never the packed-FMA one
+            gw, chunk = rf._f32_layout(s.sizes)
+            return 2 * -(-n // chunk) if gw else 1
         return rf._f32_launches(s.sizes, n, s.eng.sm_count)
     return rw._tcw_launches(s.sizes, mode, n)
 
 
 def _launches(s: Setup, gen, first: bool) -> int:
-    """One DeviceGeneration.run, restated from the host code: the draw (``_draw_launches``), the normalisation (1, open loop), the rollout (``_rollout_launches``: the wide tensor-core
+    """One DeviceGeneration.run, restated from the host code: the draw (``_draw_launches``; without action noise the
+    indices and coins alone, 1), the normalisation (1, open loop), the rollout (``_rollout_launches``: the wide tensor-core
     launcher's builder + rollout + finish per chunk, the staged float32 kernel's two per chunk, the closed loop's one
     cluster launch, which also accumulates the obs statistics), novelty (1, with an archive), the open loop's obs statistics
     (the column sums on the first generation only, coin count + accumulate), the rank (keys, histogram, scan, scatter,
     finalise), the reconstruction (1) and Adam (1).  Not counted: the jump lists (1, once per engine)."""
-    n = _draw_launches(gen.k_local // gen.n_streams, s.E * s.T * s.sizes[-1])
+    n = _draw_launches(gen.k_local // gen.n_streams, s.E * s.T * s.sizes[-1]) if s.ac_std else 1     # es_draw_indices
     n += _rollout_launches(s, gen.k_local)
     if not s.closed:
         n += 1 + (1 if first else 0) + 2
@@ -196,13 +203,13 @@ def _run(s: Setup, gen, nps):
                      streams1=_streams(gen), behv=None if gen.behv is None else gen.behv.cpu().numpy(),
                      act_noise=gen.act_noise if gen.ac_std else None,
                      archive=None if gen.archive is None else gen.archive.cpu().numpy(), nov_k=gen.nov_k, moo_w=gen.moo_w,
-                     episodes=gen.episodes, **closed, **st0)
+                     episodes=gen.episodes, activation=s.activation, **closed, **st0)
     return cap, launches
 
 
 def _judge(s: Setup, tag, cap, nl, truth=None):
     t = time.perf_counter()
-    shift, dw = RANK_BOUNDS.get((s.mode_name, cap.K), (None, None))
+    shift, dw = s.rank_bounds.get((s.mode_name, cap.K), (None, None))
     checks = gs.judge(cap, _mode(s.mode_name), s.eng.sm_count, shift, dw, truth=truth)
     print(f'\n{gs.report(f"{tag} ({nl} launches)", checks)}\n  ranks vs truth: {cap.extra.get("ranks_vs_truth")}, '
           f'fitness error: {cap.extra.get("fitness")}, saves {cap.extra.get("n_saved")}, '
@@ -264,7 +271,7 @@ def _not_vacuous(s: Setup, cap, names, truth=None):
         truth = gs.fitness_truth(cap)
     if cap.closed:
         truth = cap.extra['closed_truth']
-    shift, dw = RANK_BOUNDS.get((s.mode_name, cap.K), (None, None))
+    shift, dw = s.rank_bounds.get((s.mode_name, cap.K), (None, None))
     for name in names:
         what, mutate = gs.MUTATIONS[name]
         stages, margin = gs.rejection(gs.judge(mutate(cap), _mode(s.mode_name), s.eng.sm_count, shift, dw, truth=truth))
@@ -281,11 +288,13 @@ def _obstat(caps, obs):
 
 
 def _case(eng, table, name, mode_name, generations=1, archive=None, moo_ws=(0.5,), archives=None, closed=False,
-          mutations=(), mutate_gen=-1, cfg=None):
+          mutations=(), mutate_gen=-1, cfg=None, activation=None, rank_bounds=None):
     """Run ``generations`` generations of config ``name``, judge each, re-judge generation ``mutate_gen`` with the modelled
-    bugs ``mutations``, rerun the last one; every failed check returned, per generation."""
+    bugs ``mutations``, rerun the last one; every failed check returned, per generation.  ``activation``, ``rank_bounds``:
+    as Setup's."""
     cfg = dict(SHIPPED[name] if cfg is None else cfg)
-    s = Setup(eng, table, cfg, mode_name, archive=archive, moo_w=moo_ws[0], closed=closed)
+    s = Setup(eng, table, cfg, mode_name, archive=archive, moo_w=moo_ws[0], closed=closed, activation=activation,
+              rank_bounds=rank_bounds)
     gen, nps = s.gen, cfg['K'] // STREAMS
     caps, bad = [], []
     for g in range(generations):
@@ -412,9 +421,10 @@ def test_closed_loop(eng, table, name, cluster):
     _assert_ok(_case(eng, table, name, 'tc3', closed=True, mutations=muts))
 
 
-def _e2e(eng, table, name, archive=None, moo_w=None):
+def _e2e(eng, table, name, archive=None, moo_w=None, module=None, activation=None):
     """es.step (BatchedRollout over the 8 streams, the env resident on the device) against a DeviceGeneration from the same
-    state: indices, fitness, weights and theta' bit for bit, and the callers' streams."""
+    state: indices, fitness, weights and theta' bit for bit, and the callers' streams.  ``module``: the policy's activation
+    module in place of tanh, ``activation`` its nn.Activation (es.step through BatchedRollout(fuse_activations=True))."""
     from es_pytorch_b200 import _lib, dist
     from es_pytorch_b200.core import es
     from es_pytorch_b200.core.noisetable import NoiseTable
@@ -425,17 +435,19 @@ def _e2e(eng, table, name, archive=None, moo_w=None):
     from es_pytorch_b200.utils.rankers import CenteredRanker, MultiObjectiveRanker
     from es_pytorch_b200.utils.reporters import Reporter
     cfg = SHIPPED[name]
-    s = Setup(eng, table, cfg, 'tc3', archive=archive, moo_w=0.5 if moo_w is None else moo_w)
+    s = Setup(eng, table, cfg, 'tc3', archive=archive, moo_w=0.5 if moo_w is None else moo_w, activation=activation)
     nps = cfg['K'] // STREAMS
     gen = s.gen
     gen.run(nps)
-    net = FeedForward(list(s.sizes[1:-1]), torch.nn.Tanh(), s.env, cfg['ac_std'], 5)
+    net = FeedForward(list(s.sizes[1:-1]), torch.nn.Tanh() if module is None else module, s.env, cfg['ac_std'], 5)
+    assert (net.activation() if module is not None else None) == activation
     policy = Policy(net, SIGMA, Adam(s.P, LR))
     policy.flat_params[...] = _theta0(s.sizes, False)
     nt = NoiseTable(s.P, table)
     streams = [np.random.RandomState(1000 + r) for r in range(STREAMS)]
     fit_fn = BatchedRollout(s.env, s.T, coins_per_eval=1, save_obs_chance=CHANCE, rank_streams=streams,
-                            rollout_mode=_lib.ES_ROLLOUT_TC3, archive=archive, nov_k=NOV_K, episodes=cfg['E'])
+                            rollout_mode=_lib.ES_ROLLOUT_TC3, archive=archive, nov_k=NOV_K, episodes=cfg['E'],
+                            fuse_activations=module is not None)
     fit_fn.stream_env_from_host = False
 
     class _Cfg(dict):
@@ -445,7 +457,7 @@ def _e2e(eng, table, name, archive=None, moo_w=None):
             s.env, fit_fn, streams[0], ranker, Reporter())
     eng.sync()
     g2 = fit_fn._gen
-    assert g2 is not gen and g2.K == gen.K == cfg['K'] and g2.episodes == cfg['E']
+    assert g2 is not gen and g2.K == gen.K == cfg['K'] and g2.episodes == cfg['E'] and g2.activation == activation
     assert torch.equal(g2.idx, gen.idx) and torch.equal(g2.fit_local, gen.fit_local) and torch.equal(g2.weights, gen.weights)
     assert np.array_equal(np.asarray(ranker.noise_inds).astype(np.int64), gen.idx.cpu().numpy())
     assert np.array_equal(np.asarray(ranker.ranked_fits).reshape(-1), gen.weights.cpu().numpy())
