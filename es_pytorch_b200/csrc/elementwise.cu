@@ -37,7 +37,7 @@ __global__ void normalise_kernel(const float* __restrict__ obs, const double* __
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const int d = (int)(i % obs_dim);
         double x = __ddiv_rn(__dsub_rn((double)obs[i], mean[d]), std[d]);
-        x = fmin(fmax(x, -clip), clip);
+        x = isnan(x) ? x : fmin(fmax(x, -clip), clip);              // torch.clamp passes a NaN (fmax(NaN, -clip) is -clip)
         out[i] = (float)x;
     }
 }

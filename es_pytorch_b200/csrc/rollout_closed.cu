@@ -87,7 +87,7 @@ __host__ __device__ inline ClLayout cl_layout(int JL, int obs, int act, int band
 // ~2^28 values (and then by one float32 ulp) -- far inside the tolerance this variant is held to
 __device__ __forceinline__ float cl_normalise(float o, double mean, double rstd, double clip) {
     double x = ((double)o - mean) * rstd;
-    x = fmin(fmax(x, -clip), clip);
+    x = isnan(x) ? x : fmin(fmax(x, -clip), clip);    // torch.clamp passes a NaN (fmax(NaN, -clip) is -clip)
     return (float)x;
 }
 // the float32 pairs (es_f32x2) of this kernel hold (+, -) of a weight times (x+, x-) of an input

@@ -60,7 +60,7 @@ __host__ __device__ inline CwLayout cw_layout(int n_layers, const int* dims, int
 
 __device__ __forceinline__ float cw_normalise(float o, double mean, double std, double clip) {
     double x = ((double)o - mean) / std;
-    x = fmin(fmax(x, -clip), clip);
+    x = isnan(x) ? x : fmin(fmax(x, -clip), clip);    // torch.clamp passes a NaN (fmax(NaN, -clip) is -clip)
     return (float)x;
 }
 // the warp-wide sums of v[0..3] in 7 shuffles (transposing butterfly, the xor-16, 8, 4, 2, 1 tree for every row): lane L

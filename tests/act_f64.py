@@ -121,7 +121,7 @@ def closed_truth(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, e
         pos, mag = np.zeros((N, 3)), np.zeros((N, 3))
         osum, osq, oabs = (np.zeros((N, obs)) for _ in range(3))
         for t in range(T):
-            h = np.clip((ob - mean) / std, -float(clip), float(clip))
+            h = closed_f64.normalise(ob, mean, std, float(clip))
             for (WT, b, _), act_fn in zip(layers, per_layer(activation, len(layers))):
                 h = act_fn(np.matmul(h[:, None, :], WT)[:, 0, :] + b)
             a = h if nz_all is None else h + nz_all[:, e, t]

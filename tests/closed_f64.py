@@ -154,6 +154,12 @@ def _weights(table, idx, theta, sigma, sizes, pairs):
     return out
 
 
+def normalise(ob, mean, std, clip):
+    """nn.py:45's ``torch.clamp((ob - mean) / std, -clip, clip)`` in float64: np.clip keeps a NaN and clips +-inf, as
+    torch.clamp does."""
+    return np.clip((ob - mean) / std, -clip, clip)
+
+
 def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a, env_b, rew_vec, pos_scale,
              act_noise=None, episodes: int = 1, pairs: Optional[Sequence[int]] = None, variants=(None,), obs0_shift=None,
              activation=np.tanh):
@@ -240,7 +246,7 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
         osum, osq, oabs = (np.zeros((N, V, obs)) for _ in range(3))
         for t in range(T):
             live = ~(drop_last & (t == T - 1))                                  # [V]
-            h = np.clip((ob - vmean[None]) / std, -vclip, vclip)
+            h = normalise(ob, vmean[None], std, vclip)
             for l, (WT, _, _) in enumerate(layers):
                 if any_masks[1][l]:
                     h = h * in_mask[l][None]

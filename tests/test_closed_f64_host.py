@@ -148,3 +148,33 @@ def test_every_mutation_fails_some_problem_of_each_shape(key):
             best[mu] = max(best[mu], r)
     missed = {mu: r for mu, r in best.items() if r < MUT_MIN}
     assert not missed, (key, missed)
+
+
+def test_the_observation_clip_is_torch_clamp():
+    """The oracle's normalise_obs and the float64 truths' clip (closed_f64.normalise, which act_f64 uses too) against torch.clamp
+    (nn.py:45): a NaN stays NaN, +-inf becomes +-clip, +-clip and the values next to it are exact.  The GPU tests of a NaN
+    in the observation mean compare against these."""
+    import torch
+    import act_f64
+    clip = 5.0
+    x = np.array([np.nan, np.inf, -np.inf, clip, -clip, np.nextafter(clip, 9), np.nextafter(-clip, -9), np.nextafter(clip, 0),
+                  0.0, -0.0, 1e30, -1e-30])
+    want = torch.clamp(torch.from_numpy(x), -clip, clip).numpy()
+    assert np.isnan(want[0]) and list(want[1:5]) == [clip, -clip, clip, -clip]
+    got = cf.normalise(x, np.zeros_like(x), np.ones_like(x), clip)
+    assert np.array_equal(got, want, equal_nan=True) and np.array_equal(np.signbit(got), np.signbit(want))
+    ob = x.astype(np.float32)
+    got32 = orc.normalise_obs(ob, np.zeros_like(x), np.ones_like(x), clip)
+    want32 = torch.clamp(torch.from_numpy(ob).double(), -clip, clip).float().numpy()
+    assert np.array_equal(got32, want32, equal_nan=True)
+    # a NaN in the mean, and an infinite one, through both closed-loop truths: every fitness NaN / every fitness finite
+    sizes, T = [4, 3, 2], 3
+    P = orc.n_params(orc.layer_dims(4, [3], 2))
+    rs = np.random.RandomState(0)
+    table, theta, idx = rs.randn(P + 10).astype(np.float32), rs.randn(P).astype(np.float32), np.array([0, 5])
+    spec = orc.ClosedLoopEnvSpec(4, 2, T, band=2)
+    for m, finite in (([np.nan, 0, 0, 0], False), ([np.inf, -np.inf, 0, 0], True)):
+        args = (table, idx, theta, 0.02, sizes, np.array(m), np.ones(4), clip, spec.obs_stream[0], spec.env_a.T, spec.env_b.T,
+                spec.rew_vec, spec.pos_scale)
+        for f in (cf.truth(*args)['fit'], act_f64.closed_truth(*args)['fit']):
+            assert (np.isfinite(f) if finite else np.isnan(f)).all(), f

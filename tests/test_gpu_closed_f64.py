@@ -239,3 +239,68 @@ def test_closed_kernels_match_the_float64_truth(eng, p):
     assert got[5] == 1
     args, kw = truth_args(p, d)
     _check(f'{p.id} C={C}', p, got[:5], cf.truth(*args, **kw), d['saved'], d['spec'].pos_scale)
+
+
+# ---------------------------------------------------------------------------------------------- a NaN in the observation mean
+# torch.clamp (nn.py:45) keeps a NaN, so a NaN in ob_mean makes that observation column NaN at every step: every output of a
+# tanh or activation stack and every fitness is NaN, in the float64 truth and on the device.  A binned head's arg-max over
+# all-NaN outputs is bin 0 (torch.argmax), so its fitness stays finite and is held to the binned tests' bound.
+_NAN_FAMILIES = [('one_cta', (17, 64, 64, 6), None, 0), ('wide', (15, 256, 256, 3), None, 0),
+                 ('activation', (17, 64, 64, 6), 'relu', 0), ('binned', (15, 64, 64, 15), None, 5)]
+
+
+@pytest.mark.parametrize('loop', ['open', 'closed'])
+@pytest.mark.parametrize('name,sizes,act_kind,bins', _NAN_FAMILIES, ids=[f[0] for f in _NAN_FAMILIES])
+def test_nan_in_the_observation_mean_reaches_the_fitness(eng, name, sizes, act_kind, bins, loop):
+    import act_f64
+    from es_pytorch_b200 import _lib
+    from es_pytorch_b200.nn.nn import Activation, BinnedHead
+    sizes, T, n = list(sizes), 30, 3
+    obs = sizes[0]
+    adim = sizes[-1] // bins if bins else sizes[-1]
+    head = BinnedHead(bins, np.float32([-1.0, 0.0, 0.5]), np.float32([1.0, 2.0, 0.75])) if bins else None
+    activation = Activation(_lib.ES_ACT_RELU, 0.0) if act_kind else None
+    f64_act = act_f64.relu if act_kind else np.tanh
+    P = orc.n_params(orc.layer_dims(obs, sizes[1:-1], sizes[-1]))
+    rs = np.random.RandomState(len(sizes) + obs)
+    table, theta = rs.randn(P + 20_000).astype(np.float32), (rs.randn(P) * 0.1).astype(np.float32)
+    idx = rs.randint(0, 20_000, size=n).astype(np.int64)
+    mean, std, clip = rs.randn(obs) * 0.05, 0.5 + rs.rand(obs), 1.0
+    mean[1] = np.nan
+    dv = eng.to_device
+    spec = orc.ClosedLoopEnvSpec(obs, adim, T, band=8) if loop == 'closed' else orc.SyntheticEnvSpec(obs, adim, T)
+    fit = torch.zeros(2, n, dtype=torch.float64, device=eng.device)
+    behv = torch.zeros(2, n, 3, dtype=torch.float32, device=eng.device)
+    if loop == 'open':
+        obsn = eng.normalise_obs(dv(spec.obs_stream[:T]), dv(mean), dv(std), clip)
+        eng.rollout(dv(table), dv(idx), dv(theta), SIGMA, sizes, obsn, dv(spec.rew_vec[:T]), spec.pos_scale, fit[0], fit[1], 1,
+                    behv[0], behv[1], head=head, activation=activation)
+    else:
+        eng.rollout_closed_mlp(dv(table), dv(idx), dv(theta), SIGMA, sizes, dv(mean), dv(std), clip, dv(spec.obs_stream[0].copy()),
+                               dv(np.ascontiguousarray(spec.env_a.T)), dv(np.ascontiguousarray(spec.env_b.T)), dv(spec.rew_vec),
+                               spec.pos_scale, fit[0], fit[1], 1, behv[0].view(-1), behv[1].view(-1), head=head,
+                               activation=activation)
+    eng.sync()
+    f = fit.cpu().numpy()
+    if bins:                                   # the oracle's per-step loop: torch.argmax of the NaN outputs
+        dims = orc.layer_dims(obs, sizes[1:-1], sizes[-1])
+        want, bound = np.zeros((2, n)), np.zeros((2, n))
+        for k, i in enumerate(idx):
+            for s, sign in enumerate((1.0, -1.0)):
+                layers = orc.unflatten(orc.pheno_params(theta, SIGMA, sign * orc.table_get(table, int(i), P)), dims)
+                rews = orc.run_model(spec, layers, mean, std, clip, T, binned=(bins, head.low, head.high))[0]
+                want[s, k], bound[s, k] = sum(rews), 2e-5 * max(1.0, np.abs(rews).sum())
+        assert np.isfinite(want).all()
+    elif loop == 'open':
+        obsn_h = orc.normalise_obs(spec.obs_stream[:T], mean, std, clip)
+        want, _, mass, _ = act_f64.rollout_f64(table, idx, theta, SIGMA, sizes, obsn_h, spec.rew_vec[:T], spec.pos_scale, f64_act)
+        bound = EVAL_REL * mass
+        assert np.isnan(want).all()
+    else:
+        tr = act_f64.closed_truth(table, idx, theta, SIGMA, sizes, mean, std, clip, spec.obs_stream[0], spec.env_a.T,
+                                  spec.env_b.T, spec.rew_vec, spec.pos_scale, activation=f64_act)
+        want, bound = tr['fit'], EVAL_REL * tr['mass']
+        assert np.isnan(want).all()
+    nan = np.isnan(want)
+    assert np.array_equal(np.isnan(f), nan), f
+    assert np.all(np.abs(f[~nan] - want[~nan]) <= bound[~nan]), (f, want)
