@@ -64,11 +64,15 @@ SIGNATURES = {
                                                     _vp, _vp, _vp, _i32, _i32, _f32, _vp]),
     'es_rollout_closedloop_mlp_activation_plan': (_i32, [_vp, C.POINTER(_i32), _i32, _i32, _i32, C.POINTER(_i32), C.POINTER(_i32),
                                                          C.POINTER(_i64)]),
+    'es_rollout_closedloop_terminal': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64,
+                                              _vp, _vp, _i32, _vp, _vp, _i32, _f32, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _vp, _vp,
+                                              _vp, _i32, _vp, _vp, _i32, _f32, _vp, _i32, _f32, _vp, _vp, _vp]),
     'es_draw_noisy': (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _u64, _i32, _i32, _f64, _vp, _vp, _vp, _vp]),
     'es_randn': (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
     'es_randn_plan': (_i32, [_vp, _i64, C.POINTER(C.c_size_t), C.POINTER(_i32)]),
     'es_novelty': (_i32, [_vp, _vp, _i32, _vp, _i32, _i32, _vp, _i32, _vp]),
     'es_fitness_objective': (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _i32, _vp]),
+    'es_fitness_objective_steps': (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _vp]),
     'es_centered_rank': (_i32, [_vp, _vp, _vp, _i32, _i32, _f32, _f32, _i32, _i32, _vp, _vp, _vp]),
     'es_rank_transform': (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _f64, _f64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                  _vp, _vp]),

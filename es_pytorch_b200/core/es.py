@@ -79,7 +79,7 @@ def _queue_common_downloads(eng, gen, fpos, fneg):
     nk = R * gen.mt_key.shape[1]
     h_key, h_mtpos = h_state[:nk].view(R, -1), h_state[nk:nk + R]
     gen._h_gauss = (h_state[nk + R:nk + 2 * R], h_state[nk + 2 * R:].view(torch.float64))    # valid after the synchronisation
-    h_stats = eng.download_async(gen._gen_stats, 'gstats') if gen.extra_words else None
+    h_stats = eng.download_async(gen._gen_stats, 'gstats') if (gen.extra_words or gen.fall_height is not None) else None
     return h_pos, h_neg, h_key, h_mtpos, h_stats
 
 
@@ -95,6 +95,26 @@ def _obstat_from(h_stats, obs_dim):
     return a[:obs_dim].copy(), a[obs_dim:2 * obs_dim].copy(), float(a[2 * obs_dim])
 
 
+def _steps_from(gen, h_stats, max_steps: int) -> int:
+    """The generation's steps as test_params sums them (es.py:76): every evaluation's t_d on an env whose episodes end early
+    (the sum rode with the obs statistics), else 2K (T - 1) (run_model returns the last loop index, gym_runner.py:50,67)."""
+    if gen.fall_height is None:
+        return 2 * gen.K * (max_steps - 1)
+    return int(h_stats.numpy()[2 * gen.obs_dim + 2])
+
+
+def _terminates(fit_fn) -> bool:
+    return bool(getattr(fit_fn, 'terminates', False))
+
+
+def _noisy_terminal(policy: Policy, fit_fn) -> bool:
+    """Whether ``fit_fn`` evaluates ``policy`` with action noise on an env whose episodes end early (a binned head draws no
+    noise: FFBinned.forward ignores rs)."""
+    fused = _fused_policy(policy._module, fit_fn)
+    return (_terminates(fit_fn) and fused is not None and fused[0] == 'tanh'
+            and float(getattr(policy._module, '_action_std', 0) or 0) != 0)
+
+
 def _can_fuse_step(comm, policy: Policy, fit_fn, ranker: Ranker) -> bool:
     """``step`` can keep the whole generation on the device (one synchronisation) when the evaluation is a
     ``BatchedRollout`` of a network the fused rollouts evaluate (a tanh MLP or a binned-action one: ``BaseNet.head``; with
@@ -103,6 +123,11 @@ def _can_fuse_step(comm, policy: Policy, fit_fn, ranker: Ranker) -> bool:
     they take the call-by-call route)."""
     from .._lib import ES_RANK_MAX_NORMALIZED
     if not getattr(fit_fn, 'is_batched_rollout', False) or _fused_policy(policy._module, fit_fn) is None:
+        return False
+    if _terminates(fit_fn) and (fit_fn.objective == 'mean_reward' or _noisy_terminal(policy, fit_fn)):
+        # MeanRewardResult raises ZeroDivisionError for an evaluation that falls at its first step, before anything is ranked:
+        # test_params -> rank -> approx_grad leaves the device theta untouched when it does.  Action noise runs one evaluation
+        # at a time (test_params)
         return False
     if comm.size != dist.world().size:                       # a communicator this package does not drive
         return False
@@ -156,6 +181,7 @@ def _step_fused(cfg, comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: O
     h_w = eng.download_async(w_all, ('ranked', id(ranker)))
     h_theta = eng.download_async(gen.theta, ('theta', id(policy)))
     h_fit0, h_behv0 = eng.download_async(fit0, 'nlfit'), eng.download_async(behv0, 'nlbehv')
+    h_steps0 = eng.download_async(gen.nl_steps, 'nlsteps') if gen.fall_height is not None else None
     _mark('t3_all_queued')
     eng.sync()
     _mark('t4_synced')
@@ -165,9 +191,9 @@ def _step_fused(cfg, comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: O
     neg = devcache.attach(h_neg.numpy().reshape(gen.K, gen.n_obj).copy(), fneg, valid)
     inds = devcache.attach(h_idx.numpy().astype(np.float64), idx_all, valid)
     gen.store_states(streams, h_key.numpy().copy(), h_mtpos.numpy().copy(), _host_gauss(gen))
-    if h_stats is not None:
+    if h_stats is not None and gen.extra_words:
         gen_obstat.inc(*_obstat_from(h_stats, gen.obs_dim))
-    steps = 2 * gen.K * (fit_fn.max_steps - 1)
+    steps = _steps_from(gen, h_stats, fit_fn.max_steps)
     if not _silent(reporter):
         reporter.print(f'n dupes: {len(inds) - len(set(inds))}')
     # what Ranker.rank leaves behind (rankers.py:37-50)
@@ -181,10 +207,16 @@ def _step_fused(cfg, comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: O
     # what approx_grad and policy.pheno(zeros) leave behind: flat_params and the module carry the new theta
     policy.flat_params[...] = h_theta.numpy()
     policy.set_nn_params(torch.from_numpy(policy.flat_params.copy()))
-    noiseless_result = fit_fn.result_from_device(float(h_fit0.numpy()[0]), h_behv0.numpy()[0].astype(np.float64))
+    noiseless_result = fit_fn.result_from_device(float(h_fit0.numpy()[0]), h_behv0.numpy()[0].astype(np.float64),
+                                                 None if h_steps0 is None else int(h_steps0.numpy()[0, 0]))
     reporter.log_gen(ranker.fits, noiseless_result, policy, steps)
     _mark('t5_done')
     return noiseless_result, gen_obstat
+
+
+def _fall_height(fit_fn):
+    """The env's fall height as the generation keeps it (a python float), or None when its episodes run to the end."""
+    return float(fit_fn.env.fall_height) if _terminates(fit_fn) else None
 
 
 def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> DeviceGeneration:
@@ -201,7 +233,8 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
     if (gen is None or gen.theta is not theta or gen.n_streams != len(streams) or gen.table is not nt.device_table(eng)
             or gen.coins_per_eval != int(fit_fn.coins_per_eval) or gen.rollout_mode != fit_fn.rollout_mode
             or (gen.archive is None) != (fit_fn.archive is None) or gen.episodes != fit_fn.episodes
-            or gen.head_key != head_key or gen.act_key != act_key or gen.objective != objective):
+            or gen.head_key != head_key or gen.act_key != act_key or gen.objective != objective
+            or gen.fall_height != _fall_height(fit_fn)):
         env = fit_fn.env
         obs_dev, rew_dev = env.device_arrays(eng)
         T = fit_fn.max_steps
@@ -214,7 +247,7 @@ def _device_generation(fit_fn, policy: Policy, nt: NoiseTable, streams) -> Devic
                                ac_std=float(getattr(policy._module, '_action_std', 0.0) or 0.0),
                                closed=env.device_closed(eng) if getattr(env, 'is_synthetic_closedloop', False) else None,
                                episodes=fit_fn.episodes, head=head, closed_act_noise=True, objective=objective,
-                               activation=activation)
+                               activation=activation, fall_height=_fall_height(fit_fn))
         fit_fn._gen = gen
     else:
         gen.load_states(streams)
@@ -248,6 +281,8 @@ def _test_params_batched(comm, n: int, policy: Policy, nt: NoiseTable, gen_obsta
         raise NotImplementedError('the fused rollout evaluates tanh MLPs (FeedForward or FFBinned with torch.nn.Tanh), and with '
                                   'BatchedRollout(fuse_activations=True) FeedForward with ReLU, LeakyReLU, ELU or Sigmoid')
     streams = fit_fn.rank_streams if fit_fn.rank_streams is not None else [rs]
+    if _noisy_terminal(policy, fit_fn):
+        return _test_params_per_eval(comm, n, policy, nt, gen_obstat, fit_fn, streams)
     gen = _device_generation(fit_fn, policy, nt, streams)
     fpos, fneg = gen.evaluate(n)
     # one device->host hop for everything the reference API returns as ndarrays
@@ -266,10 +301,84 @@ def _test_params_batched(comm, n: int, policy: Policy, nt: NoiseTable, gen_obsta
     inds = h_idx.numpy().astype(np.float64)
     if gen.comm.size == 1:
         inds = devcache.attach(inds, gen.idx, valid)
-    if h_stats is not None:
+    if h_stats is not None and gen.extra_words:
         gen_obstat.inc(*_obstat_from(h_stats, gen.obs_dim))
-    steps = 2 * gen.K * (fit_fn.max_steps - 1)          # run_model returns the last loop index (gym_runner.py:50,67)
+    steps = _steps_from(gen, h_stats, fit_fn.max_steps)
+    if gen.fall_height is not None and gen.objective == 'mean_reward' and int(gen.steps_dev.min().item()) == 0:
+        # MeanRewardResult.get_result of an evaluation that fell at its first step: sum(rewards) / 0 (training_result.py:69),
+        # raised in test_params before anything is ranked
+        raise ZeroDivisionError('MeanRewardResult of an episode that ended at its first step: the reward is divided by steps = 0')
     return pos, neg, inds, steps
+
+
+def _test_params_per_eval(comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: ObStat, fit_fn, streams):
+    """test_params for a BatchedRollout on an env whose episodes end early, with action noise: one evaluation per launch.
+    Every draw of a RandomState stream comes after the previous evaluation's gaussians, and how many those are depends on
+    where that evaluation fell, so the next evaluation's noise index is unknown until it has run.  Per stream (one reference
+    rank) and pair, in the reference's order (es.py:67-74): ``nt.sample``, then per sign the save_obs coin(s), the rollout
+    (es_rollout_closedloop_terminal: the perturbed weights, es_perturb's, in both evaluations of a sigma = 0 pair) with
+    ``episodes x T x act`` gaussians drawn from a copy of the stream, and the stream advanced by the gaussians the executed
+    steps consumed, so that its state is the reference's.  Rows are rank-major, as test_params returns them."""
+    eng = get_engine()
+    module = policy._module
+    env, T, E = fit_fn.env, fit_fn.max_steps, fit_fn.episodes
+    head, activation = _fused_policy(module, fit_fn)
+    sizes = module.layer_sizes()
+    act, P = int(sizes[-1]), len(policy)
+    ac_std = float(module._action_std)
+    coins, chance = int(fit_fn.coins_per_eval), float(fit_fn.save_obs_chance)
+    if coins not in (0, 1):
+        # both evaluations of the sigma = 0 pair read the + slot's coin only when there is one coin per evaluation
+        raise ValueError(f'fit_fns draw at most one save_obs coin per evaluation, got coins_per_eval={coins}')
+    fit_fn._streams_in_use = streams                    # BatchedRollout.__call__ draws the noiseless call's coin from them
+    theta, table = policy.theta_dev(eng), nt.device_table(eng)
+    mean = eng.to_device(np.ascontiguousarray(module._obmean, dtype=np.float64).reshape(-1), torch.float64)
+    std = eng.to_device(np.ascontiguousarray(module._obstd, dtype=np.float64).reshape(-1), torch.float64)
+    rew = env.device_arrays(eng)[1][:T].contiguous()
+    obs0, env_a, env_b = env.device_closed(eng)
+    f64, dev = torch.float64, eng.device
+    fit, behv = torch.zeros(2, dtype=f64, device=dev), torch.zeros(2, 3, dtype=torch.float32, device=dev)
+    steps, used = torch.zeros(2, 1, dtype=torch.int32, device=dev), torch.zeros(2, 1, dtype=torch.int64, device=dev)
+    obs_dim = int(sizes[0])
+    stats = torch.zeros(2 * obs_dim + 2, dtype=f64, device=dev)
+    idx0 = torch.zeros(1, dtype=torch.int64, device=dev)
+    results_pos, results_neg, inds, total_steps = [], [], [], 0
+    for rs in streams:
+        for _ in range(n):
+            idx = nt.sample_idx(rs, P)                                   # nt.sample(rs) (es.py:67)
+            inds.append(idx)
+            w_pos, w_neg = eng.perturb(theta, table, torch.tensor([idx], dtype=torch.int64, device=dev), policy.std)
+            for w, results in ((w_pos, results_pos), (w_neg, results_neg)):
+                # the fit_fn's coin(s): rs.random() consumes the two 32-bit words randint(0, 2^32) returns, in that order
+                words = rs.randint(0, 2 ** 32, size=2 * coins, dtype=np.uint32) if coins else None
+                src = np.random.RandomState()
+                src.set_state(rs.get_state())
+                nz = (src.randn(E * T * act) * ac_std).astype(np.float32)
+                # both evaluations of the sigma = 0 pair are this one: the statistics come back doubled (exactly: 0 + x + x)
+                cw = None if words is None else eng.to_device(np.concatenate([words, words]).view(np.int32))
+                stats.zero_()
+                eng.rollout_closed_terminal(
+                    table, idx0, w.view(-1), 0.0, sizes, mean, std, float(module.ob_clip), obs0, env_a, env_b, rew,
+                    env.pos_scale, fit[0:1], fit[1:2], 1, behv[0], behv[1], coin_words=cw, save_obs_chance=chance,
+                    ob_sum=stats[:obs_dim] if coins else None, ob_sumsq=stats[obs_dim:2 * obs_dim] if coins else None,
+                    ob_count=stats[2 * obs_dim:] if coins else None, head=head, activation=activation,
+                    act_noise=eng.to_device(np.stack([nz, nz]).reshape(1, 2, -1)), episodes=E,
+                    fall_height=env.fall_height, steps=steps, noise_used=used)
+                h = torch.cat([fit, behv[0].to(f64), steps[0].to(f64), used[0].to(f64), stats]).cpu().numpy()
+                eng.sync()
+                total, pos, t_d, n_used, st = h[0], h[2:5], int(h[5]), int(h[6]), h[7:] / 2
+                rs.randn(n_used)
+                tr = fit_fn.result_from_device(total, pos, t_d)
+                results.append(tr)
+                if coins and st[2 * obs_dim] > 0:
+                    gen_obstat.inc(st[:obs_dim], st[obs_dim:2 * obs_dim], st[2 * obs_dim])
+                total_steps += t_d
+    n_objectives = len(results_pos[0].result)
+    results = _share_results(comm, [tr.result for tr in results_pos], [tr.result for tr in results_neg], inds)
+    gen_obstat.mpi_inc(comm)
+    if comm.size > 1:
+        total_steps = int(sum(dist.world().allgather_object(total_steps)))
+    return results[:, 0:n_objectives], results[:, n_objectives:2 * n_objectives], results[:, -1], total_steps
 
 
 def test_params(comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: ObStat, fit_fn: Callable,

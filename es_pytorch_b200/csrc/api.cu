@@ -421,8 +421,10 @@ static bool es_closed_one_cta_covers(const int* dims, int n_layers) {
 // a closed-loop entry point after ES_ENTER: its checks in order (the cluster plan refuses a shape whatever n_pairs is;
 // rollout_closed.cu checks its own coverage when it runs), the scratch rows of E > 1 episodes, then the kernel; `fn` names it in
 // every message
+// `term`: es_rollout_closedloop_terminal's outputs (NULL for the other entry points)
+struct EsTermArgs { float fall_height; int32_t* steps; int64_t* noise_used; };
 static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* layer_sizes, EsClosedEnv env, EsHead head,
-                         cudaStream_t stream) {
+                         cudaStream_t stream, const EsTermArgs* term = nullptr) {
     int rc = es_rollout_check(fn, env.ob_mean && env.ob_std && env.obs0 && env.env_a && env.env_b, layer_sizes, r);
     if (rc) return rc;
     if (head == ES_HEAD_TANH_ONE_CTA && r.n_layers != 3) {
@@ -442,6 +444,15 @@ static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* la
     }
     if (rc) return rc;
     if (r.n_pairs == 0) return ES_OK;
+    if (term) {
+        // the scratch: the evaluation counter of dynamic scheduling, then the episode rows
+        void* s = nullptr;
+        rc = es_ctx_scratch(ctx, 256 + (r.n_episodes > 1 ? (size_t)2 * ctx->sm_count * r.T * sizeof(double) : 0), &s);
+        if (rc) return rc;
+        if (r.n_episodes > 1) env.ep_rows = (double*)((char*)s + 256);
+        return es_impl_rollout_closedt(ctx, r, env, term->fall_height, term->steps, (long long*)term->noise_used, (unsigned*)s,
+                                       stream);
+    }
     if (r.n_episodes > 1) {
         void* rows = nullptr;
         rc = es_ctx_scratch(ctx, (size_t)2 * ctx->sm_count * r.T * sizeof(double), &rows);
@@ -581,6 +592,36 @@ int es_rollout_closedloop_mlp_activation(es_ctx* ctx, const float* table, int64_
     return es_closedloop(ctx, fn, r, layer_sizes, env, ES_HEAD_ACT, (cudaStream_t)stream);
 }
 
+int es_rollout_closedloop_terminal(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                   const float* theta, int P, float sigma, const int* layer_sizes, int n_layers, const double* ob_mean,
+                                   const double* ob_std, double ob_clip, const float* obs0, const float* env_a, int band,
+                                   const float* env_b, const float* rew_vec, int T, float pos_scale, const uint32_t* coin_words,
+                                   double save_obs_chance, double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos,
+                                   float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins, const float* low,
+                                   const float* range, int activation, float act_param, const float* act_noise, int n_episodes,
+                                   float fall_height, int32_t* steps, int64_t* noise_used, void* stream) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_closedloop_terminal";
+    ES_REQUIRE(isfinite(fall_height) && fall_height > 0.f, "%s: fall_height must be finite and > 0, got %g", fn, (double)fall_height);
+    ES_REQUIRE(steps != nullptr, "%s: NULL steps", fn);
+    ES_REQUIRE(n_episodes >= 1, "%s: n_episodes must be >= 1, got %d", fn, n_episodes);
+    int rc = es_activation_check(fn, activation, act_param);
+    if (rc) return rc;
+    ES_REQUIRE(bins == 0 || (activation == ES_ACT_TANH && act_noise == nullptr),
+               "%s: a binned head is a tanh stack that draws no action noise (FFBinned.forward ignores rs)", fn);
+    // without action noise the episodes are identical: one runs (as es_rollout_closedloop_mlp_episodes)
+    const EsRollout r = {.table = table, .table_len = table_len, .idx = idx, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .activation = activation, .obsn = nullptr, .rew_vec = rew_vec,
+                         .T = T, .pos_scale = pos_scale, .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride,
+                         .behv_pos = behv_pos, .behv_neg = behv_neg, .act_noise = act_noise, .err = ctx->err_dev,
+                         .n_episodes = act_noise ? n_episodes : 1, .bins = bins, .head_low = low, .head_range = range,
+                         .act_param = act_param};
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    const EsTermArgs term = {fall_height, steps, noise_used};
+    return es_closedloop(ctx, fn, r, layer_sizes, env, bins ? ES_HEAD_BINNED : activation == ES_ACT_TANH ? ES_HEAD_TANH : ES_HEAD_ACT,
+                         (cudaStream_t)stream, &term);
+}
+
 int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int activation,
                                               int* cluster_size, int* clusters, int64_t* smem_bytes) {
     ES_ENTER(ctx);
@@ -643,6 +684,16 @@ int es_fitness_objective(es_ctx* ctx, int kind, double* fit, int fit_stride, con
     if (n == 0) return ES_OK;
     ES_REQUIRE(fit && (kind == ES_OBJ_MEAN_REWARD || behv), "es_fitness_objective: NULL pointer");
     return es_impl_fitness_objective(ctx, kind, fit, fit_stride, behv, n, steps, (cudaStream_t)stream);
+}
+
+int es_fitness_objective_steps(es_ctx* ctx, int kind, double* fit, int fit_stride, const float* behv, int n, const int32_t* steps,
+                               void* stream) {
+    ES_ENTER(ctx);
+    if (kind != ES_OBJ_MEAN_REWARD) return es_fitness_objective(ctx, kind, fit, fit_stride, behv, n, 1, stream);
+    ES_REQUIRE(n >= 0 && fit_stride >= 1, "es_fitness_objective_steps: bad sizes");
+    if (n == 0) return ES_OK;
+    ES_REQUIRE(fit && steps, "es_fitness_objective_steps: NULL pointer");
+    return es_impl_mean_reward_steps(ctx, fit, fit_stride, steps, n, (cudaStream_t)stream);
 }
 
 int es_centered_rank(es_ctx* ctx, const double* fpos, const double* fneg, int K, int n_obj, float w0, float w1,

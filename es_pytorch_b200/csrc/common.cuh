@@ -199,6 +199,11 @@ int es_impl_rollout_closedw_act(es_ctx*, const EsRollout&, const EsClosedEnv&, c
 int es_launch_ubase(es_ctx*, const EsRollout&, int n_tiles, float* ubase, cudaStream_t);
 int es_impl_novelty(es_ctx*, const float*, int, const double*, int, int, double*, int, cudaStream_t);
 int es_impl_fitness_objective(es_ctx*, int, double*, int, const float*, int, int, cudaStream_t);
+int es_impl_mean_reward_steps(es_ctx*, double*, int, const int*, int, cudaStream_t);
+// the closed loop on an env whose episodes end when the position falls (rollout_closedt.cu): every shape, head and activation
+// the cluster kernel covers; steps / noise_used [2][n_pairs], `next` a device word the launch zeroes
+int es_impl_rollout_closedt(es_ctx*, const EsRollout&, const EsClosedEnv&, float fall_height, int* steps, long long* noise_used,
+                            unsigned* next, cudaStream_t);
 int es_impl_rank_transform(es_ctx*, const double*, const double*, int, int, int, double, double, int, int, int,
                            const int64_t*, float*, double*, int32_t*, double*, int32_t*, int64_t*, cudaStream_t);
 int es_impl_grad_reconstruct(es_ctx*, const float*, int64_t, const int64_t*, const float*, int, int, float*,

@@ -35,9 +35,23 @@ __global__ void fitness_objective_kernel(int kind, double* __restrict__ fit, int
     }
 }
 
+// ES_OBJ_MEAN_REWARD with every evaluation's own steps (an env whose episodes end early): total / steps[e], the same operations
+__global__ void mean_reward_steps_kernel(double* __restrict__ fit, int fit_stride, const int* __restrict__ steps, int n) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    double* f = fit + (size_t)e * fit_stride;
+    *f = __ddiv_rn(__dadd_rn(0.0, *f), (double)steps[e]);
+}
+
 int es_impl_fitness_objective(es_ctx* ctx, int kind, double* fit, int fit_stride, const float* behv, int n, int steps,
                               cudaStream_t stream) {
     fitness_objective_kernel<<<es_div_up(n, 256), 256, 0, stream>>>(kind, fit, fit_stride, behv, n, (double)steps);
+    ES_LAUNCHED(ctx);
+    return ES_OK;
+}
+
+int es_impl_mean_reward_steps(es_ctx* ctx, double* fit, int fit_stride, const int* steps, int n, cudaStream_t stream) {
+    mean_reward_steps_kernel<<<es_div_up(n, 256), 256, 0, stream>>>(fit, fit_stride, steps, n);
     ES_LAUNCHED(ctx);
     return ES_OK;
 }

@@ -423,6 +423,53 @@ class Engine:
         check(self.lib.es_rollout_closedloop_mlp_episodes(*args, _ptr(act_noise), episodes, self.stream),
               'es_rollout_closedloop_mlp' if plain else 'es_rollout_closedloop_mlp_episodes')
 
+    def rollout_closed_terminal(self, table, idx, theta, sigma: float, layer_sizes: Sequence[int], ob_mean, ob_std,
+                                ob_clip: float, obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos, fit_neg,
+                                fit_stride: int = 1, behv_pos=None, behv_neg=None, coin_words=None, save_obs_chance: float = 0.0,
+                                ob_sum=None, ob_sumsq=None, ob_count=None, head=None, act_noise=None, episodes: int = 1,
+                                activation=None, fall_height: float = None, steps=None, noise_used=None):
+        """``rollout_closed_mlp`` (same arguments and checks) on an env whose episodes end when the position falls
+        (``ClosedLoopEnv(fall_height=h)``, es_rollout_closedloop_terminal): every evaluation stops at the step t_d whose
+        position leaves |z| <= h (or at T - 1).  ``steps`` int32 [2, n] (+ then -) receives the last episode's t_d,
+        ``noise_used`` (int64 [2, n] or None) the action-noise values each evaluation consumed; episode e reads its noise from
+        where episode e - 1 stopped.  Returns (steps, noise_used)."""
+        binned = head is not None and head != 'tanh'
+        if binned and activation is not None:
+            raise ValueError('a binned head is a tanh stack: activation must be None')
+        if binned and act_noise is not None:
+            raise ValueError('a binned head draws no action noise (FFBinned.forward ignores rs): act_noise must be None')
+        if fall_height is None:
+            raise ValueError('rollout_closed_terminal needs a fall_height')
+        episodes = int(episodes)
+        if episodes < 1:
+            raise ValueError(f'episodes must be >= 1, got {episodes}')
+        n, ls = self._check_rollout(table, idx, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg)
+        act = head.adim if binned else int(layer_sizes[-1])
+        T, band = self._check_closed_env(n, layer_sizes, act, ob_mean, ob_std, obs0, env_a, env_b, rew_vec, coin_words, ob_sum,
+                                         ob_sumsq, ob_count)
+        if act_noise is not None:
+            _req(act_noise, torch.float32, 'act_noise', self.device)
+            assert act_noise.numel() == n * 2 * episodes * T * act
+        if steps is None:
+            steps = self.empty((2, n), torch.int32)
+        _req(steps, torch.int32, 'steps', self.device)
+        assert steps.numel() == 2 * n
+        if noise_used is not None:
+            _req(noise_used, torch.int64, 'noise_used', self.device)
+            assert noise_used.numel() == 2 * n
+        low = rng = None
+        if binned:
+            low, rng = self._head_arrays(head)
+        kind, param = (_lib.ES_ACT_TANH, 0.0) if activation is None else (int(activation.kind), float(activation.param))
+        check(self.lib.es_rollout_closedloop_terminal(
+            self._ctx, _ptr(table), table.numel(), _ptr(idx), n, _ptr(theta), theta.numel(), float(sigma), ls, len(layer_sizes) - 1,
+            _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b), _ptr(rew_vec), T,
+            float(pos_scale), _ptr(coin_words), float(save_obs_chance), _ptr(fit_pos), _ptr(fit_neg), int(fit_stride),
+            _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), int(head.bins) if binned else 0,
+            _ptr(low), _ptr(rng), kind, param, _ptr(act_noise), episodes, float(fall_height), _ptr(steps), _ptr(noise_used),
+            self.stream), 'es_rollout_closedloop_terminal')
+        return steps, noise_used
+
     def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int, head=None, activation=None):
         """How ``rollout_closed_mlp`` runs a shape: (CTAs per cluster, clusters resident at once, shared memory bytes per CTA);
         (0, SM count, 0) for ``rollout_closed``'s one-CTA kernel.  Raises EsLibraryError for a shape it does not cover.
@@ -457,13 +504,22 @@ class Engine:
     def fitness_objective(self, kind: int, fit, fit_stride: int, behv, n: int, steps: int):
         """Column 0 of ``n`` evaluations' fitness rows (element e * fit_stride of ``fit``), rewritten in place from the episode
         total there and the final position ``behv`` [n][3] as ES_OBJ_MEAN_REWARD / ES_OBJ_DIST / ES_OBJ_XDIST
-        (MeanRewardResult / DistResult / XDistResult, training_result.py:67-79).  ``behv`` may be None for the mean reward."""
+        (MeanRewardResult / DistResult / XDistResult, training_result.py:67-79).  ``behv`` may be None for the mean reward.
+        ``steps``: an int (every evaluation's), or an int32 tensor of each evaluation's own (es_fitness_objective_steps: an
+        env whose episodes end early)."""
         d = self.device
         _req(fit, torch.float64, 'fit', d)
         assert n == 0 or fit.numel() >= (n - 1) * fit_stride + 1
         if behv is not None:
             _req(behv, torch.float32, 'behv', d)
             assert behv.numel() >= 3 * n
+        if isinstance(steps, torch.Tensor):
+            # every evaluation's own steps (an env whose episodes end early): es_fitness_objective_steps
+            _req(steps, torch.int32, 'steps', d)
+            assert steps.numel() >= n
+            check(self.lib.es_fitness_objective_steps(self._ctx, int(kind), _ptr(fit), int(fit_stride), _ptr(behv), int(n),
+                                                      _ptr(steps), self.stream), 'es_fitness_objective_steps')
+            return
         check(self.lib.es_fitness_objective(self._ctx, int(kind), _ptr(fit), int(fit_stride), _ptr(behv), int(n), int(steps),
                                             self.stream), 'es_fitness_objective')
 

@@ -80,7 +80,7 @@ class DeviceGeneration:
                  save_obs_chance: float = 0.0, archive: Optional[torch.Tensor] = None, nov_k: int = 10,
                  moo_w: float = 1.0, rollout_mode: int = ES_ROLLOUT_F32, comm: Optional[dist.Comm] = None,
                  engine: Optional[Engine] = None, ranker=None, ac_std: float = 0.0, closed=None, episodes: int = 1, head=None,
-                 closed_act_noise: bool = False, objective: str = 'reward', activation=None):
+                 closed_act_noise: bool = False, objective: str = 'reward', activation=None, fall_height=None):
         self.eng = engine or get_engine()
         if objective not in OBJECTIVES:
             raise ValueError(f'objective must be one of {OBJECTIVES}, got {objective!r}')
@@ -97,6 +97,12 @@ class DeviceGeneration:
         # evaluate() refuses it otherwise
         self.closed = closed
         self.closed_act_noise = bool(closed_act_noise)
+        # a closed-loop env whose episodes end when the position falls (ClosedLoopEnv(fall_height=h)): the rollout is
+        # es_rollout_closedloop_terminal, every evaluation's t_d lands in steps_dev and the generation's sum of them in
+        # steps_total (shared with the obs statistics)
+        if fall_height is not None and closed is None:
+            raise ValueError('fall_height is the closed-loop env\'s: pass closed= too')
+        self.fall_height = None if fall_height is None else float(fall_height)
         self.ranker = ranker                            # a utils.rankers.Ranker; None = Centered / MultiObjective(moo_w)
         e = self.eng
         self.comm = comm or dist.world()
@@ -189,14 +195,17 @@ class DeviceGeneration:
         # signs and the noise index as float64, es.py:89-91) plus the generation's obs statistics (ObStat.mpi_inc, es.py:77)
         # -- so that one allgather serves the ranks, the indices and the statistics:
         #   [fitness [pos|neg][k][obj] | idx [k] | obs sum, sumsq, count, n_saved]
-        nf, ns = 2 * self.k_local * self.n_obj, 2 * self.obs_dim + 2
+        #   (+ the sum of the evaluations' steps on an env whose episodes end early)
+        nf, ns = 2 * self.k_local * self.n_obj, 2 * self.obs_dim + 2 + (self.fall_height is not None)
         self.share_local = torch.zeros(nf + self.k_local + ns, dtype=f64, device=e.device)
         self.fit_local = self.share_local[:nf].view(2, self.k_local, self.n_obj)
         self.idx_f64 = self.share_local[nf:nf + self.k_local]
         self._gen_stats = self.share_local[nf + self.k_local:]
         self.gen_sum = self._gen_stats[:self.obs_dim]
         self.gen_sumsq = self._gen_stats[self.obs_dim:2 * self.obs_dim]
-        self.gen_count = self._gen_stats[2 * self.obs_dim:]
+        self.gen_count = self._gen_stats[2 * self.obs_dim:2 * self.obs_dim + 2]
+        self.steps_dev = e.empty((2, self.k_local), torch.int32) if self.fall_height is not None else None
+        self.steps_total = self._gen_stats[2 * self.obs_dim + 2:] if self.fall_height is not None else None
         G = self.comm.size
         self.share_all = e.empty((G, nf + self.k_local + ns), f64) if G > 1 else None
         self.fit_all = self.share_all[:, :nf].view(G, 2, self.k_local, self.n_obj) if G > 1 else None
@@ -248,16 +257,33 @@ class DeviceGeneration:
             noisy = self.ac_std != 0.0
             self._gen_stats.zero_()
             obs0, env_a, env_b = self.closed
-            with self._timed('rollout'):
-                e.rollout_closed_mlp(self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.ob_mean, self.ob_std,
-                                     self.ob_clip, obs0, env_a, env_b, self.rew_vec, self.pos_scale, fp, fn, self.n_obj,
-                                     None if self.behv is None else self.behv[0], None if self.behv is None else self.behv[1],
-                                     coin_words=self.extras if self.extra_words else None, save_obs_chance=self.save_obs_chance,
-                                     ob_sum=self.gen_sum if self.extra_words else None,
-                                     ob_sumsq=self.gen_sumsq if self.extra_words else None,
-                                     ob_count=self.gen_count if self.extra_words else None, head=self.head,
-                                     act_noise=self.act_noise if noisy else None, episodes=self.episodes if noisy else 1,
-                                     activation=self.activation)
+            if self.fall_height is not None:
+                if noisy:
+                    raise NotImplementedError('action noise on an env whose episodes end early cannot be drawn ahead: how many '
+                                              'gaussians an evaluation consumes is known when it has fallen (es.step and '
+                                              'es.test_params run such generations one evaluation at a time)')
+                with self._timed('rollout'):
+                    e.rollout_closed_terminal(
+                        self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,
+                        obs0, env_a, env_b, self.rew_vec, self.pos_scale, fp, fn, self.n_obj,
+                        None if self.behv is None else self.behv[0], None if self.behv is None else self.behv[1],
+                        coin_words=self.extras if self.extra_words else None, save_obs_chance=self.save_obs_chance,
+                        ob_sum=self.gen_sum if self.extra_words else None, ob_sumsq=self.gen_sumsq if self.extra_words else None,
+                        ob_count=self.gen_count if self.extra_words else None, head=self.head, activation=self.activation,
+                        fall_height=self.fall_height, steps=self.steps_dev)
+                self.steps_total.copy_(self.steps_dev.sum(dtype=torch.float64).view(1))
+            else:
+                with self._timed('rollout'):
+                    e.rollout_closed_mlp(self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.ob_mean, self.ob_std,
+                                         self.ob_clip, obs0, env_a, env_b, self.rew_vec, self.pos_scale, fp, fn, self.n_obj,
+                                         None if self.behv is None else self.behv[0], None if self.behv is None else self.behv[1],
+                                         coin_words=self.extras if self.extra_words else None,
+                                         save_obs_chance=self.save_obs_chance,
+                                         ob_sum=self.gen_sum if self.extra_words else None,
+                                         ob_sumsq=self.gen_sumsq if self.extra_words else None,
+                                         ob_count=self.gen_count if self.extra_words else None, head=self.head,
+                                         act_noise=self.act_noise if noisy else None, episodes=self.episodes if noisy else 1,
+                                         activation=self.activation)
             self._score()
         else:
             self._evaluate_openloop(fp, fn)
@@ -307,8 +333,10 @@ class DeviceGeneration:
         elif self.objective == 'novelty':
             e.novelty(self.behv.view(-1, 3), self.archive, self.nov_k, fit, 1)
         elif self.objective != 'reward':
-            # steps = T - 1: the last loop index run_model returns (gym_runner.py:50,67)
-            e.fitness_objective(_OBJ_KINDS[self.objective], fit, 1, self.behv, 2 * self.k_local, self.T - 1)
+            # steps = T - 1: the last loop index run_model returns (gym_runner.py:50,67); each evaluation's t_d when its
+            # episode can end early
+            steps = self.T - 1 if self.steps_dev is None else self.steps_dev.view(-1)
+            e.fitness_objective(_OBJ_KINDS[self.objective], fit, 1, self.behv, 2 * self.k_local, steps)
 
     def _alloc_act_noise(self, nrm: int) -> torch.Tensor:
         """The [k_local, 2, episodes * T * act] float32 buffer of the generation's action noise."""
@@ -356,6 +384,16 @@ class DeviceGeneration:
                              torch.zeros(2, 3, dtype=torch.float32, device=e.device),
                              torch.zeros(1, dtype=torch.int64, device=e.device))
         fit0, behv0, idx0 = self._nl_bufs
+        if self.closed is not None and self.fall_height is not None:
+            # the evaluation's t_d in nl_steps[0, 0]
+            if getattr(self, 'nl_steps', None) is None:
+                self.nl_steps = torch.zeros(2, 1, dtype=torch.int32, device=e.device)
+            obs0, env_a, env_b = self.closed
+            e.rollout_closed_terminal(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,
+                                      obs0, env_a, env_b, self.rew_vec, self.pos_scale, fit0[0:1], fit0[1:2], 1, behv0[0].view(-1),
+                                      behv0[1].view(-1), head=self.head, activation=self.activation,
+                                      fall_height=self.fall_height, steps=self.nl_steps)
+            return fit0, behv0
         if self.closed is not None:
             obs0, env_a, env_b = self.closed
             e.rollout_closed_mlp(self.table, idx0, self.theta, 0.0, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,

@@ -88,13 +88,21 @@ class BatchedRollout:
             return self.result(rews, behv[-3:], obs, steps, self.archive, self.nov_k)
         return self.result(rews, behv, obs, steps)
 
-    def result_from_device(self, total: float, pos) -> TrainingResult:
-        """The TrainingResult ``__call__`` would build, from an episode total and final position computed on the device."""
+    def result_from_device(self, total: float, pos, steps: Optional[int] = None) -> TrainingResult:
+        """The TrainingResult ``__call__`` would build, from an episode total and final position computed on the device.
+        ``steps``: the step t_d at which the episode ended on an env whose episodes end early; None, the episode ran
+        ``max_steps`` steps."""
         rews = [float(total)]
         behv = [float(pos[0]), float(pos[1]), float(pos[2])] * int(self.max_steps)
         no_obs = np.array([np.zeros(self.env.observation_space.shape)])
-        steps = self.max_steps - 1                              # run_model returns the last loop index (gym_runner.py:50,67)
-        return self._result(rews, behv, no_obs, steps)
+        if steps is None:
+            steps = self.max_steps - 1                          # run_model returns the last loop index (gym_runner.py:50,67)
+        return self._result(rews, behv, no_obs, int(steps))
+
+    @property
+    def terminates(self) -> bool:
+        """Whether the env's episodes can end before ``max_steps`` (``ClosedLoopEnv(fall_height=h)``)."""
+        return bool(getattr(self.env, 'is_synthetic_closedloop', False) and getattr(self.env, 'terminates', False))
 
     def __call__(self, model, use_ac_noise=True) -> TrainingResult:
         """Single-policy evaluation with the reference's fit_fn contract.  Like the scripts' fit_fn (simple_example.py:38,
@@ -117,8 +125,8 @@ class BatchedRollout:
                                  or self._closed_on_device(model.layer_sizes(), head, activation)):
             # the evaluation, all its episodes, as one launch (the observations are not returned: this result never carries them)
             from .gym_runner import _device_episode
-            total, pos, _ = _device_episode(model, self.env, self.max_steps, noise_rs if noisy else None, episodes, activation)
-            return self.result_from_device(total, pos)
+            total, pos, ran = _device_episode(model, self.env, self.max_steps, noise_rs if noisy else None, episodes, activation)
+            return self.result_from_device(total, pos, ran - 1 if self.terminates else None)
         if episodes > 1:
             rews, behv, steps = self._run_episodes(model, noise_rs, episodes)
         else:
@@ -138,9 +146,11 @@ class BatchedRollout:
         """Whether a closed-loop episode of a tanh MLP runs as one launch (es_rollout_closedloop_mlp): two hidden layers always
         do (a shape outside the kernels' coverage raises there); three or four when the kernels cover the shape; anything else
         runs run_model's python loop.  A binned head (es_rollout_closedloop_mlp_binned) runs as one launch when the cluster
-        kernel covers the shape, and so does a policy with another activation (es_rollout_closedloop_mlp_activation)."""
+        kernel covers the shape, and so does a policy with another activation (es_rollout_closedloop_mlp_activation).  On an env
+        whose episodes end early every policy runs the cluster kernel (es_rollout_closedloop_terminal) when it covers the
+        shape."""
         n_hidden = len(sizes) - 2
-        if n_hidden == 2 and head == 'tanh' and activation is None:
+        if n_hidden == 2 and head == 'tanh' and activation is None and not self.terminates:
             return True
         if n_hidden not in (2, 3, 4):
             return False

@@ -39,7 +39,10 @@ def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1, acti
     """One evaluation on the open- or closed-loop synthetic env as one launch (sigma = 0).  With ``rs`` and a tanh model's
     ac_std != 0: the action noise of ``episodes`` episodes drawn back to back from ``rs``, the per-step mean over the episodes
     (obj.py:54-63).  ``activation``: the model's ``nn.Activation`` when it is not a tanh one (its outputs are the actions, as
-    a tanh model's).  Returns (fitness, the last episode's final position, steps)."""
+    a tanh model's).  Returns (fitness, the last episode's final position, steps), steps the number of steps the last episode
+    ran: T, or t_d + 1 on a closed-loop env whose episode ended at step t_d (``ClosedLoopEnv(fall_height=h)``).  There the
+    noise of ``episodes`` x T steps is drawn from a copy of ``rs``, and ``rs`` then advances by exactly the gaussians the
+    executed steps consumed, as the reference's per-step ``rs.randn(act)`` calls leave it."""
     from ..engine import get_engine
     from ..core.policy import Policy
     eng = get_engine()
@@ -55,16 +58,32 @@ def _device_episode(model, env, max_steps: int, rs=None, episodes: int = 1, acti
     behv = torch.zeros(2, 3, dtype=torch.float32, device=eng.device)
     noise = None
     ac_std = float(getattr(model, '_action_std', 0) or 0)
+    closed = getattr(env, 'is_synthetic_closedloop', False)
+    term = closed and getattr(env, 'terminates', False)
     if rs is not None and ac_std != 0 and head == 'tanh':
         # nn.py:47-48: T calls of rs.randn(act) * ac_std per episode; one call of rs.randn(episodes * T * act) consumes the stream
         # identically (legacy gaussians are produced one by one, cached second value included; neither env's noise depends on
         # its state).  [pair 0][+ | -][episodes][T][act]: both evaluations of the sigma = 0 "pair" see it, only + is used.
-        nz = (rs.randn(episodes * T * sizes[-1]) * ac_std).astype(np.float32)
+        src = rs
+        if term:                                        # how many are consumed is known after the rollout
+            src = np.random.RandomState()
+            src.set_state(rs.get_state())
+        nz = (src.randn(episodes * T * sizes[-1]) * ac_std).astype(np.float32)
         noise = eng.to_device(np.stack([nz, nz]).reshape(1, 2, -1))
     else:
         episodes = 1
     out = (fit[0:1], fit[1:2], 1, behv[0:1].view(-1), behv[1:2].view(-1))
-    if getattr(env, 'is_synthetic_closedloop', False):
+    if term:
+        steps, used = eng.rollout_closed_terminal(
+            table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), *env.device_closed(eng), rew_dev[:T].contiguous(),
+            env.pos_scale, *out, head=head, act_noise=noise, episodes=episodes, activation=activation,
+            fall_height=env.fall_height, steps=torch.zeros(2, 1, dtype=torch.int32, device=eng.device),
+            noise_used=torch.zeros(2, 1, dtype=torch.int64, device=eng.device))
+        t_d, n_used = int(steps[0, 0].item()), int(used[0, 0].item())
+        if noise is not None:
+            rs.randn(n_used)
+        return float(fit[0].item()), behv[0].cpu().numpy().astype(np.float64), t_d + 1
+    if closed:
         eng.rollout_closed_mlp(table, idx, theta, 0.0, sizes, mean, std, float(model.ob_clip), *env.device_closed(eng),
                                rew_dev[:T].contiguous(), env.pos_scale, *out, head=head, act_noise=noise, episodes=episodes,
                                activation=activation)

@@ -9,7 +9,7 @@ used by the per-perturbation compatibility path of ``gym_runner.run_model``) and
 """
 from __future__ import annotations
 
-from typing import Tuple
+from typing import Optional, Tuple
 
 import numpy as np
 
@@ -142,12 +142,27 @@ class ClosedLoopEnv(SyntheticEnv):
     headline): ``obs_{t+1} = tanh(A obs_t + B a_t)`` -- what the policy sees depends on what it did, so the episode cannot
     be batched over time.  A is banded with wrap-around (``band`` diagonals centred on the main one, gain ``a_gain`` keeps
     the map contractive), B dense; obs_0 is row 0 of the open-loop stream; reward and position as in the open-loop env.
-    float32 throughout, pre-activation accumulated in index order (A's diagonals, then B's columns)."""
+    float32 throughout, pre-activation accumulated in index order (A's diagonals, then B's columns).
+
+    ``fall_height``: None (the default), every episode runs ``max_episode_steps`` steps.  A float h > 0: the episode also ends
+    (``step`` returns ``done``) at the first step after which the third position component leaves [-h, h], evaluated in
+    float32 after that step's position update -- a torso height that drifts out of its healthy range, as the pybullet Hopper
+    and Ant envs end an episode when the robot falls.  A NaN position ends the episode too."""
     is_synthetic_openloop = False
     is_synthetic_closedloop = True
 
     def __init__(self, obs_dim: int, act_dim: int, max_episode_steps: int = 1000, band: int = 8, a_seed: int = 17,
-                 b_seed: int = 19, a_gain: float = 0.5, b_gain: float = 0.5, name: str = 'SyntheticClosedLoop-v0', **kwargs):
+                 b_seed: int = 19, a_gain: float = 0.5, b_gain: float = 0.5, name: str = 'SyntheticClosedLoop-v0',
+                 fall_height: Optional[float] = None, **kwargs):
+        if fall_height is not None:
+            if isinstance(fall_height, bool) or not isinstance(fall_height, (int, float, np.integer, np.floating)):
+                raise TypeError(f'fall_height must be a number or None, got {fall_height!r}')
+            with np.errstate(over='ignore'):
+                h = np.float32(fall_height)
+            if not (np.isfinite(h) and h > 0):
+                raise ValueError(f'fall_height must be finite and > 0 as a float32, got {fall_height!r}')
+            fall_height = h
+        self.fall_height = fall_height
         super().__init__(obs_dim, act_dim, max_episode_steps, name=name, **kwargs)
         self.band = int(band)
         self.env_a = (np.random.RandomState(a_seed).randn(self.obs_dim, self.band) * (a_gain / np.sqrt(self.band))).astype(np.float32)
@@ -170,7 +185,14 @@ class ClosedLoopEnv(SyntheticEnv):
         for j in range(self.act_dim):
             acc = (acc + (self.env_b[:, j] * a[j]).astype(f32)).astype(f32)
         self.ob = np.tanh(acc).astype(f32)
+        if self.fall_height is not None:
+            done = bool(done or not (abs(self.pos[2]) <= self.fall_height))      # float32 |z| against float32 h; NaN falls
         return self.ob.copy(), rew, done, info
+
+    @property
+    def terminates(self) -> bool:
+        """Whether an episode can end before ``max_episode_steps`` (a ``fall_height`` is set)."""
+        return self.fall_height is not None
 
     def device_closed(self, engine):
         """(obs_0 [obs], A transposed [band][obs], B transposed [act][obs]) as float32 tensors in HBM."""

@@ -290,6 +290,32 @@ int es_rollout_closedloop_mlp_activation(es_ctx* ctx, const float* table, int64_
 int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int activation,
                                               int* cluster_size, int* clusters, int64_t* smem_bytes);
 
+/* The closed loop on an env whose episodes end early (ClosedLoopEnv(fall_height=h)): run_model's `if done: break`
+ * (src/gym/gym_runner.py:50-67) inside obj.py:54-63's episode loop, for every policy the cluster kernel covers.  Step t returns
+ * done when t = T - 1 or !(|z_t| <= fall_height), z_t the third position component after step t's float32 update (a NaN
+ * falls); fall_height must be finite and > 0.  One call for every head: bins == 0 with `activation` (ES_ACT_*, act_param as
+ * es_rollout_openloop_activation) is a plain MLP whose outputs are the actions; bins >= 2 a binned head as
+ * es_rollout_closedloop_mlp_binned (activation ES_ACT_TANH, no action noise).  act_noise / n_episodes as
+ * es_rollout_closedloop_mlp_episodes, except that episode e reads its gaussians from where episode e - 1 stopped (the reference
+ * draws rs.randn(act) only for the steps it executes): the buffer holds E T act values per evaluation, of which the first
+ * sum_e (t_{d,e} + 1) act are read.  Every shape es_rollout_closedloop_mlp covers runs rollout_closedt.cu, the cluster kernel's
+ * code (a cluster of one CTA included); clusters take evaluations from a device counter, so early falls free them for others.
+ * Per evaluation, everything stops at the step t_d that returned done:
+ *   fitness      sum_t (sum_e r_{e,t}) / E to the longest episode's end (obj.py: rews[:len(rew)] += rew; rews /= E)
+ *   behv         the last episode's final position
+ *   ObStat       the last episode's t_d + 1 post-step rows; ob_count[0] += t_d + 1 per saved evaluation (es.py:73-74)
+ *   steps        dev int32 [2][n_pairs] (+ then -): the last episode's t_d (T - 1 if nothing fell), run_model's `step`
+ *   noise_used   dev int64 [2][n_pairs] or NULL: the action-noise values the evaluation consumed, sum_e (t_{d,e} + 1) act  */
+int es_rollout_closedloop_terminal(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
+                                   const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
+                                   const double* ob_mean, const double* ob_std, double ob_clip, const float* obs0,
+                                   const float* env_a, int band, const float* env_b, const float* rew_vec, int T, float pos_scale,
+                                   const uint32_t* coin_words, double save_obs_chance, double* fit_pos, double* fit_neg,
+                                   int fit_stride, float* behv_pos, float* behv_neg, double* ob_sum, double* ob_sumsq,
+                                   double* ob_count, int bins, const float* low, const float* range, int activation,
+                                   float act_param, const float* act_noise, int n_episodes, float fall_height, int32_t* steps,
+                                   int64_t* noise_used, void* stream);
+
 /* ---- a2 + a4 with action noise: all draws of a generation in stream order ---------------------------------------------
  * When FeedForward._action_std != 0 every step of every rollout draws rs.randn(act_dim) from the SAME RandomState that
  * draws the noise indices and the save_obs coins (src/nn/nn.py:47-48, src/core/es.py:66-72, simple_example.py:37-40).  Per
@@ -348,6 +374,11 @@ int es_novelty(es_ctx* ctx, const float* behv, int n, const double* archive, int
 enum { ES_OBJ_MEAN_REWARD = 1, ES_OBJ_DIST = 2, ES_OBJ_XDIST = 3 };
 int es_fitness_objective(es_ctx* ctx, int kind, double* fit, int fit_stride, const float* behv, int n, int steps,
                          void* stream);
+/* es_fitness_objective with every evaluation's own steps (dev int32 [n], es_rollout_closedloop_terminal's): MEAN_REWARD is
+ * fit[e * fit_stride] / steps[e] with the same operations; DIST and XDIST ignore steps.  A steps[e] of 0 divides by zero on
+ * the device (inf or NaN): the caller raises ZeroDivisionError first, as MeanRewardResult does.                        */
+int es_fitness_objective_steps(es_ctx* ctx, int kind, double* fit, int fit_stride, const float* behv, int n, const int32_t* steps,
+                               void* stream);
 
 /* ---- a8/a9: centered rank -> antithetic weights -------------------------------------------
  * Replaces Ranker.rank with CenteredRanker (src/utils/rankers.py:9-17,37-58) and, for
