@@ -419,12 +419,10 @@ static bool es_closed_one_cta_covers(const int* dims, int n_layers) {
 }
 
 // a closed-loop entry point after ES_ENTER: its checks in order (the cluster plan refuses a shape whatever n_pairs is;
-// rollout_closed.cu checks its own coverage when it runs), the scratch rows of E > 1 episodes, then the kernel; `fn` names it in
-// every message
-// `term`: es_rollout_closedloop_terminal's outputs (NULL for the other entry points)
-struct EsTermArgs { float fall_height; int32_t* steps; int64_t* noise_used; };
+// rollout_closed.cu checks its own coverage when it runs), the scratch, then the kernel; `fn` names it in every message.
+// `term`: es_rollout_closedloop_terminal's early end (steps NULL for the other entry points), always on the cluster kernel
 static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* layer_sizes, EsClosedEnv env, EsHead head,
-                         cudaStream_t stream, const EsTermArgs* term = nullptr) {
+                         cudaStream_t stream, const EsTerm& term = EsTerm{}) {
     int rc = es_rollout_check(fn, env.ob_mean && env.ob_std && env.obs0 && env.env_a && env.env_b, layer_sizes, r);
     if (rc) return rc;
     if (head == ES_HEAD_TANH_ONE_CTA && r.n_layers != 3) {
@@ -444,25 +442,14 @@ static int es_closedloop(es_ctx* ctx, const char* fn, EsRollout r, const int* la
     }
     if (rc) return rc;
     if (r.n_pairs == 0) return ES_OK;
-    if (term) {
-        // the scratch: the evaluation counter of dynamic scheduling, then the episode rows
-        void* s = nullptr;
-        rc = es_ctx_scratch(ctx, 256 + (r.n_episodes > 1 ? (size_t)2 * ctx->sm_count * r.T * sizeof(double) : 0), &s);
-        if (rc) return rc;
-        if (r.n_episodes > 1) env.ep_rows = (double*)((char*)s + 256);
-        return es_impl_rollout_closedt(ctx, r, env, term->fall_height, term->steps, (long long*)term->noise_used, (unsigned*)s,
-                                       stream);
-    }
-    if (r.n_episodes > 1) {
-        void* rows = nullptr;
-        rc = es_ctx_scratch(ctx, (size_t)2 * ctx->sm_count * r.T * sizeof(double), &rows);
-        if (rc) return rc;
-        env.ep_rows = (double*)rows;
-    }
-    if (head == ES_HEAD_ACT) return es_impl_rollout_closedw_act(ctx, r, env, stream);
-    if (head == ES_HEAD_TANH_ONE_CTA || (head == ES_HEAD_TANH && es_closed_one_cta_covers(r.dims, r.n_layers)))
+    // the scratch: the cluster kernel's evaluation counter (dynamic scheduling), then the per-step rows of E > 1 episodes
+    void* s = nullptr;
+    rc = es_ctx_scratch(ctx, 256 + (r.n_episodes > 1 ? (size_t)2 * ctx->sm_count * r.T * sizeof(double) : 0), &s);
+    if (rc) return rc;
+    if (r.n_episodes > 1) env.ep_rows = (double*)((char*)s + 256);
+    if (!term.steps && (head == ES_HEAD_TANH_ONE_CTA || (head == ES_HEAD_TANH && es_closed_one_cta_covers(r.dims, r.n_layers))))
         return es_impl_rollout_closed(ctx, r, env, stream);
-    return es_impl_rollout_closedw(ctx, r, env, stream);
+    return es_impl_rollout_closedw(ctx, r, env, term, (unsigned*)s, stream);
 }
 
 int es_rollout_closedloop(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs, const float* theta,
@@ -499,8 +486,7 @@ static int es_closedloop_plan(es_ctx* ctx, const char* fn, const int* layer_size
         return ES_OK;
     }
     *cluster_size = C; *smem_bytes = (int64_t)smem;
-    return head == ES_HEAD_ACT ? es_closedw_act_max_clusters(n_layers, C, smem, clusters)
-                               : es_closedw_max_clusters(n_layers, bins, C, smem, clusters);
+    return es_closedw_max_clusters(n_layers, bins, head == ES_HEAD_ACT, C, smem, clusters);
 }
 
 int es_rollout_closedloop_mlp_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int* cluster_size, int* clusters,
@@ -617,9 +603,9 @@ int es_rollout_closedloop_terminal(es_ctx* ctx, const float* table, int64_t tabl
                          .n_episodes = act_noise ? n_episodes : 1, .bins = bins, .head_low = low, .head_range = range,
                          .act_param = act_param};
     const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, coin_words, save_obs_chance, ob_sum, ob_sumsq, ob_count};
-    const EsTermArgs term = {fall_height, steps, noise_used};
+    const EsTerm term = {fall_height, steps, noise_used};
     return es_closedloop(ctx, fn, r, layer_sizes, env, bins ? ES_HEAD_BINNED : activation == ES_ACT_TANH ? ES_HEAD_TANH : ES_HEAD_ACT,
-                         (cudaStream_t)stream, &term);
+                         (cudaStream_t)stream, term);
 }
 
 int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int activation,

@@ -154,6 +154,15 @@ struct EsClosedEnv {
     double* ep_rows;
 };
 
+// an env whose episodes end early (es_rollout_closedloop_terminal), uniform over the launch.  Every other closed-loop call
+// passes steps == NULL: its episodes run T steps whatever the position (a NaN included; fall_height = inf would not do that,
+// since !(|NaN| <= inf))
+struct EsTerm {
+    float fall_height;          // h > 0: an episode ends after the step whose position leaves |z| <= h (or at T - 1)
+    int32_t* steps;             // [2][n_pairs] (+ then -): the last episode's t_d
+    int64_t* noise_used;        // [2][n_pairs] action-noise values the evaluation consumed (sum_e (t_{d,e} + 1) act), or NULL
+};
+
 // ---- entry points implemented one per .cu file (called from api.cu) -------------------------
 int es_impl_draw_indices(es_ctx*, uint32_t*, int32_t*, int, int, uint64_t, int, int64_t*, uint32_t*, cudaStream_t);
 int es_impl_mt_skip(es_ctx*, uint32_t*, int32_t*, int, int, cudaStream_t);
@@ -179,31 +188,25 @@ int es_impl_rollout_tcw(es_ctx*, const EsRollout&, int split, cudaStream_t);
 // adim * bins <= 256
 bool es_tcw_covers_binned(const EsRollout&);
 int es_impl_rollout_closed(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
-// the closed loop for tanh MLPs with 2 to 4 hidden layers of <= 256 units, obs <= 384, act <= 64, an even band <= 16, on a
-// thread-block cluster per evaluation (rollout_closedw.cu): the cluster size and shared memory per CTA of a shape (or
-// ES_ERR_UNSUPPORTED with the limit in es_last_error()), the clusters resident at once (bins: 0 for a tanh head, else the
-// binned head's), and the rollout
+// the closed loop for MLPs with 2 to 4 hidden layers of <= 256 units, obs <= 384, act <= 64, an even band <= 16, on a
+// thread-block cluster per evaluation (rollout_closedw.cu): tanh, binned heads (EsRollout::bins >= 2: every shape
+// es_closedw_plan covers with act = adim) and the other activations, with or without action noise and an early end.  The
+// cluster size and shared memory per CTA of a shape (or ES_ERR_UNSUPPORTED with the limit in es_last_error()), the clusters
+// resident at once (bins: 0, or the binned head's; act: an activation other than tanh), and the rollout (`next`: a device
+// word the launch zeroes)
 int es_closedw_plan(const int* layer_sizes, int n_layers, int band, int* cluster_size, size_t* smem_bytes);
-int es_closedw_max_clusters(int n_layers, int bins, int cluster_size, size_t smem_bytes, int* clusters);
-int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
-// binned heads (EsRollout::bins >= 2): every shape es_closedw_plan covers with act = adim; the cluster kernel at every C
 int es_closedw_binned_plan(const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes);
-// policies with an activation other than tanh (EsRollout::activation != ES_ACT_TANH): on ES_ROLLOUT_TC3 the shapes of
-// es_tcw_covers_act, rollout_tcw.cu's code (rollout_tcw_act.cu); in the closed loop every shape es_closedw_plan covers, on the
-// cluster kernel's code at every C (rollout_closedw_act.cu), and its resident clusters
+int es_closedw_max_clusters(int n_layers, int bins, bool act, int cluster_size, size_t smem_bytes, int* clusters);
+int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, const EsTerm&, unsigned* next, cudaStream_t);
+// policies with an activation other than tanh (EsRollout::activation != ES_ACT_TANH) on ES_ROLLOUT_TC3: the shapes of
+// es_tcw_covers_act, rollout_tcw.cu's code (rollout_tcw_act.cu)
 bool es_tcw_covers_act(const EsRollout&);
 int es_impl_rollout_tcw_act(es_ctx*, const EsRollout&, cudaStream_t);
-int es_closedw_act_max_clusters(int n_layers, int cluster_size, size_t smem_bytes, int* clusters);
-int es_impl_rollout_closedw_act(es_ctx*, const EsRollout&, const EsClosedEnv&, cudaStream_t);
 // U = Xn . theta1^T + b1 of an obs-64-... MLP for the pair kernels (rollout_tc2.cu): row-major [n_tiles * 128][64], 0 beyond T
 int es_launch_ubase(es_ctx*, const EsRollout&, int n_tiles, float* ubase, cudaStream_t);
 int es_impl_novelty(es_ctx*, const float*, int, const double*, int, int, double*, int, cudaStream_t);
 int es_impl_fitness_objective(es_ctx*, int, double*, int, const float*, int, int, cudaStream_t);
 int es_impl_mean_reward_steps(es_ctx*, double*, int, const int*, int, cudaStream_t);
-// the closed loop on an env whose episodes end when the position falls (rollout_closedt.cu): every shape, head and activation
-// the cluster kernel covers; steps / noise_used [2][n_pairs], `next` a device word the launch zeroes
-int es_impl_rollout_closedt(es_ctx*, const EsRollout&, const EsClosedEnv&, float fall_height, int* steps, long long* noise_used,
-                            unsigned* next, cudaStream_t);
 int es_impl_rank_transform(es_ctx*, const double*, const double*, int, int, int, double, double, int, int, int,
                            const int64_t*, float*, double*, int32_t*, double*, int32_t*, int64_t*, cudaStream_t);
 int es_impl_grad_reconstruct(es_ctx*, const float*, int64_t, const int64_t*, const float*, int, int, float*,

@@ -1,6 +1,9 @@
 // rollout_closedw.cu -- the CLOSED-LOOP synthetic env (obs_{t+1} = tanh(A obs_t + B a_t)) for policies too wide for
-// rollout_closed.cu's one pair per CTA: tanh MLPs with 2 to 4 hidden layers of 1 .. 256 units, obs <= 384, act <= 64 -- every
-// shipped config's policy (15-256-256-3, 17/26/28-256-256-256-6/8, 28-128-256-256-128-8) and a Humanoid-shaped 376-256-256-17.
+// rollout_closed.cu's one pair per CTA: MLPs with 2 to 4 hidden layers of 1 .. 256 units, obs <= 384, act <= 64 -- every
+// shipped config's policy (15-256-256-3, 17/26/28-256-256-256-6/8, 28-128-256-256-128-8) and a Humanoid-shaped 376-256-256-17 --
+// with tanh, a binned head or another activation, with or without action noise and episodes, on an env whose episodes run T
+// steps or end when the position falls.  One kernel family, cw_rollout<depth, binned, noisy, activation> in
+// rollout_closedw.cuh: 15 instantiations, each serving every call of its variant.
 //
 // Semantics are rollout_closed.cu's: theta +- sigma eps through es_pheno_pm (slices checked by es_checked_slice and the ctx's
 // error word), clip((o - mean) / std) in float64 (here an exact float64 division, as the reference), Linear + tanh after every
@@ -42,13 +45,13 @@
 //     might still store into its shared memory;
 //   * arithmetic on float32 CUDA cores: each weight matrix meets one activation column per step, so a wgmma (N >= 8) would
 //     run at most 1/8 full.
-// Binned-action policies (FFBinned, src/nn/nn.py:99-117; rollout_closedw_binned_kernel): the last layer has adim * bins outputs
+// Binned-action policies (FFBinned, src/nn/nn.py:99-117; BINNED): the last layer has adim * bins outputs
 // and every CTA holds all of them after B_{L-1}, so each CTA forms the adim actions locally (threads j < adim: the first
 // maximal bin, as torch.argmax, mapped to low[j] + range[j] * idx / (bins - 1) in the reference's float32 operation order) into
 // a local action buffer, then a __syncthreads, before the env step.  The env's B, the reward and the position use adim.  That
 // buffer is written after B_{L-1}(t) and read within step t only, so the barrier argument above is unchanged.  Binned shapes
 // always run here (C = 1 included): rollout_closed.cu has no head.
-// Action noise and episodes (rollout_closedw_noisy_kernel, es_rollout_closedloop_mlp_episodes; tanh heads only): the lane that
+// Action noise and episodes (NOISY, es_rollout_closedloop_mlp_episodes; no binned head): the lane that
 // owns an output row adds its noise value (loaded at the top of the step: a CTA owns <= 64 output rows, so one pass of its 16
 // warps covers them) before the remote stores above, which is the only change inside a step, so the barrier argument holds as
 // it is.  The E episodes of an evaluation run in sequence in its cluster, the weights left in place: each restarts x, the raw
@@ -56,18 +59,64 @@
 // float64 per-step sums of episodes 0 .. E - 2 in a [T] row per cluster in global memory, and the last episode adds
 // (row[t] + r) / E to the fitness and keeps the behaviour and the ObStat sums.  Spreading the episodes over clusters would
 // only help with fewer evaluations than resident clusters, and would make the result depend on the grid.
+// Other activations (ACT; es_rollout_closedloop_mlp_activation): the lane that owns a row applies ReLU, leaky ReLU, ELU or
+// sigmoid (es_act, in float32) where the tanh variants apply es_tanh_exp; the env's tanh(A obs + B a) is the env's and stays.
+// The kind is uniform over the launch and the branch sits in the per-row epilogue, outside the dot products, so one kernel per
+// depth and noise variant serves every kind.
+// Episodes that end early (EsTerm, es_rollout_closedloop_terminal: ClosedLoopEnv(fall_height=h)): the reference's run_model
+// leaves its step loop when env.step returns done (src/gym/gym_runner.py:50-67), and the pybullet Hopper and Ant envs the
+// shipped configs name return it when the robot falls.  Here step t returns done when t = T - 1 or !(|z_t| <= h), z_t the third
+// position component after step t's update (a NaN falls).  One cluster steps one evaluation, so stopping at a data-dependent
+// step costs nothing.  The flag is uniform over the launch; it gates only the position the other ranks form, the fall and the
+// break, and the steps / noise_used stores.  Everything else below takes its general form in every call, and with nothing
+// falling that form is the fixed-length one: t_d = T - 1, the noise offset is e T act, `reach` is T after the first episode,
+// and the fold after the last episode is empty.  A call without the flag never ends an episode early, a NaN position included:
+//   * uniform exit: the last warp's lane 0 of EVERY CTA forms the position (rank 0's is the reward lane, which already does;
+//     every CTA holds the same action after B_{L-1}, or forms the same binned action from the same outputs), with rank 0's
+//     operations in rank 0's order, and writes its CTA's fell flag before the step's closing __syncthreads; every thread reads
+//     it after that barrier and leaves the step loop at the same t_d in every CTA, without another cluster barrier;
+//   * barrier argument: a step that ends the episode has run all its barriers B_0 .. B_{L-1} and its __syncthreads, as any
+//     step.  The next cluster barrier is REUSE (or B_0 of the next episode's first step) instead of B_0(t_d + 1): every read
+//     of a_{L-1} (env step, reward, position) precedes the reader's arrival there, and the next write of any a_l comes from
+//     a later step's layer, after its writer waited at that barrier -- the write-after-read order above with B_0(t + 1)
+//     replaced by the next barrier the cluster meets.  The fell flag is local: written after the reader's last read of it
+//     (the previous step's __syncthreads, then the step's cluster barriers) and read after the step's __syncthreads;
+//   * the accumulators stop at t_d: the fitness (float64, step order) and position, the ObStat column sums over the t_d + 1
+//     post-step rows, and the ObStat count, which adds t_d + 1 per saved evaluation;
+//   * steps [2][n_pairs]: the last episode's t_d (T - 1 if nothing fell), what run_model returns;
+//   * episodes (obj.py:54-63): each episode ends on its own; rank 0's reward lane keeps the per-step float64 sums of the
+//     earlier episodes in the cluster's [T] row as far as the longest of them reached (`reach`; a step beyond it adds to 0),
+//     and after the last episode folds row[t] / E into the fitness for t_d < t < reach, so the fitness is
+//     sum_t (sum_e r_{e,t}) / E in step order to the longest episode's end.  Behaviour, ObStat and steps are the last
+//     episode's.  Without action noise the call runs one episode (the E are identical);
+//   * action noise: the reference draws randn(act) for executed steps only, so episode e reads its gaussians from where
+//     episode e - 1 stopped, at offset sum_{e' < e} (t_{d,e'} + 1) act of the evaluation's E T act values; noise_used
+//     reports the total.
+// Dynamic scheduling (every call): a cluster takes its next evaluation from a device counter (rank 0's thread 0 adds to it
+// after the step loop and stores the result into every CTA's shared memory, which the REUSE barrier publishes; every CTA read
+// the previous value before the evaluation's first cluster barrier, which that thread has passed), so a cluster whose
+// evaluations fall early takes more of them.  An evaluation's arithmetic does not depend on the cluster that runs it.
 // Alternatives not built (so not measured): weights partly in registers (rollout_closed.cu's layer 1), and a pair (both signs)
 // per cluster, which doubles the footprint to save only the load-time reads of eps.
 #include "rollout_closedw.cuh"
 
 namespace {
 
-template <int NL>
-__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) { cw_rollout<NL, false, false>(p); }
-template <int NL>
-__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_binned_kernel(const CwParams p) { cw_rollout<NL, true, false>(p); }
-template <int NL>
-__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_noisy_kernel(const CwParams p) { cw_rollout<NL, false, true>(p); }
+template <int NL, bool BINNED, bool NOISY, bool ACT>
+__global__ void __launch_bounds__(CW_THREADS, 1) rollout_closedw_kernel(const CwParams p) { cw_rollout<NL, BINNED, NOISY, ACT>(p); }
+
+template <bool BINNED, bool NOISY, bool ACT>
+CwKernel cw_depth(int n_layers) {
+    return n_layers == 3 ? rollout_closedw_kernel<3, BINNED, NOISY, ACT>
+         : n_layers == 4 ? rollout_closedw_kernel<4, BINNED, NOISY, ACT> : rollout_closedw_kernel<5, BINNED, NOISY, ACT>;
+}
+
+// binned heads are tanh stacks that draw no noise (FFBinned.forward ignores rs)
+CwKernel cw_kernel(int n_layers, bool binned, bool noisy, bool act) {
+    if (binned) return cw_depth<true, false, false>(n_layers);
+    if (act) return noisy ? cw_depth<false, true, true>(n_layers) : cw_depth<false, false, true>(n_layers);
+    return noisy ? cw_depth<false, true, false>(n_layers) : cw_depth<false, false, false>(n_layers);
+}
 
 }  // namespace
 
@@ -122,36 +171,31 @@ int es_closedw_binned_plan(const int* dims, int n_layers, int band, int bins, in
     return cw_plan(fn, dims, n_layers, band, out / bins, true, cluster_size, smem_bytes);
 }
 
-static CwKernel cw_kernel(int n_layers, bool binned = false, bool noisy = false) {
-    if (noisy)
-        return n_layers == 3 ? rollout_closedw_noisy_kernel<3> : n_layers == 4 ? rollout_closedw_noisy_kernel<4>
-                                                                                : rollout_closedw_noisy_kernel<5>;
-    if (binned)
-        return n_layers == 3 ? rollout_closedw_binned_kernel<3> : n_layers == 4 ? rollout_closedw_binned_kernel<4>
-                                                                                 : rollout_closedw_binned_kernel<5>;
-    return n_layers == 3 ? rollout_closedw_kernel<3> : n_layers == 4 ? rollout_closedw_kernel<4> : rollout_closedw_kernel<5>;
-}
-int es_closedw_max_clusters(int n_layers, int bins, int C, size_t smem, int* clusters) {
-    return cw_max_clusters(cw_kernel(n_layers, bins != 0), C, smem, clusters);
+// the plan entry points' resident clusters (the noise-free variant's: every variant runs one CTA per SM)
+int es_closedw_max_clusters(int n_layers, int bins, bool act, int C, size_t smem, int* clusters) {
+    return cw_max_clusters(cw_kernel(n_layers, bins != 0, false, act), C, smem, clusters);
 }
 
-int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, cudaStream_t stream) {
+int es_impl_rollout_closedw(es_ctx* ctx, const EsRollout& r, const EsClosedEnv& env, const EsTerm& term, unsigned* next,
+                            cudaStream_t stream) {
     int C = 0, max_clusters = 0;
     size_t smem = 0;
-    const bool binned = r.bins != 0, noisy = r.act_noise != nullptr;       // (never both: the binned entry passes no noise)
+    const bool binned = r.bins != 0;
     int rc = binned ? es_closedw_binned_plan(r.dims, r.n_layers, env.band, r.bins, &C, &smem)
                     : es_closedw_plan(r.dims, r.n_layers, env.band, &C, &smem);
     if (rc) return rc;
-    const CwKernel kernel = cw_kernel(r.n_layers, binned, noisy);
+    const CwKernel kernel = cw_kernel(r.n_layers, binned, r.act_noise != nullptr, r.activation != ES_ACT_TANH);
     rc = cw_max_clusters(kernel, C, smem, &max_clusters);
     if (rc) return rc;
     if (max_clusters < 1) {
-        es_set_error("es_rollout_closedloop_mlp: no cluster of %d CTAs with %zu bytes of shared memory each fits on this device", C, smem);
+        es_set_error("the closed-loop cluster rollout: no cluster of %d CTAs with %zu bytes of shared memory each fits on this "
+                     "device", C, smem);
         return ES_ERR_UNSUPPORTED;
     }
-    const CwParams p = {r, env};
+    const CwParams p = {r, env, term, next};
     const long long evals = 2ll * r.n_pairs;
     const int clusters = evals < max_clusters ? (int)evals : max_clusters;
+    ES_CHECK_CUDA(cudaMemsetAsync(next, 0, sizeof(unsigned), stream));
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cw_config(C, smem, clusters, stream, &attr);
     ES_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));

@@ -1,6 +1,5 @@
 // rollout_closedw.cuh -- the closed-loop cluster rollout's code (see rollout_closedw.cu for the design and the barrier argument):
-// the shared-memory layout, the body every CTA of a cluster runs and the launch configuration.  rollout_closedw.cu instantiates
-// it for tanh policies and binned heads, rollout_closedw_act.cu for the other activations.
+// the shared-memory layout, the body every CTA of a cluster runs and the launch configuration.
 #pragma once
 #include <math.h>
 #include "common.cuh"
@@ -20,6 +19,8 @@ constexpr int CW_SMEM_MAX = 227 * 1024 - 1024;    // dynamic shared memory per C
 struct CwParams {
     EsRollout r;
     EsClosedEnv env;                        // ep_rows: [clusters][T] per-step episode sums (n_episodes > 1)
+    EsTerm term;                            // term.steps == NULL: the episodes run T steps whatever the position
+    unsigned* next;                         // the evaluation counter of dynamic scheduling, zero before the launch
 };
 
 __host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
@@ -101,19 +102,11 @@ __device__ __forceinline__ void cw_store_remote(float* local, unsigned rank, flo
 // one layer of this CTA in the step loop (read from shared memory: a per-layer index into registers would go to local memory)
 struct CwLayer { int in, nr, S, r0, w, bias, xin, out, woff, boff; };
 
-// what a terminating env adds to a call (rollout_closedt.cu; TERM = false ignores it)
-struct CwTerm {
-    float fall_height;          // h > 0: an episode ends after the step whose position leaves |z| <= h (or at T - 1)
-    int* steps;                 // [2][n_pairs] (+ then -): the last episode's t_d
-    long long* noise_used;      // [2][n_pairs] action-noise values the evaluation consumed (Σ_e (t_{d,e} + 1) act), or NULL
-    unsigned* next;             // the evaluation counter of dynamic scheduling, zero before the launch
-};
-
 // ACT: every layer of the policy applies the call's activation (p.r.activation, es_act) instead of tanh; the env's own
-// tanh(A obs + B a) stays tanh.  TERM: the env ends an episode when its position falls (rollout_closedt.cu: the changes and
-// why the barrier argument holds are stated there)
-template <int NL, bool BINNED, bool NOISY, bool ACT = false, bool TERM = false>
-__device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm = CwTerm{}) {
+// tanh(A obs + B a) stays tanh.  p.term.steps set: the env ends an episode when its position falls (rollout_closedw.cu states
+// the changes and why the barrier argument holds); unset, no episode ends before T, whatever the position (a NaN included)
+template <int NL, bool BINNED, bool NOISY, bool ACT>
+__device__ __forceinline__ void cw_rollout(const CwParams& p) {
     extern __shared__ __align__(16) float cw_smem[];
     __shared__ CwLayer cw_layers[NL];
     const unsigned C = cw_cluster_nctas(), rank = cw_cluster_rank();
@@ -134,6 +127,7 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const bool rew_warp = rank == 0 && warp == CW_WARPS - 1;
+    const bool term = p.term.steps != nullptr;
 
     for (int i = tid; i < band * obs; i += CW_THREADS) cw_smem[L.env_a + i] = p.env.env_a[i];
     for (int i = tid; i < act * obs; i += CW_THREADS) cw_smem[L.env_b + i] = p.env.env_b[i];
@@ -149,11 +143,11 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
     }
     cw_cluster_sync();                                      // START: every CTA of the cluster runs and has zeroed its buffers
 
-    // TERM: the fell flag of the step (every CTA's own) and the cluster's next evaluation (rank 0 stores it into every CTA)
-    // in the two free words after the position
+    // the fell flag of the step (every CTA's own) and the cluster's next evaluation (rank 0 stores it into every CTA) in the
+    // two free words after the position
     int* __restrict__ tflag = reinterpret_cast<int*>(cw_smem + L.racc + 5);
     int* __restrict__ tnext = reinterpret_cast<int*>(cw_smem + L.racc + 6);
-    for (int ev = cluster; ev < 2 * p.r.n_pairs; ev = TERM ? *tnext : ev + n_clusters) {
+    for (int ev = cluster; ev < 2 * p.r.n_pairs; ev = *tnext) {
         const int pair = ev >> 1, neg = ev & 1;
         const long long base = es_checked_slice(p.r.idx[pair], p.r.P, p.r.table_len, p.r.err);
         const float* __restrict__ eps = p.r.table + base;
@@ -193,8 +187,8 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
         __syncthreads();
 
         const int n_eps = NOISY ? p.r.n_episodes : 1;
-        // TERM: the step the episode ended at (the same in every thread of the cluster), the noise values consumed so far, and
-        // the steps the earlier episodes' per-step sums reach (the longest of them)
+        // the step the episode ended at (the same in every thread of the cluster), the noise values consumed so far, and the
+        // steps the earlier episodes' per-step sums reach (the longest of them)
         int t_end = T - 1, reach = 0;
         long long used = 0;
         for (int ep = 0; ep < n_eps; ++ep) {
@@ -214,8 +208,7 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
                 const CwLayer& lo = cw_layers[NL - 1];
                 const int r = 4 * warp + (lane >> 3);
                 if (r < lo.nr)
-                    nzp = TERM ? p.r.act_noise + ((size_t)pair * 2 + neg) * n_eps * T * act + used + lo.r0 + r
-                               : p.r.act_noise + (((size_t)pair * 2 + neg) * n_eps + ep) * T * act + lo.r0 + r;
+                    nzp = p.r.act_noise + ((size_t)pair * 2 + neg) * n_eps * T * act + used + lo.r0 + r;
             }
 
             t_end = T - 1;
@@ -227,7 +220,7 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
                     const float* __restrict__ c = p.r.rew_vec + (size_t)t * act;
                     if (lane < act) crow0 = __ldg(c + lane);
                     if (lane + 32 < act) crow1 = __ldg(c + lane + 32);
-                    if (NOISY && lane == 0 && ep > 0 && (!TERM || t < reach)) esum = erow[t];
+                    if (NOISY && lane == 0 && ep > 0 && t < reach) esum = erow[t];
                 }
                 float nz = 0.f;                                 // this lane's action noise: in flight under the layers
                 if (NOISY && nzp) nz = __ldg(nzp + (size_t)t * act);
@@ -305,34 +298,33 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
                     }
                     __syncwarp();
                 }
-                if (TERM && warp == CW_WARPS - 1 && lane == 0) {
+                if (warp == CW_WARPS - 1 && lane == 0) {
                     // every CTA forms the position as rank 0's reward lane does (same action, same operations), so every CTA
-                    // decides the fall alike
-                    if (rank != 0) {
+                    // decides the fall alike.  The flag is stored and read at every step, also without an early end: a read
+                    // gated on `term` made the step loop measurably slower
+                    if (term && rank != 0) {
                         const float ps = p.r.pos_scale;
                         rpos[0] = __fadd_rn(rpos[0], __fmul_rn(ps, action[0]));
                         rpos[1] = __fadd_rn(rpos[1], __fmul_rn(ps, action[1 % act]));
                         rpos[2] = __fadd_rn(rpos[2], __fmul_rn(ps, action[2 % act]));
                     }
-                    *tflag = !(fabsf(rpos[2]) <= tm.fall_height);
+                    *tflag = term && !(fabsf(rpos[2]) <= p.term.fall_height);
                 }
                 __syncthreads();                                // x and the raw observation before the next step's layer 0
-                if (TERM && *tflag) { t_end = t; break; }
+                if (*tflag) { t_end = t; break; }
             }
-            if (TERM) {
-                used += (long long)(t_end + 1) * act;
-                if (NOISY && rew_warp && lane == 0 && last_ep)  // the steps only earlier episodes reached (obj.py:58-61)
-                    for (int t = t_end + 1; t < reach; ++t) rfit[0] += erow[t] / n_eps;
-                reach = max(reach, t_end + 1);
-            }
+            used += (long long)(t_end + 1) * act;
+            if (NOISY && rew_warp && lane == 0 && last_ep)      // the steps only earlier episodes reached (obj.py:58-61)
+                for (int t = t_end + 1; t < reach; ++t) rfit[0] += erow[t] / n_eps;
+            reach = max(reach, t_end + 1);
         }
         if (rew_warp && lane == 0) {
             (neg ? p.r.fit_neg : p.r.fit_pos)[(size_t)pair * p.r.fit_stride] = rfit[0];
             float* bv = neg ? p.r.behv_neg : p.r.behv_pos;
             if (bv) { bv[(size_t)pair * 3 + 0] = rpos[0]; bv[(size_t)pair * 3 + 1] = rpos[1]; bv[(size_t)pair * 3 + 2] = rpos[2]; }
-            if (TERM) {
-                tm.steps[(size_t)neg * p.r.n_pairs + pair] = t_end;
-                if (tm.noise_used) tm.noise_used[(size_t)neg * p.r.n_pairs + pair] = used;
+            if (term) {
+                p.term.steps[(size_t)neg * p.r.n_pairs + pair] = t_end;
+                if (p.term.noise_used) p.term.noise_used[(size_t)neg * p.r.n_pairs + pair] = used;
             }
         }
         if (keep_stat) {
@@ -342,10 +334,10 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p, const CwTerm& tm =
                 atomicAdd(p.env.ob_sum + i, (double)st.x);
                 atomicAdd(p.env.ob_sumsq + i, (double)st.y);
             }
-            if (tid == 0) { atomicAdd(p.env.ob_count, (double)(TERM ? t_end + 1 : T)); atomicAdd(p.env.ob_count + 1, 1.0); }
+            if (tid == 0) { atomicAdd(p.env.ob_count, (double)(t_end + 1)); atomicAdd(p.env.ob_count + 1, 1.0); }
         }
-        if (TERM && rank == 0 && tid == 0) {                // the cluster's next evaluation, into every CTA before REUSE
-            const int nx = n_clusters + (int)atomicAdd(tm.next, 1u);
+        if (rank == 0 && tid == 0) {                        // the cluster's next evaluation, into every CTA before REUSE
+            const int nx = n_clusters + (int)atomicAdd(p.next, 1u);
             for (unsigned q = 0; q < C; ++q) cw_store_remote(reinterpret_cast<float*>(tnext), q, __int_as_float(nx));
         }
         cw_cluster_sync();                                  // REUSE (the last one: EXIT)

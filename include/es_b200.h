@@ -274,8 +274,8 @@ int es_rollout_closedloop_mlp_binned_plan(es_ctx* ctx, const int* layer_sizes, i
                                           int* cluster_size, int* clusters, int64_t* smem_bytes);
 
 /* es_rollout_closedloop_mlp_episodes for a policy with any activation of es_rollout_openloop_activation.  ES_ACT_TANH is
- * es_rollout_closedloop_mlp_episodes itself, bit for bit.  The other kinds run rollout_closedw_act.cu, the cluster kernel's
- * code, at every shape es_rollout_closedloop_mlp covers, a cluster of one CTA included; the env's own tanh(A obs + B a) stays
+ * es_rollout_closedloop_mlp_episodes itself, bit for bit.  The other kinds run rollout_closedw.cu, the cluster kernel, at
+ * every shape es_rollout_closedloop_mlp covers, a cluster of one CTA included; the env's own tanh(A obs + B a) stays
  * tanh.  One kernel launch per call.                                                                                   */
 int es_rollout_closedloop_mlp_activation(es_ctx* ctx, const float* table, int64_t table_len, const int64_t* idx, int n_pairs,
                                          const float* theta, int P, float sigma, const int* layer_sizes, int n_layers,
@@ -298,8 +298,8 @@ int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_size
  * es_rollout_closedloop_mlp_binned (activation ES_ACT_TANH, no action noise).  act_noise / n_episodes as
  * es_rollout_closedloop_mlp_episodes, except that episode e reads its gaussians from where episode e - 1 stopped (the reference
  * draws rs.randn(act) only for the steps it executes): the buffer holds E T act values per evaluation, of which the first
- * sum_e (t_{d,e} + 1) act are read.  Every shape es_rollout_closedloop_mlp covers runs rollout_closedt.cu, the cluster kernel's
- * code (a cluster of one CTA included); clusters take evaluations from a device counter, so early falls free them for others.
+ * sum_e (t_{d,e} + 1) act are read.  Every shape es_rollout_closedloop_mlp covers runs rollout_closedw.cu, the cluster kernel
+ * (a cluster of one CTA included); clusters take evaluations from a device counter, so early falls free them for others.
  * Per evaluation, everything stops at the step t_d that returned done:
  *   fitness      sum_t (sum_e r_{e,t}) / E to the longest episode's end (obj.py: rews[:len(rew)] += rew; rews /= E)
  *   behv         the last episode's final position

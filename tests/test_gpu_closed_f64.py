@@ -244,7 +244,9 @@ def test_closed_kernels_match_the_float64_truth(eng, p):
 # ---------------------------------------------------------------------------------------------- a NaN in the observation mean
 # torch.clamp (nn.py:45) keeps a NaN, so a NaN in ob_mean makes that observation column NaN at every step: every output of a
 # tanh or activation stack and every fitness is NaN, in the float64 truth and on the device.  A binned head's arg-max over
-# all-NaN outputs is bin 0 (torch.argmax), so its fitness stays finite and is held to the binned tests' bound.
+# all-NaN outputs is bin 0 (torch.argmax), so its fitness stays finite and is held to the binned tests' bound.  On the
+# cluster kernel (the closed loop's wide and activation families) the position is NaN too, and an env without a fall height
+# still runs every saved evaluation's T steps: ob_count is [T saved, saved].
 _NAN_FAMILIES = [('one_cta', (17, 64, 64, 6), None, 0), ('wide', (15, 256, 256, 3), None, 0),
                  ('activation', (17, 64, 64, 6), 'relu', 0), ('binned', (15, 64, 64, 15), None, 5)]
 
@@ -271,6 +273,16 @@ def test_nan_in_the_observation_mean_reaches_the_fitness(eng, name, sizes, act_k
     spec = orc.ClosedLoopEnvSpec(obs, adim, T, band=8) if loop == 'closed' else orc.SyntheticEnvSpec(obs, adim, T)
     fit = torch.zeros(2, n, dtype=torch.float64, device=eng.device)
     behv = torch.zeros(2, n, 3, dtype=torch.float32, device=eng.device)
+    ob, saved = {}, []
+    if loop == 'closed' and name in ('wide', 'activation'):
+        saved = [(s, k) for s in range(2) for k in range(n) if (k + s) % 2 == 0]
+        coins = np.full((n, 4), 0xFFFFFFFF, dtype=np.uint32)
+        for s, k in saved:
+            coins[k, 2 * s:2 * s + 2] = 0                                       # u = 0 < chance
+        ob = dict(coin_words=dv(coins.view(np.int32)), save_obs_chance=0.5,
+                  ob_sum=torch.zeros(obs, dtype=torch.float64, device=eng.device),
+                  ob_sumsq=torch.zeros(obs, dtype=torch.float64, device=eng.device),
+                  ob_count=torch.zeros(2, dtype=torch.float64, device=eng.device))
     if loop == 'open':
         obsn = eng.normalise_obs(dv(spec.obs_stream[:T]), dv(mean), dv(std), clip)
         eng.rollout(dv(table), dv(idx), dv(theta), SIGMA, sizes, obsn, dv(spec.rew_vec[:T]), spec.pos_scale, fit[0], fit[1], 1,
@@ -279,9 +291,11 @@ def test_nan_in_the_observation_mean_reaches_the_fitness(eng, name, sizes, act_k
         eng.rollout_closed_mlp(dv(table), dv(idx), dv(theta), SIGMA, sizes, dv(mean), dv(std), clip, dv(spec.obs_stream[0].copy()),
                                dv(np.ascontiguousarray(spec.env_a.T)), dv(np.ascontiguousarray(spec.env_b.T)), dv(spec.rew_vec),
                                spec.pos_scale, fit[0], fit[1], 1, behv[0].view(-1), behv[1].view(-1), head=head,
-                               activation=activation)
+                               activation=activation, **ob)
     eng.sync()
     f = fit.cpu().numpy()
+    if ob:
+        assert ob['ob_count'].cpu().tolist() == [float(T * len(saved)), float(len(saved))]
     if bins:                                   # the oracle's per-step loop: torch.argmax of the NaN outputs
         dims = orc.layer_dims(obs, sizes[1:-1], sizes[-1])
         want, bound = np.zeros((2, n)), np.zeros((2, n))

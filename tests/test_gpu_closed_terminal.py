@@ -8,8 +8,9 @@
   delta (and, for the binned head, those whose top two outputs come within 1e-5) are counted, shown to be few, and skipped.
   Fitness within that file's EVAL_REL times the reward mass summed to t_d, the final position within its bound, steps, and
   the ObStat sums and count of the saved evaluations;
-* nothing falls: bit for bit the fall_height=None result of the existing cluster kernels; at a shape fall_height=None runs
-  on the one-CTA kernel, both within the float64 bound;
+* nothing falls: bit for bit the fall_height=None result of the cluster kernel, also with action noise over E = 3 episodes
+  (tanh and leaky ReLU at C = 1 and C = 2); at a shape fall_height=None runs on the one-CTA kernel, both within the float64
+  bound;
 * episodes: noise-free E = 3 is E = 1 bit for bit; with noise, E = 3 where an episode ends before an earlier one (the fold
   to the longest episode) against the truth, and the consumed gaussians sum_e (t_{d,e} + 1) act;
 * es.test_params / es.step with ac_std = 0: the fused route against the same generation driven call by call with a python
@@ -187,16 +188,27 @@ def test_terminal_kernel_matches_the_float64_truth(eng, name, sizes, T, kind, C)
 
 
 @pytest.mark.parametrize('name,sizes,kind', [('simple_conf', (15, 256, 256, 3), 'tanh'), ('obj', (17, 256, 256, 256, 6), 'tanh'),
-                                             ('binned', (15, 64, 64, 15), 'binned'), ('leaky', (17, 64, 64, 6), 'leaky')])
+                                             ('binned', (15, 64, 64, 15), 'binned'), ('leaky', (17, 64, 64, 6), 'leaky'),
+                                             # action noise, E = 3: the noise offset and the episode fold
+                                             ('noisy_c1', (15, 128, 64, 3), 'tanh+noise'),
+                                             ('noisy_c2', (15, 256, 256, 3), 'tanh+noise'),
+                                             ('noisy_leaky_c1', (17, 64, 64, 6), 'leaky+noise'),
+                                             ('noisy_leaky_c2', (15, 256, 256, 3), 'leaky+noise')])
 def test_nothing_falls_is_the_existing_kernels_bit_for_bit(eng, name, sizes, kind):
+    kind, noisy = kind.split('+')[0], kind.endswith('+noise')
     head, activation, _, _ = _head(kind)
-    d = build(sizes, 120, adim=3 if kind == 'binned' else None)
+    T, E = 120, 3 if noisy else 1
+    d = build(sizes, T, adim=3 if kind == 'binned' else None, E=E, ac_std=0.3 if noisy else 0.0)
+    if noisy:
+        assert eng.closed_mlp_plan(list(sizes), 8, head, activation)[0] == (2 if sizes[1] == 256 else 1)
     saved = [(s, k) for s in range(2) for k in range(d['n']) if (k + s) % 2 == 0]
     a = run(eng, d, 1e30, head, activation, saved)
     b = run(eng, d, None, head, activation, saved, terminal=False)
     for key in ('fit', 'behv', 'osum', 'osq', 'ocnt'):
         assert np.array_equal(a[key], b[key]), key
-    assert (a['steps'] == 119).all()
+    assert (a['steps'] == T - 1).all()
+    if noisy:
+        assert (a['used'] == E * T * sizes[-1]).all()
 
 
 def test_one_launch_equals_pairs_launched_one_at_a_time(eng):

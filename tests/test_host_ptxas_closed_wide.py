@@ -1,5 +1,6 @@
-"""CPU (no GPU): the closed-loop cluster rollout (rollout_closedw.cu) compiles for sm_90a without spills, and the shared memory
-it requests fits an H100 CTA (227 KiB, static included) for every shape it accepts.
+"""CPU (no GPU): the closed-loop cluster rollout (rollout_closedw.cu) compiles for sm_90a to one kernel per depth and variant
+(tanh, binned head, action noise, another activation, another activation with action noise), none with a stack frame or
+spills, and the shared memory it requests fits an H100 CTA (227 KiB, static included) for every shape it accepts.
 
 The plan (es_closedw_plan: coverage, cluster size, dynamic shared memory per CTA) is host code, so a small host program that
 includes the source runs it here over the shipped shapes and a grid of covered shapes up to every limit."""
@@ -22,25 +23,43 @@ def _nvcc():
     return cand if (os.path.isabs(cand) and os.path.exists(cand)) or shutil.which(cand) else None
 
 
-def _compile_log(tmp):
-    cmd = [_nvcc(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-Xptxas', '-v', '-c',
-           '-o', os.path.join(tmp, 'rollout_closedw.o'), SRC]
-    res = subprocess.run(cmd, capture_output=True, text=True)
+@pytest.fixture(scope='module')
+def ptxas_log():
+    if _nvcc() is None:
+        pytest.skip('needs nvcc')
+    with tempfile.TemporaryDirectory() as tmp:
+        cmd = [_nvcc(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-Xptxas', '-v', '-c',
+               '-o', os.path.join(tmp, 'rollout_closedw.o'), SRC]
+        res = subprocess.run(cmd, capture_output=True, text=True)
     log = res.stdout + res.stderr
     assert res.returncode == 0, log
     return log
 
 
-@pytest.mark.skipif(_nvcc() is None, reason='needs nvcc')
-def test_rollout_closedw_compiles_without_spills():
-    with tempfile.TemporaryDirectory() as tmp:
-        log = _compile_log(tmp)
-    # one instantiation per depth (2, 3 and 4 hidden layers), none spilling
-    props = re.findall(r'Function properties for (\S*rollout_closedw_kernel\S*)\n\s*(\d+) bytes stack frame, (\d+) bytes spill '
-                       r'stores, (\d+) bytes spill loads', log)
-    assert len(props) == 3, log
-    for name, _, st, ld in props:
-        assert st == '0' and ld == '0', f'{name}: {st} bytes spill stores, {ld} bytes spill loads'
+def _props(log):
+    """(name, stack, spill stores, spill loads) of every cluster-kernel instantiation in the ptxas log."""
+    return re.findall(r'Function properties for (\S*rollout_closedw_kernel\S*)\n\s*(\d+) bytes stack frame, (\d+) bytes spill '
+                      r'stores, (\d+) bytes spill loads', log)
+
+
+def test_cluster_kernel_variants_compile_without_spills(ptxas_log):
+    props = _props(ptxas_log)
+    assert len(props) == 15, ptxas_log
+    for name, stack, st, ld in props:
+        assert stack == '0' and st == '0' and ld == '0', f'{name}: {stack} bytes stack, {st} bytes spill stores, {ld} loads'
+
+
+def test_cluster_kernel_has_three_depths_of_each_variant(ptxas_log):
+    assert 'rollout_closedw.cu' in build.SOURCES and 'rollout_closedw.cuh' in build.HEADERS
+    # (depth, binned, noisy, activation) from the mangled template arguments <NL, BINNED, NOISY, ACT>
+    variants = []
+    for name, _, _, _ in _props(ptxas_log):
+        m = re.search(r'rollout_closedw_kernelILi(\d)ELb([01])ELb([01])ELb([01])E', name)
+        assert m, name
+        variants.append(tuple(int(g) for g in m.groups()))
+    # 2, 3 and 4 hidden layers x (tanh, binned, tanh + noise, activation, activation + noise): binned heads draw no noise
+    want = {(nl, b, n, a) for nl in (3, 4, 5) for b, n, a in ((0, 0, 0), (1, 0, 0), (0, 1, 0), (0, 0, 1), (0, 1, 1))}
+    assert len(variants) == 15 and set(variants) == want, ptxas_log
 
 
 HARNESS = r'''
@@ -82,12 +101,11 @@ int main() {
 '''
 
 
-@pytest.mark.skipif(_nvcc() is None, reason='needs nvcc')
-def test_rollout_closedw_shared_memory_fits_every_covered_shape():
+def test_rollout_closedw_shared_memory_fits_every_covered_shape(ptxas_log):
+    # (the source's only kernels are the rollout_closedw_kernel instantiations)
+    static = [int(x) for x in re.findall(r'Used \d+ registers, used \d+ barriers, (\d+) bytes smem', ptxas_log)]
+    assert len(static) == 15, ptxas_log
     with tempfile.TemporaryDirectory() as tmp:
-        log = _compile_log(tmp)
-        # (the source's only kernels are the rollout_closedw_kernel instantiations)
-        static = [int(x) for x in re.findall(r'Used \d+ registers, used \d+ barriers, (\d+) bytes smem', log)]
         src = os.path.join(tmp, 'plan.cu')
         with open(src, 'w') as f:
             f.write(HARNESS % SRC.replace('\\', '/'))
@@ -96,8 +114,8 @@ def test_rollout_closedw_shared_memory_fits_every_covered_shape():
                              capture_output=True, text=True)
         assert res.returncode == 0, res.stdout + res.stderr
         out = subprocess.run([exe], capture_output=True, text=True, timeout=120).stdout
-    static_max = max(static) if static else 0
-    assert static_max <= 1024, log                      # the 1 KiB the plan leaves for the kernel's static shared memory
+    static_max = max(static)
+    assert static_max <= 1024, ptxas_log                     # the 1 KiB the plan leaves for the kernel's static shared memory
     plans = {m.group(1): (int(m.group(2)), int(m.group(3)), int(m.group(4)))
              for m in re.finditer(r'^(\w+) rc (-?\d+) C (\d+) smem (\d+)$', out, re.M)}
     # every shipped policy is covered, with the cluster size the README states

@@ -2,7 +2,7 @@
 alternating within each row.  Open loop: ES_ROLLOUT_F32 and ES_ROLLOUT_TC3 at config 3 (376-64-64-17, K = 10 000, T = 1000:
 tanh runs the headline kernels, rollout_f32x.cu and rollout_tc2.cu, the other kinds the general float32 kernel and, where
 obs <= 256, the wide tensor-core kernel's code) and at the shipped shapes (simple_conf, obj, flagrun).  Closed loop: the cluster
-kernel (rollout_closedw.cu / rollout_closedw_act.cu) at simple_conf and obj.  Per row and kind: CUDA-event ms per rollout after a
+kernel (rollout_closedw.cu) at simple_conf and obj.  Per row and kind: CUDA-event ms per rollout after a
 warm-up (REPS rounds, kinds interleaved) and pairs/s; a kind a mode refuses prints the refusal.  The card, its power limit and
 its max SM clock are printed first.  ROWS=name,... picks rows."""
 import os, subprocess, sys
