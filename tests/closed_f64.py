@@ -1,22 +1,30 @@
-"""Float64 reference of the closed-loop rollout (es_rollout_closedloop_mlp / _episodes): what both closed-loop kernels
-approximate.
+"""Float64 reference of the closed-loop rollout (es_rollout_closedloop_mlp / _episodes / _terminal): what every closed-loop
+kernel approximates.
 
 TEST INFRASTRUCTURE ONLY.  It takes the data the kernels get and evaluates them in float64 without intermediate rounding:
 
 * the weights are ``theta +- f64(sigma) * eps`` exactly (``sigma`` as the float32 the kernels receive), state-dict layout;
-* every step normalises the raw observation, ``clip((ob - mean) / std, -clip, clip)``, runs ``tanh(W x + b)`` after every
-  layer, adds the episode's action noise ``nz`` (``act_noise`` [n_pairs][2][E][T][act], the scaled float32 gaussians), earns
-  ``<a + nz, c_t>``, integrates the position ``pos_scale * (a + nz)[i % act]`` and steps the env,
+* every step normalises the raw observation, ``clip((ob - mean) / std, -clip, clip)``, runs ``activation(W x + b)`` after
+  every layer (tanh, or f64_rollout's float64 forms of the other activations; a binned head, ``binned = (bins, low, high)``,
+  runs tanh and takes each action dimension's arg-max in bin order, ``low + (high - low) bin / (bins - 1)``), adds the
+  episode's action noise ``nz`` (``act_noise`` [n_pairs][2][E T act], the scaled float32 gaussians), earns ``<a + nz, c_t>``,
+  integrates the position ``pos_scale * (a + nz)[i % act]`` and steps the env,
   ``ob_i <- tanh(sum_d A[i, d] ob[(i + d - half) mod n] + sum_j B[i, j] (a + nz)_j)``;
-* every episode restarts from ``obs0`` with the position at 0; the fitness is ``sum_t mean_e r_{e,t}``, the reward mass
-  ``sum_t mean_e sum_j |a_tj c_tj|`` (the scale of the fitness error of an implementation whose actions carry a relative
-  error, as in f64_rollout.py);
+* with ``fall_height`` h (ClosedLoopEnv(fall_height=h)), step t ends an episode when t = T - 1 or not |z_t| <= f32(h), z_t
+  the third position component after step t's update, so a NaN position ends it too (run_model's ``if done: break``
+  inside obj.py's episode loop); without one every episode runs T steps whatever the position;
+* every episode restarts from ``obs0`` with the position at 0 and reads its noise from the evaluation's flat run where the
+  previous episode stopped (offset ``used + t act``); the fitness is ``sum_t (sum_e r_{e,t}) / E`` over the executed steps,
+  the reward mass ``sum_t (sum_e sum_j |a_tj c_tj|) / E`` (the scale of the fitness error of an implementation whose actions
+  carry a relative error, as in f64_rollout.py);
 * behaviour, position magnitude (f64_rollout.episode's), the float64 column sums of the post-step observations and of their
-  squares (the ObStat increments) and the final observation ``olast`` are the last episode's.
+  squares (the ObStat increments), the final observation ``olast`` and the last executed step t_d are the last episode's.
 
 The evaluations of a call are stacked, so that a step is one batched matrix product per layer; so are *variants* of every
 evaluation: ``simulate(variants=)`` runs, beside the truth, copies of it computed wrongly on purpose (the bugs a kernel could have, see
-``MUTATIONS``), and ``growth`` runs copies whose start observation is moved by 1e-9.  Nothing here imports the kernels.
+``MUTATIONS``), and ``growth`` runs copies whose start observation is moved by 1e-9.  One step loop with an alive mask runs
+every episode, so an env where nothing falls gives the fixed-length result by construction.  Nothing here imports the
+kernels.
 """
 from __future__ import annotations
 
@@ -24,8 +32,16 @@ from typing import Optional, Sequence
 
 import numpy as np
 
+import f64_rollout as f64
+
 U = 2.0 ** -24
 TANH_APPROX = 2.0 ** -11            # the relative error of tanh.approx.f32
+
+# The bounds a closed-loop kernel is held to against this truth (tests/test_gpu_closed_f64.py explains and measures them):
+EVAL_REL = 1e-5                     # per evaluation |f - truth| <= EVAL_REL * mass
+RMS_BOUND = 3e-4                    # over the evaluations rms(f - truth) <= RMS_BOUND * spread
+ACT_ERR = 1e-5                      # the error of one action, in the position bound 2 U mag + ACT_ERR pos_scale T
+OBS_ERR = 1e-6                      # the error of one observation, in the ObStat bounds
 
 
 # ---------------------------------------------------------------------------------------------- the cluster kernel's plan, restated
@@ -111,8 +127,8 @@ drop_last_step     the last step (reward, position, env step) is not taken
 skip_first_env_step  the env does not step at t = 0 (the observation stays obs_0)
 tanh_approx        every tanh is off by a relative 2^-11 (tanh.approx.f32's grade)
 env_clean / rew_clean  the env step / the reward (and position) use the noise-free action
-swap_sign_noise    the + evaluation takes the - evaluation's noise and vice versa
-ep0_noise          every episode takes episode 0's noise
+swap_sign_noise    the + evaluation takes the - evaluation's noise run and vice versa (each at its own offset)
+ep0_noise          every episode reads its noise from offset 0, where episode 0 does
 no_reset_obs / no_reset_pos  an episode after the first continues from the previous one's last observation / position
 first_episode_outputs  behaviour and ObStat come from the first episode instead of the last
 """
@@ -162,15 +178,21 @@ def normalise(ob, mean, std, clip):
 
 def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a, env_b, rew_vec, pos_scale,
              act_noise=None, episodes: int = 1, pairs: Optional[Sequence[int]] = None, variants=(None,), obs0_shift=None,
-             activation=np.tanh):
+             activation=np.tanh, fall_height=None, binned=None):
     """The truth (variant None) and its variants for the pairs ``pairs`` (default: all).  ``variants``: mutations (tuples of
     ``mutations``) or None.  ``obs0_shift``: [V][obs] added to obs0 per variant (``growth``).  ``activation``: the policy's
-    float64 activation after every layer in place of tanh (tests/act_f64.py's forms), or a list of one per layer; the env's
-    own tanh stays.
+    float64 activation after every layer in place of tanh (f64_rollout's forms), or a list of one per layer; the env's
+    own tanh stays.  ``fall_height``: the env's h (None: no episode ends early, a NaN position included).  ``binned``:
+    (bins, low, high) of an FFBinned head, whose last layer has act * bins outputs.  ``act_noise``: [n_pairs][2][E T act]
+    (or any shape of that size).
 
-    Returns a dict of float64 arrays indexed [V][2][n] ([V][2][n][...] for vectors): 'fit', 'mass', 'behv' (3), 'mag' (3),
-    'osum', 'osq', 'oabs' (obs: the column sums of ob, ob^2 and |ob|) and, with ``obs0_shift``, 'dev' [V][2][n]: the largest
-    ||ob_v - ob_0|| over the steps and episodes."""
+    Returns a dict of arrays indexed [V][2][n] ([V][2][n][...] for vectors): float64 'fit', 'mass', 'behv' (3), 'mag' (3),
+    'osum', 'osq', 'oabs' (obs: the column sums of ob, ob^2 and |ob|), 'olast' (obs), 'gap' (the smallest | |z_t| - h | over
+    the executed steps: a position off by less decides every fall as the truth does; inf without h), 'margin' (a binned
+    head's smallest gap between a dimension's two largest outputs over the executed steps; inf without one), 'zmax' (the
+    largest |z_t| executed), 'z0' (|z| after the last episode's first step); int64 'steps' (the last episode's t_d), 'used'
+    (noise values consumed, sum_e (t_{d,e} + 1) act), 'eps' ([E]: every episode's t_d); and, with ``obs0_shift``, 'dev': the
+    largest ||ob_v - ob_0|| over the steps and episodes."""
     idx = np.asarray(idx)
     pairs = list(range(len(idx)) if pairs is None else pairs)
     T, act = rew_vec.shape
@@ -179,19 +201,17 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
     V = len(variants)
     N = 2 * len(pairs)
     layers = _weights(table, idx, theta, sigma, sizes, pairs)
-    acts = list(activation) if isinstance(activation, (list, tuple)) else [activation] * L
-    assert len(acts) == L
+    acts = [np.tanh] * L if binned is not None else f64.per_layer(activation, L)
     c = np.asarray(rew_vec, np.float64)
     B = np.asarray(env_b, np.float64)                      # [act][obs]: pre += a @ B
     A = _env_matrix(env_a, obs).T.copy()                   # pre += ob @ A
     mean = np.asarray(ob_mean, np.float64)
     std = np.asarray(ob_std, np.float64)
     ps = float(np.float32(pos_scale))
+    h_fall = None if fall_height is None else float(np.float32(fall_height))
+    nz_all = None                                          # [N][E T act]: each evaluation's flat run
     if act_noise is not None:
-        nz_all = np.asarray(act_noise, np.float32).reshape(len(idx), 2, E, T, act)
-        nz_all = nz_all[pairs].reshape(N, E, T, act).astype(np.float64)
-    else:
-        nz_all = None
+        nz_all = np.asarray(act_noise, np.float32).reshape(len(idx), 2, -1)[pairs].reshape(N, -1).astype(np.float64)
 
     # per-variant parameters
     def flag(name):
@@ -214,8 +234,6 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
             unpert[m[1]][v] = True
     alt_A = [(v, _env_matrix(env_a, obs, shift=1).T.copy() if m[0] == 'band_shift' else _env_matrix(env_a, obs, wrap=False).T.copy())
              for v, m in enumerate(variants) if m is not None and m[0] in ('band_shift', 'band_nowrap')]
-    B_alt = B.copy()
-    B_alt[-1] = 0.0
     b_last = flag('b_last_col')
     vmean = np.where(flag('no_mean')[:, None], 0.0, mean[None, :])            # [V][obs]
     vclip = np.where(flag('no_clip'), np.inf, float(clip))[None, :, None]     # [1][V][1]
@@ -223,7 +241,7 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
     drop_last, skip_first = flag('drop_last_step'), flag('skip_first_env_step')
     env_clean, rew_clean = flag('env_clean'), flag('rew_clean')
     no_reset_obs, no_reset_pos, first_out = flag('no_reset_obs'), flag('no_reset_pos'), flag('first_episode_outputs')
-    ep_src = np.where(flag('ep0_noise')[:, None], 0, np.arange(E)[None, :])    # [V][E]
+    ep0_noise = flag('ep0_noise')[None, :]                                     # [1][V]
     ev_src = np.where(flag('swap_sign_noise')[None, :], (np.arange(N) ^ 1)[:, None], np.arange(N)[:, None])  # [N][V]
     any_masks = [not np.all(m == 1.0) for m in act_mask], [not np.all(m == 1.0) for m in in_mask]
     o0 = np.broadcast_to(np.asarray(obs0, np.float64), (N, V, obs)).copy()
@@ -239,13 +257,22 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
     prev = [np.zeros((N, V, d)) for d in sizes[1:]]
     dev = np.zeros((N, V))
     cols = [0, 1 % act, 2 % act]
+    used = np.zeros((N, V), np.int64)
+    eps = np.zeros((N, V, E), np.int64)
+    gap, margin = np.full((N, V), np.inf), np.full((N, V), np.inf)
+    zmax, z0 = np.zeros((N, V)), np.zeros((N, V))
     for e in range(E):
         ob = np.where(no_reset_obs[None, :, None] & (e > 0), ob, o0)
         pos = np.where(no_reset_pos[None, :, None] & (e > 0), pos, 0.0)
         mag = np.zeros((N, V, 3))
         osum, osq, oabs = (np.zeros((N, V, obs)) for _ in range(3))
+        alive = np.ones((N, V), bool)
+        t_d = np.full((N, V), T - 1, np.int64)
+        start = np.where(ep0_noise, 0, used)                                     # [N][V]: this episode's noise offset
         for t in range(T):
-            live = ~(drop_last & (t == T - 1))                                  # [V]
+            if not alive.any():
+                break
+            run = alive & ~(drop_last & (t == T - 1))                           # [N][V]: the step is taken
             h = normalise(ob, vmean[None], std, vclip)
             for l, (WT, _, _) in enumerate(layers):
                 if any_masks[1][l]:
@@ -260,10 +287,18 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
                     h = nxt
                 else:
                     h = y
-            a = h                                                               # [N][V][act]
+            if binned is not None:
+                bins, low, high = binned
+                out = h.reshape(N, V, act, bins)
+                top = np.sort(out, axis=3)
+                margin = np.where(alive, np.minimum(margin, (top[..., -1] - top[..., -2]).min(axis=2)), margin)
+                lo = np.asarray(low, np.float64)
+                a = lo + (np.asarray(high, np.float64) - lo) * out.argmax(axis=3) / (bins - 1.0)
+            else:
+                a = h                                                           # [N][V][act]
             if nz_all is not None:
-                nz = nz_all[ev_src, ep_src[None, :, e], t]                       # [N][V][act]
-                if np.any(act_mask[L - 1] == 0.0):
+                nz = nz_all[ev_src[:, :, None], start[:, :, None] + t * act + np.arange(act)]    # [N][V][act]
+                if binned is None and any_masks[0][L - 1]:
                     nz = nz * act_mask[L - 1][None]                              # a row never written gets no noise either
                 an = a + nz
                 a_env = np.where(env_clean[None, :, None], a, an)
@@ -271,11 +306,13 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
             else:
                 a_env = a_rew = a
             prod = a_rew * c[t]
-            fit += np.where(live, prod.sum(axis=2), 0.0) / E
-            mass += np.where(live, np.abs(prod).sum(axis=2), 0.0) / E
-            term = ps * a_rew[:, :, cols] * live[None, :, None]
-            pos = pos + term
-            mag += np.abs(pos) + np.abs(term)
+            fit += np.where(run, prod.sum(axis=2), 0.0) / E
+            mass += np.where(run, np.abs(prod).sum(axis=2), 0.0) / E
+            term = ps * a_rew[:, :, cols] * run[:, :, None]
+            npos = pos + term
+            lv = alive[:, :, None]
+            mag = np.where(lv, mag + (np.abs(npos) + np.abs(term)), mag)
+            pos = np.where(lv, npos, pos)
             pre = ob @ A
             for v, Av in alt_A:
                 pre[:, v] = ob[:, v] @ Av
@@ -285,20 +322,33 @@ def simulate(table, idx, theta, sigma, sizes, ob_mean, ob_std, clip, obs0, env_a
             nob = np.tanh(pre) * tfac
             if t == 0:
                 nob = np.where(skip_first[None, :, None], ob, nob)
-            ob = np.where(live[None, :, None], nob, ob)
+            rv = run[:, :, None]
+            ob = np.where(rv, nob, ob)
             if obs0_shift is not None:
                 dev = np.maximum(dev, np.sqrt(((ob - ob[:, :1]) ** 2).sum(axis=2)))
-            lv = live[None, :, None]
-            osum += ob * lv
-            osq += ob * ob * lv
-            oabs += np.abs(ob) * lv
+            osum += ob * rv
+            osq += ob * ob * rv
+            oabs += np.abs(ob) * rv
+            zt = np.abs(pos[:, :, 2])
+            if t == 0:
+                z0 = zt
+            zmax = np.where(alive, np.maximum(zmax, zt), zmax)
+            fell = False
+            if h_fall is not None:
+                gap = np.where(alive, np.minimum(gap, np.abs(zt - h_fall)), gap)
+                fell = ~(zt <= h_fall)
+            ended = alive & (fell | (t == T - 1))
+            t_d[ended] = t
+            alive &= ~ended
+        eps[:, :, e] = t_d
+        used += (t_d + 1) * act
         out = dict(behv=pos.copy(), mag=mag, osum=osum, osq=osq, oabs=oabs, olast=ob.copy())
         if e == 0:
             first = out
         if e == E - 1:
             for k, val in out.items():
                 res[k] = np.where(first_out.reshape((1, V) + (1,) * (val.ndim - 2)), first[k], val)
-    res['fit'], res['mass'] = fit, mass
+    res.update(fit=fit, mass=mass, steps=t_d, used=used, eps=eps, gap=gap, margin=margin, zmax=zmax, z0=z0)
     if obs0_shift is not None:
         res['dev'] = dev
 
@@ -316,7 +366,8 @@ def truth(*args, **kw):
 
 def growth(*args, directions: int = 3, delta: float = 1e-9, seed: int = 0, **kw):
     """The largest ||dob_t|| / ||dob_0|| over the steps and episodes (and the evaluations) for obs0 moved by ``delta`` along a
-    few random directions: how far the loop carries a rounding difference."""
+    few random directions: how far the loop carries a rounding difference.  ``kw`` as ``simulate`` takes them (activation,
+    fall_height, binned, ...)."""
     obs = args[4][0]                                                           # sizes[0]
     rs = np.random.RandomState(seed)
     d = rs.randn(directions, obs)

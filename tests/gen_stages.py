@@ -13,10 +13,10 @@ near-tie that flips one rank cannot cascade into the checks of later stages:
   3 normalise   the normalised observations bit for bit against orc.normalise_obs with the generation's mean / std;
   4 fitness     every evaluation against float64 (``fitness_truth``: torch.float64 on the tensors' device, from the device's
                 indices, theta, normalised observations and action noise, with the policy's activation
-                ``Capture.activation`` in tests/act_f64.py's forms), judged by test_gpu_rollout_f64._check (EVAL_REL of
+                ``Capture.activation`` in tests/f64_rollout.py's forms), judged by test_gpu_rollout_f64._check (EVAL_REL of
                 the reward mass per evaluation, RMS_BOUND of the spread -- test_gpu_activations.RMS with an activation --,
                 behaviours within float32 rounding); the float64 truth tied to the plain CPU reference
-                tests/f64_rollout.rollout_f64 (act_f64.rollout_f64 with an activation) on sampled pairs to TIE_REL of the mass;
+                tests/f64_rollout.rollout_f64 (with the activation) on sampled pairs to TIE_REL of the mass;
   5 novelty     (archive) bit for bit against orc.novelty of the device's behaviours, in column 1 of the [pos|neg][k][2] rows;
   6 weights     bit for bit against orc.centered_ranker / orc.moo_ranker on the device's fitness, n_ranked equal; and against
                 the ranks of the float64 truth: how many ranks differ, the largest shift and the largest |dw| (bounded by
@@ -32,10 +32,10 @@ MultiObjective blend w r_0 + (1 - w) r_1 with w = ``moo_w``); a capture with an 
 
 The closed loop (``Capture.obs0`` given: ClosedLoopEnv's obs_0, A^T [band, obs], B^T [act, obs]) has no full-population truth:
   2 obstat      count and n_saved exact; sum and sumsq against the float64 truth's osum / osq of the saved evaluations within
-                test_gpu_closed_f64's bound (T ulps of their magnitude per saved evaluation plus OBS_ERR per observation);
+                closed_f64's bound (T ulps of their magnitude per saved evaluation plus OBS_ERR per observation);
   3 normalise   inside the rollout kernel: judged through the fitness;
   4 fitness     closed_f64.truth (with the policy's activation) on a sample (``closed_sample``: every saved evaluation, the first and last pair of each
-                stream, random pairs up to about 64 evaluations), with test_gpu_closed_f64's bounds, after closed_f64.growth
+                stream, random pairs up to about 64 evaluations), with closed_f64's bounds, after closed_f64.growth
                 has shown that the sample does not amplify rounding (<= GROWTH_BOUND);
   6 weights     exact against the oracle on the device's fitness; the ranks against the truth are not compared (reported).
 
@@ -58,12 +58,10 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from oracle import es_oracle as orc  # noqa: E402
-import act_f64  # noqa: E402
 import closed_f64 as cf  # noqa: E402
 import f64_rollout as f64  # noqa: E402
 import rc_f64 as rc  # noqa: E402
 import test_gpu_activations as act_bounds  # noqa: E402
-import test_gpu_closed_f64 as closed_bounds  # noqa: E402
 import test_gpu_noise_table as noise_criterion  # noqa: E402
 import test_gpu_rollout_f64 as rollout_f64  # noqa: E402
 
@@ -335,7 +333,7 @@ def _truth_columns(truth, saved: np.ndarray):
 
 def _stage_obstat_closed(cap: Capture, truth) -> List[Check]:
     """Every evaluation's ObStat increment is its own post-step observations (obs_1 .. obs_T of the last episode): count and
-    n_saved exact, the sums within test_gpu_closed_f64's bound of the truth's (the device adds them with float64 atomics,
+    n_saved exact, the sums within closed_f64's bound of the truth's (the device adds them with float64 atomics,
     in no fixed order)."""
     obs, T = cap.obs_dim, cap.T
     saved = replayed_saves(cap)
@@ -345,8 +343,8 @@ def _stage_obstat_closed(cap: Capture, truth) -> List[Check]:
     U, ns = 2.0 ** -24, max(1, n_saved)
     want_s = truth['osum'][s_idx, j_idx].sum(axis=0)
     want_q = truth['osq'][s_idx, j_idx].sum(axis=0)
-    bound_s = 2 * T * U * truth['oabs'][s_idx, j_idx].sum(axis=0) + closed_bounds.OBS_ERR * T * ns
-    bound_q = 2 * T * U * want_q + 2 * closed_bounds.OBS_ERR * T * ns
+    bound_s = 2 * T * U * truth['oabs'][s_idx, j_idx].sum(axis=0) + cf.OBS_ERR * T * ns
+    bound_q = 2 * T * U * want_q + 2 * cf.OBS_ERR * T * ns
     rs = float((np.abs(cap.stats[:obs] - want_s) / bound_s).max())
     rq = float((np.abs(cap.stats[obs:2 * obs] - want_q) / bound_q).max())
     return [Check('obstat', 'sum err/bound against the float64 truth', rs, 1.0, rs <= 1.0),
@@ -368,14 +366,14 @@ ACT_BYTES = 2 ** 29       # fitness_truth: the float64 activations of one layer 
 
 
 def layer_forms(cap: Capture, xp=np) -> list:
-    """The float64 activation of every layer of ``cap``'s policy (act_f64.form of ``cap.activation``; tanh for None), for
+    """The float64 activation of every layer of ``cap``'s policy (f64_rollout.form of ``cap.activation``; tanh for None), for
     numpy arrays or (``xp=torch``) torch tensors."""
-    return [act_f64.form(cap.activation, xp)] * (len(cap.sizes) - 1)
+    return [f64.form(cap.activation, xp)] * (len(cap.sizes) - 1)
 
 
 def fitness_truth(cap: Capture, chunk: Optional[int] = None, behaviour_episode: int = -1, noise=None, acts=None):
     """(fitness [2, K], behaviour [2, K, 3], reward mass [2, K], position magnitude [2, K, 3]) in float64 (f64_rollout's
-    definitions, with the policy's activation in act_f64's forms), computed with torch.float64 on the table's device in
+    definitions, with the policy's activation in its forms), computed with torch.float64 on the table's device in
     chunks of pairs: a measurement reference.  The forward pass is shared by the E episodes (only the noise differs); fitness
     and mass are the per-step means over them, behaviour and magnitude the episode ``behaviour_episode``'s.  ``chunk``
     (default: up to 200 pairs, fewer where one layer's activations over T steps would pass ACT_BYTES); ``noise``: in place of
@@ -471,7 +469,7 @@ def closed_truth(cap: Capture, pairs: Optional[Sequence[int]] = None, growth: bo
 
 
 def _stage_fitness_closed(cap: Capture, truth) -> List[Check]:
-    """The sampled evaluations against the float64 truth, with test_gpu_closed_f64._check's bounds."""
+    """The sampled evaluations against the float64 truth, with closed_f64's bounds (test_gpu_closed_f64._check's)."""
     pairs = truth['pairs']
     U = 2.0 ** -24
     f = cap.fit[:, pairs, 0]
@@ -483,10 +481,10 @@ def _stage_fitness_closed(cap: Capture, truth) -> List[Check]:
     g = truth['growth']
     out = [Check('fitness', 'closed loop: growth of a 1e-9 move of obs_0 (the sample is not chaotic)', g, GROWTH_BOUND,
                  g <= GROWTH_BOUND, f'{2 * len(pairs)} evaluations sampled'),
-           Check('fitness', 'max err/mass', worst, closed_bounds.EVAL_REL, worst <= closed_bounds.EVAL_REL),
-           Check('fitness', 'rms/spread', rms / spread, closed_bounds.RMS_BOUND, rms <= closed_bounds.RMS_BOUND * spread)]
+           Check('fitness', 'max err/mass', worst, cf.EVAL_REL, worst <= cf.EVAL_REL),
+           Check('fitness', 'rms/spread', rms / spread, cf.RMS_BOUND, rms <= cf.RMS_BOUND * spread)]
     if cap.behv is not None:
-        tol = 2 * U * truth['mag'] + closed_bounds.ACT_ERR * float(np.float32(cap.pos_scale)) * cap.T
+        tol = 2 * U * truth['mag'] + cf.ACT_ERR * float(np.float32(cap.pos_scale)) * cap.T
         r = float((np.abs(cap.behv[:, pairs] - truth['behv']) / tol).max())
         out.append(Check('fitness', 'behaviour err/tol', r, 1.0, r <= 1.0))
     cap.extra['fitness'] = dict(sampled_evaluations=2 * len(pairs), rms_over_spread=rms / spread, max_err_over_mass=worst,
@@ -541,11 +539,8 @@ def stage_fitness(cap: Capture, mode: int, truth, tie: Optional[Sequence[int]] =
     if cap.ac_std:
         noise = np.stack([_np(cap.act_noise[k]) for k in tie])
     tie_args = (table_np, np.arange(len(tie)) * P, cap.theta0, cap.sigma, cap.sizes, cap.obsn, cap.rew_vec, cap.pos_scale)
-    if cap.activation is None:
-        cf, cb, cm, cmag = f64.rollout_f64(*tie_args, noise, cap.episodes)
-    else:
-        cf, cb, cm, cmag = act_f64.rollout_f64(*tie_args, act_f64.form(cap.activation), noise, cap.episodes)
-    rel = float(max((np.abs(cf - tf[:, tie]) / cm).max(), (np.abs(cb - tb[:, tie]) / np.maximum(cmag, 1e-300)).max()))
+    rf, rb, rm, rmag = f64.rollout_f64(*tie_args, noise, cap.episodes, activation=f64.form(cap.activation))
+    rel = float(max((np.abs(rf - tf[:, tie]) / rm).max(), (np.abs(rb - tb[:, tie]) / np.maximum(rmag, 1e-300)).max()))
     out.append(Check('fitness', f'float64 truth vs CPU reference ({2 * len(tie)} evaluations), rel', rel, TIE_REL, rel <= TIE_REL))
     return out
 
@@ -874,7 +869,7 @@ def _act_forms_bug(c: Capture, which: str, xp) -> list:
         acts[0] = xp.tanh
     elif which == 'default_param':
         default = {_lib.ES_ACT_LEAKY_RELU: 0.01, _lib.ES_ACT_ELU: 1.0}[int(c.activation.kind)]
-        acts = [act_f64.form(Activation(c.activation.kind, default), xp)] * len(acts)
+        acts = [f64.form(Activation(c.activation.kind, default), xp)] * len(acts)
     else:
         acts[-1] = lambda z: z
     return acts

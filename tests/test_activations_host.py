@@ -7,8 +7,8 @@
   networks ``activation`` describes;
 * the Activation alone rebuilds the network's arithmetic: a forward through the torch module it names equals the module's own
   forward bit for bit (what the GPU tests take as the float32 truth);
-* the float64 truth of the GPU tests (tests/act_f64.py) is f64_rollout's and closed_f64's with np.tanh, and its activation
-  forms are torch's in float64;
+* the float64 truths of the GPU tests (tests/f64_rollout.py, tests/closed_f64.py) with each activation's form are the
+  float32 forward through torch's modules to float32 rounding, and the forms are torch's in float64;
 * the new sources compile for sm_90a without spills or serialised wgmma, within the closed-loop plan's static shared memory;
 * the entry points are declared, bound and exported, and the kinds match the header.
 """
@@ -221,17 +221,18 @@ def test_activation_entry_points_are_declared_bound_and_built():
 def _f64_helpers():
     import sys
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    import act_f64
     import closed_f64
     import f64_rollout
-    return act_f64, closed_f64, f64_rollout
+    return closed_f64, f64_rollout
 
 
 @pytest.mark.parametrize('E,noisy', [(1, False), (3, True)])
 def test_float64_truth_with_tanh_is_the_tanh_truth(E, noisy):
-    """act_f64 with np.tanh reproduces f64_rollout (open loop) and closed_f64 (closed loop): the GPU tests' bounds, built on
-    those, carry over to the other activations."""
-    act_f64, closed_f64, f64_rollout = _f64_helpers()
+    """Open loop: the float64 truth with every kind's form is the float32 forward through torch's own modules to float32
+    rounding (fitness and behaviour, per evaluation).  Closed loop: tanh given per layer is the default bit for bit, and
+    another activation changes the policy, not the env: a ReLU truth differs."""
+    from es_pytorch_b200.nn.nn import Activation
+    closed_f64, f64_rollout = _f64_helpers()
     rs = np.random.RandomState(4)
     sizes, T, n = [9, 16, 12, 4], 7, 3
     P = f64_rollout.n_params(sizes)
@@ -241,27 +242,36 @@ def test_float64_truth_with_tanh_is_the_tanh_truth(E, noisy):
     obsn = rs.randn(T, sizes[0]).astype(np.float32)
     rew = rs.randn(T, sizes[-1]).astype(np.float32)
     noise = (rs.randn(n, 2, E, T, sizes[-1]) * 0.1).astype(np.float32) if noisy else None
-    want = f64_rollout.rollout_f64(table, idx, theta, 0.02, sizes, obsn, rew, 0.05, noise, E)
-    got = act_f64.rollout_f64(table, idx, theta, 0.02, sizes, obsn, rew, 0.05, np.tanh, noise, E)
-    for g, w in zip(got, want):
-        np.testing.assert_allclose(g, w, rtol=1e-13, atol=1e-15)
+    c, cols = rew.astype(np.float64), [j % sizes[-1] for j in range(3)]
+    for _, kind, param in KINDS:
+        act = Activation(kind, param)
+        fit, behv, mass, mag = f64_rollout.rollout_f64(table, idx, theta, 0.02, sizes, obsn, rew, 0.05, noise, E,
+                                                       activation=f64_rollout.form(act))
+        for k in range(n):
+            for s, sign in enumerate((1.0, -1.0)):
+                w = f64_rollout.perturbed(table, idx[k], theta, 0.02, sign).astype(np.float32)
+                a = mlp_forward(w, sizes, obsn, act).numpy().astype(np.float64)
+                nz = np.zeros((1, T, sizes[-1])) if noise is None else noise[k, s].astype(np.float64)
+                f32_fit = np.mean([((a + z) * c).sum() for z in nz])
+                f32_behv = 0.05 * (a + nz[-1])[:, cols].sum(axis=0)
+                assert abs(f32_fit - fit[s, k]) <= 1e-6 * mass[s, k], (kind, k, s)
+                assert np.all(np.abs(f32_behv - behv[s, k]) <= 1e-6 * mag[s, k]), (kind, k, s)
     band = 4
     args = (table, idx, theta, 0.02, sizes, rs.randn(sizes[0]) * 0.1, 0.5 + rs.rand(sizes[0]), 1.0,
             rs.randn(sizes[0]).astype(np.float32), (rs.randn(band, sizes[0]) * 0.4).astype(np.float32),
             (rs.randn(sizes[-1], sizes[0]) * 0.4).astype(np.float32), rew, 0.05)
     want = closed_f64.truth(*args, act_noise=noise, episodes=E)
-    got = act_f64.closed_truth(*args, act_noise=noise, episodes=E)
-    for k in ('fit', 'mass', 'behv', 'mag', 'osum', 'osq', 'oabs'):
-        np.testing.assert_allclose(got[k], want[k], rtol=1e-13, atol=1e-15, err_msg=k)
-    # another activation changes the policy, not the env: a ReLU truth differs
-    relu = act_f64.closed_truth(*args, act_noise=noise, episodes=E, activation=act_f64.relu)
+    got = closed_f64.truth(*args, act_noise=noise, episodes=E, activation=[np.tanh] * (len(sizes) - 1))
+    for k in want:
+        assert np.array_equal(got[k], want[k]), k
+    relu = closed_f64.truth(*args, act_noise=noise, episodes=E, activation=f64_rollout.relu)
     assert not np.allclose(relu['fit'], want['fit'])
 
 
 def test_float64_activation_forms_match_torch_in_float64():
-    act_f64, _, _ = _f64_helpers()
+    _, f64_rollout = _f64_helpers()
     z = np.linspace(-30, 30, 2001)
     t = torch.from_numpy(z)
-    for f, m in ((act_f64.relu, torch.nn.ReLU()), (act_f64.leaky_relu(0.1), torch.nn.LeakyReLU(float(np.float32(0.1)))),
-                 (act_f64.elu(0.7), torch.nn.ELU(float(np.float32(0.7)))), (act_f64.sigmoid, torch.nn.Sigmoid())):
+    for f, m in ((f64_rollout.relu, torch.nn.ReLU()), (f64_rollout.leaky_relu(0.1), torch.nn.LeakyReLU(float(np.float32(0.1)))),
+                 (f64_rollout.elu(0.7), torch.nn.ELU(float(np.float32(0.7)))), (f64_rollout.sigmoid, torch.nn.Sigmoid())):
         np.testing.assert_allclose(f(z), m(t).numpy(), rtol=1e-14, atol=1e-300)

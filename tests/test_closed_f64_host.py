@@ -123,7 +123,7 @@ def test_truth_at_sigma_zero_matches_the_float32_oracle(p):
     rews, bh, ob, _ = _oracle(p, d, 0, 0, sigma=0.0)
     assert abs(sum(rews) - tr['fit'][0, 0]) <= 1e-6 * tr['mass'][0, 0]
     assert np.abs(np.array(bh[-3:]) - tr['behv'][0, 0]).max() <= 2 * cf.U * tr['mag'][0, 0].max() + 1e-7 * p.T
-    assert np.abs(ob.astype(np.float64).sum(axis=0) - tr['osum'][0, 0]).max() <= G.OBS_ERR * p.T
+    assert np.abs(ob.astype(np.float64).sum(axis=0) - tr['osum'][0, 0]).max() <= cf.OBS_ERR * p.T
 
 
 def _groups():
@@ -151,11 +151,10 @@ def test_every_mutation_fails_some_problem_of_each_shape(key):
 
 
 def test_the_observation_clip_is_torch_clamp():
-    """The oracle's normalise_obs and the float64 truths' clip (closed_f64.normalise, which act_f64 uses too) against torch.clamp
+    """The oracle's normalise_obs and the float64 truth's clip (closed_f64.normalise) against torch.clamp
     (nn.py:45): a NaN stays NaN, +-inf becomes +-clip, +-clip and the values next to it are exact.  The GPU tests of a NaN
     in the observation mean compare against these."""
     import torch
-    import act_f64
     clip = 5.0
     x = np.array([np.nan, np.inf, -np.inf, clip, -clip, np.nextafter(clip, 9), np.nextafter(-clip, -9), np.nextafter(clip, 0),
                   0.0, -0.0, 1e30, -1e-30])
@@ -167,7 +166,7 @@ def test_the_observation_clip_is_torch_clamp():
     got32 = orc.normalise_obs(ob, np.zeros_like(x), np.ones_like(x), clip)
     want32 = torch.clamp(torch.from_numpy(ob).double(), -clip, clip).float().numpy()
     assert np.array_equal(got32, want32, equal_nan=True)
-    # a NaN in the mean, and an infinite one, through both closed-loop truths: every fitness NaN / every fitness finite
+    # a NaN in the mean, and an infinite one, through the closed-loop truth: every fitness NaN / every fitness finite
     sizes, T = [4, 3, 2], 3
     P = orc.n_params(orc.layer_dims(4, [3], 2))
     rs = np.random.RandomState(0)
@@ -176,5 +175,5 @@ def test_the_observation_clip_is_torch_clamp():
     for m, finite in (([np.nan, 0, 0, 0], False), ([np.inf, -np.inf, 0, 0], True)):
         args = (table, idx, theta, 0.02, sizes, np.array(m), np.ones(4), clip, spec.obs_stream[0], spec.env_a.T, spec.env_b.T,
                 spec.rew_vec, spec.pos_scale)
-        for f in (cf.truth(*args)['fit'], act_f64.closed_truth(*args)['fit']):
-            assert (np.isfinite(f) if finite else np.isnan(f)).all(), f
+        f = cf.truth(*args)['fit']
+        assert (np.isfinite(f) if finite else np.isnan(f)).all(), f

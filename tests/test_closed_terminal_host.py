@@ -4,11 +4,14 @@
 * run_model's python loop on a terminating env against a restatement from the oracle's env and forward: rewards, t_d, the
   padded behaviour and the observation rows;
 * obj.py's E-episode fold (BatchedRollout's python route) with a last episode shorter than an earlier one;
+* the float64 truth (tests/closed_f64.py): a fall height nothing reaches is no fall height, for the truth and every modelled
+  bug, and a NaN position ends an episode only when there is a fall height;
 * argument validation, and the new entry points' declarations and bindings (the cluster kernel's compilation for sm_90a is
   checked in test_host_ptxas_closed_wide.py)."""
 import os
 import re
 import sys
+from typing import Optional
 
 import numpy as np
 import pytest
@@ -17,10 +20,41 @@ import torch
 from oracle import es_oracle as orc
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import closed_terminal_f64 as ctf  # noqa: E402
+import closed_f64 as cf  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32 = np.float32
+
+
+def run_model_loop(env, model_fn, max_steps: int, rs: Optional[np.random.RandomState] = None, ac_std: float = 0.0):
+    """run_model's python loop (gym_runner.py:33-67) restated on a ClosedLoopEnv-like ``env`` with the float32 forward
+    ``model_fn(ob) -> action``: every step adds ``rs.randn(act) * ac_std`` when given, steps the env, records the reward,
+    the observation and the position, and breaks on done; the behaviour is padded with the last position.  Returns (rews,
+    behv, obs [steps][obs], step)."""
+    behv, rews, obs = [], [], []
+    ob = env.reset()
+    step = 0
+    for step in range(max_steps):
+        a = np.asarray(model_fn(ob), dtype=F32)
+        if rs is not None and ac_std != 0:
+            a = (a.astype(np.float64) + rs.randn(a.shape[0]) * ac_std).astype(F32)
+        ob, rew, done, _ = env.step(a)
+        rews.append(rew)
+        obs.append(ob)
+        behv.extend(float(x) for x in env.pos)
+        if done:
+            break
+    behv += behv[-3:] * (max_steps - len(behv) // 3)
+    return rews, behv, np.array(obs), step
+
+
+def episodes_fold(episode_rewards, max_steps: int):
+    """obj.py:56-61: ``rews = zeros(max_steps); rews[:len(rew)] += rew`` per episode in order, ``rews /= E``."""
+    rews = np.zeros(max_steps)
+    for rew in episode_rewards:
+        rews[:len(rew)] += np.array(rew)
+    rews /= max(1, len(episode_rewards))
+    return rews
 
 
 def _env(T=40, h=None, obs=15, act=3, **kw):
@@ -165,7 +199,7 @@ def test_fold_of_episodes_where_the_last_is_shorter():
             break
     assert found is not None
     seed, eps = found
-    want = ctf.episodes_fold([e[0] for e in eps], T)
+    want = episodes_fold([e[0] for e in eps], T)
     br = BatchedRollout(env, T, coins_per_eval=0, episodes=E)
     rs = np.random.RandomState(seed)
     rews, behv, steps = br._run_episodes(model, rs, E)
@@ -183,7 +217,7 @@ def test_restated_loop_matches_the_packages_run_model_with_noise():
     a, b = np.random.RandomState(4), np.random.RandomState(4)
     got = run_model(model, env, T, a)
     fwd = lambda ob: model(torch.from_numpy(np.asarray(ob)).float(), rs=None).detach().numpy()
-    want = ctf.run_model_loop(env, fwd, T, b, 0.2)
+    want = run_model_loop(env, fwd, T, b, 0.2)
     assert got[3] == want[3] and got[0] == want[0] and got[1] == want[1]
     sa, sb = a.get_state(), b.get_state()
     assert np.array_equal(sa[1], sb[1]) and sa[2:] == sb[2:]
@@ -198,6 +232,37 @@ def test_coin_words_are_the_words_random_consumes():
         assert orc.words_to_double(int(w[0]), int(w[1])) == b.random()
         sa, sb = a.get_state(), b.get_state()
         assert np.array_equal(sa[1], sb[1]) and sa[2:] == sb[2:]
+
+
+# ---------------------------------------------------------------------------------------------- the float64 truth
+def test_fall_height_nothing_reaches_is_no_fall_height():
+    """closed_f64.simulate at h = 1e30 is its fall_height=None result bit for bit, for the truth and every modelled bug, with
+    action noise over E = 3 episodes.  A NaN in ob_mean makes the position NaN from step 0: without a fall height every
+    episode still runs T steps, with one every episode ends at step 0."""
+    sizes, band, T, n, E = [15, 32, 32, 3], 4, 40, 3, 3
+    act = sizes[-1]
+    P = orc.n_params(orc.layer_dims(sizes[0], sizes[1:-1], act))
+    rs = np.random.RandomState(6)
+    table = rs.randn(P + 1000).astype(F32)
+    theta = np.concatenate([rs.randn(fi * fo + fo) / np.sqrt(fi) for fi, fo in zip(sizes[:-1], sizes[1:])]).astype(F32)
+    spec = orc.ClosedLoopEnvSpec(sizes[0], act, T, band=band)
+    idx, mean, std = rs.randint(0, 1000, size=n), rs.randn(sizes[0]) * 0.05, 0.5 + rs.rand(sizes[0])
+    args = lambda mean: (table, idx, theta, 0.02, sizes, mean, std, 1.0, spec.obs_stream[0].copy(),
+                         np.ascontiguousarray(spec.env_a.T), np.ascontiguousarray(spec.env_b.T), spec.rew_vec, spec.pos_scale)
+    kw = dict(act_noise=(rs.randn(n, 2, E * T * act) * 0.3).astype(F32), episodes=E)
+    variants = [None] + cf.mutations(sizes, band, True, E)
+    free = cf.simulate(*args(mean), variants=variants, **kw)
+    high = cf.simulate(*args(mean), variants=variants, fall_height=1e30, **kw)
+    assert free.keys() == high.keys()
+    for k in free:
+        if k != 'gap':                                   # |z - h|: inf without a height
+            assert np.array_equal(free[k], high[k]), k
+    assert (free['steps'] == T - 1).all() and (free['used'] == E * T * act).all()
+    mean[1] = np.nan
+    free, fall = cf.truth(*args(mean), **kw), cf.truth(*args(mean), fall_height=1e30, **kw)
+    assert np.isnan(free['fit']).all() and np.isnan(free['z0']).all()
+    assert (free['eps'] == T - 1).all() and (free['used'] == E * T * act).all()
+    assert (fall['eps'] == 0).all() and (fall['used'] == E * act).all()
 
 
 # ---------------------------------------------------------------------------------------------- C ABI

@@ -186,8 +186,9 @@ def test_judge_rejects_activation_bugs_in_the_closed_loop(name):
 def test_activation_of_tanh_is_the_tanh_truth():
     """A capture whose activation is tanh gets the truths of one without (no activation): open loop with episodes and
     action noise, closed loop with its growth, to 1e-13 relative; and the closed loop's truth with another activation is
-    tests/act_f64.closed_truth's."""
-    import act_f64
+    closed_f64.truth's of the sampled pairs, sliced from the table by hand."""
+    import closed_f64
+    import f64_rollout
     tanh = _act('ES_ACT_TANH', 0.0)
     cap = _cap('episodes')
     for want, got in zip(gs.fitness_truth(cap), gs.fitness_truth(gs._copy(cap, activation=tanh))):
@@ -203,8 +204,8 @@ def test_activation_of_tanh_is_the_tanh_truth():
     pairs = got['pairs']
     P = c.P
     table = np.concatenate([c.table[int(c.idx[k]):int(c.idx[k]) + P].numpy() for k in pairs])
-    want = act_f64.closed_truth(table, np.arange(len(pairs)) * P, c.theta0, c.sigma, c.sizes, c.ob_mean, c.ob_std, c.ob_clip,
-                                c.obs0, c.env_a, c.env_b, c.rew_vec, c.pos_scale, activation=act_f64.elu(0.7))
+    want = closed_f64.truth(table, np.arange(len(pairs)) * P, c.theta0, c.sigma, c.sizes, c.ob_mean, c.ob_std, c.ob_clip,
+                            c.obs0, c.env_a, c.env_b, c.rew_vec, c.pos_scale, activation=f64_rollout.elu(0.7))
     for k in ('fit', 'mass', 'behv', 'mag', 'osum', 'osq', 'oabs'):     # sums in another order: relative to their largest
         np.testing.assert_allclose(got[k], want[k], rtol=1e-13, atol=1e-13 * np.abs(want[k]).max(), err_msg=k)
     assert not np.allclose(got['fit'], gs.closed_truth(cap, pairs=pairs, growth=False)['fit'])

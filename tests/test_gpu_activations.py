@@ -2,9 +2,9 @@
 
 * open loop, ES_ROLLOUT_F32 (the general float32 kernel) and ES_ROLLOUT_TC3 (the wide tensor-core kernel's code) at the
   shipped shapes, judged as the tanh kernels are (test_gpu_rollout_f64's EVAL_REL / RMS_BOUND / ACT_ERR against
-  act_f64, f64_rollout's truth with the float64 activation); action noise and episodes, T = 1 and partial tiles, sigma = 0, pair counts
+  f64_rollout's truth with the float64 activation); action noise and episodes, T = 1 and partial tiles, sigma = 0, pair counts
   around the SM count and multi-launch float32 chunks;
-* closed loop at clusters of 1, 2 and 4 CTAs against act_f64.closed_truth (closed_f64's, with the activation; test_gpu_closed_f64's
+* closed loop at clusters of 1, 2 and 4 CTAs against closed_f64.truth with the activation (test_gpu_closed_f64's
   bounds), ObStat sums included;
 * launch edges: TC3 around its launch chunk, F32 with 8 ragged layers and around the switch to staged weights (H = 196 ..
   198), the wide kernel's layer shapes (widths 192 and mixed, act 32, obs 1 and 256, four hidden layers), the closed loop in
@@ -31,7 +31,6 @@ from es_pytorch_b200 import _lib
 from es_pytorch_b200.nn.nn import Activation
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import act_f64  # noqa: E402
 import f64_rollout as f64  # noqa: E402
 from test_gpu_rollout_f64 import ACT_ERR, EVAL_REL, RMS_BOUND, U, Case, _sample  # noqa: E402
 import closed_f64  # noqa: E402
@@ -43,10 +42,10 @@ pytestmark = pytest.mark.gpu
 
 F32, TC, TC3 = _lib.ES_ROLLOUT_F32, _lib.ES_ROLLOUT_TC, _lib.ES_ROLLOUT_TC3
 ACTS = {
-    'relu': (Activation(_lib.ES_ACT_RELU, 0.0), act_f64.relu),
-    'leaky': (Activation(_lib.ES_ACT_LEAKY_RELU, float(np.float32(0.1))), act_f64.leaky_relu(0.1)),
-    'elu': (Activation(_lib.ES_ACT_ELU, float(np.float32(0.7))), act_f64.elu(0.7)),
-    'sigmoid': (Activation(_lib.ES_ACT_SIGMOID, 0.0), act_f64.sigmoid),
+    'relu': (Activation(_lib.ES_ACT_RELU, 0.0), f64.relu),
+    'leaky': (Activation(_lib.ES_ACT_LEAKY_RELU, float(np.float32(0.1))), f64.leaky_relu(0.1)),
+    'elu': (Activation(_lib.ES_ACT_ELU, float(np.float32(0.7))), f64.elu(0.7)),
+    'sigmoid': (Activation(_lib.ES_ACT_SIGMOID, 0.0), f64.sigmoid),
 }
 TANH = Activation(_lib.ES_ACT_TANH, 0.0)
 # rms error over the checked evaluations relative to their fitness spread, about twice the largest value measured on an H100
@@ -104,8 +103,8 @@ class ActCase(Case):
 
     def truth(self, pairs, f64act=None):
         """``f64act``: in place of the policy's float64 activation (one function, or a list of one per layer)."""
-        return act_f64.rollout_f64(self.table, self.idx, self.theta, self.sigma, self.sizes, self.obsn, self.rew, self.ps,
-                                   self.f64act if f64act is None else f64act, self.noise, self.E, pairs)
+        return f64.rollout_f64(self.table, self.idx, self.theta, self.sigma, self.sizes, self.obsn, self.rew, self.ps,
+                               self.noise, self.E, pairs, activation=self.f64act if f64act is None else f64act)
 
 
 def _check(tag, mode, case, f, b, pairs, rms_check=True, truth=None):
@@ -241,7 +240,7 @@ def _mutated_forms(name, which):
     """The policy's float64 activation per layer, evaluated wrongly on purpose (tests/gen_stages.py's modelled bugs)."""
     act, f = ACTS[name]
     if which == 'default_param':
-        return {'leaky': act_f64.leaky_relu(0.01), 'elu': act_f64.elu(1.0)}[name]
+        return {'leaky': f64.leaky_relu(0.01), 'elu': f64.elu(1.0)}[name]
     return lambda n_layers: ([np.tanh] + [f] * (n_layers - 1) if which == 'tanh_layer' else [f] * (n_layers - 1) + [lambda z: z])
 
 
@@ -287,12 +286,12 @@ def _place_in_sigmoid_tails(theta, sizes, rs):
 # digit) or None)
 SMALL = np.float32(3e-4)
 REGIMES = {
-    'sigmoid_tails': (Activation(_lib.ES_ACT_SIGMOID, 0.0), act_f64.sigmoid, 'tails'),
+    'sigmoid_tails': (Activation(_lib.ES_ACT_SIGMOID, 0.0), f64.sigmoid, 'tails'),
     'elu_near_zero': (ACTS['elu'][0], ACTS['elu'][1], 'small'),
-    'leaky_slope_0': (Activation(_lib.ES_ACT_LEAKY_RELU, 0.0), act_f64.leaky_relu(0.0), None),
-    'leaky_slope_-0.5': (Activation(_lib.ES_ACT_LEAKY_RELU, -0.5), act_f64.leaky_relu(-0.5), None),
-    'leaky_slope_3': (Activation(_lib.ES_ACT_LEAKY_RELU, 3.0), act_f64.leaky_relu(3.0), None),
-    'elu_alpha_0': (Activation(_lib.ES_ACT_ELU, 0.0), act_f64.elu(0.0), None),
+    'leaky_slope_0': (Activation(_lib.ES_ACT_LEAKY_RELU, 0.0), f64.leaky_relu(0.0), None),
+    'leaky_slope_-0.5': (Activation(_lib.ES_ACT_LEAKY_RELU, -0.5), f64.leaky_relu(-0.5), None),
+    'leaky_slope_3': (Activation(_lib.ES_ACT_LEAKY_RELU, 3.0), f64.leaky_relu(3.0), None),
+    'elu_alpha_0': (Activation(_lib.ES_ACT_ELU, 0.0), f64.elu(0.0), None),
 }
 
 
@@ -450,7 +449,7 @@ def test_closed_loop_against_float64(eng, name, shape, C, noisy):
     got = _closed_run(eng, p, d, act)
     assert got[5] == 1                                                        # one launch
     args, kw = cf.truth_args(p, d)
-    tr = act_f64.closed_truth(*args, activation=f64act, **kw)
+    tr = closed_f64.truth(*args, activation=f64act, **kw)
     cf._check(f'{name} {shape}', p, got[:5], tr, d['saved'], d['spec'].pos_scale)
     again = _closed_run(eng, p, d, act)
     assert np.array_equal(got[0], again[0]) and np.array_equal(got[1], again[1]) and np.array_equal(got[4], again[4])
@@ -490,7 +489,7 @@ def test_closed_loop_clusters_and_pair_order(eng, name, shape, band, C, T):
     got = _closed_run(eng, p, d, act)
     assert got[5] == 1
     args, kw = cf.truth_args(p, d)
-    tr = act_f64.closed_truth(*args, activation=f64act, **kw)
+    tr = closed_f64.truth(*args, activation=f64act, **kw)
     cf._check(f'{name} {shape}', p, got[:5], tr, d['saved'], d['spec'].pos_scale)
     rev = _closed_run(eng, p, _reversed(p, d), act)
     assert np.array_equal(got[0], rev[0][:, ::-1]) and np.array_equal(got[1], rev[1][:, ::-1]), 'the reversed run differs'
@@ -514,7 +513,7 @@ def test_closed_loop_activation_regimes(eng, regime):
     growth = closed_f64.growth(*args, activation=form, **kw)
     assert growth <= 100, growth
     got = _closed_run(eng, p, d, act)
-    tr = act_f64.closed_truth(*args, activation=form, **kw)
+    tr = closed_f64.truth(*args, activation=form, **kw)
     cf._check(f'closed {regime} (growth {growth:.3g})', p, got[:5], tr, d['saved'], d['spec'].pos_scale)
 
 

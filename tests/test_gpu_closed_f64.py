@@ -39,15 +39,11 @@ from oracle import es_oracle as orc
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import closed_f64 as cf  # noqa: E402
+from closed_f64 import ACT_ERR, EVAL_REL, OBS_ERR, RMS_BOUND, U  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24
 SIGMA = 0.02
-EVAL_REL = 1e-5
-RMS_BOUND = 3e-4
-ACT_ERR = 1e-5
-OBS_ERR = 1e-6
 
 
 class Problem(NamedTuple):
@@ -254,7 +250,7 @@ _NAN_FAMILIES = [('one_cta', (17, 64, 64, 6), None, 0), ('wide', (15, 256, 256, 
 @pytest.mark.parametrize('loop', ['open', 'closed'])
 @pytest.mark.parametrize('name,sizes,act_kind,bins', _NAN_FAMILIES, ids=[f[0] for f in _NAN_FAMILIES])
 def test_nan_in_the_observation_mean_reaches_the_fitness(eng, name, sizes, act_kind, bins, loop):
-    import act_f64
+    import f64_rollout as f64
     from es_pytorch_b200 import _lib
     from es_pytorch_b200.nn.nn import Activation, BinnedHead
     sizes, T, n = list(sizes), 30, 3
@@ -262,7 +258,7 @@ def test_nan_in_the_observation_mean_reaches_the_fitness(eng, name, sizes, act_k
     adim = sizes[-1] // bins if bins else sizes[-1]
     head = BinnedHead(bins, np.float32([-1.0, 0.0, 0.5]), np.float32([1.0, 2.0, 0.75])) if bins else None
     activation = Activation(_lib.ES_ACT_RELU, 0.0) if act_kind else None
-    f64_act = act_f64.relu if act_kind else np.tanh
+    f64_act = f64.relu if act_kind else np.tanh
     P = orc.n_params(orc.layer_dims(obs, sizes[1:-1], sizes[-1]))
     rs = np.random.RandomState(len(sizes) + obs)
     table, theta = rs.randn(P + 20_000).astype(np.float32), (rs.randn(P) * 0.1).astype(np.float32)
@@ -307,12 +303,13 @@ def test_nan_in_the_observation_mean_reaches_the_fitness(eng, name, sizes, act_k
         assert np.isfinite(want).all()
     elif loop == 'open':
         obsn_h = orc.normalise_obs(spec.obs_stream[:T], mean, std, clip)
-        want, _, mass, _ = act_f64.rollout_f64(table, idx, theta, SIGMA, sizes, obsn_h, spec.rew_vec[:T], spec.pos_scale, f64_act)
+        want, _, mass, _ = f64.rollout_f64(table, idx, theta, SIGMA, sizes, obsn_h, spec.rew_vec[:T], spec.pos_scale,
+                                           activation=f64_act)
         bound = EVAL_REL * mass
         assert np.isnan(want).all()
     else:
-        tr = act_f64.closed_truth(table, idx, theta, SIGMA, sizes, mean, std, clip, spec.obs_stream[0], spec.env_a.T,
-                                  spec.env_b.T, spec.rew_vec, spec.pos_scale, activation=f64_act)
+        tr = cf.truth(table, idx, theta, SIGMA, sizes, mean, std, clip, spec.obs_stream[0], spec.env_a.T, spec.env_b.T,
+                      spec.rew_vec, spec.pos_scale, activation=f64_act)
         want, bound = tr['fit'], EVAL_REL * tr['mass']
         assert np.isnan(want).all()
     nan = np.isnan(want)

@@ -1,12 +1,12 @@
 """GPU: episodes that end early on the closed-loop env (ClosedLoopEnv(fall_height=h), es_rollout_closedloop_terminal).
 
-* the kernel against the float64 truth (tests/closed_terminal_f64.py) at every shipped config's policy (C = 2 for 15-256-256-3,
+* the kernel against the float64 truth (tests/closed_f64.py with the fall height) at every shipped config's policy (C = 2 for 15-256-256-3,
   C = 4 for 17-256-256-256-6 and 28-128-256-256-128-8), a C = 1 shape, a binned head and a leaky-ReLU policy, at fall heights
   from "half fall at step 0" to "nothing falls".  Per evaluation: t_d exactly wherever the truth's |z| stays at least delta
-  from h over the executed steps, delta the position bound of tests/test_gpu_closed_f64.py (2 ulp of the summed magnitude
-  plus ACT_ERR pos_scale T: a kernel position within its bound decides each step as the truth does); the evaluations within
-  delta (and, for the binned head, those whose top two outputs come within 1e-5) are counted, shown to be few, and skipped.
-  Fitness within that file's EVAL_REL times the reward mass summed to t_d, the final position within its bound, steps, and
+  from h over the executed steps, delta the closed loop's position bound (2 ulp of the summed magnitude plus ACT_ERR
+  pos_scale T: a kernel position within its bound decides each step as the truth does); the evaluations within delta (and,
+  for the binned head, those whose top two outputs come within 1e-5) are counted, shown to be few, and skipped.  Fitness
+  within the closed loop's EVAL_REL times the reward mass summed to t_d, the final position within its bound, steps, and
   the ObStat sums and count of the saved evaluations;
 * nothing falls: bit for bit the fall_height=None result of the cluster kernel, also with action noise over E = 3 episodes
   (tanh and leaky ReLU at C = 1 and C = 2); at a shape fall_height=None runs on the one-CTA kernel, both within the float64
@@ -31,16 +31,13 @@ from es_pytorch_b200 import _lib
 from oracle import es_oracle as orc
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import act_f64  # noqa: E402
-import closed_terminal_f64 as ctf  # noqa: E402
+import closed_f64 as cf  # noqa: E402
+import f64_rollout as f64  # noqa: E402
+from closed_f64 import ACT_ERR, EVAL_REL, OBS_ERR, U  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24
 SIGMA = 0.02
-EVAL_REL = 1e-5                 # tests/test_gpu_closed_f64.py's per-evaluation fitness bound (of the reward mass)
-ACT_ERR = 1e-5
-OBS_ERR = 1e-6
 LOW = np.array([-1.0, -0.5, -2.0], np.float32)
 HIGH = np.array([1.0, 1.5, 0.5], np.float32)
 
@@ -50,7 +47,7 @@ def _head(kind):
     if kind == 'binned':
         return BinnedHead(5, LOW.copy(), HIGH.copy()), None, (5, LOW, HIGH), np.tanh
     if kind == 'leaky':
-        return None, Activation(_lib.ES_ACT_LEAKY_RELU, float(np.float32(0.1))), None, act_f64.leaky_relu(0.1)
+        return None, Activation(_lib.ES_ACT_LEAKY_RELU, float(np.float32(0.1))), None, f64.leaky_relu(0.1)
     return None, None, None, np.tanh
 
 
@@ -73,9 +70,9 @@ def build(sizes, T, n_pairs=8, seed=3, g=1.0, band=8, E=1, ac_std=0.0, adim=None
 
 def truth(d, h, binned=None, activation=np.tanh):
     s = d['spec']
-    return ctf.truth(d['table'], d['idx'], d['theta'], SIGMA, d['sizes'], d['mean'], d['std'], d['clip'], d['obs0'], d['env_a'],
-                     d['env_b'], s.rew_vec, s.pos_scale, h, act_noise=d['noise'], episodes=d['E'], activation=activation,
-                     binned=binned)
+    return cf.truth(d['table'], d['idx'], d['theta'], SIGMA, d['sizes'], d['mean'], d['std'], d['clip'], d['obs0'], d['env_a'],
+                    d['env_b'], s.rew_vec, s.pos_scale, act_noise=d['noise'], episodes=d['E'], activation=activation,
+                    fall_height=h, binned=binned)
 
 
 def coins(n, saved):

@@ -1,6 +1,6 @@
 """GPU: whole generations of policies with ReLU, leaky-ReLU, ELU and sigmoid activations (DeviceGeneration(activation=...),
 es.step with BatchedRollout(fuse_activations=True)) at the shipped configs' shapes, judged stage by stage (tests/gen_stages.py)
-against exact and float64 references, the float64 truth applying the policy's activation (tests/act_f64.py's forms).
+against exact and float64 references, the float64 truth applying the policy's activation (tests/f64_rollout.py's forms).
 
 Built as test_gpu_generation_shipped_configs.py (its Setup, runs, judge, rerun and modelled bugs; the same table, streams,
 theta0, sigma, Adam and save_obs coins), with one activation per config:
