@@ -67,6 +67,10 @@ SIGNATURES = {
     'es_rollout_closedloop_terminal': (_i32, [_vp, _vp, _i64, _vp, _i32, _vp, _i32, _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64,
                                               _vp, _vp, _i32, _vp, _vp, _i32, _f32, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _vp, _vp,
                                               _vp, _i32, _vp, _vp, _i32, _f32, _vp, _i32, _f32, _vp, _vp, _vp]),
+    'es_rollout_closedloop_terminal_streams': (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _u64, _i32, _f64, _vp, _i64, _vp, _i32,
+                                                      _f32, C.POINTER(_i32), _i32, _vp, _vp, _f64, _vp, _vp, _i32, _vp, _vp, _i32,
+                                                      _f32, _f64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32,
+                                                      _i32, _f32, _vp, _vp, _vp, _vp]),
     'es_draw_noisy': (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _u64, _i32, _i32, _f64, _vp, _vp, _vp, _vp]),
     'es_randn': (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp]),
     'es_randn_plan': (_i32, [_vp, _i64, C.POINTER(C.c_size_t), C.POINTER(_i32)]),

@@ -18,7 +18,7 @@ LIB = os.path.join(HERE, 'libes_b200.so')
 STAMP = os.path.join(HERE, '.libes_b200.stamp')
 
 SOURCES = ['api.cu', 'reconstruct.cu', 'rank.cu', 'elementwise.cu', 'mt_draw.cu', 'mt_gauss.cu', 'rollout_f32.cu', 'rollout_f32x.cu', 'rollout_tc2.cu', 'rollout_tcw.cu', 'rollout_tcw_act.cu',
-           'rollout_closed.cu', 'rollout_closedw.cu', 'objective.cu']
+           'rollout_closed.cu', 'rollout_closedw.cu', 'rollout_closedw_walk.cu', 'objective.cu']
 HEADERS = ['common.cuh', 'pipeline.cuh', 'wgmma.cuh', 'mt19937.cuh', 'rollout_tcw.cuh', 'rollout_closedw.cuh', 'mt_jump_polys.inc', os.path.join('..', '..', 'include', 'es_b200.h')]
 
 NVCC_FLAGS = [

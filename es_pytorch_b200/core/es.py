@@ -115,6 +115,12 @@ def _noisy_terminal(policy: Policy, fit_fn) -> bool:
             and float(getattr(policy._module, '_action_std', 0) or 0) != 0)
 
 
+def _walks(fit_fn) -> bool:
+    """Whether a noisy evaluation on an env whose episodes end early runs fused (``BatchedRollout(fuse_noisy_terminal=True)``:
+    the rollout walks each stream's draws, es_rollout_closedloop_terminal_streams) instead of one evaluation per launch."""
+    return bool(getattr(fit_fn, 'fuse_noisy_terminal', False))
+
+
 def _can_fuse_step(comm, policy: Policy, fit_fn, ranker: Ranker) -> bool:
     """``step`` can keep the whole generation on the device (one synchronisation) when the evaluation is a
     ``BatchedRollout`` of a network the fused rollouts evaluate (a tanh MLP or a binned-action one: ``BaseNet.head``; with
@@ -124,10 +130,10 @@ def _can_fuse_step(comm, policy: Policy, fit_fn, ranker: Ranker) -> bool:
     from .._lib import ES_RANK_MAX_NORMALIZED
     if not getattr(fit_fn, 'is_batched_rollout', False) or _fused_policy(policy._module, fit_fn) is None:
         return False
-    if _terminates(fit_fn) and (fit_fn.objective == 'mean_reward' or _noisy_terminal(policy, fit_fn)):
+    if _terminates(fit_fn) and (fit_fn.objective == 'mean_reward' or (_noisy_terminal(policy, fit_fn) and not _walks(fit_fn))):
         # MeanRewardResult raises ZeroDivisionError for an evaluation that falls at its first step, before anything is ranked:
         # test_params -> rank -> approx_grad leaves the device theta untouched when it does.  Action noise runs one evaluation
-        # at a time (test_params)
+        # at a time (test_params) unless the BatchedRollout opts into the fused route (fuse_noisy_terminal)
         return False
     if comm.size != dist.world().size:                       # a communicator this package does not drive
         return False
@@ -282,7 +288,10 @@ def _test_params_batched(comm, n: int, policy: Policy, nt: NoiseTable, gen_obsta
                                   'BatchedRollout(fuse_activations=True) FeedForward with ReLU, LeakyReLU, ELU or Sigmoid')
     streams = fit_fn.rank_streams if fit_fn.rank_streams is not None else [rs]
     if _noisy_terminal(policy, fit_fn):
-        return _test_params_per_eval(comm, n, policy, nt, gen_obstat, fit_fn, streams)
+        if not _walks(fit_fn):
+            return _test_params_per_eval(comm, n, policy, nt, gen_obstat, fit_fn, streams)
+        if int(fit_fn.coins_per_eval) not in (0, 1):
+            raise ValueError(f'fit_fns draw at most one save_obs coin per evaluation, got coins_per_eval={fit_fn.coins_per_eval}')
     gen = _device_generation(fit_fn, policy, nt, streams)
     fpos, fneg = gen.evaluate(n)
     # one device->host hop for everything the reference API returns as ndarrays
@@ -312,7 +321,9 @@ def _test_params_batched(comm, n: int, policy: Policy, nt: NoiseTable, gen_obsta
 
 
 def _test_params_per_eval(comm, n: int, policy: Policy, nt: NoiseTable, gen_obstat: ObStat, fit_fn, streams):
-    """test_params for a BatchedRollout on an env whose episodes end early, with action noise: one evaluation per launch.
+    """test_params for a BatchedRollout on an env whose episodes end early, with action noise: one evaluation per launch (the
+    default; ``BatchedRollout(fuse_noisy_terminal=True)`` runs the whole generation in one launch that walks each stream's draws
+    inside the rollout, es_rollout_closedloop_terminal_streams, with CUDA's log in the gaussians instead of numpy's).
     Every draw of a RandomState stream comes after the previous evaluation's gaussians, and how many those are depends on
     where that evaluation fell, so the next evaluation's noise index is unknown until it has run.  Per stream (one reference
     rank) and pair, in the reference's order (es.py:67-74): ``nt.sample``, then per sign the save_obs coin(s), the rollout

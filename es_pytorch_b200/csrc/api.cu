@@ -122,6 +122,10 @@ static int es_async_error(es_ctx* ctx, const char* where) {
             es_set_error("%s: a previous ES_ROLLOUT_TC3 rollout met a hidden activation beyond float16 range (|h| > 65504), which its "
                          "split float16 operands cannot hold: the results of that call are invalid; use ES_ROLLOUT_F32 for such "
                          "policies", where);
+        else if (code == ES_ASYNC_WALK_OVERFLOW)
+            es_set_error("%s: es_rollout_closedloop_terminal_streams walked a stream past the MT19937 words generated for it (a > "
+                         "12 sigma event of the polar method's acceptance count, or a bug): the results of that call are invalid",
+                         where);
         else if (code == ES_ASYNC_RANDN_OVERFLOW)
             es_set_error("%s: es_randn needed more MT19937 words than its windows had generated (a > 12 sigma event of the "
                          "polar method's acceptance count, or a bug): the values of that call are invalid", where);
@@ -606,6 +610,68 @@ int es_rollout_closedloop_terminal(es_ctx* ctx, const float* table, int64_t tabl
     const EsTerm term = {fall_height, steps, noise_used};
     return es_closedloop(ctx, fn, r, layer_sizes, env, bins ? ES_HEAD_BINNED : activation == ES_ACT_TANH ? ES_HEAD_TANH : ES_HEAD_ACT,
                          (cudaStream_t)stream, term);
+}
+
+int es_rollout_closedloop_terminal_streams(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss,
+                                           int n_streams, int n_per_stream, uint64_t upper_bound, int coins_per_eval, double ac_std,
+                                           const float* table, int64_t table_len, const float* theta, int P, float sigma,
+                                           const int* layer_sizes, int n_layers, const double* ob_mean, const double* ob_std,
+                                           double ob_clip, const float* obs0, const float* env_a, int band, const float* env_b,
+                                           const float* rew_vec, int T, float pos_scale, double save_obs_chance, int64_t* idx_out,
+                                           uint32_t* coin_out, double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos,
+                                           float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins,
+                                           int activation, float act_param, int n_episodes, float fall_height, int32_t* steps,
+                                           int64_t* noise_used, float* noise_trace, void* stream) {
+    ES_ENTER(ctx);
+    const char* fn = "es_rollout_closedloop_terminal_streams";
+    ES_REQUIRE(mt_key && mt_pos && has_gauss && gauss && idx_out, "%s: NULL stream state or idx_out", fn);
+    ES_REQUIRE(n_streams >= 0 && n_per_stream >= 0, "%s: negative count", fn);
+    ES_REQUIRE((long long)n_streams * n_per_stream <= 0x3FFFFFFFLL, "%s: %d streams x %d pairs exceed 2^30 pairs", fn, n_streams,
+               n_per_stream);
+    if (bins != 0) {
+        es_set_error("%s: a binned head draws no action noise (FFBinned.forward ignores rs): use es_rollout_closedloop_terminal", fn);
+        return ES_ERR_UNSUPPORTED;
+    }
+    if (coins_per_eval < 0 || coins_per_eval > 1) {
+        es_set_error("%s: fit_fns draw at most one save_obs coin per evaluation, got coins_per_eval %d", fn, coins_per_eval);
+        return ES_ERR_UNSUPPORTED;
+    }
+    ES_REQUIRE(coins_per_eval == 0 || coin_out, "%s: coin_out is NULL", fn);
+    ES_REQUIRE(isfinite(ac_std) && ac_std != 0.0, "%s: ac_std must be finite and != 0 (without action noise use "
+               "es_rollout_closedloop_terminal), got %g", fn, ac_std);
+    ES_REQUIRE(isfinite(fall_height) && fall_height > 0.f, "%s: fall_height must be finite and > 0, got %g", fn, (double)fall_height);
+    ES_REQUIRE(steps != nullptr, "%s: NULL steps", fn);
+    ES_REQUIRE(n_episodes >= 1, "%s: n_episodes must be >= 1, got %d", fn, n_episodes);
+    int rc = es_activation_check(fn, activation, act_param);
+    if (rc) return rc;
+    rc = es_randint_check(fn, upper_bound);
+    if (rc) return rc;
+    if (upper_bound == 1) {
+        es_set_error("%s: upper_bound == 1 is not supported", fn);
+        return ES_ERR_UNSUPPORTED;
+    }
+    const int n_pairs = n_streams * n_per_stream;
+    EsRollout r = {.table = table, .table_len = table_len, .idx = idx_out, .n_pairs = n_pairs, .theta = theta, .P = P,
+                         .sigma = sigma, .n_layers = n_layers, .activation = activation, .obsn = nullptr, .rew_vec = rew_vec,
+                         .T = T, .pos_scale = pos_scale, .fit_pos = fit_pos, .fit_neg = fit_neg, .fit_stride = fit_stride,
+                         .behv_pos = behv_pos, .behv_neg = behv_neg, .act_noise = nullptr, .err = ctx->err_dev,
+                         .n_episodes = n_episodes, .act_param = act_param};
+    rc = es_rollout_check(fn, ob_mean && ob_std && obs0 && env_a && env_b, layer_sizes, r);
+    if (rc) return rc;
+    ES_REQUIRE(band >= 1 && band <= r.dims[0], "%s: band must be in [1, obs_dim]", fn);
+    ES_REQUIRE((ob_sum == nullptr) == (ob_sumsq == nullptr) && (ob_sum == nullptr) == (ob_count == nullptr),
+               "%s: ob_sum/ob_sumsq/ob_count must all be set or NULL", fn);
+    const EsClosedEnv env = {ob_mean, ob_std, ob_clip, obs0, env_a, band, env_b, nullptr, save_obs_chance, ob_sum, ob_sumsq, ob_count};
+    const EsTerm term = {fall_height, steps, noise_used};
+    const EsStreamWalk walk = {mt_key, mt_pos, has_gauss, gauss, n_streams, n_per_stream, upper_bound, coins_per_eval, ac_std,
+                               idx_out, coin_out, noise_trace};
+    if (n_pairs == 0) {
+        // (the plan still refuses a shape it does not cover)
+        int C = 0;
+        size_t smem = 0;
+        return es_closedw_plan(r.dims, r.n_layers, band, &C, &smem);
+    }
+    return es_impl_rollout_closedw_walk(ctx, r, env, term, walk, (cudaStream_t)stream);
 }
 
 int es_rollout_closedloop_mlp_activation_plan(es_ctx* ctx, const int* layer_sizes, int n_layers, int band, int activation,

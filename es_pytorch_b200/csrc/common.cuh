@@ -41,6 +41,7 @@ struct es_ctx {
 #define ES_ASYNC_RNG_OVERFLOW 2      // es_draw_noisy (jump-ahead path): the stream consumed more words than were generated ahead
 #define ES_ASYNC_RANDN_OVERFLOW 3    // es_randn: the n values needed more words than its windows generated
 #define ES_ASYNC_F16_RANGE 4         // es_rollout_openloop_activation (TC3): a hidden activation beyond float16 range
+#define ES_ASYNC_WALK_OVERFLOW 5     // es_rollout_closedloop_terminal_streams: a stream walked past the words generated ahead
 
 void es_set_error(const char* fmt, ...);
 
@@ -198,6 +199,28 @@ int es_closedw_plan(const int* layer_sizes, int n_layers, int band, int* cluster
 int es_closedw_binned_plan(const int* layer_sizes, int n_layers, int band, int bins, int* cluster_size, size_t* smem_bytes);
 int es_closedw_max_clusters(int n_layers, int bins, bool act, int cluster_size, size_t smem_bytes, int* clusters);
 int es_impl_rollout_closedw(es_ctx*, const EsRollout&, const EsClosedEnv&, const EsTerm&, unsigned* next, cudaStream_t);
+// The words of es_rollout_closedloop_terminal_streams (mt_gauss.cu): every stream's tempered MT19937 words from its block 0 on,
+// as far as n_pairs pairs of evaluations of N gaussians and `coins` coins each reach at es_draw_noisy's mean + 12 sigma, by
+// the jump-ahead fill.  plan: no device work; ES_ERR_UNSUPPORTED beyond the jump-ahead range
+struct EsStreamWords {
+    int lb_log2, n_seg;
+    size_t stride_words;        // per stream (a chunk of padding past the generated words included)
+    uint32_t limit;             // the last word index a walk may reach
+    size_t words_bytes, order_bytes;    // the scratch of the fill (256-byte multiples)
+};
+int es_impl_stream_words_plan(const es_ctx*, const char* fn, int n_streams, int n_pairs, int coins, int N, EsStreamWords*);
+int es_impl_stream_words_fill(es_ctx*, const uint32_t* mt_key, int n_streams, const EsStreamWords&, uint32_t* words,
+                              uint16_t* order, cudaStream_t);
+// the stream walk (rollout_closedw_walk.cu): the arguments of es_rollout_closedloop_terminal_streams beyond the rollout's
+struct EsStreamWalk {
+    uint32_t* mt_key; int32_t* mt_pos; int32_t* has_gauss; double* gauss;
+    int n_streams, n_per_stream;
+    uint64_t upper_bound;
+    int coins;
+    double ac_std;
+    int64_t* idx_out; uint32_t* coin_out; float* noise_trace;
+};
+int es_impl_rollout_closedw_walk(es_ctx*, const EsRollout&, const EsClosedEnv&, const EsTerm&, const EsStreamWalk&, cudaStream_t);
 // policies with an activation other than tanh (EsRollout::activation != ES_ACT_TANH) on ES_ROLLOUT_TC3: the shapes of
 // es_tcw_covers_act, rollout_tcw.cu's code (rollout_tcw_act.cu)
 bool es_tcw_covers_act(const EsRollout&);

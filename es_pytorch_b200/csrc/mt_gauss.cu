@@ -702,13 +702,17 @@ int mj_segment_lb(long long n_streams, long long blocks, int sm_count) {
 // How many words can a stream consume?  Per rollout ceil(N / 2) accepted attempts at acceptance pi / 4 (a negative binomial
 // count), 4 words each; per pair one index draw (~1.08 words with rejections, bounded generously) and the coins.  The
 // jump-ahead pass generates the mean + 12 sigma of the total (+ slack); the walk flags an overflow.
-int mg_plan(const es_ctx* ctx, int n_streams, int n_pairs, int coins, int N, MgPlan& pl) {
+long long mg_blocks_needed(int n_pairs, int coins, int N) {
     const double p_acc = 0.78539816339744830962, n_acc = (N + 1) / 2;
     const double att_mean = n_acc / p_acc, att_sd = sqrt(n_acc * (1.0 - p_acc)) / p_acc;
     const double evals = 2.0 * n_pairs;
     const double words_max = 624.0 + n_pairs * (8.0 + 4.0 * coins) + 4.0 * (evals * att_mean + 12.0 * sqrt(evals) * att_sd + 64.0) +
                              2.0 * MG_WIN + 16.0 * MT_NW;
-    const long long blocks_needed = (long long)(words_max / MT_NW) + 1;
+    return (long long)(words_max / MT_NW) + 1;
+}
+
+int mg_plan(const es_ctx* ctx, int n_streams, int n_pairs, int coins, int N, MgPlan& pl) {
+    const long long blocks_needed = mg_blocks_needed(n_pairs, coins, N);
     // jump-ahead when a stream is long enough to be worth splitting (ES_MT_JUMP=0 / 1 overrides; ES_MT_JUMP_LB: log2 of the
     // segment length in blocks, for tests)
     const char* ej = getenv("ES_MT_JUMP");
@@ -1065,6 +1069,59 @@ int es_impl_randn(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_g
         ES_LAUNCHED(ctx);
     }
     return ES_OK;
+}
+
+// The stream walk consumes words only for the steps that run, so its bound is the no-fall consumption: mg_plan's sizing with
+// the jump-ahead fill always (the walk reads the words directly, no accept masks or prefixes)
+static bool sw_fits(long long blocks, long long n_streams, int sm_count, int* lb, long long* n_seg) {
+    *lb = mj_segment_lb(n_streams, blocks, sm_count);
+    // mj_segment_lb lengthens the segments until the fill has at most ~4 per SM; with more streams than that it would stop
+    // only at its maximum, and every stream would be generated that long.  A segment longer than the stream's need buys no
+    // parallelism: at most ceil(log2(blocks)), so the words generated stay under twice the bound
+    int need = 0;
+    while ((1LL << need) < blocks) ++need;
+    if (*lb > need) *lb = need;
+    *n_seg = (blocks + (1LL << *lb) - 1) >> *lb;
+    return ((*n_seg << *lb) >> MJ_BITS_RANGE) == 0 && *n_seg <= 65535;
+}
+
+int es_impl_stream_words_plan(const es_ctx* ctx, const char* fn, int n_streams, int n_pairs, int coins, int N, EsStreamWords* pl) {
+    const long long blocks = mg_blocks_needed(n_pairs, coins, N);
+    int lb = 0;
+    long long n_seg = 0;
+    if (!sw_fits(blocks, n_streams, ctx->sm_count, &lb, &n_seg)) {
+        int lo = 0, hi = n_pairs;                                  // the most pairs per stream that fit
+        while (lo < hi) {
+            const int mid = lo + (hi - lo + 1) / 2;
+            int l2;
+            long long s2;
+            if (sw_fits(mg_blocks_needed(mid, coins, N), n_streams, ctx->sm_count, &l2, &s2)) lo = mid; else hi = mid - 1;
+        }
+        const long long pairs = (long long)n_streams * n_pairs;
+        if (lo == 0)
+            es_set_error("%s: one pair of %d gaussians per evaluation needs %lld blocks of 624 words, beyond the jump-ahead "
+                         "range of 2^%d blocks per stream: no number of streams fits; use fewer episodes or steps", fn, N,
+                         mg_blocks_needed(1, coins, N), MJ_BITS_RANGE);
+        else
+            es_set_error("%s: %d pairs per stream need %lld blocks of 624 words each (%d gaussians per evaluation), beyond the "
+                         "jump-ahead range of 2^%d blocks per stream; at most %d pairs per stream fit, so the %lld pairs need "
+                         "at least %lld streams", fn, n_pairs, blocks, N, MJ_BITS_RANGE, lo, pairs, (pairs + lo - 1) / lo);
+        return ES_ERR_UNSUPPORTED;
+    }
+    pl->lb_log2 = lb;
+    pl->n_seg = (int)n_seg;
+    const size_t gen_words = (size_t)(1 + (n_seg << lb)) * MT_NW;
+    const size_t n_chunks = (gen_words + MJ_CW - 1) / MJ_CW;
+    pl->stride_words = (n_chunks + 1) * MJ_CW;                   // (+ a chunk: the walk stages up to 256 words past its cursor)
+    pl->limit = (uint32_t)(gen_words - 8);
+    pl->words_bytes = mg_pad((size_t)n_streams * pl->stride_words * sizeof(uint32_t));
+    pl->order_bytes = mg_pad((size_t)n_seg * sizeof(uint16_t));
+    return ES_OK;
+}
+
+int es_impl_stream_words_fill(es_ctx* ctx, const uint32_t* mt_key, int n_streams, const EsStreamWords& pl, uint32_t* words,
+                              uint16_t* order, cudaStream_t stream) {
+    return mj_launch_fill(ctx, mt_key, n_streams, pl.n_seg, pl.lb_log2, order, words, pl.stride_words, stream);
 }
 
 int es_impl_draw_noisy(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss, int n_streams,

@@ -23,6 +23,30 @@ struct CwParams {
     unsigned* next;                         // the evaluation counter of dynamic scheduling, zero before the launch
 };
 
+// The stream walk of es_rollout_closedloop_terminal_streams (rollout_closedw_walk.cu states the design): every stream's
+// tempered MT19937 words from its block 0 on, and what the walk reads and writes of the streams
+struct CwWalk {
+    const uint32_t* words;      // [n_streams][stride] (mj_launch_fill)
+    size_t stride;
+    uint32_t limit;             // a cursor past it has left the generated words (the buffer is padded past it by >= 4096 words)
+    uint32_t rng, mask;         // the randint bound (mt19937_randint_bound)
+    int n_per_stream, coins;
+    double ac_std;
+    uint32_t* mt_key;           // [n_streams][624], position, has_gauss, gauss: in and out
+    int32_t* mt_pos;
+    int32_t* has_gauss;
+    double* gauss;
+    int64_t* idx_out;           // [n_streams * n_per_stream]
+    uint32_t* coin_out;         // [n_streams * n_per_stream][4 coins] or NULL
+    float* trace;               // [n_streams * n_per_stream][2][E T act] the noise each executed step added, or NULL
+};
+struct CwWalkParams : CwParams { CwWalk w; };
+
+// the walk's shared memory after the layout's end (floats): the noise of the step being run and of the next one, the staged
+// words of the next step's attempts, the pair's index and the evaluation's save_obs decision
+constexpr int CW_WALK_NZ = CW_MAX_ACT, CW_WALK_STAGE = 256;
+constexpr int CW_WALK_FLOATS = 2 * CW_WALK_NZ + CW_WALK_STAGE + 4;
+
 __host__ __device__ inline int cw_pad32(int n) { return (n + 31) & ~31; }
 __host__ __device__ inline int cw_pad4(int n) { return (n + 3) & ~3; }
 
@@ -102,11 +126,137 @@ __device__ __forceinline__ void cw_store_remote(float* local, unsigned rank, flo
 // one layer of this CTA in the step loop (read from shared memory: a per-layer index into registers would go to local memory)
 struct CwLayer { int in, nr, S, r0, w, bias, xin, out, woff, boff; };
 
+// One stream's walk, run by one warp (every lane holds the same state): the committed state after the draws of every executed
+// step (cur, hg, gv: word cursor, has_gauss, cached gaussian) and the state after the draws formed ahead for a step that may not
+// run (fcur, fhg, fgv).  Draws act on the formed state; commit() keeps them, discard() drops them.  numpy's order per pair:
+// randint, then per evaluation the coin words and randn(act) per executed step (legacy_gauss: the cached value first, then
+// polar attempts of 4 words, f x2 returned and f x1 cached).
+struct CwWalker {
+    const uint32_t* gw;
+    uint32_t cur, fcur;
+    int hg, fhg;
+    double gv, fgv;
+    bool bad;
+
+    __device__ void load(const CwWalk& w, int sid) {
+        gw = w.words + (size_t)sid * w.stride;
+        cur = fcur = (uint32_t)w.mt_pos[sid];
+        hg = fhg = w.has_gauss[sid] ? 1 : 0;
+        gv = fgv = w.gauss[sid];
+        bad = false;
+    }
+    __device__ void commit() { cur = fcur; hg = fhg; gv = fgv; }
+    __device__ void discard() { fcur = cur; fhg = hg; fgv = gv; }
+    // n more words from the formed cursor must lie in the generated words; otherwise the ctx's error word is set and the walk
+    // stops consuming (its remaining draws are garbage, es_check_async raises)
+    __device__ bool room(const CwWalk& w, uint32_t n, int* err) {
+        if (!bad && fcur + n > w.limit) {
+            bad = true;
+            if (err) *(volatile int*)err = ES_ASYNC_WALK_OVERFLOW;
+        }
+        return !bad;
+    }
+    // rs.randint(0, upper_bound): masked rejection, 32 candidates at a time
+    __device__ uint32_t randint(const CwWalk& w, int lane, int* err) {
+        while (room(w, 32, err)) {
+            const uint32_t v = __ldg(gw + fcur + lane) & w.mask;
+            const unsigned ok = __ballot_sync(0xffffffffu, v <= w.rng);
+            if (ok) {
+                const int f = __ffs((int)ok) - 1;
+                fcur += (uint32_t)f + 1u;
+                return __shfl_sync(0xffffffffu, v, f);
+            }
+            fcur += 32u;
+        }
+        return 0u;
+    }
+    // the next two words (one rs.random() coin)
+    __device__ uint2 coin(const CwWalk& w, int* err) {
+        if (!room(w, 2, err)) return make_uint2(0u, 0u);
+        const uint2 c = make_uint2(__ldg(gw + fcur), __ldg(gw + fcur + 1));
+        fcur += 2u;
+        return c;
+    }
+    // start copying the CW_WALK_STAGE words from the formed cursor into `stage` (cp.async: no registers held across the layers)
+    __device__ void prefetch(uint32_t* stage, int lane) const {
+#pragma unroll
+        for (int j = 0; j < CW_WALK_STAGE / 32; ++j) {
+            const int i = lane + 32 * j;
+            const unsigned s = (unsigned)__cvta_generic_to_shared(stage + i);
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gw + fcur + i) : "memory");
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    }
+    // randn(act) * ac_std rounded to float32 into out[0 .. act), from the formed state; `stage`: the words prefetch() copied
+    // from the same cursor, or NULL
+    __device__ void form(const CwWalk& w, int act, float* out, const uint32_t* stage, int lane, int* err) {
+        if (stage) {
+            asm volatile("cp.async.wait_all;" ::: "memory");
+            __syncwarp();
+        }
+        const uint32_t s0 = fcur;
+        int k = 0;
+        if (fhg) {
+            if (lane == 0) out[0] = (float)__dmul_rn(fgv, w.ac_std);
+            k = 1; fhg = 0; fgv = 0.0;
+        }
+        while (k < act && room(w, 128, err)) {
+            const int need = (act - k + 1) >> 1;                  // accepted attempts still to find
+            uint32_t wd[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const uint32_t rel = fcur - s0 + 4u * (uint32_t)lane + (uint32_t)q;
+                wd[q] = (stage && rel < (uint32_t)CW_WALK_STAGE) ? stage[rel] : __ldg(gw + fcur + 4u * (uint32_t)lane + q);
+            }
+            const bool acc = mt19937_polar_accept(wd[0], wd[1], wd[2], wd[3]);
+            const unsigned bal = __ballot_sync(0xffffffffu, acc);
+            const int rank = __popc(bal & ((1u << lane) - 1u));
+            double cache = 0.0;
+            if (acc && rank < need) {
+                const double2 g = mt19937_polar_pair(wd[0], wd[1], wd[2], wd[3]);
+                const int v = k + 2 * rank;
+                out[v] = (float)__dmul_rn(g.x, w.ac_std);
+                if (v + 1 < act) out[v + 1] = (float)__dmul_rn(g.y, w.ac_std);
+                else cache = g.y;
+            }
+            const int n_acc = __popc(bal);
+            if (n_acc >= need) {                                 // the need-th accepted attempt (lane L) ends the draw
+                const int L = __ffs((int)__ballot_sync(0xffffffffu, acc && rank == need - 1)) - 1;
+                const double c = __shfl_sync(0xffffffffu, cache, L);
+                fhg = (act - k) & 1;
+                fgv = fhg ? c : 0.0;
+                fcur += 4u * (uint32_t)(L + 1);
+                k = act;
+            } else {
+                fcur += 128u;
+                k += 2 * n_acc;
+            }
+        }
+        __syncwarp();
+    }
+    // the committed state into the stream's state, in DeviceGeneration.mt_state's layout: the raw words behind the tempered
+    // words of the cursor's block (position 624: the block is exhausted), the position and the gaussian cache
+    __device__ void store(const CwWalk& w, int sid, int lane) const {
+        const uint32_t blk = cur / MT_NW, off = cur % MT_NW;
+        const bool at_end = off == 0 && blk > 0;
+        const uint32_t b_last = at_end ? blk - 1 : blk;
+        for (int i = lane; i < MT_NW; i += 32) w.mt_key[(size_t)sid * MT_NW + i] = mt19937_untemper(__ldg(gw + (size_t)b_last * MT_NW + i));
+        if (lane == 0) {
+            w.mt_pos[sid] = at_end ? MT_NW : (int32_t)off;
+            w.has_gauss[sid] = hg;
+            w.gauss[sid] = gv;
+        }
+    }
+};
+
 // ACT: every layer of the policy applies the call's activation (p.r.activation, es_act) instead of tanh; the env's own
 // tanh(A obs + B a) stays tanh.  p.term.steps set: the env ends an episode when its position falls (rollout_closedw.cu states
-// the changes and why the barrier argument holds); unset, no episode ends before T, whatever the position (a NaN included)
-template <int NL, bool BINNED, bool NOISY, bool ACT>
-__device__ __forceinline__ void cw_rollout(const CwParams& p) {
+// the changes and why the barrier argument holds); unset, no episode ends before T, whatever the position (a NaN included).
+// WALK (NOISY, with p a CwWalkParams and p.term.steps set): clusters take streams, not evaluations, and one warp per CTA walks
+// the stream's words into the indices, coins and action noise (rollout_closedw_walk.cu)
+template <int NL, bool BINNED, bool NOISY, bool ACT, bool WALK = false, class Params = CwParams>
+__device__ __forceinline__ void cw_rollout(const Params& p) {
+    static_assert(!WALK || (NOISY && !BINNED), "the stream walk draws action noise");
     extern __shared__ __align__(16) float cw_smem[];
     __shared__ CwLayer cw_layers[NL];
     const unsigned C = cw_cluster_nctas(), rank = cw_cluster_rank();
@@ -147,9 +297,50 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
     // two free words after the position
     int* __restrict__ tflag = reinterpret_cast<int*>(cw_smem + L.racc + 5);
     int* __restrict__ tnext = reinterpret_cast<int*>(cw_smem + L.racc + 6);
-    for (int ev = cluster; ev < 2 * p.r.n_pairs; ev = *tnext) {
+    // the stream walk: its warp (idle in the env step, obs <= 384), the step noise [2][CW_WALK_NZ] (by step parity), the staged
+    // words, and the pair's index and the save_obs decision it publishes
+    [[maybe_unused]] const bool walker = WALK && warp == CW_WARPS - 2;
+    [[maybe_unused]] float* __restrict__ wnz = cw_smem + L.total;
+    [[maybe_unused]] uint32_t* __restrict__ wstage = reinterpret_cast<uint32_t*>(cw_smem + L.total + 2 * CW_WALK_NZ);
+    [[maybe_unused]] uint32_t* __restrict__ wmisc = wstage + CW_WALK_STAGE;
+    [[maybe_unused]] CwWalker wk;
+    [[maybe_unused]] int n_ev = 0;                          // a stream's evaluations (WALK)
+    int ev0 = cluster;
+    if constexpr (WALK) {
+        n_ev = 2 * p.w.n_per_stream;
+        ev0 = cluster * n_ev;                               // (>= 2 n_pairs when the cluster has no stream)
+    }
+    for (int ev = ev0; ev < 2 * p.r.n_pairs; ev = *tnext) {
         const int pair = ev >> 1, neg = ev & 1;
-        const long long base = es_checked_slice(p.r.idx[pair], p.r.P, p.r.table_len, p.r.err);
+        [[maybe_unused]] const int e_loc = WALK ? ev % n_ev : 0;
+        if constexpr (WALK) {
+            // the pair's index (before +), the evaluation's coin and its first step's noise, published by the barrier below
+            // (every read of this CTA's previous evaluation preceded REUSE)
+            if (walker) {
+                const CwWalk& w = p.w;
+                if (e_loc == 0) wk.load(w, ev / n_ev);
+                if (!neg) {
+                    const uint32_t ix = wk.randint(w, lane, p.r.err);
+                    if (lane == 0) {
+                        wmisc[0] = ix;
+                        if (rank == 0) w.idx_out[pair] = (int64_t)ix;
+                    }
+                }
+                if (w.coins) {
+                    const uint2 c = wk.coin(w, p.r.err);
+                    if (lane == 0) {
+                        wmisc[1] = mt19937_random_sample(c.x, c.y) < p.env.save_obs_chance;
+                        if (rank == 0 && w.coin_out) { w.coin_out[(size_t)pair * 4 + 2 * neg] = c.x; w.coin_out[(size_t)pair * 4 + 2 * neg + 1] = c.y; }
+                    }
+                } else if (lane == 0) {
+                    wmisc[1] = 0u;
+                }
+                wk.form(w, act, wnz, nullptr, lane, p.r.err);
+                wk.commit();
+            }
+            __syncthreads();
+        }
+        const long long base = es_checked_slice(WALK ? (long long)wmisc[0] : p.r.idx[pair], p.r.P, p.r.table_len, p.r.err);
         const float* __restrict__ eps = p.r.table + base;
         const float* __restrict__ th = p.r.theta;
         const float sg = p.r.sigma;
@@ -179,7 +370,9 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
         start_episode();
         if (tid == 0) { rfit[0] = 0.0; rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
         bool save = false;                                  // the evaluation's save_obs coin (legacy random_sample < chance)
-        if (p.env.coins) {
+        if constexpr (WALK) {
+            save = wmisc[1] != 0u;
+        } else if (p.env.coins) {
             const uint32_t* c = p.env.coins + (size_t)pair * 4 + 2 * neg;
             save = mt19937_random_sample(c[0], c[1]) < p.env.save_obs_chance;
         }
@@ -197,6 +390,9 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
             if (NOISY && ep > 0) {
                 start_episode();
                 if (tid == 0) { rpos[0] = 0.f; rpos[1] = 0.f; rpos[2] = 0.f; }
+                if constexpr (WALK) {                       // the episode's first step draws where the last one stopped
+                    if (walker) { wk.form(p.w, act, wnz, nullptr, lane, p.r.err); wk.commit(); }
+                }
                 __syncthreads();
             }
 
@@ -204,11 +400,18 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
             // layer's pass, lanes 8 i)
             double* __restrict__ erow = NOISY ? p.env.ep_rows + (size_t)cluster * T : nullptr;
             const float* __restrict__ nzp = nullptr;
+            [[maybe_unused]] float* __restrict__ trp = nullptr;    // (WALK) the row's noise trace
             if (NOISY && (lane & 7) == 0) {
                 const CwLayer& lo = cw_layers[NL - 1];
                 const int r = 4 * warp + (lane >> 3);
-                if (r < lo.nr)
-                    nzp = p.r.act_noise + ((size_t)pair * 2 + neg) * n_eps * T * act + used + lo.r0 + r;
+                if (r < lo.nr) {
+                    if constexpr (WALK) {
+                        nzp = wnz + lo.r0 + r;
+                        if (p.w.trace) trp = p.w.trace + ((size_t)pair * 2 + neg) * n_eps * T * act + used + lo.r0 + r;
+                    } else {
+                        nzp = p.r.act_noise + ((size_t)pair * 2 + neg) * n_eps * T * act + used + lo.r0 + r;
+                    }
+                }
             }
 
             t_end = T - 1;
@@ -223,7 +426,15 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                     if (NOISY && lane == 0 && ep > 0 && t < reach) esum = erow[t];
                 }
                 float nz = 0.f;                                 // this lane's action noise: in flight under the layers
-                if (NOISY && nzp) nz = __ldg(nzp + (size_t)t * act);
+                if constexpr (WALK) {
+                    if (nzp) {
+                        nz = nzp[(t & 1) * CW_WALK_NZ];
+                        if (trp) trp[(size_t)t * act] = nz;
+                    }
+                    if (walker && t + 1 < T) wk.prefetch(wstage, lane);     // the next step's words, under the layers
+                } else {
+                    if (NOISY && nzp) nz = __ldg(nzp + (size_t)t * act);
+                }
                 // ---- the layers: 4 rows per warp and pass, each row's tanh stored into every CTA's a_l, then B_l ----
 #pragma unroll 1
                 for (int l = 0; l < NL; ++l) {
@@ -310,7 +521,13 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
                     }
                     *tflag = term && !(fabsf(rpos[2]) <= p.term.fall_height);
                 }
+                if constexpr (WALK) {                           // the next step's noise, kept if the step runs
+                    if (walker && t + 1 < T) wk.form(p.w, act, wnz + ((t + 1) & 1) * CW_WALK_NZ, wstage, lane, p.r.err);
+                }
                 __syncthreads();                                // x and the raw observation before the next step's layer 0
+                if constexpr (WALK) {
+                    if (walker) { if (*tflag) wk.discard(); else wk.commit(); }
+                }
                 if (*tflag) { t_end = t; break; }
             }
             used += (long long)(t_end + 1) * act;
@@ -336,8 +553,21 @@ __device__ __forceinline__ void cw_rollout(const CwParams& p) {
             }
             if (tid == 0) { atomicAdd(p.env.ob_count, (double)(t_end + 1)); atomicAdd(p.env.ob_count + 1, 1.0); }
         }
+        if constexpr (WALK) {                               // the stream's state after its last evaluation
+            if (walker && rank == 0 && e_loc == n_ev - 1) wk.store(p.w, ev / n_ev, lane);
+        }
         if (rank == 0 && tid == 0) {                        // the cluster's next evaluation, into every CTA before REUSE
-            const int nx = n_clusters + (int)atomicAdd(p.next, 1u);
+            int nx;
+            if constexpr (WALK) {                           // the stream's next one, or the first of the next stream
+                if (e_loc + 1 < n_ev) {
+                    nx = ev + 1;
+                } else {
+                    const long long s = n_clusters + (long long)atomicAdd(p.next, 1u);
+                    nx = s * n_ev < 2ll * p.r.n_pairs ? (int)(s * n_ev) : 2 * p.r.n_pairs;
+                }
+            } else {
+                nx = n_clusters + (int)atomicAdd(p.next, 1u);
+            }
             for (unsigned q = 0; q < C; ++q) cw_store_remote(reinterpret_cast<float*>(tnext), q, __int_as_float(nx));
         }
         cw_cluster_sync();                                  // REUSE (the last one: EXIT)
@@ -357,7 +587,8 @@ static cudaLaunchConfig_t cw_config(int C, size_t smem, int clusters, cudaStream
 }
 
 // the number of clusters of the shape that can be resident at once (the persistent grid), 0 when none fits
-static int cw_max_clusters(CwKernel k, int C, size_t smem, int* clusters) {
+template <class Kernel>
+static int cw_max_clusters(Kernel k, int C, size_t smem, int* clusters) {
     ES_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaLaunchAttribute attr;
     const cudaLaunchConfig_t cfg = cw_config(C, smem, 1, nullptr, &attr);

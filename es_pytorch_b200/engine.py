@@ -470,6 +470,71 @@ class Engine:
             self.stream), 'es_rollout_closedloop_terminal')
         return steps, noise_used
 
+    def rollout_closed_terminal_streams(self, mt_key, mt_pos, has_gauss, gauss, n_per_stream: int, upper_bound: int,
+                                        coins_per_eval: int, ac_std: float, table, theta, sigma: float, layer_sizes: Sequence[int],
+                                        ob_mean, ob_std, ob_clip: float, obs0, env_a, env_b, rew_vec, pos_scale: float, fit_pos,
+                                        fit_neg, fit_stride: int = 1, behv_pos=None, behv_neg=None, save_obs_chance: float = 0.0,
+                                        ob_sum=None, ob_sumsq=None, ob_count=None, head=None, episodes: int = 1, activation=None,
+                                        fall_height: float = None, idx_out=None, coin_out=None, steps=None, noise_used=None,
+                                        noise_trace=None):
+        """``draw_noisy`` and ``rollout_closed_terminal`` in one launch (es_rollout_closedloop_terminal_streams), for action noise
+        (``ac_std`` != 0) on an env whose episodes end early: every stream (mt_key int32 [R, 624], mt_pos / has_gauss int32
+        [R], gauss float64 [R], updated in place) draws, per pair, its index, then per sign ``coins_per_eval`` (0 or 1) coins
+        and randn(act) for each step its episodes execute, in the reference's order.  Fitness, behaviour, ObStat, ``steps`` and
+        ``noise_used`` as ``rollout_closed_terminal`` for the R * n_per_stream pairs, stream-major.  ``noise_trace`` (float32
+        [R * n, 2, episodes * T * act] or None) receives the noise each executed step added.  A binned head draws no noise and
+        is refused.  Returns (idx int64 [R * n], coin words int32 [R * n, 4] or None, steps, noise_used)."""
+        if head is not None and head != 'tanh':
+            raise ValueError('a binned head draws no action noise (FFBinned.forward ignores rs): use rollout_closed_terminal')
+        if int(coins_per_eval) not in (0, 1):
+            raise ValueError(f'fit_fns draw at most one save_obs coin per evaluation, got coins_per_eval={coins_per_eval}')
+        if fall_height is None:
+            raise ValueError('rollout_closed_terminal_streams needs a fall_height')
+        if not float(ac_std):
+            raise ValueError('rollout_closed_terminal_streams draws action noise: ac_std must be != 0 (else use '
+                             'draw_indices and rollout_closed_terminal)')
+        episodes = int(episodes)
+        if episodes < 1:
+            raise ValueError(f'episodes must be >= 1, got {episodes}')
+        d = self.device
+        R = mt_key.shape[0]
+        _req(mt_key, torch.int32, 'mt_key', d); _req(mt_pos, torch.int32, 'mt_pos', d)
+        _req(has_gauss, torch.int32, 'has_gauss', d); _req(gauss, torch.float64, 'gauss', d)
+        assert mt_key.shape == (R, ES_MT_N) and mt_pos.numel() == R and has_gauss.numel() == R and gauss.numel() == R
+        n = R * int(n_per_stream)
+        if idx_out is None:
+            idx_out = self.empty((n,), torch.int64)
+        if coins_per_eval and coin_out is None:
+            coin_out = self.empty((n, 4), torch.int32)
+        _req(idx_out, torch.int64, 'idx_out', d)
+        assert idx_out.numel() == n
+        if coin_out is not None:
+            _req(coin_out, torch.int32, 'coin_out', d)
+            assert coin_out.numel() == 4 * n
+        _, ls = self._check_rollout(table, idx_out, theta, layer_sizes, fit_pos, fit_neg, fit_stride, behv_pos, behv_neg)
+        act = int(layer_sizes[-1])
+        T, band = self._check_closed_env(n, layer_sizes, act, ob_mean, ob_std, obs0, env_a, env_b, rew_vec, None, ob_sum, ob_sumsq,
+                                         ob_count)
+        if steps is None:
+            steps = self.empty((2, n), torch.int32)
+        _req(steps, torch.int32, 'steps', d)
+        assert steps.numel() == 2 * n
+        if noise_used is not None:
+            _req(noise_used, torch.int64, 'noise_used', d)
+            assert noise_used.numel() == 2 * n
+        if noise_trace is not None:
+            _req(noise_trace, torch.float32, 'noise_trace', d)
+            assert noise_trace.numel() == n * 2 * episodes * T * act
+        kind, param = (_lib.ES_ACT_TANH, 0.0) if activation is None else (int(activation.kind), float(activation.param))
+        check(self.lib.es_rollout_closedloop_terminal_streams(
+            self._ctx, _ptr(mt_key), _ptr(mt_pos), _ptr(has_gauss), _ptr(gauss), R, int(n_per_stream), int(upper_bound),
+            int(coins_per_eval), float(ac_std), _ptr(table), table.numel(), _ptr(theta), theta.numel(), float(sigma), ls,
+            len(layer_sizes) - 1, _ptr(ob_mean), _ptr(ob_std), float(ob_clip), _ptr(obs0), _ptr(env_a), int(band), _ptr(env_b),
+            _ptr(rew_vec), T, float(pos_scale), float(save_obs_chance), _ptr(idx_out), _ptr(coin_out), _ptr(fit_pos), _ptr(fit_neg),
+            int(fit_stride), _ptr(behv_pos), _ptr(behv_neg), _ptr(ob_sum), _ptr(ob_sumsq), _ptr(ob_count), 0, kind, param, episodes,
+            float(fall_height), _ptr(steps), _ptr(noise_used), _ptr(noise_trace), self.stream), 'es_rollout_closedloop_terminal_streams')
+        return idx_out, coin_out, steps, noise_used
+
     def closed_mlp_plan(self, layer_sizes: Sequence[int], band: int, head=None, activation=None):
         """How ``rollout_closed_mlp`` runs a shape: (CTAs per cluster, clusters resident at once, shared memory bytes per CTA);
         (0, SM count, 0) for ``rollout_closed``'s one-CTA kernel.  Raises EsLibraryError for a shape it does not cover.

@@ -236,19 +236,22 @@ class DeviceGeneration:
         e = self.eng
         self._ensure_buffers(n_per_stream)
         self.version += 1
-        with self._timed('draw_indices'):
-            if self.ac_std != 0.0:
-                # indices, coins and the action noise of every rollout, in the reference's stream order (mt_gauss.cu); the
-                # episodes of one evaluation are back to back in the stream
-                nrm = self.episodes * self.T * self.act_dim
-                if self.act_noise is None or self.act_noise.shape != (self.k_local, 2, nrm):
-                    self.act_noise = None
-                    self.act_noise = self._alloc_act_noise(nrm)
-                e.draw_noisy(self.mt_key, self.mt_pos, self.mt_has, self.mt_gauss, n_per_stream, self.table.numel() - self.P,
-                             self.coins_per_eval, nrm, self.ac_std, self.idx, self.extras, self.act_noise)
-            else:
-                e.draw_indices(self.mt_key, self.mt_pos, n_per_stream, self.table.numel() - self.P, self.extra_words,
-                               self.idx, self.extras)
+        # action noise on an env whose episodes end early: the rollout draws the indices, coins and noise itself
+        streams_walk = self.closed is not None and self.fall_height is not None and self.ac_std != 0.0 and self.closed_act_noise
+        if not streams_walk:
+            with self._timed('draw_indices'):
+                if self.ac_std != 0.0:
+                    # indices, coins and the action noise of every rollout, in the reference's stream order (mt_gauss.cu); the
+                    # episodes of one evaluation are back to back in the stream
+                    nrm = self.episodes * self.T * self.act_dim
+                    if self.act_noise is None or self.act_noise.shape != (self.k_local, 2, nrm):
+                        self.act_noise = None
+                        self.act_noise = self._alloc_act_noise(nrm)
+                    e.draw_noisy(self.mt_key, self.mt_pos, self.mt_has, self.mt_gauss, n_per_stream, self.table.numel() - self.P,
+                                 self.coins_per_eval, nrm, self.ac_std, self.idx, self.extras, self.act_noise)
+                else:
+                    e.draw_indices(self.mt_key, self.mt_pos, n_per_stream, self.table.numel() - self.P, self.extra_words,
+                                   self.idx, self.extras)
         fp, fn = self.fit_local[0], self.fit_local[1]
         if self.closed is not None:
             if self.ac_std != 0.0 and not self.closed_act_noise:
@@ -257,11 +260,22 @@ class DeviceGeneration:
             noisy = self.ac_std != 0.0
             self._gen_stats.zero_()
             obs0, env_a, env_b = self.closed
-            if self.fall_height is not None:
-                if noisy:
-                    raise NotImplementedError('action noise on an env whose episodes end early cannot be drawn ahead: how many '
-                                              'gaussians an evaluation consumes is known when it has fallen (es.step and '
-                                              'es.test_params run such generations one evaluation at a time)')
+            if streams_walk:
+                # how many gaussians an evaluation consumes is known when it has fallen, so the next pair's draws cannot be
+                # made ahead: each stream's draws are walked inside the rollout, its evaluations in the reference's order
+                with self._timed('rollout'):
+                    e.rollout_closed_terminal_streams(
+                        self.mt_key, self.mt_pos, self.mt_has, self.mt_gauss, n_per_stream, self.table.numel() - self.P,
+                        self.coins_per_eval, self.ac_std, self.table, self.theta, self.sigma, self.layer_sizes, self.ob_mean,
+                        self.ob_std, self.ob_clip, obs0, env_a, env_b, self.rew_vec, self.pos_scale, fp, fn, self.n_obj,
+                        None if self.behv is None else self.behv[0], None if self.behv is None else self.behv[1],
+                        save_obs_chance=self.save_obs_chance, ob_sum=self.gen_sum if self.extra_words else None,
+                        ob_sumsq=self.gen_sumsq if self.extra_words else None,
+                        ob_count=self.gen_count if self.extra_words else None, episodes=self.episodes,
+                        activation=self.activation, fall_height=self.fall_height, idx_out=self.idx, coin_out=self.extras,
+                        steps=self.steps_dev)
+                self.steps_total.copy_(self.steps_dev.sum(dtype=torch.float64).view(1))
+            elif self.fall_height is not None:
                 with self._timed('rollout'):
                     e.rollout_closed_terminal(
                         self.table, self.idx, self.theta, self.sigma, self.layer_sizes, self.ob_mean, self.ob_std, self.ob_clip,

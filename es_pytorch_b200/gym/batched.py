@@ -18,6 +18,12 @@ exactly the single episode (E copies of a float32 sum exactly in float64, and (E
 run the fused device rollouts too (es_rollout_*_activation) -- in ``es.step``, ``es.test_params`` and this object's own
 call.  Off by default: such a policy then runs run_model's python loop with the module's own forward, as the reference does.
 
+``fuse_noisy_terminal``: a policy with action noise on an env whose episodes end early (``ClosedLoopEnv(fall_height=h)``) runs
+the whole generation in one launch that walks each stream's index, coin and noise draws inside the rollout
+(es_rollout_closedloop_terminal_streams), in ``es.step`` and ``es.test_params``.  Off by default: such a generation then runs
+one evaluation per launch with numpy's own gaussians.  The fused route's gaussians use CUDA's log (<= 1 ulp of float64), so a
+float32 noise value can differ from numpy's where it lies next to a rounding midpoint; this object's own call is unchanged.
+
 ``result`` is the TrainingResult adaptor the script's fit_fn builds (training_result.py:62-97): RewardResult (the default
 without an archive), MeanRewardResult, DistResult, XDistResult, NSResult (novelty alone) or NSRResult (reward and novelty,
 the default with an archive).  The fused generation computes the same column(s) on the device.
@@ -44,7 +50,7 @@ class BatchedRollout:
                  archive: Optional[np.ndarray] = None, nov_k: int = 10,
                  rank_streams: Optional[Sequence[np.random.RandomState]] = None,
                  rollout_mode: int = _lib.ES_ROLLOUT_F32, episodes: int = 1, result: Optional[type] = None,
-                 fuse_activations: bool = False):
+                 fuse_activations: bool = False, fuse_noisy_terminal: bool = False):
         if not (getattr(env, 'is_synthetic_openloop', False) or getattr(env, 'is_synthetic_closedloop', False)):
             raise TypeError('BatchedRollout needs a synthetic env (es_pytorch_b200.gym.synthetic_env: open- or closed-loop)')
         self.env = env
@@ -56,6 +62,7 @@ class BatchedRollout:
         self.rank_streams = list(rank_streams) if rank_streams is not None else None
         self.rollout_mode = rollout_mode
         self.fuse_activations = bool(fuse_activations)
+        self.fuse_noisy_terminal = bool(fuse_noisy_terminal)
         if isinstance(episodes, bool) or not isinstance(episodes, (int, np.integer)):
             raise TypeError(f'episodes must be an integer, got {episodes!r}')
         if episodes < 0:

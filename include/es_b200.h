@@ -315,6 +315,34 @@ int es_rollout_closedloop_terminal(es_ctx* ctx, const float* table, int64_t tabl
                                    double* ob_count, int bins, const float* low, const float* range, int activation,
                                    float act_param, const float* act_noise, int n_episodes, float fall_height, int32_t* steps,
                                    int64_t* noise_used, void* stream);
+/* es_draw_noisy followed by es_rollout_closedloop_terminal in ONE launch, for the case they cannot be split: action noise
+ * (ac_std != 0) on an env whose episodes end early.  The reference draws rs.randn(act) only for the steps it executes
+ * (src/nn/nn.py:47-48, src/gym/gym_runner.py:50-67), so where a pair's index lies in its stream (src/core/es.py:66-74) depends
+ * on where the stream's previous evaluations fell, and nothing can be drawn ahead.  Per stream, in the reference's order:
+ * randint(0, upper_bound) per pair, then for + and -: coins_per_eval (0 or 1) doubles and randn(act) per executed step of
+ * each of the n_episodes episodes, the noise float32(g * ac_std) added to the policy's outputs.  Clusters take whole streams
+ * (one at a time each: fewer streams than resident clusters leave part of the GPU idle) and walk their words, generated
+ * beforehand by MT19937 jump-ahead up to the no-fall consumption at es_draw_noisy's mean + 12 sigma (a walk past them makes
+ * es_check_async fail; a stream whose bound exceeds 2^20 blocks of 624 words is refused with the pairs per stream that fit).
+ *   mt_key / mt_pos / has_gauss / gauss   dev, in/out: the streams' RandomState.get_state()[1..4] (as es_draw_noisy)
+ *   idx_out   dev int64 [n_streams * n_per_stream]; coin_out dev uint32 [n_streams * n_per_stream][4] (coins_per_eval 1) or NULL
+ *   fit_pos .. ob_count, steps, noise_used: as es_rollout_closedloop_terminal for those pairs, stream-major
+ *   noise_trace  dev float [n_streams * n_per_stream][2][n_episodes T act] or NULL: the noise each executed step added, at
+ *                offset sum_{e' < e} (t_{d,e'} + 1) act + t act of its evaluation (other entries untouched; for tests)
+ * Every other argument is es_rollout_closedloop_terminal's; bins must be 0 (a binned head draws no noise).  Results equal
+ * drawing each evaluation's noise from a copy of its stream, rolling it out with es_rollout_closedloop_terminal and advancing
+ * the stream by noise_used gaussians; indices, coins, key, position and has_gauss bit-exact, the gaussians with CUDA's log
+ * (<= 1 ulp of float64: a float32 noise value can differ where it lies next to a rounding midpoint).                   */
+int es_rollout_closedloop_terminal_streams(es_ctx* ctx, uint32_t* mt_key, int32_t* mt_pos, int32_t* has_gauss, double* gauss,
+                                           int n_streams, int n_per_stream, uint64_t upper_bound, int coins_per_eval, double ac_std,
+                                           const float* table, int64_t table_len, const float* theta, int P, float sigma,
+                                           const int* layer_sizes, int n_layers, const double* ob_mean, const double* ob_std,
+                                           double ob_clip, const float* obs0, const float* env_a, int band, const float* env_b,
+                                           const float* rew_vec, int T, float pos_scale, double save_obs_chance, int64_t* idx_out,
+                                           uint32_t* coin_out, double* fit_pos, double* fit_neg, int fit_stride, float* behv_pos,
+                                           float* behv_neg, double* ob_sum, double* ob_sumsq, double* ob_count, int bins,
+                                           int activation, float act_param, int n_episodes, float fall_height, int32_t* steps,
+                                           int64_t* noise_used, float* noise_trace, void* stream);
 
 /* ---- a2 + a4 with action noise: all draws of a generation in stream order ---------------------------------------------
  * When FeedForward._action_std != 0 every step of every rollout draws rs.randn(act_dim) from the SAME RandomState that
